@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- sorted-KV GB/s of the Tez shuffle sort/merge hot path on B200 (BASELINE.json metric).
+"""bench.py -- sorted-KV GB/s of the Tez shuffle sort/merge hot path on H100 (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 N=1 workload = BASELINE config 2: 1e8 records, 16 B key / 64 B value, 64 partitions (HashPartitioner,
 TezBytesComparator) -> file.out bytes bit-identical to the reference format.  A "step" is one complete pass of the
@@ -13,6 +13,8 @@ hot path over that batch (partition + sort + IFile emit with CRC).
 N>1 (torchrun, one rank per GPU): BASELINE config 4 shape, weak scaling -- every rank sorts its own records into
 1024 partitions, partitions are exchanged with an all-to-all over NVLink (owner(p) = p*N/P), each rank merges the
 N runs of every partition it owns.
+--dump-outputs DIR (N=1, config 2): after the timed steps, writes what the last timed step computed as .npy files
+(float64, about 17 MB in all; see dump_outputs).
 --impl reference: the CPU restatement of PipelinedSorter (oracle/, "port") timed on the host cores.
 """
 import argparse
@@ -41,7 +43,7 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 class ClockSampler:
@@ -226,14 +228,31 @@ def workload_config(gpus, records, config=4):
             "l2": "inputs larger than L2, no flush needed"}
 
 
-def load_traffic():
-    p = os.path.join(ROOT, "profiles", "emit_traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:
-            return None
-    return None
+DUMP_SAMPLE = 1 << 20   # file.out bytes sampled by --dump-outputs
+
+
+def dump_outputs(out_dir, d_out, out_len, index):
+    """What the caller of tezgpu_sorter_sort_device_fixed receives, as float64 .npy files (about 17 MB in all):
+      index.npy           [P, 3] spill index (start offset, raw length, part length) of every partition
+      segment_crc32.npy   [P] CRC32 trailer of every non-empty partition segment (-1 for empty ones); covers every byte
+      file_out_sample.npy [DUMP_SAMPLE, 2] (offset, byte) of file.out at offsets drawn by a fixed-seed generator
+      file_out_len.npy    [1] length of file.out"""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    index = np.asarray(index, dtype=np.int64)
+    crc = np.full(len(index), -1.0)
+    ends = [int(a + c - 4) for a, _, c in index if c >= 4]
+    if ends:
+        t = torch.tensor(ends, dtype=torch.int64, device=d_out.device)
+        w = d_out[(t[:, None] + torch.arange(4, device=d_out.device)).flatten()].view(-1, 4).to(torch.int64).cpu().numpy()
+        crc[index[:, 2] >= 4] = (w[:, 0] << 24) | (w[:, 1] << 16) | (w[:, 2] << 8) | w[:, 3]
+    offs = np.sort(np.random.default_rng(12345).integers(0, out_len, DUMP_SAMPLE))
+    vals = d_out[torch.from_numpy(offs).to(d_out.device)].cpu().numpy()
+    np.save(os.path.join(out_dir, "index.npy"), index.astype(np.float64))
+    np.save(os.path.join(out_dir, "segment_crc32.npy"), crc)
+    np.save(os.path.join(out_dir, "file_out_sample.npy"), np.stack([offs, vals]).T.astype(np.float64))
+    np.save(os.path.join(out_dir, "file_out_len.npy"), np.array([out_len], dtype=np.float64))
 
 
 def single_gpu(args):
@@ -274,14 +293,15 @@ def single_gpu(args):
     ms_step = ev0.elapsed_time(ev1) / args.steps
     value = n * REC / (ms_step * 1e-3) / 1e9
     assert out_len == n * OUT_REC + 10 * int((index[:, 1] > 0).sum())
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, d_out, out_len, index)
 
     peak, peak_src = hbm_peak()
     emit = sum(emit_ms) / len(emit_ms)
     achieved = n * ALGO_BYTES_PER_RECORD / (emit * 1e-3) / 1e9
-    traffic = load_traffic()
     roofline = {"bound": "hbm", "kernel": "k_emit_fast4<5,1> (software-pipelined gather + IFile framing + CRC32 + coalesced store)",
                 "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 4),
-                "traffic": traffic["dram_bytes_per_launch"] if traffic else None, "peak_source": peak_src,
+                "traffic": None, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": n * ALGO_BYTES_PER_RECORD, "ms_per_launch": round(emit, 4)}
     pipeline = {"algorithmic_bytes_per_step": n * ALGO_BYTES_PER_RECORD,
                 "achieved": round(n * ALGO_BYTES_PER_RECORD / (ms_step * 1e-3) / 1e9, 1),
@@ -330,6 +350,7 @@ def single_gpu(args):
         mg[0].close()
         s4.close()
         del d_out4, d_merged
+        torch.cuda.empty_cache()       # the e2e leg's sorters allocate outside torch's caching allocator
 
     # ---- e2e through the C ABI with host buffers (pinned), H2D + D2H inside the timed region.
     # Two task slots (as a node runs several map tasks per GPU): each slot is one sorter handle doing
@@ -555,17 +576,23 @@ def main():
                          "5 (Zipf keys, 4 KB values, 256 partitions; any --gpus)")
     ap.add_argument("--c1-text-mb", type=int, default=100)
     ap.add_argument("--c3-segments", type=int, default=256)
-    ap.add_argument("--c3-segment-mb", type=int, default=64)
+    ap.add_argument("--c3-segment-mb", type=int, default=32,
+                    help="MiB per segment (32: 8 GiB of segments; their parse and sort workspace and the output fit 80 GB)")
     ap.add_argument("--c3-cpu-segments", type=int, default=16)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="N=1, config 2: write the last timed step's spill index, segment CRC32s and a seeded sample of "
+                         "file.out to DIR/*.npy")
     args = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.records is None:
         if args.config == 5:
-            args.records = 4_000_000      # 16.4 GB of records per GPU
+            args.records = 2_000_000      # 8.2 GB of records per GPU (inputs, output slots and merge buffers fit 80 GB)
         else:
             args.records = 100_000_000 if (args.gpus == 1 and world == 1) else 125_000_000
     if args.warmup < 3 and args.impl != "reference":
         args.warmup = 3
+    if args.dump_outputs and (args.impl == "reference" or args.config != 2 or args.gpus != 1 or world != 1):
+        ap.error("--dump-outputs is implemented for the single-GPU config 2 line")
     if args.impl == "reference":
         return reference_arm(args)
     if args.config == 1:

@@ -1,5 +1,5 @@
 /*
- * tezgpu.h -- C ABI of libtezgpu.so: B200-native (sm_100a) replacement of the Tez shuffle sort/merge hot path.
+ * tezgpu.h -- C ABI of libtezgpu.so: H100-native (sm_90a) replacement of the Tez shuffle sort/merge hot path.
  *
  * This is the drop-in boundary (SURVEY.md 8b).  Plain pointers and sizes only -- no torch / C++ types.
  * Each entry point names the reference interface it replaces.  Paths are relative to

@@ -1,4 +1,4 @@
-"""tez_b200 -- B200-native (sm_100a) implementation of Apache Tez's shuffle sort/merge hot path.
+"""tez_b200 -- H100-native (sm_90a) implementation of Apache Tez's shuffle sort/merge hot path.
 
 The compute path lives in libtezgpu.so (hand-written CUDA behind the C ABI of include/tezgpu.h).
 This package is the host-side mirror used where no JVM exists; it never falls back to CPU code.

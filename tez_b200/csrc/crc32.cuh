@@ -107,7 +107,7 @@ static inline void crc_build_tables(CrcTables &t, int stride_words) {
 // ---------------------------------------------------------------------------------------------- warp-resident maps
 // Every step of the interleaved checksum is a GF(2)-linear map of a 32-bit word ("multiply by a fixed power of x"),
 // classically four 256-entry table look-ups in shared memory.  Random byte values make those look-ups collide on
-// banks (measured: 58 % of the emit kernel's shared-load wavefronts were replays).  The same map split into seven
+// banks and replay.  The same map split into seven
 // 5-bit digits needs only 32-entry tables, and a 32-entry table is exactly one register across the lanes of a warp:
 // digit k of x selects lane (x >> 5k) & 31 of register t[k] with one SHFL -- no shared memory, no conflicts.
 // All 32 lanes must execute apply() together (lanes with nothing to fold pass 0, which maps to 0).
@@ -142,9 +142,8 @@ struct WarpLinearMap {
 // with W instead of S in the textbook form; the two-deep form applies S there too and the constant factor
 // x^(128*(T-1)) this adds to every partial is divided out once, in the per-lane alignment multiplier of the final fold
 // (CrcTables::einv; the inverse exists because the CRC-32 polynomial is primitive: tests/test_abi_cpu.py).
-// The third digit table costs 7 registers: measured on B200, kernels already at their register cap lose more to the
-// spills than they gain (k_emit_fast4 at 80 registers: 5.44 -> 6.94 ms, k_emit_fast4u 8.5 -> 9.8 ms), kernels with
-// headroom gain a little (k_emit_runs 8.98 -> 8.85 ms).  Hence a template flag per kernel.
+// The third digit table costs 7 registers: kernels already at their register cap (k_emit_fast4, k_emit_fast4u at 80)
+// spill, kernels with headroom can afford the shorter chain.  Hence a template flag per kernel.
 template <bool ILP>
 struct CrcChunkFoldT {
   WarpLinearMap w, s;

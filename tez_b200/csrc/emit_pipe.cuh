@@ -1,8 +1,7 @@
 // emit_pipe.cuh -- software-pipelined variant of the source-oriented emit kernel (emit_fast.cuh) for packed,
 // 16-byte aligned fixed-width records.
 //
-// What the profile of k_emit_fast showed (profiles/r01_emit_shfl_*): no pipe saturated (LSU data pipe 65 %, issue 53 %),
-// 25 % of the warp samples waiting on the gather's global loads, 19 % at barriers (11 % of it behind warp 0 folding
+// k_emit_fast saturates no pipe: its warps wait on the gather's global loads and at barriers (behind warp 0 folding
 // the tile's partial checksums while seven warps idle).  This kernel keeps the same tile algorithm and byte-exact
 // output but reorders the work of a persistent CTA:
 //   * the 128-bit gather loads of tile N+1 are issued into registers BEFORE the checksum / write-out loop of tile N
@@ -333,7 +332,7 @@ __global__ void __launch_bounds__(FE_THREADS * SUBS, SUBS > 1 ? 1 : TEZGPU_EMIT4
     if (!has1) break;
     // the descriptor prefetches are consumed HERE: without this the compiler renames them straight into the next
     // iteration, where their scoreboard is shared with the freshly issued gather loads and the first use stalls on
-    // those (measured: 20 % of all warp samples on one integer add in the middle of the gather)
+    // those (the first use of a prefetched descriptor then waits for the whole gather)
     asm volatile("" : "+r"(nr2n), "+r"(fl2n), "+l"(abs2n), "+r"(r0_3), "+r"(nr3));
     nr0 = nr1; fl0 = fl1; abs0 = abs1;
     nr1 = nr2n; fl1 = fl2n; abs1 = abs2n;

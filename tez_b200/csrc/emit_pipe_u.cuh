@@ -8,12 +8,12 @@
 //   * the loads of tile N+1 are issued before the checksum loop of tile N; source offsets (two dependent global loads:
 //     sorted order -> record index -> byte offset) are fetched three / two tiles ahead;
 //   * batched second-level checksum folds, two barriers per tile (as emit_pipe.cuh).
-// Measured on the batched reduce-side merge of 1e8 records (tools/merge_profile.py): 7.88 ms against 9.78 ms for
-// k_emit_fast<5,false>.  TEZGPU_EMIT_PIPE_UNALIGNED=0 selects the older kernel.
+// TEZGPU_EMIT_PIPE_UNALIGNED=0 selects the older kernel k_emit_fast<5,false> (tools/merge_profile.py times the
+// batched reduce-side merge both ways).
 //
 // The checksum / write-out loop and the batched fold are the same text as in k_emit_fast4 on purpose: moving them into
-// shared __device__ functions changed ptxas' register allocation (spill stores 28 -> 136 bytes in k_emit_fast4<5,1>,
-// 72 -> 132 here), so the duplication stays until that can be re-measured.
+// shared __device__ functions changed ptxas' register allocation (more spill stores in both kernels), so the
+// duplication stays until that can be re-measured.
 #pragma once
 #include "emit_pipe.cuh"
 

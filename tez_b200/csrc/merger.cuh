@@ -1,4 +1,4 @@
-// merger.cuh -- reduce side of the hot path on sm_100a: k-way merge of sorted IFile segments.
+// merger.cuh -- reduce side of the hot path on sm_90a: k-way merge of sorted IFile segments.
 // Device counterpart of TezMerger.MergeQueue (SORT/TezMerger.java:465-1065): segments are checksum-verified and
 // parsed on the device, the union of their records is ordered with the same radix-sort + key-refinement machinery
 // as the map side (a stable sort of already sorted runs IS their k-way merge: equal keys keep (segment, position)
@@ -631,7 +631,7 @@ class Merger {
     ParseArrays pa{d_koff.as<uint64_t>(), d_voff.as<uint64_t>(), d_klen.as<uint32_t>(), d_vlen.as<uint32_t>(), d_tag.as<uint32_t>(), d_part.as<int32_t>()};
     if (n) {
       const uint32_t hl = vint_size_u32(fixed_klen) + vint_size_u32(fixed_vlen);
-      k_fill_fixed_arrays<<<(uint32_t)std::min<uint64_t>(div_up(n, 256), 148 * 16), 256, 0, st>>>(
+      k_fill_fixed_arrays<<<(uint32_t)std::min<uint64_t>(div_up(n, 256), (uint64_t)pipe.num_sms * 16), 256, 0, st>>>(
           d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), fixed_klen, fixed_vlen, hl, pa);
       launches++;
       TG_CUDA(cudaGetLastError());

@@ -137,10 +137,10 @@ struct PwWalk {
 // EMIT: PW_EMIT_GROUP lanes walk the SAME window from the same entry (identical control flow, broadcast loads) and lane
 // (record number mod PW_EMIT_GROUP) writes that record's metadata: consecutive records go out from consecutive lanes
 // within a few iterations, so every 32-byte sector of the six output arrays is completed while it is still in L2.
-// One THREAD per window had 483 k windows x 6 arrays = 2.9 M concurrent write streams -- 370 MB of open cache lines,
-// more than the L2 -- and ran at 140 GB/s of useful writes (144 ms of config 3's step); a whole warp per window
-// removed that but issued every walk instruction once per window instead of once per 32 windows (109 ms).  Groups of
-// eight lanes keep four windows per warp and ~230 k open lines (29 MB).
+// One THREAD per window keeps 483 k windows x 6 arrays = 2.9 M concurrent write streams open at config 3 -- 370 MB of
+// partial cache lines, more than the L2; a whole warp per window avoids that but issues every walk instruction once
+// per window instead of once per 32 windows.  Groups of eight lanes keep four windows per warp and ~230 k open lines
+// (29 MB).
 template <bool EMIT>
 __device__ __forceinline__ PwWalk pw_walk(const uint8_t *__restrict__ seg, const PwSeg &sd, uint32_t s, uint64_t wend, bool last_win,
                                           uint64_t e, uint64_t base, uint64_t carry_off, uint64_t carry_len, const PwArrays &out,
@@ -237,8 +237,8 @@ struct PwFixedHint {
 // survives usually fell into step with the true chain (two walks are identical from the first (position, state) they
 // share) and so reports the true exit.  The exceptions are flukes that decode a large length and "survive" by jumping
 // out of the window, and walks in the "previous record was a repeat" state, which read every byte they land on as a
-// value length and hop on for a long time (measured on word-count data: 5 % wrong guesses when the first survivor is
-// taken).  Hence:
+// value length and hop on for a long time (on word-count data, taking the first survivor guesses wrong for a few
+// percent of the windows).  Hence:
 //   * EOF markers count only where a well-formed body has them (its last two bytes);
 //   * an exit beyond the NEXT window is only the fallback (records longer than a window are rare; when they exist every
 //     walk on the true chain reports the same far exit and the fallback is right);

@@ -1,10 +1,10 @@
-// radix_sort.cuh -- hand-written LSD radix sort for sm_100a ("onesweep": one read + one write of the data per
+// radix_sort.cuh -- hand-written LSD radix sort for sm_90a ("onesweep": one read + one write of the data per
 // 8-bit digit, chained-scan with decoupled look-back across tiles, warp-match ranking, shared-memory reorder so the
 // scatter leaves the SM as contiguous per-digit runs).
 //
-// Tried in round 2 and reverted: a second instantiation of the tile body without the per-item validity predicates
-// (every tile but the last is full) -- 27 % fewer SASS instructions in that path, but the pass got SLOWER on the B200
-// (4 passes 2.30 -> 2.44 ms at 1e8 pairs; twice the code for the instruction cache of a kernel that is issue-bound).
+// Tried and reverted: a second instantiation of the tile body without the per-item validity predicates (every tile but
+// the last is full) -- fewer SASS instructions in that path, but twice the code for the instruction cache of a kernel
+// that is issue-bound, and the pass got slower.
 //
 // Used by the sorter for the (partition|key-prefix, record-index) pairs of the hot path -- the device counterpart of
 // PipelinedSorter's per-span QuickSort + SpanMerger (SORT/PipelinedSorter.java:965-1023,1116-1503) -- and by the
@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS)
 
   // Tile id = block index: blocks of a 1-D grid are dispatched in index order, which is what the look-back's forward
   // progress needs (same assumption as CUB's decoupled look-back scan).  A global ticket counter costs one same-address
-  // atomic per tile -- measured ~20 ns each, i.e. 0.25 ms of a 0.58 ms pass at 12 K tiles.
+  // atomic per tile, serialised on one address across all tiles of a pass.
 #ifdef TEZGPU_TICKET_ATOMIC
   if (tid == 0) s_misc[0] = atomicAdd(tile_counter, 1u);
 #else

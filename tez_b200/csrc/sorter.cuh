@@ -20,8 +20,8 @@ namespace tezgpu {
 
 // Small device -> host results (flags, counters, the spill index) are WRITTEN BY A KERNEL into mapped pinned memory
 // instead of going through cudaMemcpyAsync: a tiny copy is queued on a copy engine, and when another task slot's
-// multi-GB upload occupies that engine the sort's one host round trip waits for all of it (measured: a flush next to
-// another slot's upload took 297 ms = 144 ms behind the upload + 153 ms of its own; tools/e2e_probe.py).
+// multi-GB upload occupies that engine the sort's one host round trip waits for all of it (tools/e2e_probe.py shows
+// the timeline of two task slots).
 __global__ void k_store_to_host(uint32_t *__restrict__ dst0, const uint32_t *__restrict__ src0, uint32_t n0, uint32_t *__restrict__ dst1,
                                 const uint32_t *__restrict__ src1, uint32_t n1, uint32_t *__restrict__ dst2,
                                 const uint32_t *__restrict__ src2, uint32_t n2) {
@@ -70,7 +70,7 @@ class SortPipeline {
   int pbits;
   cudaStream_t stream = nullptr;
   EventTimer timer;
-  int num_sms = 148;
+  int num_sms = 132;
 
   // workspace (grow-only, reused across flushes)
   DeviceBuffer keysA, keysB, valsA, valsB, same, blk, small, tile_state, sizes, rec_off;
@@ -95,7 +95,7 @@ class SortPipeline {
     TG_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
     TG_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, c.device));
     // The path is dominated by sparse reads (16-byte keys out of 80-byte records, 80-byte record gathers): ask L2 to
-    // fetch 32-byte sectors instead of wider granules (measured: stage 1.28 -> 0.70 ms).  TEZGPU_L2_FETCH=0 leaves
+    // fetch 32-byte sectors instead of wider granules (k_stage reads 16 of every 80 bytes).  TEZGPU_L2_FETCH=0 leaves
     // the device limit untouched, any other value overrides.
     {
       const char *g = getenv("TEZGPU_L2_FETCH");
@@ -143,7 +143,7 @@ class SortPipeline {
   bool merge_inputs_plain = false;
   uint32_t merge_max_runs = 0;   // run-table mode: most runs any output partition has (emit_runs.cuh plans <= 32 per warp)
   static bool runs_emit_enabled() {
-    // opt-in: measured 8.85 ms per 1e8 records against 8.55 ms for the pipelined gather (emit_pipe_u.cuh), DESIGN.md 7
+    // opt-in: the pipelined gather (emit_pipe_u.cuh) is the default for these records
     static const bool on = getenv("TEZGPU_EMIT_RUNS") && atoi(getenv("TEZGPU_EMIT_RUNS")) != 0;
     return on;
   }
@@ -169,7 +169,7 @@ class SortPipeline {
     return e;
   }
   static bool pipe_unaligned_enabled() {
-    // on by default (measured: 9.8 -> 7.9 ms for the 1e8-record reduce-side emit); TEZGPU_EMIT_PIPE_UNALIGNED=0 falls back
+    // on by default; TEZGPU_EMIT_PIPE_UNALIGNED=0 falls back to k_emit_fast<5,false>
     static const bool on = !(getenv("TEZGPU_EMIT_PIPE_UNALIGNED") && atoi(getenv("TEZGPU_EMIT_PIPE_UNALIGNED")) == 0);
     return on;
   }
@@ -304,7 +304,7 @@ class SortPipeline {
       TG_CUDA(cudaMemsetAsync(same.p, 0, n, stream));
       const bool fast16 = rec.fixed && !rec.key_off && !rec.use_runs && rec.klen == 16 && ((rec.klen + rec.vlen) % 16 == 0) && rec.cmp == CMP_BYTES &&
                           (((uintptr_t)rec.kv & 15u) == 0);
-      int sgrid = (int)std::min<uint64_t>(div_up(n, 256), 148 * 16);
+      int sgrid = (int)std::min<uint64_t>(div_up(n, 256), (uint64_t)num_sms * 16);
       if (fast16) k_stage<true><<<sgrid, 256, 0, stream>>>(rec, K, d_hist(), d_error());
       else k_stage<false><<<sgrid, 256, 0, stream>>>(rec, K, d_hist(), d_error());
       TG_CUDA(cudaGetLastError());
@@ -427,7 +427,7 @@ class SortPipeline {
           k_ref_build_keys<<<(uint32_t)div_up(m, 256), 256, 0, stream>>>(rec, t_gid[cur].as<uint32_t>(), t_lidx[cur].as<uint32_t>(), m,
                                                                     depth, t_key64[0].as<uint64_t>());
           TG_CUDA(cudaMemsetAsync(d_hist(), 0, 8 * RADIX * 4, stream));
-          k_radix_hist<uint64_t, 8><<<(int)std::min<uint64_t>(div_up(m, 512 * 8), 148 * 4), 512, 0, stream>>>(t_key64[0].as<uint64_t>(), m, 0, d_hist());
+          k_radix_hist<uint64_t, 8><<<(int)std::min<uint64_t>(div_up(m, 512 * 8), (uint64_t)num_sms * 4), 512, 0, stream>>>(t_key64[0].as<uint64_t>(), m, 0, d_hist());
           k_radix_scan_hist<<<1, RADIX, 0, stream>>>(d_hist(), 8, m, d_trivial());
           launches += 3;
           TG_CUDA(cudaGetLastError());
@@ -570,10 +570,9 @@ class SortPipeline {
     if (tiles) {
       if (fast_emit) {
         int per_sm = 0;
-        // opt-in (TEZGPU_EMIT_TMA=1): byte-exact (68 GPU parity tests), but measured 15.4 ms against 5.45 ms for the
-        // register-staged kernel on 1e8 records -- the bulk-copy gather itself is as fast as the LDG gather
-        // (tools/bench_gather.cu: 4.4 ms either way, the memory system's rate for random 80-byte reads), the warp-divergent
-        // chunk assembly of the consumers is what costs (profiles/README.md, round 2)
+        // opt-in (TEZGPU_EMIT_TMA=1): byte-exact (the GPU parity tests run it), but slower than the register-staged
+        // kernel -- the bulk-copy gather itself is no faster than the LDG gather (tools/bench_gather.cu times both), and
+        // bulk copies are warp-uniform instructions whose per-record issue and chunk assembly cost more than they save
         static const bool use_tma = getenv("TEZGPU_EMIT_TMA") && atoi(getenv("TEZGPU_EMIT_TMA")) != 0;
         if (fast_aligned && use_tma && emit_tma_fits(e.recs_per_tile, stride)) {
           // gather by the bulk-copy engine into a shared-memory ring, chunks assembled straight from the staged
@@ -590,8 +589,8 @@ class SortPipeline {
         } else if (fast_aligned && emit4_fits(e.recs_per_tile, fp.cpr) && !getenv("TEZGPU_EMIT_V2")) {
           // software-pipelined kernel (emit_pipe.cuh): a tile's pieces must fit the registers of one gather round.
           // Default: independent 256-thread CTAs, three per SM.  TEZGPU_EMIT_SUBS=3 selects the variant with one CTA
-          // per SM whose three groups share lane-private checksum tables -- measured SLOWER (8.39 vs 5.44 ms): its
-          // 219 KB of shared memory leave the SM ~30 KB of L1 and the random gather loses its memory-level parallelism.
+          // per SM whose three groups share lane-private checksum tables -- slower: its 219 KB of shared memory leave
+          // the SM little L1 and the random gather loses its memory-level parallelism.
           static const bool subs1 = !(getenv("TEZGPU_EMIT_SUBS") && atoi(getenv("TEZGPU_EMIT_SUBS")) == 3);
           if (!subs1) {
             constexpr int SUBS = 3;

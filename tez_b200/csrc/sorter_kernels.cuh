@@ -1,4 +1,4 @@
-// sorter_kernels.cuh -- map-output side of the hot path on sm_100a:
+// sorter_kernels.cuh -- map-output side of the hot path on sm_90a:
 //   stage (key -> partition, sort word)  ->  onesweep radix sort  ->  tie refinement on key suffixes
 //   ->  partition bounds / layout  ->  gather + IFile emit (vint framing, RLE markers, per-segment CRC32).
 // Device counterpart of PipelinedSorter.collect/sort/spill + IFile.Writer

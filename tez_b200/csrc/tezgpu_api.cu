@@ -262,8 +262,8 @@ static void sorter_run(tezgpu_sorter *h, uint8_t *host_out, uint64_t out_cap, ui
   st.output_bytes = (int64_t)h->payload_bytes;
   TG_CHECK(len <= out_cap, TEZGPU_E_NOMEM, "output buffer too small for file.out");
   if (len) {
-    // one copy, not pieces: with 64 MB pieces a download running next to another task slot's upload was measured at
-    // 26 GB/s (312 ms) instead of 40-47 GB/s (tools/e2e_probe.py, profiles/r02_e2e_probe*.log)
+    // one copy, not pieces: 64 MB pieces of a download running next to another task slot's upload were slower than
+    // one whole copy (tools/e2e_probe.py)
     TG_CUDA(cudaMemcpyAsync(host_out, h->d_out.p, len, cudaMemcpyDeviceToHost, h->pipe.stream));
     TG_CUDA(cudaStreamSynchronize(h->pipe.stream));
   }
@@ -418,7 +418,7 @@ int32_t tezgpu_fetch_ranges(int32_t device, const tezgpu_copy_range *ranges, uin
     cudaEventRecord(e0, st);
   }
   if (err == cudaSuccess) {
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     uint32_t grid = (uint32_t)std::min<uint64_t>(chunks, (uint64_t)sms * 2);
     grid = fetch_grid_cap(grid);
@@ -495,7 +495,7 @@ int32_t tezgpu_fetch_segments_verified(int32_t device, const tezgpu_fetch_segmen
     cudaEventCreate(&e1);
     cudaEventRecord(e0, st);
   }
-  int sms = 148, per_sm = 0;
+  int sms = 132, per_sm = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fetch_verify, FV_THREADS, 0);
   const uint32_t grid = fetch_grid_cap((uint32_t)std::min<uint64_t>(np, (uint64_t)sms * (per_sm > 0 ? per_sm : 1)));

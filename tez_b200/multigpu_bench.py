@@ -108,9 +108,9 @@ def run(args, workload_config, ClockSampler, hbm_peak, run_cpu, host_cores, veri
     overlap = px is not None and os.environ.get("TEZ_SHUFFLE_OVERLAP", "0") == "1"
     if overlap:
         import threading
-        # a pull grid that fills every SM serialises with the sort kernels instead of overlapping (measured: exchange =
-        # sort + pull); about one CTA per SM keeps NVLink busy and leaves the other half of each SM to the sort
-        os.environ.setdefault("TEZGPU_FETCH_CTAS", "148")
+        # a pull grid that fills every SM serialises with the sort kernels instead of overlapping (exchange = sort +
+        # pull); about one CTA per SM keeps NVLink busy and leaves the other half of each SM to the sort
+        os.environ.setdefault("TEZGPU_FETCH_CTAS", str(torch.cuda.get_device_properties(dev).multi_processor_count))
         pull_stream = torch.cuda.Stream(device=dev)
         pending = {}
 
@@ -229,7 +229,7 @@ def run(args, workload_config, ClockSampler, hbm_peak, run_cpu, host_cores, veri
                            "achieved_GBps_per_gpu": round(sent / (avg["exchange"] * 1e-3) / 1e9, 1) if avg["exchange"] else None,
                            "fetch_kernel_ms": round(sum(fetch_ms) / len(fetch_ms), 3) if fetch_ms else None,
                            "fetch_kernel_GBps_per_gpu": round(sent / (sum(fetch_ms) / len(fetch_ms) * 1e-3) / 1e9, 1) if fetch_ms and sum(fetch_ms) else None,
-                           "transport": transport + (" + sort(k+1) overlapped with pull(k)" if overlap else ""), "reference_GBps": 770,
+                           "transport": transport + (" + sort(k+1) overlapped with pull(k)" if overlap else ""),
                            "note": ("peer pull: index all-gather (NCCL) + one fetch kernel over CUDA IPC mappings; own partitions merged in place"
                                     if px else "variable-size all-to-all (NCCL send/recv) incl. index all-gather")},
                 "roofline": {"bound": "hbm", "achieved": round(n * (2 * (REC + OUT_REC)) / (ms_step * 1e-3) / 1e9, 1), "peak": peak,

@@ -72,8 +72,7 @@ def pull_plan(all_idx, rank, num_partitions, peer_ptrs):
     """What rank `rank` pulls: all_idx is the gathered [world, P, 3] spill index, peer_ptrs[g] the address of rank g's
     file.out in this process.  Returns (ranges, seg_src, need): ranges = [(g, src_address, offset_in_receive_buffer,
     nbytes)], one per producer, in ring order starting at rank+1 (the classic all-to-all schedule: at any moment every
-    producer's HBM / NVLink egress serves one consumer instead of all consumers pulling from rank 0 first -- measured
-    at 4 GPUs with the naive order: the fetch kernel took 9.1 ms on one rank and 19.7 ms on another);
+    producer's HBM / NVLink egress serves one consumer instead of all consumers pulling from rank 0 first);
     seg_src[g] = (receive offset, file offset) of g's range; need = receive buffer bytes.  Receive offsets agree
     with the source address modulo 16 so the copy moves 128-bit words (the receive buffer is 16-byte aligned)."""
     world = all_idx.shape[0]
@@ -199,7 +198,7 @@ class PeerExchange:
             src_of = {g: (peer_ptrs[g] + a) - (base + off) for g, (off, a) in seg_src.items()}   # src - dst per producer
             # ring order, like pull_plan: producer rank+1 first, so that at any moment a producer serves one consumer
             # (the segment table itself is ordered by source rank -- pulling in THAT order sends all consumers to rank 0
-            # first: measured at 8 GPUs, the pull kernel took 15 ms on the luckiest rank and 47 ms on the others)
+            # first, and every rank but the first waits for the others)
             remote = [(ptr + src_of[g], ptr, ln) for ptr, ln, _, g in ring_order(segs, self.rank, self.world)]
             self.last_fetch_ms = native.fetch_segments_verified(remote, self.device, stream)
             self.last_verified = [g != self.rank for _, _, _, g in segs]

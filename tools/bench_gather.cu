@@ -1,10 +1,12 @@
 // bench_gather.cu -- ceiling for the emit kernel's memory pattern: out[i] = in[perm[i]] for 80-byte records
 // (16-byte pieces, 5 lanes per record, streaming stores), no checksum, no framing.  Prints ms and GB/s moved.
-// build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/bench_gather tools/bench_gather.cu
+// build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/bench_gather tools/bench_gather.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
+
+static int g_sms = 132;   // SM count of the device, read in main()
 
 __device__ __forceinline__ uint4 ldg_stream_v4(const void *p) {
   uint4 r;
@@ -159,7 +161,7 @@ static void run_tma(const uint8_t *in, const uint32_t *perm, uint8_t *out, uint3
   const uint32_t ntiles = n / TILE_RECS;
   for (int rep = 0; rep < 2; rep++) {
     cudaEventRecord(e0);
-    k_gather_tma<STAGES, MODE, PW, CW><<<148 * ctas_per_sm, 32 * (PW + CW), smem>>>(in, perm, out, ntiles);
+    k_gather_tma<STAGES, MODE, PW, CW><<<g_sms * ctas_per_sm, 32 * (PW + CW), smem>>>(in, perm, out, ntiles);
     cudaEventRecord(e1);
     cudaEventSynchronize(e1);
     float ms;
@@ -191,14 +193,15 @@ __global__ void k_fill_data(uint32_t *p, uint64_t words) {
 }
 
 int main(int argc, char **argv) {
+  cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0);
   const uint32_t n = argc > 1 ? (uint32_t)atoll(argv[1]) : 100000000u;
   uint8_t *in, *out;
   uint32_t *perm;
   cudaMalloc(&in, (size_t)n * 80);
   cudaMalloc(&out, (size_t)n * 80);
   cudaMalloc(&perm, (size_t)n * 4);
-  k_fill_data<<<148 * 8, 256>>>(reinterpret_cast<uint32_t *>(in), (uint64_t)n * 20);
-  k_fill_perm<<<148 * 8, 256>>>(perm, n, 48271u * 7919u + 2u * 3u * 0u + 0u | 1u);
+  k_fill_data<<<g_sms * 8, 256>>>(reinterpret_cast<uint32_t *>(in), (uint64_t)n * 20);
+  k_fill_perm<<<g_sms * 8, 256>>>(perm, n, 48271u * 7919u + 2u * 3u * 0u + 0u | 1u);
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0);
   cudaEventCreate(&e1);
@@ -206,7 +209,7 @@ int main(int argc, char **argv) {
   for (int ctas = 2; ctas <= 8; ctas += 2) {
     for (int rep = 0; rep < 2; rep++) {
       cudaEventRecord(e0);
-      k_gather<5><<<148 * ctas, 256>>>(in, perm, out, npieces);
+      k_gather<5><<<g_sms * ctas, 256>>>(in, perm, out, npieces);
       cudaEventRecord(e1);
       cudaEventSynchronize(e1);
       float ms;

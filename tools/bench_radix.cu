@@ -1,5 +1,5 @@
 // tools/bench_radix.cu -- micro-benchmark of the onesweep radix pass (tuning aid; not part of the product path).
-// nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -DTEZGPU_RADIX_THREADS32=.. -DTEZGPU_RADIX_IPT32=.. tools/bench_radix.cu
+// nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -DTEZGPU_RADIX_THREADS32=.. -DTEZGPU_RADIX_IPT32=.. tools/bench_radix.cu
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -20,6 +20,8 @@ __global__ void k_fill(uint32_t *k, uint32_t n) {
 }
 
 int main(int argc, char **argv) {
+  int sms = 132;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   uint32_t n = argc > 1 ? (uint32_t)atoll(argv[1]) : 100000000u;
   uint32_t *ka, *kb, *va, *vb, *small;
   cudaMalloc(&ka, n * 4ull); cudaMalloc(&kb, n * 4ull); cudaMalloc(&va, n * 4ull); cudaMalloc(&vb, n * 4ull);
@@ -36,7 +38,7 @@ int main(int argc, char **argv) {
   for (int it = 0; it < 6; it++) {
     k_fill<<<(n + 255) / 256, 256, 0, st>>>(ka, n);
     cudaMemsetAsync(small, 0, 16384, st);
-    k_radix_hist<uint32_t, 4><<<148 * 8, 512, 0, st>>>(ka, n, 0, ws.hist);
+    k_radix_hist<uint32_t, 4><<<sms * 8, 512, 0, st>>>(ka, n, 0, ws.hist);
     k_radix_scan_hist<<<1, RADIX, 0, st>>>(ws.hist, 4, n, ws.trivial);
     cudaEventRecord(e0, st);
     int launches = 0;
