@@ -293,6 +293,9 @@ uint32_t tezgpu_debug_assemble_emulate(const uint8_t *stage, uint32_t nr, uint32
 /* diagnostics: host-side run of the chunk-interleaved CRC fold of the emit / verify kernels (ilp: two-deep form) */
 uint32_t tezgpu_debug_chunk_fold_emulate(const uint8_t *data, uint32_t nchunks, int32_t ilp);
 
+/* diagnostics: host-side run of the per-thread-run CRC fold of the packed fixed-width emit kernel (nchunks <= 1280) */
+uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks);
+
 uint32_t tezgpu_debug_runs_assemble_emulate(const uint8_t *staging, uint32_t staging_len, const uint32_t *src, uint32_t nr,
                                             uint32_t rec_size, uint32_t lead, int32_t first, int32_t last,
                                             uint8_t *image_out, uint32_t image_cap);

@@ -142,7 +142,7 @@ struct WarpLinearMap {
 // with W instead of S in the textbook form; the two-deep form applies S there too and the constant factor
 // x^(128*(T-1)) this adds to every partial is divided out once, in the per-lane alignment multiplier of the final fold
 // (CrcTables::einv; the inverse exists because the CRC-32 polynomial is primitive: tests/test_abi_cpu.py).
-// The third digit table costs 7 registers: kernels already at their register cap (k_emit_fast4, k_emit_fast4u at 80)
+// The third digit table costs 7 registers: kernels already at their register cap (k_emit_fast4u at 80)
 // spill, kernels with headroom can afford the shorter chain.  Hence a template flag per kernel.
 template <bool ILP>
 struct CrcChunkFoldT {

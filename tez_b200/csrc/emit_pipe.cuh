@@ -2,19 +2,23 @@
 // 16-byte aligned fixed-width records.
 //
 // k_emit_fast saturates no pipe: its warps wait on the gather's global loads and at barriers (behind warp 0 folding
-// the tile's partial checksums while seven warps idle).  This kernel keeps the same tile algorithm and byte-exact
-// output but reorders the work of a persistent CTA:
-//   * the 128-bit gather loads of tile N+1 are issued into registers BEFORE the checksum / write-out loop of tile N
-//     and stored to the image after it (record indices are fetched two tiles ahead, tile descriptors three), so the
-//     DRAM latency of the random gather hides behind ~190 instructions per thread-chunk of CRC work;
-//   * the per-tile second-level checksum fold is deferred: partials of FE4_BATCH tiles are parked in shared memory
+// the tile's partial checksums while seven warps idle).  This kernel keeps the same byte-exact output but reorders the
+// work of a persistent CTA:
+//   * the 128-bit gather loads of tile N+1 are issued into registers BEFORE the checksum / write-out of tile N and
+//     stored to the image after it (record indices are fetched two tiles ahead, tile descriptors three), so the DRAM
+//     latency of the random gather hides behind the checksum work;
+//   * the per-tile second-level checksum fold is deferred: partials of FE4_PARKED tiles are parked in shared memory
 //     and folded together, one tile per warp, so no warp waits for another's serial fold;
 //   * two barriers per tile instead of three.
+// Checksum organisation (CRC32 in parallel, see DESIGN.md): a tile image holds at most FE_THREADS * FE4_RUN 16-byte
+// chunks; thread t folds the FE4_RUN whole chunks at distance [FE4_RUN*(255-t), FE4_RUN*(256-t)) from the end of the
+// tile body with the textbook chain c = W(c ^ word) ("next word" map W = * x^32 only), so its alignment multiplier
+// x^(8*80*(255-t)) does not depend on the tile's length.  W runs on lane-private digit tables in shared memory.
 #pragma once
 #include "emit_fast.cuh"
 
 #ifndef TEZGPU_EMIT4_MIN_CTAS
-#define TEZGPU_EMIT4_MIN_CTAS 3
+#define TEZGPU_EMIT4_MIN_CTAS 3  // CTAs per SM of k_emit_fast4u (emit_pipe_u.cuh)
 #endif
 #ifndef TEZGPU_EMIT4_MAP16
 #define TEZGPU_EMIT4_MAP16 0
@@ -22,17 +26,69 @@
 
 namespace tezgpu {
 
-constexpr int FE4_BATCH = FE_THREADS / 32;  // one parked tile per warp
+constexpr int FE4_BATCH = FE_THREADS / 32;  // one parked tile per warp (k_emit_fast4u)
 constexpr int FE4_UNROLL = TEZGPU_EMIT4_MAP16 ? 6 : 5;  // gather rounds held in registers
+constexpr int FE4_RUN = 5;                  // 16-byte chunks per thread-run of the checksum
+constexpr uint32_t FE4_RUN_BYTES = 16u * FE4_RUN;
+constexpr int FE4_IMG_BYTES = FE_THREADS * FE4_RUN * 16;  // 20480: the tile image is exactly FE4_RUN rounds of chunks
+// Shared-memory footprint decides this kernel on H100 (DESIGN.md §7): the CTA's total picks the carveout, and what the
+// carveout leaves as L1 bounds the random gather's loads in flight.  Two groups, four parked tiles and 7-bit digits
+// come to 125 KB (the 132 KB carveout).  8-bit digits (4 tables, 16 LDS per chunk instead of 20) take 128 KB of
+// tables alone and were 1.8 ms slower than 7-bit ones at the same layout; 6-bit digits with three groups fit the
+// 132 KB carveout too and were 0.07 ms slower.
+// independent 256-thread groups per CTA (one CTA per SM); they share the checksum tables
+constexpr int FE4_GROUPS = 2;
+// tiles whose partials a group parks before folding them (one warp each)
+constexpr int FE4_PARKED = 4;
+// digit width of the lane-private tables of W: 7 bits -> tables of 128, 128, 128, 128 and 16 entries (66 KB, 20 LDS
+// per chunk)
+constexpr int FE4_WBITS = 7;
+constexpr int FE4_WDIGITS = (32 + FE4_WBITS - 1) / FE4_WBITS;
+constexpr int FE4_WENTRIES = ((FE4_WDIGITS - 1) << FE4_WBITS) + (1 << (32 - FE4_WBITS * (FE4_WDIGITS - 1)));
 
-// can a tile of `recs` records with `cpr` pieces each be gathered in FE4_UNROLL rounds?
-static inline bool emit4_fits(uint32_t recs, uint32_t cpr) {
+// records of `rec_size` bytes a tile image holds in the worst case (lead <= 15, segment header 4, EOF marker 2)
+static inline uint32_t emit4_max_recs(uint32_t rec_size) {
+  return std::min<uint32_t>(FE_MAX_RECS, (FE4_IMG_BYTES - 15 - 4 - 2) / rec_size);
+}
+
+// pieces per record the kernel serves: the packed piece map of full tiles (k_emit_fast4) keeps a piece's byte offset
+// in its record, 16c, in 7 bits
+constexpr uint32_t FE4_MAX_CPR = 8;
+
+// can a tile of `recs` records of `rec_size` bytes with `cpr` pieces each be gathered in FE4_UNROLL rounds and fit the
+// image?
+static inline bool emit4_fits(uint32_t recs, uint32_t cpr, uint32_t rec_size) {
+  if (cpr > FE4_MAX_CPR || recs > emit4_max_recs(rec_size)) return false;
 #if TEZGPU_EMIT4_MAP16
   const uint32_t rph = 16u / cpr;
-  return cpr <= 8 && 16ull * ((recs + rph - 1) / rph) <= (uint64_t)FE4_UNROLL * FE_THREADS;
+  return 16ull * ((recs + rph - 1) / rph) <= (uint64_t)FE4_UNROLL * FE_THREADS;
 #else
   return (uint64_t)recs * cpr <= (uint64_t)FE4_UNROLL * FE_THREADS;
 #endif
+}
+
+// W = "* x^32" on a word whose digit k (FE4_WBITS wide, the top one narrower) is e: the value of entry e of digit
+// table k (host and device: the host emulation in tezgpu_api.cu builds the same tables)
+__host__ __device__ __forceinline__ uint32_t emit4_wtab_value(const CrcTables *__restrict__ t, uint32_t k, uint32_t e) {
+  const uint32_t v = e << (FE4_WBITS * k);
+  return t->slice[3][v & 0xFF] ^ t->slice[2][(v >> 8) & 0xFF] ^ t->slice[1][(v >> 16) & 0xFF] ^ t->slice[0][v >> 24];
+}
+
+// W (* x^32) of x through the lane-private digit tables (layout: Emit4Smem); `wt` is this lane's word of entry 0 of
+// table 0.  Entry e of a table is e * 128 bytes from its start: digit k is shifted straight to that position and
+// masked (shift, and, add, load per digit).  Host and device: the host emulation in tezgpu_api.cu runs this code on a
+// table laid out like the kernel's.
+__host__ __device__ __forceinline__ uint32_t emit4_next_word(const uint8_t *wt, uint32_t x) {
+  uint32_t r = 0;
+#pragma unroll
+  for (int k = 0; k < FE4_WDIGITS; k++) {
+    constexpr int E = 7;  // log2(32 lanes * 4 bytes)
+    const int sh = FE4_WBITS * k - E;
+    const uint32_t m = (k + 1 < FE4_WDIGITS ? (1u << FE4_WBITS) - 1 : (1u << (32 - FE4_WBITS * k)) - 1) << E;
+    const uint32_t off = (sh >= 0 ? x >> sh : x << -sh) & m;
+    r ^= *reinterpret_cast<const uint32_t *>(wt + off + ((size_t)k << (FE4_WBITS + E)));
+  }
+  return r;
 }
 
 struct FoldMeta {
@@ -49,59 +105,47 @@ __device__ __forceinline__ uint4 lds_v4(uint32_t a) {
   return v;
 }
 
-// SUBS = 1: one 256-thread group per CTA, TEZGPU_EMIT4_MIN_CTAS CTAs per SM, both checksum maps as SHFL digit tables.
-// SUBS = 3: one CTA per SM hosts three independent 256-thread groups (named barriers) that share a LANE-PRIVATE copy
-//           of the four "next word" byte tables (entry e of table k for lane l lives at word (k*256+e)*32+l, always
-//           bank l): the look-up that runs three times per chunk becomes 4 conflict-free LDS instead of 7 SHFL.
-//           Measured on the SHFL-only kernel: a SHFL occupies the LSU data pipe for two cycles, so its 28 SHFL per
-//           chunk cost as much pipe time as the conflicting byte-table look-ups they replaced; the pipe, not issue
-//           or DRAM, bounded the kernel.
-template <int SUBS>
+// Shared memory: the lane-private digit tables of W (entry e of table k for lane l at word (k << FE4_WBITS + e) * 32
+// + l, always bank l: conflict-free whatever the digits), the classic byte table (trailing bytes) and the byte tables
+// of the second-level Horner step; then per group the tile image, three tiles' record indices and the parked tiles.
 struct Emit4Smem {
-  static constexpr int BATCH = SUBS > 1 ? 4 : FE4_BATCH;
-  static constexpr size_t WTAB = SUBS > 1 ? (size_t)4 * 256 * 32 * 4 : 0;
+  static constexpr size_t WTAB = (size_t)FE4_WENTRIES * 32 * 4;
   static constexpr size_t SHARED = WTAB + 256 * 4 + 4 * 256 * 4;
-  static constexpr size_t GROUP = FE_IMG_BYTES + 3 * FE_MAX_RECS * 4 + (size_t)BATCH * FE_THREADS * 4 + (size_t)BATCH * sizeof(FoldMeta);
-  static constexpr size_t TOTAL = SHARED + SUBS * GROUP;
+  static constexpr size_t GROUP = FE4_IMG_BYTES + 3 * FE_MAX_RECS * 4 + (size_t)FE4_PARKED * FE_THREADS * 4 + (size_t)FE4_PARKED * sizeof(FoldMeta);
+  static constexpr size_t TOTAL = SHARED + FE4_GROUPS * GROUP;
 };
 
-template <int UNROLL, int SUBS>
-__global__ void __launch_bounds__(FE_THREADS * SUBS, SUBS > 1 ? 1 : TEZGPU_EMIT4_MIN_CTAS) k_emit_fast4(FastEmitParams fp) {
-  using L = Emit4Smem<SUBS>;
-  constexpr int BATCH = L::BATCH;
+template <int UNROLL>
+__global__ void __launch_bounds__(FE_THREADS * FE4_GROUPS, 1) k_emit_fast4(FastEmitParams fp) {
+  using L = Emit4Smem;
+  constexpr int BATCH = FE4_PARKED;
   extern __shared__ __align__(16) uint8_t smem4[];
-  uint32_t *s_wtab = reinterpret_cast<uint32_t *>(smem4);              // [4][256][32] lane-private (SUBS > 1)
+  uint32_t *s_wtab = reinterpret_cast<uint32_t *>(smem4);              // [FE4_WENTRIES][32] lane-private
   uint32_t *s_tab = reinterpret_cast<uint32_t *>(smem4 + L::WTAB);     // classic byte table (trailing bytes)
-  uint32_t *s_adv128 = s_tab + 256;                                    // * x^(32*128): second-level fold
+  uint32_t *s_hor = s_tab + 256;                                       // * x^(8*80*32): second-level Horner step
   const int sub = threadIdx.x / FE_THREADS, tid = threadIdx.x % FE_THREADS, lane = tid & 31, warp = tid >> 5;
   uint8_t *gbase = smem4 + L::SHARED + (size_t)sub * L::GROUP;
   uint8_t *s_img = gbase;
-  uint32_t(*s_idx)[FE_MAX_RECS] = reinterpret_cast<uint32_t(*)[FE_MAX_RECS]>(gbase + FE_IMG_BYTES);  // tiles N, N+1, N+2
-  uint32_t(*s_part)[FE_THREADS] = reinterpret_cast<uint32_t(*)[FE_THREADS]>(gbase + FE_IMG_BYTES + 3 * FE_MAX_RECS * 4);
-  FoldMeta *s_meta = reinterpret_cast<FoldMeta *>(gbase + FE_IMG_BYTES + 3 * FE_MAX_RECS * 4 + (size_t)BATCH * FE_THREADS * 4);
-  auto group_sync = [&]() {
-    if (SUBS == 1) __syncthreads();
-    else asm volatile("bar.sync %0, %1;" ::"r"(sub + 1), "r"(FE_THREADS) : "memory");
-  };
+  uint32_t(*s_idx)[FE_MAX_RECS] = reinterpret_cast<uint32_t(*)[FE_MAX_RECS]>(gbase + FE4_IMG_BYTES);  // tiles N, N+1, N+2
+  uint32_t(*s_part)[FE_THREADS] = reinterpret_cast<uint32_t(*)[FE_THREADS]>(gbase + FE4_IMG_BYTES + 3 * FE_MAX_RECS * 4);
+  FoldMeta *s_meta = reinterpret_cast<FoldMeta *>(gbase + FE4_IMG_BYTES + 3 * FE_MAX_RECS * 4 + (size_t)BATCH * FE_THREADS * 4);
+  auto group_sync = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(sub + 1), "r"(FE_THREADS) : "memory"); };
 
   const EmitParams &e = fp.e;
-  const uint32_t G = gridDim.x * SUBS, ntiles = fp.ntiles;
-  uint32_t tile = blockIdx.x * SUBS + sub;
-  if (SUBS > 1)
-    for (int i = threadIdx.x; i < 4 * 256 * 32; i += FE_THREADS * SUBS) s_wtab[i] = (&e.crc->slice[0][0])[i >> 5];
-  for (int i = threadIdx.x; i < 256; i += FE_THREADS * SUBS) s_tab[i] = e.crc->slice[0][i];
-  for (int i = threadIdx.x; i < 4 * 256; i += FE_THREADS * SUBS) s_adv128[i] = (&e.crc->adv128[0][0])[i];
+  const uint32_t G = gridDim.x * FE4_GROUPS, ntiles = fp.ntiles;
+  uint32_t tile = blockIdx.x * FE4_GROUPS + sub;
+  for (int i = threadIdx.x; i < FE4_WENTRIES * 32; i += FE_THREADS * FE4_GROUPS)
+    s_wtab[i] = emit4_wtab_value(e.crc, (uint32_t)(i >> 5) >> FE4_WBITS, (uint32_t)(i >> 5) & ((1u << FE4_WBITS) - 1));
+  for (int i = threadIdx.x; i < 256; i += FE_THREADS * FE4_GROUPS) s_tab[i] = e.crc->slice[0][i];
+  {
+    const uint32_t x_hor = e.crc->pow0[FE4_RUN_BYTES * 32];
+    for (int i = threadIdx.x; i < 4 * 256; i += FE_THREADS * FE4_GROUPS) s_hor[i] = crc_multmodp((uint32_t)(i & 255) << (8 * (i >> 8)), x_hor);
+  }
   __syncthreads();
   if (tile >= ntiles) return;
-  CrcChunkFoldT<false> cf;  // the chunk fold's linear maps as warp-resident digit tables (crc32.cuh)
-  cf.init(e.crc, lane);
-  const uint32_t lane_pow = SUBS == 1 ? cf.lane_pow : e.crc->pow_word[4 * (31 - lane)];
-  const WarpLinearMap &m_word = cf.w, &m_skip = cf.s;
-  const uint32_t *wt = s_wtab + lane;  // this lane's bank
-  auto next_word = [&](uint32_t x) -> uint32_t {
-    if (SUBS == 1) return m_word.apply(x);
-    return wt[(768u + (x & 0xFFu)) << 5] ^ wt[(512u + ((x >> 8) & 0xFFu)) << 5] ^ wt[(256u + ((x >> 16) & 0xFFu)) << 5] ^ wt[(x >> 24) << 5];
-  };
+  const uint32_t lane_pow = e.crc->pow0[FE4_RUN_BYTES * (31 - lane)];  // x^(8*80*(31-lane))
+  const uint8_t *wt = reinterpret_cast<const uint8_t *>(s_wtab + lane);  // this lane's bank
+  auto next_word = [&](uint32_t x) -> uint32_t { return emit4_next_word(wt, x); };
   const uint32_t img_base = (uint32_t)__cvta_generic_to_shared(s_img);
   const uint8_t *__restrict__ kv = e.rec.kv;
   const uint32_t rec_size = e.rec_size, hdr_len = e.fixed_hdr_len, stride = fp.stride, cpr = fp.cpr;
@@ -135,8 +179,9 @@ __global__ void __launch_bounds__(FE_THREADS * SUBS, SUBS > 1 ? 1 : TEZGPU_EMIT4
   };
 #endif
   // Full tiles (all but the last of a partition) share one piece map: packed once per thread as
-  // j | 16c << 8 | (j * rec_size + hdr_len + 16c) << 15, so a piece costs an index look-up and one multiply-add
-  // instead of the divide / permute arithmetic (which was ~25 % of the kernel's instructions).
+  // j | 16c << 8 | (j * rec_size + hdr_len + 16c) << 15 (j < 256, 16c < 128: cpr <= FE4_MAX_CPR, checked by
+  // emit4_fits), so a piece costs an index look-up and one multiply-add instead of the divide / permute arithmetic
+  // (which was ~25 % of the kernel's instructions).
   const uint32_t full_nr = e.recs_per_tile;
   uint32_t pk[UNROLL], onmask = 0;
 #pragma unroll
@@ -236,48 +281,40 @@ __global__ void __launch_bounds__(FE_THREADS * SUBS, SUBS > 1 ? 1 : TEZGPU_EMIT4
     // ---- gather of the next tile goes out now; it lands while this tile is checksummed and written
     if (has1) issue_gather(nr1, s_idx[(n_it + 1) % 3]);
 
-    // ---- fused CRC + write-out (emit_fast.cuh): thread t owns the chunks at distance == T-1-t (mod T) from the end
+    // ---- write-out (lane-consecutive chunks, coalesced), then the checksum of this thread's run
     const uint32_t cb0 = rec0, cb1 = body_end;
     const uint32_t ca = cb0 >> 4, cz = cb1 >> 4;
     uint8_t *dstg = e.out + (abs0 - lead);
     uint32_t c = 0;
     if (cz > ca) {
-      const uint32_t Cn = cz - ca;
-      const uint32_t iters = (Cn + FE_THREADS - 1) / FE_THREADS;
-      int32_t i = (int32_t)Cn + tid - (int32_t)(iters * FE_THREADS);
-      uint32_t sa = img_base + 16u * (uint32_t)((int32_t)ca + i);
-      uint8_t *gp = dstg + 16ll * ((int64_t)ca + i);
-      for (uint32_t it = 0; it < iters; it++, i += FE_THREADS, sa += 16u * FE_THREADS, gp += 16 * FE_THREADS) {
-        if (i + (31 - lane) < 0) continue;  // no lane of this warp owns a chunk yet (first, ragged round only)
-        uint4 w = make_uint4(0, 0, 0, 0);
-        if (i >= 0) {
-          w = lds_v4(sa);
-          if (i == 0) {
-            const uint32_t b0 = 16u * ca;
-            if (b0 >= lead) stg_stream_v4(gp, w);
-            else for (uint32_t x = lead; x < b0 + 16u; x++) dstg[x] = s_img[x];  // ragged first chunk of the tile
-            const uint32_t skip = cb0 & 15u;  // bytes before the body (segment header / previous tile) fold as zero
-            if (skip) {
-              uint32_t ww[4] = {w.x, w.y, w.z, w.w};
+      const int32_t Cn = (int32_t)(cz - ca);
+      for (int32_t i = tid; i < Cn; i += FE_THREADS) {
+        const uint4 w = lds_v4(img_base + 16u * (ca + (uint32_t)i));
+        if (i > 0 || 16u * ca >= lead) stg_stream_v4(dstg + 16u * (ca + (uint32_t)i), w);
+        else for (uint32_t x = lead; x < 16u * ca + 16u; x++) dstg[x] = s_img[x];  // ragged first chunk of the tile
+      }
+      // thread t: chunks [Cn - FE4_RUN*(256-t), Cn - FE4_RUN*(255-t)); those before the body are zeros, which leave a
+      // zero remainder unchanged
+      const int32_t i0 = Cn - FE4_RUN * (FE_THREADS - tid);
 #pragma unroll
-              for (uint32_t k = 0; k < 4; k++) {
-                if (skip >= 4 * k + 4) ww[k] = 0;
-                else if (skip > 4 * k) ww[k] &= 0xFFFFFFFFu << (8u * (skip - 4 * k));
-              }
-              w = make_uint4(ww[0], ww[1], ww[2], ww[3]);
-            }
-          } else {
-            stg_stream_v4(gp, w);
+      for (int k = 0; k < FE4_RUN; k++) {
+        const int32_t i = i0 + k;
+        if (i < 0) continue;
+        uint4 w = lds_v4(img_base + 16u * (ca + (uint32_t)i));  // 80-byte lane stride: conflict-free quarter-warps
+        if (i == 0) {
+          const uint32_t skip = cb0 & 15u;  // bytes before the body (segment header / previous tile) fold as zero
+          uint32_t ww[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+          for (uint32_t q = 0; q < 4; q++) {
+            if (skip >= 4 * q + 4) ww[q] = 0;
+            else if (skip > 4 * q) ww[q] &= 0xFFFFFFFFu << (8u * (skip - 4 * q));
           }
+          w = make_uint4(ww[0], ww[1], ww[2], ww[3]);
         }
-        if (SUBS == 1) {
-          c = cf.fold(c, w, it + 1 == iters);
-        } else {
-          uint32_t x = next_word(c ^ w.x) ^ w.y;
-          x = next_word(x) ^ w.z;
-          x = next_word(x) ^ w.w;
-          c = (it + 1 == iters) ? next_word(x) : m_skip.apply(x);
-        }
+        c = next_word(c ^ w.x);
+        c = next_word(c ^ w.y);
+        c = next_word(c ^ w.z);
+        c = next_word(c ^ w.w);
       }
     }
     s_part[slot][tid] = c;
@@ -299,12 +336,12 @@ __global__ void __launch_bounds__(FE_THREADS * SUBS, SUBS > 1 ? 1 : TEZGPU_EMIT4
 
     if (slot == (uint32_t)BATCH || !has1) {
       // ---- deferred second level: warp w folds parked tile w.  lane l folds partials l, l+32, ... (Horner with
-      // x^(128*32)), aligns by x^(128*(31-l)), xor-reduce; lane 0 appends the trailing bytes
+      // x^(8*80*32)), aligns by x^(8*80*(31-l)), xor-reduce; lane 0 appends the trailing bytes
       if ((uint32_t)warp < slot) {
         uint32_t q = 0;
 #pragma unroll
         for (int k = 0; k < FE_THREADS / 32; k++) {
-          q = s_adv128[q & 0xFF] ^ s_adv128[256 + ((q >> 8) & 0xFF)] ^ s_adv128[512 + ((q >> 16) & 0xFF)] ^ s_adv128[768 + (q >> 24)];
+          q = s_hor[q & 0xFF] ^ s_hor[256 + ((q >> 8) & 0xFF)] ^ s_hor[512 + ((q >> 16) & 0xFF)] ^ s_hor[768 + (q >> 24)];
           q ^= s_part[warp][lane + 32 * k];
         }
         q = crc_multmodp(q, lane_pow);

@@ -11,9 +11,10 @@
 // TEZGPU_EMIT_PIPE_UNALIGNED=0 selects the older kernel k_emit_fast<5,false> (tools/merge_profile.py times the
 // batched reduce-side merge both ways).
 //
-// The checksum / write-out loop and the batched fold are the same text as in k_emit_fast4 on purpose: moving them into
-// shared __device__ functions changed ptxas' register allocation (more spill stores in both kernels), so the
-// duplication stays until that can be re-measured.
+// The checksum / write-out loop and the batched fold are NOT those of k_emit_fast4 any more: that kernel folds
+// per-thread runs of five chunks on lane-private tables (one CTA of two groups per SM), this one still folds the
+// 256-thread chunk interleave with SHFL digit tables (CrcChunkFoldT<false>) at three CTAs per SM.  Porting the run fold
+// here is a separate, measured change.
 #pragma once
 #include "emit_pipe.cuh"
 

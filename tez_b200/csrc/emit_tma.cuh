@@ -10,7 +10,8 @@
 //     shift for a chunk inside one record's bytes, a short composition for the chunks that straddle the 2-byte framing
 //     of the next record), fold it into the tile's CRC32 and stream it to HBM -- the image of emit_pipe.cuh (five STS per
 //     16 bytes + one LDS.128) is never materialised.
-// Same tiles, same byte-exact output and the same per-tile checksum algebra as k_emit_fast4 (emit_pipe.cuh).
+// Same tiles and byte-exact output as k_emit_fast4 (emit_pipe.cuh); the per-tile checksum is the chunk-interleaved
+// fold of k_emit_fast4u (emit_pipe_u.cuh), not k_emit_fast4's per-thread runs.
 #pragma once
 #include "emit_pipe_u.cuh"
 

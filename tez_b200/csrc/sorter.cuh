@@ -186,13 +186,18 @@ class SortPipeline {
     // within 10 % of the cap, take the one with the most records per executed round (249 for 82-byte records).
     static const int round_fill = getenv("TEZGPU_EMIT_ROUND_FILL") ? atoi(getenv("TEZGPU_EMIT_ROUND_FILL")) : TEZGPU_EMIT_ROUND_FILL_DEFAULT;
     bool fill = round_fill != 0;
+    const uint32_t stride = rec.klen + rec.vlen;
+    const bool fast = stride >= 16 && stride % 16 == 0;
+    const bool aligned = !rec.key_off && !rec.use_runs && (((uintptr_t)rec.kv & 15u) == 0);
     if (rec.use_runs && runs_emit_enabled() && emit_runs_fits(e.recs_per_tile, e.rec_size, merge_max_runs)) {
       // run-table mode with the range-copy emit (emit_runs.cuh): full 256-record tiles
+    } else if (fast && aligned && emit4_max_recs(e.rec_size) >= 1 && emit4_fits(emit4_max_recs(e.rec_size), stride / 16, e.rec_size)) {
+      // the pipelined kernel for packed aligned records (emit_pipe.cuh): its image holds exactly FE4_RUN checksum
+      // rounds, so a tile takes as many records as fit it in the worst case (249 of 82 bytes: 1278 chunks, 1280 slots).
+      // Wider records (more than FE4_MAX_CPR pieces) keep the tiles of k_emit_fast.
+      e.recs_per_tile = std::min<uint32_t>(e.recs_per_tile, emit4_max_recs(e.rec_size));
     } else if (pipe_unaligned_enabled()) {
       // the pipelined kernel for records at arbitrary offsets (emit_pipe_u.cuh) holds a tile's words in five gather rounds
-      const uint32_t stride = rec.klen + rec.vlen;
-      const bool fast = stride >= 16 && stride % 16 == 0;
-      const bool aligned = !rec.key_off && !rec.use_runs && (((uintptr_t)rec.kv & 15u) == 0);
       if (fast && !aligned && emit4u_max_recs(stride / 16) >= 32) {
         e.recs_per_tile = std::min<uint32_t>(e.recs_per_tile, emit4u_max_recs(stride / 16));
         fill = true;
@@ -586,31 +591,19 @@ class SortPipeline {
           TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_emit_tma, ET_THREADS, smem));
           uint32_t grid = (uint32_t)std::min<uint64_t>(tiles, (uint64_t)num_sms * (per_sm > 0 ? per_sm : 1));
           k_emit_tma<<<grid, ET_THREADS, smem, stream>>>(fp, (uint32_t)EmitTmaLayout::stage_bytes(e.recs_per_tile, stride));
-        } else if (fast_aligned && emit4_fits(e.recs_per_tile, fp.cpr) && !getenv("TEZGPU_EMIT_V2")) {
-          // software-pipelined kernel (emit_pipe.cuh): a tile's pieces must fit the registers of one gather round.
-          // Default: independent 256-thread CTAs, three per SM.  TEZGPU_EMIT_SUBS=3 selects the variant with one CTA
-          // per SM whose three groups share lane-private checksum tables -- slower: its 219 KB of shared memory leave
-          // the SM little L1 and the random gather loses its memory-level parallelism.
-          static const bool subs1 = !(getenv("TEZGPU_EMIT_SUBS") && atoi(getenv("TEZGPU_EMIT_SUBS")) == 3);
-          if (!subs1) {
-            constexpr int SUBS = 3;
-            static bool attr = false;
-            if (!attr) {
-              TG_CUDA(cudaFuncSetAttribute(k_emit_fast4<FE4_UNROLL, SUBS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Emit4Smem<SUBS>::TOTAL));
-              attr = true;
-            }
-            uint32_t grid = (uint32_t)std::min<uint64_t>(div_up(tiles, SUBS), (uint64_t)num_sms);
-            k_emit_fast4<FE4_UNROLL, SUBS><<<grid, FE_THREADS * SUBS, Emit4Smem<SUBS>::TOTAL, stream>>>(fp);
-          } else {
-            static bool attr = false;
-            if (!attr) {
-              TG_CUDA(cudaFuncSetAttribute(k_emit_fast4<FE4_UNROLL, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Emit4Smem<1>::TOTAL));
-              attr = true;
-            }
-            TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_emit_fast4<FE4_UNROLL, 1>, FE_THREADS, Emit4Smem<1>::TOTAL));
-            uint32_t grid = (uint32_t)std::min<uint64_t>(tiles, (uint64_t)num_sms * (per_sm > 0 ? per_sm : 1));
-            k_emit_fast4<FE4_UNROLL, 1><<<grid, FE_THREADS, Emit4Smem<1>::TOTAL, stream>>>(fp);
+        } else if (fast_aligned && emit4_fits(e.recs_per_tile, fp.cpr, e.rec_size) && !getenv("TEZGPU_EMIT_V2")) {
+          // software-pipelined kernel (emit_pipe.cuh): a tile's pieces must fit the registers of one gather round and
+          // its bytes the FE4_IMG_BYTES image.  One CTA per SM, FE4_GROUPS independent 256-thread groups sharing the
+          // lane-private checksum tables (66 KB) next to their images, indices and parked partials (54 KB): 125 KB
+          // keeps the CTA in the 132 KB shared-memory carveout, which leaves the random gather enough L1 for its
+          // loads in flight (larger footprints measured slower, DESIGN.md §7).
+          static bool attr = false;
+          if (!attr) {
+            TG_CUDA(cudaFuncSetAttribute(k_emit_fast4<FE4_UNROLL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Emit4Smem::TOTAL));
+            attr = true;
           }
+          uint32_t grid = (uint32_t)std::min<uint64_t>(div_up(tiles, FE4_GROUPS), (uint64_t)num_sms);
+          k_emit_fast4<FE4_UNROLL><<<grid, FE_THREADS * FE4_GROUPS, Emit4Smem::TOTAL, stream>>>(fp);
         } else if (rec.use_runs && runs_emit_enabled() && emit_runs_fits(e.recs_per_tile, e.rec_size, merge_max_runs)) {
           // reduce side, fixed-framing runs in place: one bulk copy per run and tile (emit_runs.cuh)
           const size_t smem = EmitRunsLayout::total(e.recs_per_tile, e.rec_size);

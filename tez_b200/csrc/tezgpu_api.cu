@@ -650,6 +650,44 @@ uint32_t tezgpu_debug_chunk_fold_emulate(const uint8_t *data, uint32_t nchunks, 
   return total;
 }
 
+// Host emulation of the run checksum of k_emit_fast4 (emit_pipe.cuh): FE_THREADS threads, thread t folds the FE4_RUN
+// chunks ending FE4_RUN*(255-t) chunks before the end (chunks before the data are zeros) through the lane-private digit
+// tables of W, laid out and read with the kernel's code (emit4_wtab_value, emit4_next_word); lane l folds partials
+// l, l+32, ... by Horner with x^(8*80*32), multiplies by x^(8*80*(31-l)), and the lanes xor.  nchunks <= FE_THREADS * FE4_RUN.  Returns the raw remainder (init 0, no final xor) of the nchunks * 16
+// bytes.
+uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks) {
+  if (nchunks > (uint32_t)(FE_THREADS * FE4_RUN)) return 0;
+  CrcTables *t = new CrcTables();
+  crc_build_tables(*t, EMIT_CRC_STRIDE_WORDS);
+  // the kernel's shared-memory layout: entry e of table k for lane l at word ((k << FE4_WBITS) + e) * 32 + l
+  std::vector<uint32_t> wtab((size_t)FE4_WENTRIES * 32);
+  for (uint32_t i = 0; i < (uint32_t)FE4_WENTRIES * 32; i++) wtab[i] = emit4_wtab_value(t, (i >> 5) >> FE4_WBITS, (i >> 5) & ((1u << FE4_WBITS) - 1));
+  const uint32_t x_hor = t->pow0[FE4_RUN_BYTES * 32];
+  auto H = [&](uint32_t x) { return crc_multmodp(x, x_hor); };
+  const int32_t Cn = (int32_t)nchunks;
+  std::vector<uint32_t> part(FE_THREADS, 0);
+  for (int tid = 0; tid < FE_THREADS; tid++) {
+    uint32_t c = 0;
+    for (int k = 0; k < FE4_RUN; k++) {
+      const int32_t i = Cn - FE4_RUN * (FE_THREADS - tid) + k;
+      if (i < 0) continue;
+      uint32_t w[4];
+      memcpy(w, data + 16 * (size_t)i, 16);
+      const uint8_t *wt = reinterpret_cast<const uint8_t *>(wtab.data() + (tid & 31));
+      for (int q = 0; q < 4; q++) c = emit4_next_word(wt, c ^ w[q]);
+    }
+    part[tid] = c;
+  }
+  uint32_t total = 0;
+  for (int lane = 0; lane < 32; lane++) {
+    uint32_t q = 0;
+    for (int kk = 0; kk < FE_THREADS / 32; kk++) q = H(q) ^ part[lane + 32 * kk];
+    total ^= crc_multmodp(q, t->pow0[FE4_RUN_BYTES * (31 - lane)]);
+  }
+  delete t;
+  return total;
+}
+
 // Host emulation of the run-range emit kernel's chunk assembly (emit_runs.cuh): record j of the tile is the rec_size
 // bytes at staging[src[j]...]; builds the output image chunk by chunk with the kernel's template code.
 uint32_t tezgpu_debug_runs_assemble_emulate(const uint8_t *staging, uint32_t staging_len, const uint32_t *src, uint32_t nr,
