@@ -105,13 +105,15 @@ __device__ __forceinline__ uint32_t lanemask_lt() {
   return m;
 }
 
-__device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t *p) {
+// Coherent at GPU scope (L2), without the system-scope cost of `volatile`: for flags that only other CTAs of the same
+// device read, where the flag and its value share one word.
+__device__ __forceinline__ uint32_t ld_relaxed_gpu_u32(const uint32_t *p) {
   uint32_t v;
-  asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-__device__ __forceinline__ void st_volatile_u32(uint32_t *p, uint32_t v) {
-  asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+__device__ __forceinline__ void st_relaxed_gpu_u32(uint32_t *p, uint32_t v) {
+  asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
 __device__ __forceinline__ uint64_t ld_volatile_u64(const uint64_t *p) {

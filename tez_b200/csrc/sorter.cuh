@@ -73,7 +73,9 @@ class SortPipeline {
   int num_sms = 132;
 
   // workspace (grow-only, reused across flushes)
-  DeviceBuffer keysA, keysB, valsA, valsB, same, blk, small, tile_state, sizes, rec_off;
+  // sortA / sortB: the radix sort's two 8n-byte blocks (radix_sort_pairs).  The stage writes the sort words to the
+  // first half of sortA; the sorted words and the index array end up in the two halves of one block.
+  DeviceBuffer sortA, sortB, same, blk, small, tile_state, sizes, rec_off;
   DeviceBuffer t_pos[2], t_gid[2], t_lidx[2], t_key64[2], t_val[2], t_state, t_ghead, t_gneq, sym_sets, sym_tab, rep_flags;
   DeviceBuffer seg_start, tile_start, part_start, d_index, seg_crc, tile_desc, tile_crc, tie_state;
   PinnedBuffer h_small;
@@ -247,7 +249,7 @@ class SortPipeline {
     timer.mark(stream);
 
     const size_t n4 = (size_t)(n ? n : 1) * 4;
-    keysA.ensure(n4); keysB.ensure(n4); valsA.ensure(n4); valsB.ensure(n4);
+    sortA.ensure(2 * n4); sortB.ensure(2 * n4);
     same.ensure(n ? n : 1);
     const uint32_t nblk = (uint32_t)div_up(n ? n : 1, SCAN_TILE);
     blk.ensure(((size_t)nblk + 2) * 8);
@@ -263,8 +265,8 @@ class SortPipeline {
 
     uint64_t dup_count = 0;
     uint64_t tie_records = 0;
-    uint32_t *K = keysA.as<uint32_t>();
-    uint32_t *order = valsA.as<uint32_t>();
+    uint32_t *K = sortA.as<uint32_t>();
+    uint32_t *order = sortA.as<uint32_t>() + n;
 
     uint32_t sym_npos = 0;
     if (n && !rec.fixed && !unordered && !(getenv("TEZGPU_NO_SYM") && atoi(getenv("TEZGPU_NO_SYM")))) {
@@ -334,9 +336,8 @@ class SortPipeline {
         for (int q = 0; q < 4; q++) if (8 * q + 8 > 32 - pbits) pass_mask |= 1u << q;
         if (!pass_mask) pass_mask = 1;
       }
-      int done = radix_sort_passes<uint32_t>(stream, ws, keysA.as<uint32_t>(), keysB.as<uint32_t>(), valsA.as<uint32_t>(),
-                                             valsB.as<uint32_t>(), n, 0, 4, pass_mask, true, &launches);
-      if (done & 1) { K = keysB.as<uint32_t>(); order = valsB.as<uint32_t>(); }
+      int done = radix_sort_pairs(stream, ws, sortA.as<uint32_t>(), sortB.as<uint32_t>(), n, 0, 4, pass_mask, &launches);
+      if (done & 1) { K = sortB.as<uint32_t>(); order = sortB.as<uint32_t>() + n; }
       if (unordered) {
         k_flip_order<<<(uint32_t)div_up(n, 256), 256, 0, stream>>>(order, n);
         launches++;
@@ -446,7 +447,7 @@ class SortPipeline {
           t_state.ensure(w2.tile_state_words * 4);
           w2.tile_state = t_state.as<uint32_t>();
           int d2 = radix_sort_passes<uint64_t>(stream, w2, t_key64[0].as<uint64_t>(), t_key64[1].as<uint64_t>(), t_lidx[cur].as<uint32_t>(),
-                                               t_val[0].as<uint32_t>(), m, 0, 8, mask, false, &launches);
+                                               t_val[0].as<uint32_t>(), m, 0, 8, mask, &launches);
           const uint64_t *Ks = (d2 & 1) ? t_key64[1].as<uint64_t>() : t_key64[0].as<uint64_t>();
           const uint32_t *Ls = (d2 & 1) ? t_val[0].as<uint32_t>() : t_lidx[cur].as<uint32_t>();
           k_ref_apply_count<<<mblk, SCAN_THREADS, 0, stream>>>(Ks, Ls, t_pos[cur].as<uint32_t>(), m, order, same.as<uint8_t>(), d_dups(),
