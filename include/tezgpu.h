@@ -285,20 +285,11 @@ int32_t tezgpu_shuffle_receive(const uint8_t *in, uint64_t len, tezgpu_wire_segm
 /* diagnostics: host-side emulation of the device's tiled CRC algebra (same tables, no GPU needed) */
 uint32_t tezgpu_debug_crc_emulate(const uint8_t *body, uint64_t len, uint32_t piece_bytes, uint32_t lead);
 
-/* diagnostics: host-side run of the TMA emit kernel's chunk assembly (same template code, no GPU needed) */
-uint32_t tezgpu_debug_assemble_emulate(const uint8_t *stage, uint32_t nr, uint32_t stride, const uint8_t *hdr,
-                                       uint32_t hdr_len, uint32_t lead, int32_t first, int32_t last, uint8_t *image_out,
-                                       uint32_t image_cap);
-
 /* diagnostics: host-side run of the chunk-interleaved CRC fold of the emit / verify kernels (ilp: two-deep form) */
 uint32_t tezgpu_debug_chunk_fold_emulate(const uint8_t *data, uint32_t nchunks, int32_t ilp);
 
 /* diagnostics: host-side run of the per-thread-run CRC fold of the packed fixed-width emit kernel (nchunks <= 1280) */
 uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks);
-
-uint32_t tezgpu_debug_runs_assemble_emulate(const uint8_t *staging, uint32_t staging_len, const uint32_t *src, uint32_t nr,
-                                            uint32_t rec_size, uint32_t lead, int32_t first, int32_t last,
-                                            uint8_t *image_out, uint32_t image_cap);
 
 #ifdef __cplusplus
 }

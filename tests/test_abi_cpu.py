@@ -53,81 +53,3 @@ def test_segment_table_fast_path_matches_ctypes_layout():
     few = m._segments(segs[:3], parts[:3])        # the ctypes path (<= 64 runs)
     assert bytes(few)[:3 * 24] == bytes(slow)[:3 * 24]
 
-
-def test_tma_emit_chunk_assembly_matches_the_byte_image():
-    """The TMA emit kernel (emit_tma.cuh) never builds the output image in shared memory: every aligned 16-byte chunk is
-    assembled straight from the staged records (framing bytes, record straddles, segment header, EOF markers).  The same
-    template code runs here on the host (tezgpu_debug_assemble_emulate) against the obvious concatenation, for record
-    strides / vint framings / tile sizes / alignments / first-last flags the kernel can meet."""
-    import numpy as np
-    L = _lib.load()
-    rng = random.Random(1)
-    cases = 0
-    for stride in (16, 32, 80, 96, 4112):
-        for hdr in (b"\x10\x40", b"\x10", b"\x8f\x80\x40", b"\x8f\x80\x8e\x10\x00", bytes(range(1, 11))):
-            for nr in (1, 2, 3, 17, 255, 256):
-                if nr * stride > 300000:
-                    continue
-                for lead in (0, 1, 2, 7, 12, 13, 15):
-                    for first in (0, 1):
-                        for last in (0, 1):
-                            stage = np.frombuffer(rng.randbytes(nr * stride), dtype=np.uint8).copy()
-                            img = bytearray(lead)
-                            if first:
-                                img += b"TIF\x00"
-                            for j in range(nr):
-                                img += hdr + stage[j * stride:(j + 1) * stride].tobytes()
-                            if last:
-                                img += b"\xff\xff"
-                            cap = (len(img) + 31) // 16 * 16
-                            out = np.zeros(cap, dtype=np.uint8)
-                            hb = np.frombuffer(hdr, dtype=np.uint8).copy()
-                            end = L.tezgpu_debug_assemble_emulate(stage.ctypes.data, nr, stride, hb.ctypes.data, len(hdr), lead,
-                                                                  first, last, out.ctypes.data, cap)
-                            assert end == len(img)
-                            assert out[lead:end].tobytes() == bytes(img[lead:]), (stride, hdr, nr, lead, first, last)
-                            cases += 1
-    assert cases > 3000
-
-
-def test_run_range_emit_chunk_assembly_matches_the_byte_image():
-    """emit_runs.cuh (reduce side, fixed-framing runs in place): the tile's records sit in a few contiguous byte ranges
-    of the input segments, copied into shared memory at arbitrary alignments; every aligned 16-byte chunk of the output
-    is assembled from the one or two records it covers.  Same template code on the host against the concatenation."""
-    import numpy as np
-    L = _lib.load()
-    rng = random.Random(3)
-    cases = 0
-    for rec_size in (17, 18, 33, 82, 83, 100, 4114):
-        for nr in (1, 2, 5, 64, 255, 256):
-            if nr * rec_size > 400000:
-                continue
-            for lead in (0, 1, 6, 11, 15):
-                for first in (0, 1):
-                    for last in (0, 1):
-                        nruns = rng.randint(1, min(8, nr))
-                        assign = [rng.randrange(nruns) for _ in range(nr)]
-                        sizes = [assign.count(g) for g in range(nruns)]
-                        staging, run_off = bytearray(), []
-                        for g in range(nruns):
-                            staging += bytes((16 - len(staging) % 16) % 16) + rng.randbytes(rng.randint(0, 15))
-                            run_off.append(len(staging))
-                            staging += bytes(sizes[g] * rec_size)
-                        recs = [rng.randbytes(rec_size) for _ in range(nr)]
-                        at, src = [0] * nruns, []
-                        for j in range(nr):
-                            o = run_off[assign[j]] + at[assign[j]] * rec_size
-                            at[assign[j]] += 1
-                            staging[o:o + rec_size] = recs[j]
-                            src.append(o)
-                        img = bytearray(lead) + (b"TIF\x00" if first else b"") + b"".join(recs) + (b"\xff\xff" if last else b"")
-                        cap = (len(img) + 31) // 16 * 16
-                        out = np.zeros(cap, dtype=np.uint8)
-                        st = np.frombuffer(bytes(staging), dtype=np.uint8).copy()
-                        sa = np.array(src, dtype=np.uint32)
-                        end = L.tezgpu_debug_runs_assemble_emulate(st.ctypes.data, len(st), sa.ctypes.data, nr, rec_size, lead,
-                                                                   first, last, out.ctypes.data, cap)
-                        assert end == len(img)
-                        assert out[lead:end].tobytes() == bytes(img[lead:]), (rec_size, nr, lead, first, last)
-                        cases += 1
-    assert cases >= 700

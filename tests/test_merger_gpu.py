@@ -352,19 +352,3 @@ def test_config5_shape_zipf_keys_sort_and_merge_bit_exact(val_len, n):
         exp, _, _ = O.merge_ifile(mine, O.CMP_BYTES, factor=100)
         assert ln == exp.size and np.array_equal(merged[a:a + ln], exp), "partition %d" % p
 
-
-@pytest.mark.parametrize("switch", ["TEZGPU_EMIT_RUNS", "TEZGPU_EMIT_TMA"])
-def test_opt_in_tma_emit_kernels_stay_bit_exact(switch):
-    """The two emit kernels built on cp.async.bulk (emit_runs.cuh: one bulk copy per run and tile on the reduce side;
-    emit_tma.cuh: one per record on the map side) are slower than the register-staged gathers and therefore opt-in
-    (switches are read once per process): the fixed-width sorter and merger parity cases must pass with them on."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, **{switch: "1"})
-    sel = ("tests/test_merger_gpu.py::test_merge_of_gpu_sorted_fixed_width_partitions "
-           "tests/test_merger_gpu.py::test_batched_multi_partition_merge_matches_per_partition_oracle "
-           "tests/test_sorter_gpu.py::test_c2_fixed_width_bit_exact tests/test_sorter_gpu.py::test_fast_emit_other_16_byte_strides").split()
-    r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-m", "gpu"] + sel, cwd=root, env=env, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]

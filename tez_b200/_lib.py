@@ -71,8 +71,6 @@ SYMBOLS = [
     ("tezgpu_debug_crc_emulate", C.c_uint32, [_V, C.c_uint64, C.c_uint32, C.c_uint32]),
     ("tezgpu_debug_chunk_fold_emulate", C.c_uint32, [_V, C.c_uint32, C.c_int32]),
     ("tezgpu_debug_run_fold_emulate", C.c_uint32, [_V, C.c_uint32]),
-    ("tezgpu_debug_runs_assemble_emulate", C.c_uint32, [_V, C.c_uint32, _V, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.c_int32, _V, C.c_uint32]),
-    ("tezgpu_debug_assemble_emulate", C.c_uint32, [_V, C.c_uint32, C.c_uint32, _V, C.c_uint32, C.c_uint32, C.c_int32, C.c_int32, _V, C.c_uint32]),
     ("tezgpu_merge_open", C.c_int32, [_P(Conf), _P(Segment), C.c_uint32, _P(_V)]),
     ("tezgpu_merge_reopen", C.c_int32, [_V, _P(Segment), C.c_uint32]),
     ("tezgpu_merge_set_check_for_same_keys", C.c_int32, [_V, C.c_int32]),

@@ -141,17 +141,12 @@ __device__ __forceinline__ uint64_t fast_source_offset(const Records &rec, uint3
   return rec.key_off ? rec.key_off[ri] : (uint64_t)ri * stride;
 }
 
-#ifndef TEZGPU_CRC_SHFL
-#define TEZGPU_CRC_SHFL 1
-#endif
-
 template <int UNROLL, bool ALIGNED>
 __global__ void __launch_bounds__(FE_THREADS, TEZGPU_EMIT_MIN_CTAS) k_emit_fast(FastEmitParams fp) {
   __shared__ __align__(16) uint8_t s_img[FE_IMG_BYTES];
   __shared__ uint32_t s_idx[2][FE_MAX_RECS];                    // record indices of the current / next tile
   __shared__ uint64_t s_off[ALIGNED ? 1 : 2][ALIGNED ? 1 : FE_MAX_RECS];  // source offsets (explicit-offset mode)
   __shared__ uint32_t s_tab[4 * 256];    // slice-by-4 tables
-  __shared__ uint32_t s_adv[4 * 256];    // * x^(32*(4*FE_THREADS-3)): skip to this thread's next 16-byte chunk
   __shared__ uint32_t s_adv32[4 * 256];  // * x^(32*128): second-level fold
   __shared__ uint32_t s_part[FE_THREADS];
 
@@ -159,12 +154,10 @@ __global__ void __launch_bounds__(FE_THREADS, TEZGPU_EMIT_MIN_CTAS) k_emit_fast(
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int i = tid; i < 4 * 256; i += FE_THREADS) {
     s_tab[i] = (&e.crc->slice[0][0])[i];
-    s_adv[i] = (&e.crc->advc[0][0])[i];
     s_adv32[i] = (&e.crc->adv128[0][0])[i];
   }
   // constant alignment multipliers: x^(32*(31-lane)) for the final in-warp fold
   const uint32_t lane_pow = e.crc->pow_word[4 * (31 - lane)];
-#if TEZGPU_CRC_SHFL
   // the two maps of the chunk-interleaved checksum as warp-resident 5-bit digit tables (crc32.cuh): "next word"
   // (* x^32) and "skip to this thread's next chunk" (* x^(32*(4*FE_THREADS-3))), built from the global byte tables
   WarpLinearMap m_word, m_skip;
@@ -173,7 +166,6 @@ __global__ void __launch_bounds__(FE_THREADS, TEZGPU_EMIT_MIN_CTAS) k_emit_fast(
     m_word.init([&](uint32_t x) { return gt[768 + (x & 0xFF)] ^ gt[512 + ((x >> 8) & 0xFF)] ^ gt[256 + ((x >> 16) & 0xFF)] ^ gt[x >> 24]; }, lane);
     m_skip.init([&](uint32_t x) { return ga[x & 0xFF] ^ ga[256 + ((x >> 8) & 0xFF)] ^ ga[512 + ((x >> 16) & 0xFF)] ^ ga[768 + (x >> 24)]; }, lane);
   }
-#endif
   const uint32_t img_base = (uint32_t)__cvta_generic_to_shared(s_img);
   const uint8_t *__restrict__ kv = e.rec.kv;
   const uint8_t *kv_end = kv + e.rec.kv_bytes;
@@ -279,7 +271,6 @@ __global__ void __launch_bounds__(FE_THREADS, TEZGPU_EMIT_MIN_CTAS) k_emit_fast(
       uint32_t c = 0;
       if (cz > ca) {
         const uint32_t Cn = cz - ca;
-#if TEZGPU_CRC_SHFL
         // uniform trip count for the whole CTA (the maps are warp collectives); a thread whose chunk index is still
         // negative folds zeros, which stay zero
         const uint32_t iters = (Cn + FE_THREADS - 1) / FE_THREADS;
@@ -308,36 +299,6 @@ __global__ void __launch_bounds__(FE_THREADS, TEZGPU_EMIT_MIN_CTAS) k_emit_fast(
           x = m_word.apply(x) ^ v.w;
           c = (it + 1 == iters) ? m_word.apply(x) : m_skip.apply(x);
         }
-#else
-        if (Cn + tid >= FE_THREADS) {
-          const uint32_t last_i = Cn - FE_THREADS + tid;
-          for (uint32_t i = last_i % FE_THREADS; i <= last_i; i += FE_THREADS) {
-            const uint32_t b0 = 16u * (ca + i);
-            uint4 v = *reinterpret_cast<const uint4 *>(s_img + b0);
-            if (b0 >= lead) stg_stream_v4(dstg + b0, v);
-            else for (uint32_t x = lead; x < b0 + 16u; x++) dstg[x] = s_img[x];  // ragged first chunk of the tile
-            if (i == 0 && (cb0 & 15u)) {  // zero the bytes before the body (segment header / previous tile's bytes)
-              const uint32_t skip = cb0 & 15u;
-              uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-              for (uint32_t k = 0; k < 4; k++) {
-                if (skip >= 4 * k + 4) w[k] = 0;
-                else if (skip > 4 * k) w[k] &= 0xFFFFFFFFu << (8u * (skip - 4 * k));
-              }
-              v = make_uint4(w[0], w[1], w[2], w[3]);
-            }
-            uint32_t x = c ^ v.x;
-            x = s_tab[768 + (x & 0xFF)] ^ s_tab[512 + ((x >> 8) & 0xFF)] ^ s_tab[256 + ((x >> 16) & 0xFF)] ^ s_tab[x >> 24];
-            x ^= v.y;
-            x = s_tab[768 + (x & 0xFF)] ^ s_tab[512 + ((x >> 8) & 0xFF)] ^ s_tab[256 + ((x >> 16) & 0xFF)] ^ s_tab[x >> 24];
-            x ^= v.z;
-            x = s_tab[768 + (x & 0xFF)] ^ s_tab[512 + ((x >> 8) & 0xFF)] ^ s_tab[256 + ((x >> 16) & 0xFF)] ^ s_tab[x >> 24];
-            x ^= v.w;
-            if (i == last_i) c = s_tab[768 + (x & 0xFF)] ^ s_tab[512 + ((x >> 8) & 0xFF)] ^ s_tab[256 + ((x >> 16) & 0xFF)] ^ s_tab[x >> 24];
-            else c = s_adv[x & 0xFF] ^ s_adv[256 + ((x >> 8) & 0xFF)] ^ s_adv[512 + ((x >> 16) & 0xFF)] ^ s_adv[768 + (x >> 24)];
-          }
-        }
-#endif
       }
       s_part[tid] = c;
       // chunks outside [ca, cz): the tile's leading header-only chunk (cannot happen: header and body share chunk ca

@@ -20,14 +20,11 @@
 #ifndef TEZGPU_EMIT4_MIN_CTAS
 #define TEZGPU_EMIT4_MIN_CTAS 3  // CTAs per SM of k_emit_fast4u (emit_pipe_u.cuh)
 #endif
-#ifndef TEZGPU_EMIT4_MAP16
-#define TEZGPU_EMIT4_MAP16 0
-#endif
 
 namespace tezgpu {
 
 constexpr int FE4_BATCH = FE_THREADS / 32;  // one parked tile per warp (k_emit_fast4u)
-constexpr int FE4_UNROLL = TEZGPU_EMIT4_MAP16 ? 6 : 5;  // gather rounds held in registers
+constexpr int FE4_UNROLL = 5;               // gather rounds held in registers
 constexpr int FE4_RUN = 5;                  // 16-byte chunks per thread-run of the checksum
 constexpr uint32_t FE4_RUN_BYTES = 16u * FE4_RUN;
 constexpr int FE4_IMG_BYTES = FE_THREADS * FE4_RUN * 16;  // 20480: the tile image is exactly FE4_RUN rounds of chunks
@@ -59,12 +56,7 @@ constexpr uint32_t FE4_MAX_CPR = 8;
 // image?
 static inline bool emit4_fits(uint32_t recs, uint32_t cpr, uint32_t rec_size) {
   if (cpr > FE4_MAX_CPR || recs > emit4_max_recs(rec_size)) return false;
-#if TEZGPU_EMIT4_MAP16
-  const uint32_t rph = 16u / cpr;
-  return 16ull * ((recs + rph - 1) / rph) <= (uint64_t)FE4_UNROLL * FE_THREADS;
-#else
   return (uint64_t)recs * cpr <= (uint64_t)FE4_UNROLL * FE_THREADS;
-#endif
 }
 
 // W = "* x^32" on a word whose digit k (FE4_WBITS wide, the top one narrower) is e: the value of entry e of digit
@@ -151,24 +143,8 @@ __global__ void __launch_bounds__(FE_THREADS * FE4_GROUPS, 1) k_emit_fast4(FastE
   const uint32_t rec_size = e.rec_size, hdr_len = e.fixed_hdr_len, stride = fp.stride, cpr = fp.cpr;
   const TileDesc *__restrict__ tiles = fp.tiles;
 
-  // piece slot of a tile <-> (record j, 16-byte piece c).
-  // MAP16 = 0: consecutive lanes take consecutive pieces, records straddle the 8-lane quarters a 128-bit warp load is
-  //            split into, so a quarter touches the lines of up to three records;
-  // MAP16 = 1: every half-warp takes 16/cpr whole records (leftover lanes idle): fewer distinct 128-byte lines per
-  //            quarter -> fewer L1 wavefronts for the random gather.
+  // piece slot of a tile <-> (record j, 16-byte piece c): consecutive lanes take consecutive pieces.
   // Even records first, then odd ones (emit_fast.cuh): keeps a warp on one unaligned-store path.
-#if TEZGPU_EMIT4_MAP16
-  const uint32_t rph = 16u / cpr;                       // records per half-warp
-  const uint32_t hl = tid & 15u, rl = hl / cpr, pc = hl - rl * cpr;
-  const bool lane_used = rl < rph;
-  auto piece = [&](int u, uint32_t nr, uint32_t &j, uint32_t &c) -> bool {
-    const uint32_t jp = (((uint32_t)tid >> 4) + 16u * (uint32_t)u) * rph + rl;
-    c = pc;
-    const uint32_t half_up = (nr + 1) >> 1;
-    j = jp < half_up ? 2u * jp : 2u * (jp - half_up) + 1u;
-    return lane_used && jp < nr;
-  };
-#else
   auto piece = [&](int u, uint32_t nr, uint32_t &j, uint32_t &c) -> bool {
     const uint32_t q = tid + u * FE_THREADS;
     const uint32_t jp = cpr == 1 ? q : __umulhi(q, fp.cpr_magic);
@@ -177,7 +153,6 @@ __global__ void __launch_bounds__(FE_THREADS * FE4_GROUPS, 1) k_emit_fast4(FastE
     j = jp < half_up ? 2u * jp : 2u * (jp - half_up) + 1u;
     return q < nr * cpr;
   };
-#endif
   // Full tiles (all but the last of a partition) share one piece map: packed once per thread as
   // j | 16c << 8 | (j * rec_size + hdr_len + 16c) << 15 (j < 256, 16c < 128: cpr <= FE4_MAX_CPR, checked by
   // emit4_fits), so a piece costs an index look-up and one multiply-add instead of the divide / permute arithmetic

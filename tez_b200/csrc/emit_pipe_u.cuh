@@ -8,8 +8,7 @@
 //   * the loads of tile N+1 are issued before the checksum loop of tile N; source offsets (two dependent global loads:
 //     sorted order -> record index -> byte offset) are fetched three / two tiles ahead;
 //   * batched second-level checksum folds, two barriers per tile (as emit_pipe.cuh).
-// TEZGPU_EMIT_PIPE_UNALIGNED=0 selects the older kernel k_emit_fast<5,false> (tools/merge_profile.py times the
-// batched reduce-side merge both ways).
+// Records of more than 31 pieces do not fit a warp's round and take k_emit_fast<5,false> (plan_fixed_emit, sorter.cuh).
 //
 // The checksum / write-out loop and the batched fold are NOT those of k_emit_fast4 any more: that kernel folds
 // per-thread runs of five chunks on lane-private tables (one CTA of two groups per SM), this one still folds the
@@ -32,31 +31,13 @@ static inline uint32_t emit4u_max_recs(uint32_t cpr) {
   return w > 32 ? 0u : (uint32_t)FE4U_UNROLL * (FE_THREADS / 32) * (32u / w);
 }
 
-// funnel shifts that also compile for the host (the chunk-assembly algebra is unit-tested on the CPU)
-__host__ __device__ __forceinline__ uint32_t fsr32(uint32_t lo, uint32_t hi, uint32_t s) {
-#ifdef __CUDA_ARCH__
-  return __funnelshift_r(lo, hi, s);
-#else
-  s &= 31u;
-  return s ? (lo >> s) | (hi << (32u - s)) : lo;
-#endif
-}
-__host__ __device__ __forceinline__ uint32_t fsl32(uint32_t lo, uint32_t hi, uint32_t s) {
-#ifdef __CUDA_ARCH__
-  return __funnelshift_l(lo, hi, s);
-#else
-  s &= 31u;
-  return s ? (hi << s) | (lo >> (32u - s)) : hi;
-#endif
-}
-
 // bytes [sh, sh + 16) of the 32-byte window lo || hi
-__host__ __device__ __forceinline__ uint4 window16(uint4 lo, uint4 hi, uint32_t sh) {
+__device__ __forceinline__ uint4 window16(uint4 lo, uint4 hi, uint32_t sh) {
   uint32_t w0 = lo.x, w1 = lo.y, w2 = lo.z, w3 = lo.w, w4 = hi.x, w5 = hi.y, w6 = hi.z, w7 = hi.w;
   if (sh & 4u) { w0 = w1; w1 = w2; w2 = w3; w3 = w4; w4 = w5; w5 = w6; w6 = w7; }
   if (sh & 8u) { w0 = w2; w1 = w3; w2 = w4; w3 = w5; w4 = w6; }
   const uint32_t bsh = (sh & 3u) * 8u;
-  return make_uint4(fsr32(w0, w1, bsh), fsr32(w1, w2, bsh), fsr32(w2, w3, bsh), fsr32(w3, w4, bsh));
+  return make_uint4(__funnelshift_r(w0, w1, bsh), __funnelshift_r(w1, w2, bsh), __funnelshift_r(w2, w3, bsh), __funnelshift_r(w3, w4, bsh));
 }
 
 template <int UNROLL>

@@ -525,9 +525,7 @@ class Merger {
       const int P = pipe.conf.num_partitions;
       std::vector<uint32_t> pseg((size_t)P + 1, 0);
       for (uint32_t s = 0; s < nseg; s++) pseg[segs[s].partition + 1]++;
-      uint32_t max_runs = 0;
-      for (int p = 0; p < P; p++) { max_runs = std::max(max_runs, pseg[p + 1]); pseg[p + 1] += pseg[p]; }
-      pipe.merge_max_runs = max_runs;
+      for (int p = 0; p < P; p++) pseg[p + 1] += pseg[p];
       d_run_pseg.ensure(((size_t)P + 1) * 4);
       TG_CUDA(cudaMemcpyAsync(d_run_pseg.p, pseg.data(), ((size_t)P + 1) * 4, cudaMemcpyHostToDevice, st));
       d_run_off.ensure((size_t)nseg * 8); d_run_base.ensure((size_t)(nseg + 1) * 4); d_run_part.ensure((size_t)nseg * 4);

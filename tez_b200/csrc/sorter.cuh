@@ -8,12 +8,7 @@
 
 #include "../../include/tezgpu.h"
 #include "device_util.h"
-#ifndef TEZGPU_EMIT_ROUND_FILL_DEFAULT
-#define TEZGPU_EMIT_ROUND_FILL_DEFAULT 0
-#endif
 #include "emit_pipe_u.cuh"
-#include "emit_tma.cuh"
-#include "emit_runs.cuh"
 #include "sorter_kernels.cuh"
 
 namespace tezgpu {
@@ -63,6 +58,50 @@ struct DeviceConstants {
 
 // thrown by sort_phase in run-table mode (Records::use_runs): the merger then re-parses the segments with the walker
 struct FramingMismatch {};
+
+// The emit kernels for fixed-width records written without repeats (records with repeats take k_emit<false>).
+enum class FixedEmitKernel {
+  Pipe,           // k_emit_fast4: packed, 16-byte aligned records, stride a multiple of 16, at most FE4_MAX_CPR pieces
+  Fast,           // k_emit_fast<5, true>: the same, wider records
+  PipeUnaligned,  // k_emit_fast4u: records at arbitrary offsets, stride a multiple of 16, at most 31 pieces
+  FastUnaligned,  // k_emit_fast<5, false>: the same, wider records
+  General,        // k_emit<true>: strides that are not a multiple of 16
+};
+struct FixedEmitPlan {
+  FixedEmitKernel kernel;
+  uint32_t recs_per_tile;
+};
+
+// Kernel and tile size of a fixed-width emit, from the record view alone.  sort_phase lays the tiles out with it
+// speculatively and emit_phase launches the kernel it names, so the tile size always suits the kernel.
+static inline FixedEmitPlan plan_fixed_emit(const Records &rec, uint32_t rec_size) {
+  const uint32_t stride = rec.klen + rec.vlen, cpr = stride / 16;
+  // the tile image must fit the image buffer of the source-oriented emit kernels (FE_IMG_BYTES)
+  const uint32_t cap = std::max<uint32_t>(1, std::min<uint32_t>(EMIT_MAX_RECS, (FE_IMG_BYTES - 32) / rec_size));
+  if (stride < 16 || stride % 16) return {FixedEmitKernel::General, cap};
+  if (!rec.key_off && !rec.use_runs && ((uintptr_t)rec.kv & 15u) == 0) {
+    // k_emit_fast4's image holds exactly FE4_RUN checksum rounds, so a tile takes as many records as fit it in the
+    // worst case (249 of 82 bytes: 1278 chunks, 1280 slots)
+    const uint32_t m = emit4_max_recs(rec_size);
+    if (emit4_fits(m, cpr, rec_size)) return {FixedEmitKernel::Pipe, std::min(cap, m)};
+    return {FixedEmitKernel::Fast, cap};
+  }
+  // k_emit_fast4u holds a tile's words in FE4U_UNROLL gather rounds (at least 40 records when a record fits a warp)
+  const uint32_t m = emit4u_max_recs(cpr);
+  if (m == 0) return {FixedEmitKernel::FastUnaligned, cap};
+  // Round filling: its checksum / write-out loop walks a tile in rounds of FE_THREADS 16-byte chunks.  Among the tile
+  // sizes within 10 % of the cap, take the one with the most records per executed round.
+  const uint32_t top = std::min(cap, m);
+  uint32_t best = top;
+  double best_eff = 0;
+  for (uint32_t r = top; r >= top - top / 10; r--) {
+    const uint64_t chunks = ((uint64_t)r * rec_size + 15 + 4 + 2 + 15) / 16;  // worst-case lead, header, EOF
+    const uint64_t rounds = (chunks + FE_THREADS - 1) / FE_THREADS;
+    const double eff = (double)r / (double)rounds;
+    if (eff > best_eff) { best_eff = eff; best = r; }
+  }
+  return {FixedEmitKernel::PipeUnaligned, best};
+}
 
 class SortPipeline {
  public:
@@ -143,12 +182,6 @@ class SortPipeline {
   // (every segment had the plain fixed framing), which together decide whether any record can be written as a repeat
   int merge_check_same = 1;
   bool merge_inputs_plain = false;
-  uint32_t merge_max_runs = 0;   // run-table mode: most runs any output partition has (emit_runs.cuh plans <= 32 per warp)
-  static bool runs_emit_enabled() {
-    // opt-in: the pipelined gather (emit_pipe_u.cuh) is the default for these records
-    static const bool on = getenv("TEZGPU_EMIT_RUNS") && atoi(getenv("TEZGPU_EMIT_RUNS")) != 0;
-    return on;
-  }
 
   EmitParams make_emit_params(const Records &rec, const uint32_t *order, int rle, bool merge_mode, uint8_t *d_out) {
     EmitParams e;
@@ -170,54 +203,17 @@ class SortPipeline {
     e.P = conf.num_partitions;
     return e;
   }
-  static bool pipe_unaligned_enabled() {
-    // on by default; TEZGPU_EMIT_PIPE_UNALIGNED=0 falls back to k_emit_fast<5,false>
-    static const bool on = !(getenv("TEZGPU_EMIT_PIPE_UNALIGNED") && atoi(getenv("TEZGPU_EMIT_PIPE_UNALIGNED")) == 0);
-    return on;
-  }
-  void set_fixed_layout(EmitParams &e, const Records &rec) {
+  // fixed framing (vint klen, vint vlen) and the tile size of the emit kernel the plan picks, which it returns
+  FixedEmitKernel set_fixed_layout(EmitParams &e, const Records &rec) {
     int h = 0;
     for (int b = 0; b < vint_size_u32(rec.klen); b++) e.fixed_hdr[h++] = vint_byte_u32(rec.klen, b);
     for (int b = 0; b < vint_size_u32(rec.vlen); b++) e.fixed_hdr[h++] = vint_byte_u32(rec.vlen, b);
     e.fixed_hdr_len = h;
     e.rec_size = h + rec.klen + rec.vlen;
-    // the tile image must fit the image buffer of the source-oriented emit kernels (FE_IMG_BYTES)
-    e.recs_per_tile = std::max<uint32_t>(1, std::min<uint32_t>(EMIT_MAX_RECS, (FE_IMG_BYTES - 32) / e.rec_size));
-    // Round filling: the checksum / write-out loop of the source-oriented kernels walks a tile in rounds of
-    // FE_THREADS 16-byte chunks; 256 records of 82 bytes are 5.13 rounds, six are executed.  Among the tile sizes
-    // within 10 % of the cap, take the one with the most records per executed round (249 for 82-byte records).
-    static const int round_fill = getenv("TEZGPU_EMIT_ROUND_FILL") ? atoi(getenv("TEZGPU_EMIT_ROUND_FILL")) : TEZGPU_EMIT_ROUND_FILL_DEFAULT;
-    bool fill = round_fill != 0;
-    const uint32_t stride = rec.klen + rec.vlen;
-    const bool fast = stride >= 16 && stride % 16 == 0;
-    const bool aligned = !rec.key_off && !rec.use_runs && (((uintptr_t)rec.kv & 15u) == 0);
-    if (rec.use_runs && runs_emit_enabled() && emit_runs_fits(e.recs_per_tile, e.rec_size, merge_max_runs)) {
-      // run-table mode with the range-copy emit (emit_runs.cuh): full 256-record tiles
-    } else if (fast && aligned && emit4_max_recs(e.rec_size) >= 1 && emit4_fits(emit4_max_recs(e.rec_size), stride / 16, e.rec_size)) {
-      // the pipelined kernel for packed aligned records (emit_pipe.cuh): its image holds exactly FE4_RUN checksum
-      // rounds, so a tile takes as many records as fit it in the worst case (249 of 82 bytes: 1278 chunks, 1280 slots).
-      // Wider records (more than FE4_MAX_CPR pieces) keep the tiles of k_emit_fast.
-      e.recs_per_tile = std::min<uint32_t>(e.recs_per_tile, emit4_max_recs(e.rec_size));
-    } else if (pipe_unaligned_enabled()) {
-      // the pipelined kernel for records at arbitrary offsets (emit_pipe_u.cuh) holds a tile's words in five gather rounds
-      if (fast && !aligned && emit4u_max_recs(stride / 16) >= 32) {
-        e.recs_per_tile = std::min<uint32_t>(e.recs_per_tile, emit4u_max_recs(stride / 16));
-        fill = true;
-      }
-    }
-    if (fill && e.recs_per_tile >= 32) {
-      const uint32_t cap = e.recs_per_tile;
-      uint32_t best = cap;
-      double best_eff = 0;
-      for (uint32_t r = cap; r >= cap - cap / 10; r--) {
-        const uint64_t chunks = ((uint64_t)r * e.rec_size + 15 + 4 + 2 + 15) / 16;  // worst-case lead, header, EOF
-        const uint64_t rounds = (chunks + FE_THREADS - 1) / FE_THREADS;
-        const double eff = (double)r / (double)rounds;
-        if (eff > best_eff) { best_eff = eff; best = r; }
-      }
-      e.recs_per_tile = best;
-    }
+    const FixedEmitPlan plan = plan_fixed_emit(rec, e.rec_size);
+    e.recs_per_tile = plan.recs_per_tile;
     e.rec_off = nullptr;
+    return plan.kernel;
   }
 
   void run(Records rec, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index, tezgpu_stats *stats) {
@@ -512,15 +508,13 @@ class SortPipeline {
     const bool fixed_emit = rec.fixed && (dup_count == 0 || no_repeats);
     uint64_t bound = output_bound(n, rec.fixed ? (uint64_t)n * (rec.klen + rec.vlen) : rec.kv_bytes, P);
     uint64_t *hs = h_small.as<uint64_t>();
+    const FixedEmitKernel kernel = fixed_emit ? set_fixed_layout(e, rec) : FixedEmitKernel::General;
     if (fixed_emit && state.spec_layout) {
-      // layout, totals and index triples were produced during the sort phase (same parameters): no round trip here
-      set_fixed_layout(e, rec);
+      // layout, totals and index triples were produced during the sort phase (same plan): no round trip here
       hs[0] = state.spec_file_bytes;
       hs[1] = state.spec_tiles;
     } else {
-      if (fixed_emit) {
-        set_fixed_layout(e, rec);
-      } else {
+      if (!fixed_emit) {
         uint64_t avg = n ? (rec.fixed ? (uint64_t)(rec.klen + rec.vlen) : rec.kv_bytes / n) + 4 : 16;
         e.recs_per_tile = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(EMIT_MAX_RECS, (EMIT_IMG_BYTES - 32) / avg));
         sizes.ensure(n4);
@@ -553,13 +547,12 @@ class SortPipeline {
     const uint64_t tiles = hs[1];
     TG_CHECK(file_bytes <= bound, TEZGPU_E_INVALID, "internal: output exceeds bound");
     TG_CHECK(file_bytes <= out_cap, TEZGPU_E_NOMEM, "output buffer too small for file.out");
-    // fixed-width records take the source-oriented kernel (emit_fast.cuh): 16-byte aligned packed records use one
-    // 128-bit load per piece, records at explicit / unaligned offsets two loads + a funnel shift
+    // the source-oriented kernels (emit_fast.cuh, emit_pipe*.cuh) gather 16-byte pieces of the records tile by tile
+    // and leave one checksum per tile
+    const bool source_oriented = fixed_emit && kernel != FixedEmitKernel::General;
     const uint32_t stride = rec.klen + rec.vlen;
-    const bool fast_emit = fixed_emit && stride >= 16 && (stride % 16 == 0) && !getenv("TEZGPU_NO_FAST_EMIT");
-    const bool fast_aligned = fast_emit && !rec.key_off && !rec.use_runs && (((uintptr_t)rec.kv & 15u) == 0);
     FastEmitParams fp;
-    if (tiles && fast_emit) {
+    if (tiles && source_oriented) {
       tile_desc.ensure((size_t)tiles * sizeof(TileDesc));
       k_build_tiles<<<(uint32_t)div_up(tiles, 256), 256, 0, stream>>>(e, tile_desc.as<TileDesc>());
       launches++;
@@ -574,81 +567,54 @@ class SortPipeline {
     }
     timer.mark(stream);
     if (tiles) {
-      if (fast_emit) {
+      // persistent CTAs: as many as fit the device at once
+      auto persistent_grid = [&](auto kern, int threads, size_t smem) {
         int per_sm = 0;
-        // opt-in (TEZGPU_EMIT_TMA=1): byte-exact (the GPU parity tests run it), but slower than the register-staged
-        // kernel -- the bulk-copy gather itself is no faster than the LDG gather (tools/bench_gather.cu times both), and
-        // bulk copies are warp-uniform instructions whose per-record issue and chunk assembly cost more than they save
-        static const bool use_tma = getenv("TEZGPU_EMIT_TMA") && atoi(getenv("TEZGPU_EMIT_TMA")) != 0;
-        if (fast_aligned && use_tma && emit_tma_fits(e.recs_per_tile, stride)) {
-          // gather by the bulk-copy engine into a shared-memory ring, chunks assembled straight from the staged
-          // records (emit_tma.cuh); TEZGPU_EMIT_TMA=0 selects the register-staged kernels below
-          const size_t smem = EmitTmaLayout::total(e.recs_per_tile, stride);
-          static size_t attr_smem = 0;
-          if (smem > attr_smem) {
-            TG_CUDA(cudaFuncSetAttribute(k_emit_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            attr_smem = smem;
+        TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+        return (uint32_t)std::min<uint64_t>(tiles, (uint64_t)num_sms * (per_sm > 0 ? per_sm : 1));
+      };
+      if (!fixed_emit) {
+        k_emit<false><<<persistent_grid(k_emit<false>, EMIT_THREADS, 0), EMIT_THREADS, 0, stream>>>(e);
+      } else {
+        switch (kernel) {
+          case FixedEmitKernel::Pipe: {
+            // One CTA per SM, FE4_GROUPS independent 256-thread groups sharing the lane-private checksum tables (66 KB)
+            // next to their images, indices and parked partials (54 KB): 125 KB keeps the CTA in the 132 KB
+            // shared-memory carveout, which leaves the random gather enough L1 for its loads in flight (larger
+            // footprints measured slower, DESIGN.md §7).
+            static bool attr = false;
+            if (!attr) {
+              TG_CUDA(cudaFuncSetAttribute(k_emit_fast4<FE4_UNROLL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Emit4Smem::TOTAL));
+              attr = true;
+            }
+            const uint32_t grid = (uint32_t)std::min<uint64_t>(div_up(tiles, FE4_GROUPS), (uint64_t)num_sms);
+            k_emit_fast4<FE4_UNROLL><<<grid, FE_THREADS * FE4_GROUPS, Emit4Smem::TOTAL, stream>>>(fp);
+            break;
           }
-          TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_emit_tma, ET_THREADS, smem));
-          uint32_t grid = (uint32_t)std::min<uint64_t>(tiles, (uint64_t)num_sms * (per_sm > 0 ? per_sm : 1));
-          k_emit_tma<<<grid, ET_THREADS, smem, stream>>>(fp, (uint32_t)EmitTmaLayout::stage_bytes(e.recs_per_tile, stride));
-        } else if (fast_aligned && emit4_fits(e.recs_per_tile, fp.cpr, e.rec_size) && !getenv("TEZGPU_EMIT_V2")) {
-          // software-pipelined kernel (emit_pipe.cuh): a tile's pieces must fit the registers of one gather round and
-          // its bytes the FE4_IMG_BYTES image.  One CTA per SM, FE4_GROUPS independent 256-thread groups sharing the
-          // lane-private checksum tables (66 KB) next to their images, indices and parked partials (54 KB): 125 KB
-          // keeps the CTA in the 132 KB shared-memory carveout, which leaves the random gather enough L1 for its
-          // loads in flight (larger footprints measured slower, DESIGN.md §7).
-          static bool attr = false;
-          if (!attr) {
-            TG_CUDA(cudaFuncSetAttribute(k_emit_fast4<FE4_UNROLL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Emit4Smem::TOTAL));
-            attr = true;
+          case FixedEmitKernel::Fast:
+            k_emit_fast<5, true><<<persistent_grid(k_emit_fast<5, true>, FE_THREADS, 0), FE_THREADS, 0, stream>>>(fp);
+            break;
+          case FixedEmitKernel::PipeUnaligned: {
+            static bool attr = false;
+            if (!attr) {
+              TG_CUDA(cudaFuncSetAttribute(k_emit_fast4u<FE4U_UNROLL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Emit4uSmem::TOTAL));
+              attr = true;
+            }
+            const uint32_t grid = persistent_grid(k_emit_fast4u<FE4U_UNROLL>, FE_THREADS, Emit4uSmem::TOTAL);
+            k_emit_fast4u<FE4U_UNROLL><<<grid, FE_THREADS, Emit4uSmem::TOTAL, stream>>>(fp);
+            break;
           }
-          uint32_t grid = (uint32_t)std::min<uint64_t>(div_up(tiles, FE4_GROUPS), (uint64_t)num_sms);
-          k_emit_fast4<FE4_UNROLL><<<grid, FE_THREADS * FE4_GROUPS, Emit4Smem::TOTAL, stream>>>(fp);
-        } else if (rec.use_runs && runs_emit_enabled() && emit_runs_fits(e.recs_per_tile, e.rec_size, merge_max_runs)) {
-          // reduce side, fixed-framing runs in place: one bulk copy per run and tile (emit_runs.cuh)
-          const size_t smem = EmitRunsLayout::total(e.recs_per_tile, e.rec_size);
-          static size_t attr_smem = 0;
-          if (smem > attr_smem) {
-            TG_CUDA(cudaFuncSetAttribute(k_emit_runs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            attr_smem = smem;
-          }
-          TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_emit_runs, ER_THREADS, smem));
-          uint32_t grid = (uint32_t)std::min<uint64_t>(tiles, (uint64_t)num_sms * (per_sm > 0 ? per_sm : 1));
-          k_emit_runs<<<grid, ER_THREADS, smem, stream>>>(fp, (uint32_t)EmitRunsLayout::stage_data(e.recs_per_tile, e.rec_size),
-                                                         (uint32_t)EmitRunsLayout::stage_bytes(e.recs_per_tile, e.rec_size));
-        } else if (fast_aligned) {
-          TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_emit_fast<5, true>, FE_THREADS, 0));
-          uint32_t grid = (uint32_t)std::min<uint64_t>(tiles, (uint64_t)num_sms * (per_sm > 0 ? per_sm : 1));
-          k_emit_fast<5, true><<<grid, FE_THREADS, 0, stream>>>(fp);
-        } else if (!fast_aligned && pipe_unaligned_enabled() && e.recs_per_tile <= emit4u_max_recs(fp.cpr)) {
-          // records at arbitrary offsets (reduce side), software-pipelined variant
-          static bool attr = false;
-          if (!attr) {
-            TG_CUDA(cudaFuncSetAttribute(k_emit_fast4u<FE4U_UNROLL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Emit4uSmem::TOTAL));
-            attr = true;
-          }
-          TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_emit_fast4u<FE4U_UNROLL>, FE_THREADS, Emit4uSmem::TOTAL));
-          uint32_t grid = (uint32_t)std::min<uint64_t>(tiles, (uint64_t)num_sms * (per_sm > 0 ? per_sm : 1));
-          k_emit_fast4u<FE4U_UNROLL><<<grid, FE_THREADS, Emit4uSmem::TOTAL, stream>>>(fp);
-        } else {
-          TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_emit_fast<5, false>, FE_THREADS, 0));
-          uint32_t grid = (uint32_t)std::min<uint64_t>(tiles, (uint64_t)num_sms * (per_sm > 0 ? per_sm : 1));
-          k_emit_fast<5, false><<<grid, FE_THREADS, 0, stream>>>(fp);
+          case FixedEmitKernel::FastUnaligned:
+            k_emit_fast<5, false><<<persistent_grid(k_emit_fast<5, false>, FE_THREADS, 0), FE_THREADS, 0, stream>>>(fp);
+            break;
+          case FixedEmitKernel::General:
+            k_emit<true><<<persistent_grid(k_emit<true>, EMIT_THREADS, 0), EMIT_THREADS, 0, stream>>>(e);
+            break;
         }
+      }
+      if (source_oriented) {
         k_crc_combine<<<(uint32_t)div_up(tiles, 256), 256, 0, stream>>>(fp.tile_crc, (uint32_t)tiles, d_crc, seg_crc.as<uint32_t>());
         launches++;
-      } else {
-        // general kernel, persistent CTAs (as many as fit the device at once)
-        static int per_sm_fixed = 0, per_sm_var = 0;
-        if (!per_sm_fixed) {
-          TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_fixed, k_emit<true>, EMIT_THREADS, 0));
-          TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_var, k_emit<false>, EMIT_THREADS, 0));
-        }
-        const uint32_t cap = (uint32_t)num_sms * (uint32_t)std::max(1, fixed_emit ? per_sm_fixed : per_sm_var);
-        const uint32_t grid = (uint32_t)std::min<uint64_t>(tiles, cap);
-        if (fixed_emit) k_emit<true><<<grid, EMIT_THREADS, 0, stream>>>(e);
-        else k_emit<false><<<grid, EMIT_THREADS, 0, stream>>>(e);
       }
       launches++;
       TG_CUDA(cudaGetLastError());

@@ -573,37 +573,6 @@ uint32_t tezgpu_debug_crc_emulate(const uint8_t *body, uint64_t len, uint32_t pi
   return crc;
 }
 
-// Host emulation of the TMA emit kernel's chunk assembly (emit_tma.cuh): builds the output byte image of one tile chunk
-// by chunk with the very same template code the consumer warps run, from `nr` staged records of `stride` bytes.
-// image_out receives 16 * (chunks) bytes starting at image offset 0; returns the image length (body_end).
-uint32_t tezgpu_debug_assemble_emulate(const uint8_t *stage, uint32_t nr, uint32_t stride, const uint8_t *hdr, uint32_t hdr_len,
-                                       uint32_t lead, int32_t first, int32_t last, uint8_t *image_out, uint32_t image_cap) {
-  std::vector<uint8_t> padded((size_t)nr * stride + 64, 0);
-  memcpy(padded.data(), stage, (size_t)nr * stride);
-  HostSmem sm{padded.data()};
-  TmaEmitConst kc;
-  kc.rec_size = hdr_len + stride;
-  kc.hdr_len = hdr_len;
-  kc.stride = stride;
-  kc.magic = (uint32_t)((1ull << 32) / kc.rec_size) + 1u;
-  uint32_t hw[4] = {0, 0, 0, 0};
-  for (uint32_t b = 0; b < hdr_len; b++) hw[b >> 2] |= (uint32_t)hdr[b] << (8u * (b & 3u));
-  kc.hdr = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-  TmaTileGeom g;
-  g.stg = 0;
-  g.nr = nr;
-  g.first = first != 0;
-  g.last = last != 0;
-  g.rec0 = lead + (g.first ? 4u : 0u);
-  g.body = nr * kc.rec_size;
-  const uint32_t body_end = g.rec0 + g.body + (g.last ? 2u : 0u);
-  for (uint32_t c = lead >> 4; 16u * c < body_end && 16u * c + 16u <= image_cap; c++) {
-    const uint4 v = tma_assemble(sm, kc, g, 16u * c);
-    memcpy(image_out + 16u * c, &v, 16);
-  }
-  return body_end;
-}
-
 // Host emulation of the chunk-interleaved checksum of the emit / verify kernels (crc32.cuh CrcChunkFold): 256 threads,
 // thread t folds chunks i = Cn + t - iters*256 (+256 ...), partials are combined by the adv128 second-level fold, the
 // per-lane alignment multiplier and an xor across lanes.  ilp = 1 runs the two-deep fold with the einv correction,
@@ -686,30 +655,6 @@ uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks) {
   }
   delete t;
   return total;
-}
-
-// Host emulation of the run-range emit kernel's chunk assembly (emit_runs.cuh): record j of the tile is the rec_size
-// bytes at staging[src[j]...]; builds the output image chunk by chunk with the kernel's template code.
-uint32_t tezgpu_debug_runs_assemble_emulate(const uint8_t *staging, uint32_t staging_len, const uint32_t *src, uint32_t nr,
-                                            uint32_t rec_size, uint32_t lead, int32_t first, int32_t last, uint8_t *image_out,
-                                            uint32_t image_cap) {
-  std::vector<uint8_t> padded((size_t)staging_len + 64, 0);
-  memcpy(padded.data(), staging, staging_len);
-  HostSmem sm{padded.data()};
-  RunsTileGeom g;
-  g.src = src;
-  g.nr = nr;
-  g.first = first != 0;
-  g.last = last != 0;
-  g.rec0 = lead + (g.first ? 4u : 0u);
-  g.body = nr * rec_size;
-  const uint32_t magic = (uint32_t)((1ull << 32) / rec_size) + 1u;
-  const uint32_t body_end = g.rec0 + g.body + (g.last ? 2u : 0u);
-  for (uint32_t c = lead >> 4; 16u * c < body_end && 16u * c + 16u <= image_cap; c++) {
-    const uint4 v = runs_assemble(sm, rec_size, magic, g, 16u * c);
-    memcpy(image_out + 16u * c, &v, 16);
-  }
-  return body_end;
 }
 
 }  // extern "C"
