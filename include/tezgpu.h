@@ -98,6 +98,18 @@ typedef struct tezgpu_stats {
 typedef struct tezgpu_sorter tezgpu_sorter;
 typedef struct tezgpu_merger tezgpu_merger;
 
+/* Combiner: ExternalSorter.combiner = MRCombiner running one of the sum reducers below, applied on the device between
+ * the sort and the IFile writer (SORT/PipelinedSorter.java:601-609,815-820; SORT/dflt/DefaultSorter.java:915-945).
+ * A group is a maximal run of adjacent records of one partition whose keys compare equal (ValuesIterator); it is
+ * written as one record: the key bytes, then the big-endian sum of the group's values (Java arithmetic: wraps).  Keys
+ * are then unique per partition, so no REPEAT_KEY marker is written; stats.rle_used / adjacent_equal_keys still report
+ * the decision made on the uncombined stream.  A value that is not 4 (INT) or 8 (LONG) bytes wide fails the flush /
+ * write with TEZGPU_E_INVALID.  With a combiner, stats.output_records counts the records that entered the combine
+ * (COMBINE_INPUT_RECORDS) and stats.spilled_records those written (COMBINE_OUTPUT_RECORDS); ms_total includes it. */
+#define TEZGPU_COMBINE_NONE 0
+#define TEZGPU_COMBINE_SUM_INT 1    /* IntSumReducer over IntWritable values */
+#define TEZGPU_COMBINE_SUM_LONG 2   /* LongSumReducer over LongWritable values */
+
 const char *tezgpu_last_error(void);
 int32_t tezgpu_abi_version(void);
 /* number of visible CUDA devices (0 when none; never falls back to CPU) */
@@ -149,6 +161,11 @@ int32_t tezgpu_sorter_sort_device_fixed(tezgpu_sorter *h, const void *d_kv, cons
 /* cudaStream_t of the handle, as an opaque pointer (so callers can record events on it) */
 void *tezgpu_sorter_stream(tezgpu_sorter *h);
 
+/* runs the combiner (TEZGPU_COMBINE_*) on every flush of the handle.  Call before the first collect (or right after a
+ * reset); survives reset.  Fails with TEZGPU_E_INVALID on an unordered handle (UnorderedPartitionedKVWriter has no
+ * combiner) and on a fixed-width handle whose fixed_val_len is not the combiner's value width. */
+int32_t tezgpu_sorter_set_combiner(tezgpu_sorter *h, int32_t combiner);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Merger: replaces TezMerger.merge(...) -> TezRawKeyValueIterator (SORT/TezMerger.java:717-912,
  * SORT/TezRawKeyValueIterator.java:33-87) as called from OG/MergeManager.java:804-811,899-903,1035-1041,1197-1199
@@ -184,6 +201,10 @@ int32_t tezgpu_merge_reopen(tezgpu_merger *m, const tezgpu_segment *segs, uint32
  * (adjustPriorityQueue / compareKeyWithNextTopKey, :597-652).  PipelinedSorter's final merge passes
  * merger.needsRLE() here AND as the writer's rle (SORT/PipelinedSorter.java:797-814).  Call before next_batch / write. */
 int32_t tezgpu_merge_set_check_for_same_keys(tezgpu_merger *m, int32_t check_for_same_keys);
+/* runs the combiner (TEZGPU_COMBINE_*) in tezgpu_merge_write_*: PipelinedSorter's final merge when
+ * numSpills >= tez.runtime.combine.min.spills (SORT/PipelinedSorter.java:815-820).  Call before write_*, like
+ * set_check_for_same_keys.  A merger with a combiner has no record iterator: next_batch fails with TEZGPU_E_STATE. */
+int32_t tezgpu_merge_set_combiner(tezgpu_merger *m, int32_t combiner);
 /* total records / key+value bytes of the merged stream */
 /* diagnostics: how the last open / reopen located the records -- mode 0: fixed framing, records addressed in place
  * (no parse); 1: parallel window parser (by_hand = windows whose guessed entry was wrong and that the chase walked

@@ -44,6 +44,14 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
     if (!checkForSameKeys) nativeSetCheckForSameKeys(handle, false);
   }
 
+  /**
+   * Combines the merged stream in writeIFile (PipelinedSorter's final merge from tez.runtime.combine.min.spills spills
+   * on, PipelinedSorter.java:815-820); next() then fails: a combining merge has no record iterator.
+   */
+  public void setCombiner(int combiner) throws IOException {
+    nativeSetCombiner(handle, combiner);
+  }
+
   @Override
   public boolean next() throws IOException {
     if (++i >= n) {
@@ -87,6 +95,7 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
   private static native long nativeOpen(long[] addresses, long[] lengths, int[] flags, int[] partitions, int numPartitions,
       int comparator, int device) throws IOException;
   private static native void nativeSetCheckForSameKeys(long h, boolean on) throws IOException;
+  private static native void nativeSetCombiner(long h, int combiner) throws IOException;
   private static native int nativeNextBatch(long h, ByteBuffer out, int cap, IntBuffer idx, int idxCap) throws IOException;
   private static native boolean nativeHasMore(long h);
   private static native void nativeWriteIFile(long h, String path, boolean rle, long[] rawAndPart) throws IOException;

@@ -34,6 +34,7 @@ public class GpuSorter extends ExternalSorter {
   // ids of include/tezgpu.h
   static final int CMP_BYTES = 0, CMP_TEXT = 1, CMP_BYTESWRITABLE = 2, CMP_INT = 3, CMP_LONG = 4;
   static final int PART_GIVEN = 0, PART_HASH = 1;
+  static final int COMBINE_NONE = 0, COMBINE_SUM_INT = 1, COMBINE_SUM_LONG = 2;
   private static final int BATCH_BYTES = 32 << 20;
   private static final int BATCH_RECORDS = 1 << 20;
 
@@ -60,6 +61,15 @@ public class GpuSorter extends ExternalSorter {
         Integer.parseInt(System.getenv().getOrDefault("TEZGPU_DEVICE", "0")));
     keySerializer.open(sink);
     valSerializer.open(sink);
+  }
+
+  /**
+   * Runs ExternalSorter's combiner on the device at every spill, when it is MRCombiner with IntSumReducer /
+   * LongSumReducer (COMBINE_SUM_INT / COMBINE_SUM_LONG, chosen by the caller from the reducer and value classes).
+   * Call before the first write.  Any other combiner is not run (a combiner may run zero times).
+   */
+  public void setCombiner(int combiner) throws IOException {
+    nativeSetCombiner(handle, combiner);
   }
 
   /** The device path supports a closed set of RawComparators; anything else keeps tez.runtime.sorter.class=PIPELINED. */
@@ -163,6 +173,7 @@ public class GpuSorter extends ExternalSorter {
    *  [4] OUTPUT_BYTES [5] rle used [6] adjacent equal keys [7] kernel launches */
   private static native void nativeFlush(long h, String out, String index, long[] idx, long[] counters) throws IOException;
   private static native void nativeReset(long h) throws IOException;
+  private static native void nativeSetCombiner(long h, int combiner) throws IOException;
   private static native void nativeDestroy(long h);
 
   /** DataOutputStream target that appends to the direct batch buffer. */

@@ -82,6 +82,12 @@ JNIEXPORT void JNICALL SORTER(nativeReset)(JNIEnv *env, jclass cls, jlong h) {
   failed(env, tezgpu_sorter_reset((tezgpu_sorter *)(intptr_t)h));
 }
 
+/* ExternalSorter.combiner = MRCombiner + IntSumReducer / LongSumReducer (TEZGPU_COMBINE_*) */
+JNIEXPORT void JNICALL SORTER(nativeSetCombiner)(JNIEnv *env, jclass cls, jlong h, jint combiner) {
+  (void)cls;
+  failed(env, tezgpu_sorter_set_combiner((tezgpu_sorter *)(intptr_t)h, combiner));
+}
+
 JNIEXPORT void JNICALL SORTER(nativeDestroy)(JNIEnv *env, jclass cls, jlong h) {
   (void)env; (void)cls;
   tezgpu_sorter_destroy((tezgpu_sorter *)(intptr_t)h);
@@ -124,6 +130,11 @@ JNIEXPORT jlong JNICALL MERGER(nativeOpen)(JNIEnv *env, jclass cls, jlongArray a
 JNIEXPORT void JNICALL MERGER(nativeSetCheckForSameKeys)(JNIEnv *env, jclass cls, jlong h, jboolean on) {
   (void)cls;
   failed(env, tezgpu_merge_set_check_for_same_keys((tezgpu_merger *)(intptr_t)h, on ? 1 : 0));
+}
+
+JNIEXPORT void JNICALL MERGER(nativeSetCombiner)(JNIEnv *env, jclass cls, jlong h, jint combiner) {
+  (void)cls;
+  failed(env, tezgpu_merge_set_combiner((tezgpu_merger *)(intptr_t)h, combiner));
 }
 
 JNIEXPORT jint JNICALL MERGER(nativeNextBatch)(JNIEnv *env, jclass cls, jlong h, jobject out, jint cap, jobject idx, jint idx_cap) {

@@ -66,6 +66,9 @@ static const char *K_FINAL_MERGE = "tez.runtime.enable.final-merge.in.output";  
 static const char *K_REPORT_STATS = "tez.runtime.report.partition.stats";       // :195-198 default memory_optimized
 static const char *K_COMPRESS = "tez.runtime.compress";
 static const char *K_SERIALIZATIONS = "io.serializations";
+static const char *K_VALUE_CLASS = "tez.runtime.value.class";
+static const char *K_COMBINER_CLASS = "tez.runtime.combiner.class";
+static const char *K_COMBINE_MIN_SPILLS = "tez.runtime.combine.min.spills";  // TezRuntimeConfiguration:128-130 default 3
 
 static bool ends_with(const std::string &s, const char *suf) {
   size_t n = strlen(suf);
@@ -83,6 +86,24 @@ static int comparator_for(const Configuration &c) {
     return TEZGPU_CMP_BYTESWRITABLE;
   }
   throw Err(TEZGPU_E_UNSUPPORTED, "key class '" + key + "' has no device comparator (supported: Text, BytesWritable, IntWritable, LongWritable)");
+}
+
+// The combiners the device runs: MRCombiner (tez-mapreduce combine/MRCombiner.java) with a sum reducer over the value
+// class it sums.  The reducer class is mapreduce.job.combine.class under the new API and mapred.combiner.class under
+// the old one (ConfigUtils.useNewApi: mapred.mapper.new-api, default false).  Any other combiner is not run: MR
+// semantics allow a combiner to run zero times.
+static int combiner_for(const Configuration &c) {
+  if (!ends_with(c.get(K_COMBINER_CLASS, ""), "combine.MRCombiner")) return TEZGPU_COMBINE_NONE;
+  const bool new_api = c.getBoolean("mapred.mapper.new-api", false);
+  const std::string red = c.get(new_api ? "mapreduce.job.combine.class" : "mapred.combiner.class", "");
+  const std::string val = c.get(K_VALUE_CLASS, "");
+  if ((red == "org.apache.hadoop.mapreduce.lib.reduce.IntSumReducer" || red == "org.apache.hadoop.examples.WordCount$IntSumReducer") &&
+      val == "org.apache.hadoop.io.IntWritable")
+    return TEZGPU_COMBINE_SUM_INT;
+  if ((red == "org.apache.hadoop.mapreduce.lib.reduce.LongSumReducer" || red == "org.apache.hadoop.mapred.lib.LongSumReducer") &&
+      val == "org.apache.hadoop.io.LongWritable")
+    return TEZGPU_COMBINE_SUM_LONG;
+  return TEZGPU_COMBINE_NONE;
 }
 
 // ---------------------------------------------------------------- small utilities
@@ -191,6 +212,8 @@ struct GpuSorter {
   std::vector<int64_t> final_idx;
   std::vector<int64_t> partition_stats;  // partitionStats[p] += rawLength at every spill (SORT/PipelinedSorter.java:631-633)
   int last_spill_rle = 0;                // merger.needsRLE() of the most recent spill's SpanMerger (:599,805,814)
+  int combiner = TEZGPU_COMBINE_NONE;    // runs on every spill, and on the final merge from min_spills spills on (:601-609,815-820)
+  int min_spills = 3;
   std::map<std::string, int64_t> &counters;
 
   GpuSorter(const tezgpu_conf &c, int64_t mem, bool fm, const std::string &wd, const std::string &u, std::map<std::string, int64_t> &ctr)
@@ -198,6 +221,16 @@ struct GpuSorter {
     gpu_check(tezgpu_sorter_create(&gc, &h));
   }
   ~GpuSorter() { if (h) tezgpu_sorter_destroy(h); }
+  void set_combiner(int c, int min_spills_for_combine) {
+    gpu_check(tezgpu_sorter_set_combiner(h, c));
+    combiner = c;
+    min_spills = min_spills_for_combine;
+  }
+  // MRCombiner's COMBINE_INPUT_RECORDS / COMBINE_OUTPUT_RECORDS of one combined write
+  void count_combine(const tezgpu_stats &st) {
+    counters["COMBINE_INPUT_RECORDS"] += st.output_records;
+    counters["COMBINE_OUTPUT_RECORDS"] += st.spilled_records;
+  }
 
   // TezTaskOutputFiles (RL/common/task/local/output/TezTaskOutputFiles.java:88-231)
   std::string spill_dir(int n) const { return work_dir + "/output/" + uid + "_" + std::to_string(n); }
@@ -247,6 +280,7 @@ struct GpuSorter {
     else if (num_spills > 0) { counters["ADDITIONAL_SPILLS_BYTES_WRITTEN"] += st.file_out_bytes; counters["OUTPUT_BYTES_WITH_OVERHEAD"] = 0; }
     else counters["OUTPUT_BYTES_WITH_OVERHEAD"] += st.output_bytes_with_overhead;
     counters["SPILLED_RECORDS"] += st.spilled_records;
+    if (combiner) count_combine(st);
     last_spill_rle = st.rle_used;
     partition_stats.resize((size_t)P, 0);
     for (int p = 0; p < P; p++) partition_stats[p] += idx[3 * p + 1];
@@ -311,12 +345,15 @@ struct GpuSorter {
     // TezMerger.merge(..., checkForSameKeys = merger.needsRLE()) into Writer(..., rle = merger.needsRLE()), `merger`
     // being the SpanMerger of the last spill (SORT/PipelinedSorter.java:797-814)
     int32_t rc = tezgpu_merge_set_check_for_same_keys(m, last_spill_rle);
+    const bool combine = combiner && num_spills >= min_spills;
+    if (rc == 0 && combine) rc = tezgpu_merge_set_combiner(m, combiner);
     if (rc == 0)
       rc = tezgpu_merge_write_partitions(m, final_out.c_str(), final_index.c_str(), /*rle=*/last_spill_rle, final_idx.data(), &st);
     tezgpu_merge_close(m);
     gpu_check(rc);
     const uint64_t len = (uint64_t)st.file_out_bytes;
     counters["SPILLED_RECORDS"] += st.spilled_records;
+    if (combine) count_combine(st);
     int64_t raw = 0;
     for (int p = 0; p < P; p++) raw += final_idx[3 * p + 1];
     counters["OUTPUT_BYTES_WITH_OVERHEAD"] += raw;
@@ -379,6 +416,7 @@ struct Output {
     gc.sorter_impl = sc == "LEGACY" ? 1 : 0;
     gc.mem_budget_bytes = (uint64_t)granted;
     sorter = new GpuSorter(gc, granted > 0 ? granted : requested, final_merge, work_dir, uid, counters);
+    if (const int c = combiner_for(conf)) sorter->set_combiner(c, (int)conf.getInt(K_COMBINE_MIN_SPILLS, 3));
     started = true;
   }
   void write(const uint8_t *k, uint32_t kl, const uint8_t *v, uint32_t vl, int32_t partition) {

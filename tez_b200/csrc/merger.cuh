@@ -776,6 +776,13 @@ class Merger {
 
   uint64_t output_bound() const { return SortPipeline::output_bound(n, kv_bytes, pipe.conf.num_partitions) + 16; }
 
+  // the writer behind write_*: TezMerger.writeFile semantics, or -- with a combiner -- the combined records, which carry
+  // no segment tags and unique keys (merge mode and the plain writer then write the same bytes)
+  void emit(int writer_rle, uint8_t *d_out_buf, uint64_t cap, uint64_t *out_len, int64_t *index, tezgpu_stats *st) {
+    if (pipe.combiner) pipe.emit_combined(writer_rle ? 1 : 0, d_out_buf, cap, out_len, index, st);
+    else pipe.emit_phase(writer_rle ? 1 : 0, true, d_out_buf, cap, out_len, index, st);
+  }
+
   // TezMerger.writeFile: one IFile segment, equal adjacent keys written through IFile.REPEAT_KEY
   void write_device(uint8_t *d_out_buf, uint64_t cap, int writer_rle, int64_t *raw_len, int64_t *part_len, tezgpu_stats *stats) {
     TG_CHECK(pipe.conf.num_partitions == 1, TEZGPU_E_STATE,
@@ -783,7 +790,7 @@ class Merger {
     int64_t index[3] = {0, 0, 0};
     uint64_t len = 0;
     tezgpu_stats st;
-    pipe.emit_phase(writer_rle ? 1 : 0, true, d_out_buf, cap, &len, index, &st);
+    emit(writer_rle, d_out_buf, cap, &len, index, &st);
     st.output_bytes = (int64_t)kv_bytes;
     st.kernel_launches += launches - pipe.state.launches;
     if (raw_len) *raw_len = index[1];
@@ -794,7 +801,7 @@ class Merger {
   void write_partitions_device(uint8_t *d_out_buf, uint64_t cap, int writer_rle, uint64_t *out_len, int64_t *index,
                                tezgpu_stats *stats) {
     tezgpu_stats st;
-    pipe.emit_phase(writer_rle ? 1 : 0, true, d_out_buf, cap, out_len, index, &st);
+    emit(writer_rle, d_out_buf, cap, out_len, index, &st);
     st.output_bytes = (int64_t)kv_bytes;
     st.kernel_launches += launches - pipe.state.launches;
     if (stats) *stats = st;
@@ -826,6 +833,7 @@ class Merger {
     TG_CUDA(cudaSetDevice(pipe.conf.device));
     cudaStream_t st = pipe.stream;
     *count = 0;
+    TG_CHECK(!pipe.combiner, TEZGPU_E_STATE, "a merger with a combiner has no record iterator: use tezgpu_merge_write_*");
     if (cursor >= n || idx_cap == 0) return;
     ensure_kvoff();
     uint32_t *d_cnt = pipe.d_large();

@@ -8,6 +8,7 @@
 
 #include "../../include/tezgpu.h"
 #include "device_util.h"
+#include "combine.cuh"
 #include "emit_pipe_u.cuh"
 #include "sorter_kernels.cuh"
 
@@ -177,18 +178,25 @@ class SortPipeline {
     int launches = 0;
     bool have_bounds = false, spec_layout = false;  // partition bounds / fixed-width layout already on the device
     uint64_t spec_file_bytes = 0, spec_tiles = 0;
+    const uint8_t *same = nullptr;  // the combined records' same[] (all zero); nullptr = the sort's own `same`
   } state;
   // merge mode only (the Merger sets them): MergeQueue.checkForSameKeys, and "no input record was run-length encoded"
   // (every segment had the plain fixed framing), which together decide whether any record can be written as a repeat
   int merge_check_same = 1;
   bool merge_inputs_plain = false;
+  int combiner = TEZGPU_COMBINE_NONE;  // TEZGPU_COMBINE_*: combine_phase runs between the sort and the emit
+  // combine workspace (grow-only): head flags / group ids, sums, head positions, and the combined records' sort words,
+  // order, same[], bytes and (variable width) metadata
+  DeviceBuffer c_head, c_gid, c_sums, c_hpos, c_K, c_order, c_same, c_kv, c_koff, c_klen, c_vlen, c_bad;
+  PinnedBuffer c_host;
+  EventTimer c_timer;
 
   EmitParams make_emit_params(const Records &rec, const uint32_t *order, int rle, bool merge_mode, uint8_t *d_out) {
     EmitParams e;
     memset(&e, 0, sizeof(e));
     e.rec = rec;
     e.order = order;
-    e.same = same.as<uint8_t>();
+    e.same = state.same ? state.same : same.as<uint8_t>();
     e.part_start = part_start.as<uint32_t>();
     e.seg_start = seg_start.as<uint64_t>();
     e.tile_start = tile_start.as<uint32_t>();
@@ -223,7 +231,8 @@ class SortPipeline {
     else if (conf.rle_policy == TEZGPU_RLE_OFF) rle = 0;
     else rle = (conf.sorter_impl == 1) ? 0 : ((double)state.dup_count > 0.1 * (double)rec.n);
     if (conf.sorter_impl == TEZGPU_SORTER_UNORDERED) rle = 0;   // Writer(..., codec, null, null): no run-length encoding (:1092)
-    emit_phase(rle, false, d_out, out_cap, out_len, index, stats);
+    if (combiner) emit_combined(rle, d_out, out_cap, out_len, index, stats);
+    else emit_phase(rle, false, d_out, out_cap, out_len, index, stats);
   }
 
   // partition + sort: stage, radix sort of (sort word, index), tie refinement.  Leaves K / order / same / counts.
@@ -241,6 +250,7 @@ class SortPipeline {
     TG_CHECK(rec.hash_partition || rec.partition || rec.use_runs || n == 0 || P == 1, TEZGPU_E_INVALID, "partition ids required (partitioner=GIVEN)");
     int launches = 0;
     state.have_bounds = state.spec_layout = false;
+    state.same = nullptr;
     timer.reset();
     timer.mark(stream);
 
@@ -652,6 +662,166 @@ class SortPipeline {
       stats->ms_total = timer.ms(0, b + 3);
       stats->kernel_launches = launches;
     }
+  }
+
+  // Combine (combine.cuh): replaces state.rec / K / order / same by one record per group of equal keys, in sorted order,
+  // so that the unchanged emit_phase writes them.  Returns false when no two adjacent keys are equal: the records are then
+  // their own combined form (a group of one re-encodes to its input bytes) and only the value widths are checked.
+  // Throws TEZGPU_E_INVALID, naming the record (collection / merge order), on a value of the wrong width.
+  bool combine_phase() {
+    const Records rec = state.rec;
+    const uint32_t n = rec.n, W = combine_width(combiner);
+    TG_CHECK(W, TEZGPU_E_INVALID, "unknown combiner");
+    const char *name = combiner == TEZGPU_COMBINE_SUM_INT ? "IntSumReducer needs 4-byte IntWritable values"
+                                                          : "LongSumReducer needs 8-byte LongWritable values";
+    if (n == 0) return false;
+    c_bad.ensure(16);
+    c_host.ensure(64);
+    uint32_t *bad = c_bad.as<uint32_t>();
+    TG_CUDA(cudaMemsetAsync(bad, 0xFF, 4, stream));
+    int launches = 0;
+    if (state.dup_count == 0) {
+      if (rec.fixed) {
+        TG_CHECK(rec.vlen == W, TEZGPU_E_INVALID, "combiner: record 0 has a " + std::to_string(rec.vlen) + "-byte value (" + name + ")");
+        return false;
+      }
+      k_combine_check_width<<<(uint32_t)std::min<uint64_t>(div_up(n, 256), (uint64_t)num_sms * 16), 256, 0, stream>>>(rec, W, bad);
+      TG_CUDA(cudaGetLastError());
+      state.launches += 1;
+      uint32_t *h = c_host.as<uint32_t>();
+      TG_CUDA(cudaMemcpyAsync(h, bad, 4, cudaMemcpyDeviceToHost, stream));
+      TG_CUDA(cudaStreamSynchronize(stream));
+      TG_CHECK(h[0] == 0xFFFFFFFFu, TEZGPU_E_INVALID, "combiner: record " + std::to_string(h[0]) + " has a value of the wrong width (" + name + ")");
+      return false;
+    }
+    // ---- group ids: exclusive scan of the heads
+    const uint32_t nblk = (uint32_t)div_up(n, SCAN_TILE);
+    c_head.ensure((size_t)n * 4);
+    c_gid.ensure(((size_t)n + 1) * 8);
+    blk.ensure(((size_t)nblk + 2) * 8);
+    k_combine_heads<<<(uint32_t)div_up(n, 256), 256, 0, stream>>>(same.as<uint8_t>(), n, c_head.as<uint32_t>());
+    k_sum_u32_blocks<<<nblk, SCAN_THREADS, 0, stream>>>(c_head.as<uint32_t>(), n, blk.as<uint64_t>());
+    k_scan_block_sums<<<1, 1024, 0, stream>>>(blk.as<uint64_t>(), nblk);
+    k_scan_u32_apply<<<nblk, SCAN_THREADS, 0, stream>>>(c_head.as<uint32_t>(), n, blk.as<uint64_t>(), c_gid.as<uint64_t>());
+    launches += 4;
+    // ---- segmented sums (groups <= n: sized by n, no round trip first)
+    c_sums.ensure((size_t)n * 8);
+    c_hpos.ensure((size_t)n * 4);
+    c_K.ensure((size_t)n * 4);
+    TG_CUDA(cudaMemsetAsync(c_sums.p, 0, (size_t)n * 8, stream));
+    const uint32_t sgrid = (uint32_t)div_up(div_up(n, 32 * CMB_ROWS) * 32, CMB_THREADS);
+    if (W == 4)
+      k_combine_sum<4><<<sgrid, CMB_THREADS, 0, stream>>>(rec, state.order, state.K, c_gid.as<uint64_t>(), n, c_sums.as<unsigned long long>(),
+                                                          c_hpos.as<uint32_t>(), c_K.as<uint32_t>(), bad);
+    else
+      k_combine_sum<8><<<sgrid, CMB_THREADS, 0, stream>>>(rec, state.order, state.K, c_gid.as<uint64_t>(), n, c_sums.as<unsigned long long>(),
+                                                          c_hpos.as<uint32_t>(), c_K.as<uint32_t>(), bad);
+    launches++;
+    TG_CUDA(cudaGetLastError());
+    uint32_t *h = c_host.as<uint32_t>();
+    TG_CUDA(cudaMemcpyAsync(h, bad, 4, cudaMemcpyDeviceToHost, stream));
+    TG_CUDA(cudaMemcpyAsync(h + 2, c_gid.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, stream));
+    TG_CUDA(cudaStreamSynchronize(stream));
+    TG_CHECK(h[0] == 0xFFFFFFFFu, TEZGPU_E_INVALID, "combiner: record " + std::to_string(h[0]) + " has a value of the wrong width (" + name + ")");
+    uint64_t m64;
+    memcpy(&m64, h + 2, 8);
+    const uint32_t m = (uint32_t)m64;
+    // ---- compaction
+    c_order.ensure((size_t)m * 4);
+    c_same.ensure(m);
+    TG_CUDA(cudaMemsetAsync(c_same.p, 0, m, stream));
+    Records out;
+    memset(&out, 0, sizeof(out));
+    out.n = m;
+    out.cmp = rec.cmp;
+    out.hash_partition = rec.hash_partition;
+    out.num_partitions = rec.num_partitions;
+    out.pbits = rec.pbits;
+    const uint64_t *off = nullptr;
+    uint64_t bytes;
+    if (rec.fixed) {
+      bytes = (uint64_t)m * (rec.klen + W);
+      out.fixed = 1;
+      out.klen = rec.klen;
+      out.vlen = W;
+    } else {
+      // key offsets: scan of (key length + width) over the groups; c_head / c_gid are free again
+      const uint32_t mblk = (uint32_t)div_up(m, SCAN_TILE);
+      k_combine_sizes<<<(uint32_t)div_up(m, 256), 256, 0, stream>>>(rec, state.order, c_hpos.as<uint32_t>(), m, W, c_head.as<uint32_t>());
+      k_sum_u32_blocks<<<mblk, SCAN_THREADS, 0, stream>>>(c_head.as<uint32_t>(), m, blk.as<uint64_t>());
+      k_scan_block_sums<<<1, 1024, 0, stream>>>(blk.as<uint64_t>(), mblk);
+      k_scan_u32_apply<<<mblk, SCAN_THREADS, 0, stream>>>(c_head.as<uint32_t>(), m, blk.as<uint64_t>(), c_gid.as<uint64_t>());
+      launches += 4;
+      TG_CUDA(cudaGetLastError());
+      TG_CUDA(cudaMemcpyAsync(h + 4, c_gid.as<uint64_t>() + m, 8, cudaMemcpyDeviceToHost, stream));
+      TG_CUDA(cudaStreamSynchronize(stream));
+      memcpy(&bytes, h + 4, 8);
+      off = c_gid.as<uint64_t>();
+      c_koff.ensure((size_t)m * 8);
+      c_klen.ensure((size_t)m * 4);
+      c_vlen.ensure((size_t)m * 4);
+      out.key_off = c_koff.as<uint64_t>();
+      out.key_len = c_klen.as<uint32_t>();
+      out.val_len = c_vlen.as<uint32_t>();
+    }
+    c_kv.ensure(align_up(bytes, 16) + 32);
+    out.kv = c_kv.as<uint8_t>();
+    out.kv_bytes = rec.fixed ? bytes : align_up(bytes, 16);
+    // one thread per record for short fixed keys, a warp per record otherwise (multi-KB BytesWritable keys)
+    const bool narrow = rec.fixed && rec.klen <= 64;
+    const uint32_t lanes = narrow ? 1 : 32;
+    const uint32_t wgrid = (uint32_t)div_up((uint64_t)m * lanes, 256);
+    auto write = [&](auto kern) {
+      kern<<<wgrid, 256, 0, stream>>>(rec, state.order, c_hpos.as<uint32_t>(), c_sums.as<unsigned long long>(), m, off, c_kv.as<uint8_t>(),
+                                      c_order.as<uint32_t>(), c_koff.as<uint64_t>(), c_klen.as<uint32_t>(), c_vlen.as<uint32_t>());
+    };
+    if (W == 4) narrow ? write(k_combine_write<4, 1>) : write(k_combine_write<4, 32>);
+    else narrow ? write(k_combine_write<8, 1>) : write(k_combine_write<8, 32>);
+    launches++;
+    TG_CUDA(cudaGetLastError());
+    state.rec = out;
+    state.K = c_K.as<uint32_t>();
+    state.order = c_order.as<uint32_t>();
+    state.same = c_same.as<uint8_t>();
+    state.dup_count = 0;
+    state.have_bounds = state.spec_layout = false;   // emit_phase lays the combined records out again
+    state.launches += launches;
+    return true;
+  }
+
+  // combine + emit.  The stats keep the meaning they have without a combiner (rle_used / adjacent_equal_keys describe
+  // the uncombined stream, ms_emit the emit alone) except output_records = records that entered the combine and
+  // spilled_records = records written.  The sort's state is restored afterwards, so a merger can write again.
+  void emit_combined(int rle, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index, tezgpu_stats *stats) {
+    const SortState saved = state;
+    c_timer.reset();
+    c_timer.mark(stream);
+    bool replaced = false;
+    try {
+      replaced = combine_phase();
+      c_timer.mark(stream);
+      emit_phase(rle, false, d_out, out_cap, out_len, index, stats);
+    } catch (...) {
+      restore_after_combine(saved, replaced);
+      throw;
+    }
+    const uint64_t written = state.rec.n;
+    restore_after_combine(saved, replaced);
+    if (stats) {
+      const float ms_combine = c_timer.ms(0, 1);
+      stats->output_records = (int64_t)saved.rec.n;
+      stats->spilled_records = (int64_t)written;
+      stats->adjacent_equal_keys = (int64_t)saved.dup_count;
+      stats->ms_emit = std::max(0.f, stats->ms_emit - ms_combine);
+    }
+  }
+  void restore_after_combine(const SortState &saved, bool replaced) {
+    if (!replaced) return;   // the emit ran over the sort's own records
+    const int launches = state.launches;
+    state = saved;
+    state.launches = launches;
+    // the combined emit overwrote the partition bounds and the layout of the sorted records
+    state.have_bounds = state.spec_layout = false;
   }
 };
 

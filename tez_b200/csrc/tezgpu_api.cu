@@ -331,6 +331,19 @@ int32_t tezgpu_sorter_sort_device_fixed(tezgpu_sorter *h, const void *d_kv, cons
 
 void *tezgpu_sorter_stream(tezgpu_sorter *h) { return h ? (void *)h->pipe.stream : nullptr; }
 
+int32_t tezgpu_sorter_set_combiner(tezgpu_sorter *h, int32_t combiner) {
+  TG_API_BEGIN
+  TG_CHECK(h, TEZGPU_E_INVALID, "null handle");
+  TG_CHECK(combiner == TEZGPU_COMBINE_NONE || combine_width(combiner), TEZGPU_E_INVALID, "unknown combiner");
+  TG_CHECK(!combiner || h->pipe.conf.sorter_impl != TEZGPU_SORTER_UNORDERED, TEZGPU_E_INVALID,
+           "the unordered writer (UnorderedPartitionedKVWriter) runs no combiner");
+  TG_CHECK(!combiner || !h->fixed || h->vlen == combine_width(combiner), TEZGPU_E_INVALID,
+           "fixed_val_len " + std::to_string(h->vlen) + " is not the combiner's value width");
+  TG_CHECK(h->n == 0 && !h->flushed, TEZGPU_E_STATE, "set the combiner before the first collect (or after a reset)");
+  h->pipe.combiner = combiner;
+  TG_API_END
+}
+
 // ------------------------------------------------------------------------------------------------ NVLink peer fetch
 int32_t tezgpu_peer_alloc(int32_t device, uint64_t bytes, void **dptr, uint8_t *handle_out) {
   TG_API_BEGIN

@@ -33,12 +33,24 @@ def make_conf(num_partitions, comparator=CMP_BYTES, partitioner=PART_HASH, rle_p
 
 
 class GpuSorter:
-    def __init__(self, num_partitions, **kw):
+    def __init__(self, num_partitions, combiner=COMBINE_NONE, **kw):
+        """combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG runs MRCombiner with IntSumReducer / LongSumReducer on every
+        flush (tezgpu_sorter_set_combiner)."""
         self.L = _lib.load()
         self.conf = make_conf(num_partitions, **kw)
         self.P = num_partitions
         self.h = C.c_void_p()
         check(self.L.tezgpu_sorter_create(C.byref(self.conf), C.byref(self.h)))
+        if combiner:
+            try:
+                self.set_combiner(combiner)
+            except Exception:
+                self.close()
+                raise
+
+    def set_combiner(self, combiner):
+        """Before the first collect (or after reset); survives reset."""
+        check(self.L.tezgpu_sorter_set_combiner(self.h, combiner))
 
     def close(self):
         if self.h:
@@ -116,10 +128,11 @@ class GpuSorter:
 
 class GpuMerger:
     def __init__(self, segments, comparator=CMP_BYTES, device=0, has_header=True, device_ptrs=False, fixed=None,
-                 partitions=None, num_partitions=1, send_empty=True, verified=None):
+                 partitions=None, num_partitions=1, send_empty=True, verified=None, combiner=COMBINE_NONE):
         """segments: list of bytes / uint8 arrays (host) or (ptr, len) tuples when device_ptrs.
         verified: optional per-segment booleans -- the transport already checked that segment's checksum
-        (TEZGPU_SEG_VERIFIED: fetch_segments_verified), the merge does not read it again to verify."""
+        (TEZGPU_SEG_VERIFIED: fetch_segments_verified), the merge does not read it again to verify.
+        combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG combines the merged stream in write_* (tezgpu_merge_set_combiner)."""
         self.L = _lib.load()
         self.conf = make_conf(num_partitions, comparator=comparator, partitioner=PART_GIVEN, device=device, fixed=fixed,
                               send_empty=send_empty)
@@ -128,6 +141,16 @@ class GpuMerger:
         arr = self._segments(segments, partitions, verified)
         self.h = C.c_void_p()
         check(self.L.tezgpu_merge_open(C.byref(self.conf), arr, len(segments), C.byref(self.h)))
+        if combiner:
+            try:
+                self.set_combiner(combiner)
+            except Exception:
+                self.close()
+                raise
+
+    def set_combiner(self, combiner):
+        """Combines in write_*; the record iterator is then unavailable (TEZGPU_E_STATE)."""
+        check(self.L.tezgpu_merge_set_combiner(self.h, combiner))
 
     def _segments(self, segments, partitions, verified=None):
         self._keep = []
