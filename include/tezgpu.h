@@ -110,6 +110,13 @@ typedef struct tezgpu_merger tezgpu_merger;
 #define TEZGPU_COMBINE_SUM_INT 1    /* IntSumReducer over IntWritable values */
 #define TEZGPU_COMBINE_SUM_LONG 2   /* LongSumReducer over LongWritable values */
 
+/* Codec of the IFile segments (tez.runtime.compress / tez.runtime.compress.codec, SORT/IFile.java:351-420): with
+ * DEFAULT (org.apache.hadoop.io.compress.DefaultCodec, RL/common/ConfigUtils.java:44-66) a segment is 'T','I','F',1, one
+ * zlib stream (RFC 1950) of the uncompressed body, and the CRC-32 of the compressed bytes; its index triple keeps the
+ * uncompressed rawLength and has the compressed segment length as partLength.  Other codecs are not on the device. */
+#define TEZGPU_CODEC_NONE 0
+#define TEZGPU_CODEC_DEFAULT 1
+
 const char *tezgpu_last_error(void);
 int32_t tezgpu_abi_version(void);
 /* number of visible CUDA devices (0 when none; never falls back to CPU) */
@@ -166,6 +173,14 @@ void *tezgpu_sorter_stream(tezgpu_sorter *h);
  * combiner) and on a fixed-width handle whose fixed_val_len is not the combiner's value width. */
 int32_t tezgpu_sorter_set_combiner(tezgpu_sorter *h, int32_t combiner);
 
+/* writes every segment through the codec (TEZGPU_CODEC_*) in flush, flush_to_memory and sort_device_fixed, after the
+ * combiner when one is set; unordered handles too (UnorderedPartitionedKVWriter writes through the codec).  Call before
+ * the first collect (or right after a reset); survives reset.  With a codec, tezgpu_sorter_output_bound includes the
+ * worst case (every 32 KiB chunk stored), stats.output_bytes_physical / file_out_bytes count compressed bytes,
+ * output_bytes_with_overhead is still the sum of rawLength, and ms_total includes the compression (ms_emit does not).
+ * TEZGPU_E_UNSUPPORTED for any other codec. */
+int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Merger: replaces TezMerger.merge(...) -> TezRawKeyValueIterator (SORT/TezMerger.java:717-912,
  * SORT/TezRawKeyValueIterator.java:33-87) as called from OG/MergeManager.java:804-811,899-903,1035-1041,1197-1199
@@ -195,6 +210,16 @@ int32_t tezgpu_merge_open(const tezgpu_conf *conf, const tezgpu_segment *segs, u
 /* runs a new merge through an existing handle, keeping its device allocations (the per-step reduce side of the
  * multi-GPU shuffle; a container-reused task) */
 int32_t tezgpu_merge_reopen(tezgpu_merger *m, const tezgpu_segment *segs, uint32_t nseg);
+/* tezgpu_merge_open / reopen with a codec (TEZGPU_CODEC_*).  raw_len[i] is segment i's rawLength (spill index or
+ * ShuffleHeader uncompressedLength): required for segments whose header flag is 1 (TEZGPU_E_INVALID without it), ignored
+ * for the others; raw_len may be NULL when none is compressed.  Compressed and uncompressed segments may be mixed.  A
+ * compressed segment's CRC is checked on the compressed bytes (unless TEZGPU_SEG_VERIFIED), its body must inflate to
+ * exactly raw_len[i] - 4 bytes (one or more complete zlib streams), else TEZGPU_E_FORMAT naming the segment.  Every
+ * tezgpu_merge_write_* of the handle writes through the same codec (PipelinedSorter's final merge, :774-836).
+ * TEZGPU_CODEC_NONE behaves exactly like open / reopen. */
+int32_t tezgpu_merge_open_codec(const tezgpu_conf *conf, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg,
+                                int32_t codec, tezgpu_merger **out);
+int32_t tezgpu_merge_reopen_codec(tezgpu_merger *m, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg);
 /* MergeQueue's checkForSameKeys constructor argument (SORT/TezMerger.java:560-573; default true like the reference's
  * other constructors, :519).  When 0, isSameKey() -- and therefore REPEAT_KEY in tezgpu_merge_write_* -- is reported
  * only for records that were run-length encoded in their input segment, never across segment boundaries
@@ -311,6 +336,13 @@ uint32_t tezgpu_debug_chunk_fold_emulate(const uint8_t *data, uint32_t nchunks, 
 
 /* diagnostics: host-side run of the per-thread-run CRC fold of the packed fixed-width emit kernel (nchunks <= 1280) */
 uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks);
+
+/* diagnostics: the device codec run on the host with the same code.  deflate: the zlib stream the device writes for one
+ * segment body (a compressed segment is TIF\x01 + this + CRC-32).  inflate: decodes a compressed segment body (the bytes
+ * between header and CRC) that must yield exactly body_len bytes; TEZGPU_E_FORMAT names the reason otherwise. */
+int32_t tezgpu_debug_deflate_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len);
+int32_t tezgpu_debug_inflate_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
+                                     uint64_t *out_len);
 
 #ifdef __cplusplus
 }

@@ -40,7 +40,19 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
    */
   public GpuMergeIterator(long[] addresses, long[] lengths, int[] flags, int comparator, boolean checkForSameKeys)
       throws IOException {
-    handle = nativeOpen(addresses, lengths, flags, null, 1, comparator, Integer.parseInt(System.getenv().getOrDefault("TEZGPU_DEVICE", "0")));
+    this(addresses, lengths, flags, null, GpuSorter.CODEC_NONE, comparator, checkForSameKeys);
+  }
+
+  /**
+   * @param rawLengths rawLength of every segment (TezIndexRecord, or the ShuffleHeader's uncompressedLength); required
+   *                   for the compressed ones ('T','I','F',1), may be null when none is compressed
+   * @param codec      GpuSorter.codecId(CodecUtils.getCodec(conf)): CODEC_DEFAULT inflates compressed segments on the
+   *                   device, and writeFile then writes a compressed segment
+   */
+  public GpuMergeIterator(long[] addresses, long[] lengths, int[] flags, long[] rawLengths, int codec, int comparator,
+      boolean checkForSameKeys) throws IOException {
+    handle = nativeOpen(addresses, lengths, flags, null, 1, rawLengths, codec, comparator,
+        Integer.parseInt(System.getenv().getOrDefault("TEZGPU_DEVICE", "0"))); // tezgpu_merge_open_codec
     if (!checkForSameKeys) nativeSetCheckForSameKeys(handle, false);
   }
 
@@ -86,20 +98,22 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
 
   /** PipelinedSorter.flush's final merge: all spills, all partitions, one device pass (PipelinedSorter.java:774-836). */
   static void mergeSpillsToFile(String[] spillFiles, String[] spillIndexFiles, int partitions, int comparator,
-      boolean sendEmptyPartitionDetails, boolean checkForSameKeys, boolean writerRle, String out, String index)
+      boolean sendEmptyPartitionDetails, boolean checkForSameKeys, boolean writerRle, int codec, String out, String index)
       throws IOException {
+    // tezgpu_merge_open_codec(P, the spills' rawLengths, codec) + set_check_for_same_keys + tezgpu_merge_write_partitions:
+    // with CODEC_DEFAULT the compressed spills are read and file.out is written compressed
     nativeMergeSpills(spillFiles, spillIndexFiles, partitions, comparator, sendEmptyPartitionDetails, checkForSameKeys,
-        writerRle, out, index); // tezgpu_merge_open(P) + set_check_for_same_keys + tezgpu_merge_write_partitions
+        writerRle, codec, out, index);
   }
 
   private static native long nativeOpen(long[] addresses, long[] lengths, int[] flags, int[] partitions, int numPartitions,
-      int comparator, int device) throws IOException;
+      long[] rawLengths, int codec, int comparator, int device) throws IOException;
   private static native void nativeSetCheckForSameKeys(long h, boolean on) throws IOException;
   private static native void nativeSetCombiner(long h, int combiner) throws IOException;
   private static native int nativeNextBatch(long h, ByteBuffer out, int cap, IntBuffer idx, int idxCap) throws IOException;
   private static native boolean nativeHasMore(long h);
   private static native void nativeWriteIFile(long h, String path, boolean rle, long[] rawAndPart) throws IOException;
   private static native void nativeMergeSpills(String[] files, String[] indexFiles, int partitions, int comparator,
-      boolean sendEmpty, boolean checkForSameKeys, boolean writerRle, String out, String index) throws IOException;
+      boolean sendEmpty, boolean checkForSameKeys, boolean writerRle, int codec, String out, String index) throws IOException;
   private static native void nativeClose(long h);
 }

@@ -21,6 +21,8 @@ import org.apache.hadoop.io.IntWritable;
 import org.apache.hadoop.io.LongWritable;
 import org.apache.hadoop.io.RawComparator;
 import org.apache.hadoop.io.Text;
+import org.apache.hadoop.io.compress.CompressionCodec;
+import org.apache.hadoop.io.compress.DefaultCodec;
 import org.apache.tez.runtime.api.OutputContext;
 import org.apache.tez.runtime.library.common.comparator.TezBytesComparator;
 import org.apache.tez.runtime.library.partitioner.HashPartitioner;
@@ -35,6 +37,7 @@ public class GpuSorter extends ExternalSorter {
   static final int CMP_BYTES = 0, CMP_TEXT = 1, CMP_BYTESWRITABLE = 2, CMP_INT = 3, CMP_LONG = 4;
   static final int PART_GIVEN = 0, PART_HASH = 1;
   static final int COMBINE_NONE = 0, COMBINE_SUM_INT = 1, COMBINE_SUM_LONG = 2;
+  static final int CODEC_NONE = 0, CODEC_DEFAULT = 1;
   private static final int BATCH_BYTES = 32 << 20;
   private static final int BATCH_RECORDS = 1 << 20;
 
@@ -61,6 +64,20 @@ public class GpuSorter extends ExternalSorter {
         Integer.parseInt(System.getenv().getOrDefault("TEZGPU_DEVICE", "0")));
     keySerializer.open(sink);
     valSerializer.open(sink);
+    // ExternalSorter.codec = CodecUtils.getCodec(conf): every spill and the final merge write through it
+    final int c = codecId(codec);
+    if (c != CODEC_NONE) nativeSetCodec(handle, c);
+  }
+
+  /**
+   * The device writes and reads DefaultCodec (zlib) segments only.  The class must be DefaultCodec itself: GzipCodec
+   * extends DefaultCodec but writes gzip members, so an instanceof test would be wrong.
+   */
+  static int codecId(CompressionCodec codec) throws IOException {
+    if (codec == null) return CODEC_NONE;
+    if (codec.getClass() == DefaultCodec.class) return CODEC_DEFAULT;
+    throw new IOException("tez.runtime.compress.codec=" + codec.getClass().getName()
+        + ": only org.apache.hadoop.io.compress.DefaultCodec is supported on the device path");
   }
 
   /**
@@ -147,7 +164,7 @@ public class GpuSorter extends ExternalSorter {
     finalOutputFile = mapOutputFile.getOutputFileForWrite(0);
     finalIndexFile = mapOutputFile.getOutputIndexFileForWrite(0);
     GpuMergeIterator.mergeSpillsToFile(spillFilePaths(), spillIndexPaths(), partitions,
-        comparatorId(comparator, conf), sendEmptyPartitionDetails, lastSpillRle, lastSpillRle,
+        comparatorId(comparator, conf), sendEmptyPartitionDetails, lastSpillRle, lastSpillRle, codecId(codec),
         finalOutputFile.toString(), finalIndexFile.toString());
     numShuffleChunks.setValue(1);
   }
@@ -174,6 +191,7 @@ public class GpuSorter extends ExternalSorter {
   private static native void nativeFlush(long h, String out, String index, long[] idx, long[] counters) throws IOException;
   private static native void nativeReset(long h) throws IOException;
   private static native void nativeSetCombiner(long h, int combiner) throws IOException;
+  private static native void nativeSetCodec(long h, int codec) throws IOException;
   private static native void nativeDestroy(long h);
 
   /** DataOutputStream target that appends to the direct batch buffer. */

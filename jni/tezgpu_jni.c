@@ -88,6 +88,12 @@ JNIEXPORT void JNICALL SORTER(nativeSetCombiner)(JNIEnv *env, jclass cls, jlong 
   failed(env, tezgpu_sorter_set_combiner((tezgpu_sorter *)(intptr_t)h, combiner));
 }
 
+/* ExternalSorter.codec when it is DefaultCodec itself (TEZGPU_CODEC_*; GpuSorter.codecId) */
+JNIEXPORT void JNICALL SORTER(nativeSetCodec)(JNIEnv *env, jclass cls, jlong h, jint codec) {
+  (void)cls;
+  failed(env, tezgpu_sorter_set_codec((tezgpu_sorter *)(intptr_t)h, codec));
+}
+
 JNIEXPORT void JNICALL SORTER(nativeDestroy)(JNIEnv *env, jclass cls, jlong h) {
   (void)env; (void)cls;
   tezgpu_sorter_destroy((tezgpu_sorter *)(intptr_t)h);
@@ -95,12 +101,14 @@ JNIEXPORT void JNICALL SORTER(nativeDestroy)(JNIEnv *env, jclass cls, jlong h) {
 
 /* ------------------------------------------------------------------------------------------------ GpuMergeIterator */
 JNIEXPORT jlong JNICALL MERGER(nativeOpen)(JNIEnv *env, jclass cls, jlongArray addresses, jlongArray lengths, jintArray flags,
-                                           jintArray partitions, jint num_partitions, jint comparator, jint device) {
+                                           jintArray partitions, jint num_partitions, jlongArray raw_lengths, jint codec,
+                                           jint comparator, jint device) {
   (void)cls;
   jsize n = (*env)->GetArrayLength(env, addresses);
   jlong *a = (*env)->GetLongArrayElements(env, addresses, NULL), *l = (*env)->GetLongArrayElements(env, lengths, NULL);
   jint *f = (*env)->GetIntArrayElements(env, flags, NULL);
   jint *p = partitions ? (*env)->GetIntArrayElements(env, partitions, NULL) : NULL;
+  jlong *r = raw_lengths ? (*env)->GetLongArrayElements(env, raw_lengths, NULL) : NULL;
   tezgpu_segment *segs = (tezgpu_segment *)calloc((size_t)n + 1, sizeof(tezgpu_segment));
   for (jsize i = 0; i < n; i++) {
     segs[i].data = (const void *)(intptr_t)a[i];
@@ -117,8 +125,10 @@ JNIEXPORT jlong JNICALL MERGER(nativeOpen)(JNIEnv *env, jclass cls, jlongArray a
   c.partitioner = TEZGPU_PART_GIVEN;
   c.send_empty_partition_details = 1;
   tezgpu_merger *m = NULL;
-  int32_t rc = tezgpu_merge_open(&c, segs, (uint32_t)n, &m);
+  /* rawLength of every segment: required for the compressed ones (jlong and int64_t are both 64-bit) */
+  int32_t rc = tezgpu_merge_open_codec(&c, segs, (const int64_t *)r, (uint32_t)n, codec, &m);
   free(segs);
+  if (r) (*env)->ReleaseLongArrayElements(env, raw_lengths, r, JNI_ABORT);
   (*env)->ReleaseLongArrayElements(env, addresses, a, JNI_ABORT);
   (*env)->ReleaseLongArrayElements(env, lengths, l, JNI_ABORT);
   (*env)->ReleaseIntArrayElements(env, flags, f, JNI_ABORT);
@@ -172,6 +182,6 @@ JNIEXPORT void JNICALL MERGER(nativeClose)(JNIEnv *env, jclass cls, jlong h) {
 
 /* nativeMergeSpills (PipelinedSorter.flush's final merge) reads the spill files and their TezSpillRecord indexes and
  * builds the partition-tagged segment table exactly as tez_b200/csrc/host/tez_runtime_library.cc::GpuSorter::flush does
- * (:281-330): tezgpu_merge_open(conf with num_partitions = P) -> tezgpu_merge_set_check_for_same_keys(needsRLE) ->
+ * (:281-330): tezgpu_merge_open_codec(conf with num_partitions = P, spill rawLengths, codec) -> tezgpu_merge_set_check_for_same_keys(needsRLE) ->
  * tezgpu_merge_write_partitions(out, index, rle = needsRLE).  It is that C++ code behind a JNI signature; kept there so
  * the logic exists once and is exercised by tests/test_runtime_library_gpu.py. */

@@ -63,6 +63,7 @@ SYMBOLS = [
     ("tezgpu_sorter_sort_device_fixed", C.c_int32, [_V, _V, _V, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64), _V, _P(Stats)]),
     ("tezgpu_sorter_stream", _V, [_V]),
     ("tezgpu_sorter_set_combiner", C.c_int32, [_V, C.c_int32]),
+    ("tezgpu_sorter_set_codec", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_shuffle_header_size", C.c_uint64, [C.c_char_p, C.c_int64, C.c_int64, C.c_int32]),
     ("tezgpu_shuffle_header_write", C.c_int32, [C.c_char_p, C.c_int64, C.c_int64, C.c_int32, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_shuffle_header_read", C.c_int32, [_V, C.c_uint64, _V, C.c_uint64, _P(C.c_int64), _P(C.c_int64), _P(C.c_int32), _P(C.c_uint64)]),
@@ -72,8 +73,12 @@ SYMBOLS = [
     ("tezgpu_debug_crc_emulate", C.c_uint32, [_V, C.c_uint64, C.c_uint32, C.c_uint32]),
     ("tezgpu_debug_chunk_fold_emulate", C.c_uint32, [_V, C.c_uint32, C.c_int32]),
     ("tezgpu_debug_run_fold_emulate", C.c_uint32, [_V, C.c_uint32]),
+    ("tezgpu_debug_deflate_emulate", C.c_int32, [_V, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
+    ("tezgpu_debug_inflate_emulate", C.c_int32, [_V, C.c_uint64, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_merge_open", C.c_int32, [_P(Conf), _P(Segment), C.c_uint32, _P(_V)]),
     ("tezgpu_merge_reopen", C.c_int32, [_V, _P(Segment), C.c_uint32]),
+    ("tezgpu_merge_open_codec", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, _P(_V)]),
+    ("tezgpu_merge_reopen_codec", C.c_int32, [_V, _P(Segment), _V, C.c_uint32]),
     ("tezgpu_merge_set_check_for_same_keys", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_merge_set_combiner", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_merge_parse_info", C.c_int32, [_V, _V, _V]),

@@ -1,0 +1,232 @@
+// codec.cuh -- DefaultCodec on both sides of the shuffle: the compress phase behind every emit (SortPipeline) and the
+// inflate step in front of every merge open (Merger).  Formats and kernels: deflate.cuh, inflate.cuh.
+#pragma once
+#include "inflate.cuh"
+#include "merger.cuh"
+
+namespace tezgpu {
+
+// The uncompressed file is in z_img with its index raw_index (start, rawLength, partLength per partition).  Every
+// partition that has a segment gets a compressed one: TIF\x01, the zlib stream of the same body, CRC-32 of the stream.
+// index receives (start, the same rawLength, compressed length).  One host round trip (the compressed layout).
+inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len,
+                                         int64_t *index, tezgpu_stats *stats) {
+  const int P = conf.num_partitions;
+  cudaStream_t st = stream;
+  z_timer.reset();
+  z_timer.mark(st);
+  z_host.ensure((size_t)P * sizeof(ZSeg) + 64);
+  ZSeg *hs = z_host.as<ZSeg>();
+  uint32_t nchunks = 0;
+  uint64_t nsegs = 0;
+  for (int p = 0; p < P; p++) {
+    const int64_t start = raw_index[3 * p], part = raw_index[3 * p + 2];
+    ZSeg &s = hs[p];
+    memset(&s, 0, sizeof(s));
+    s.chunk0 = nchunks;
+    s.rank = nsegs;
+    if (part > 0) {
+      s.body_off = (uint64_t)start + 4;
+      s.body_len = (uint64_t)part - 8;
+      s.nchunks = (uint32_t)std::max<uint64_t>(1, div_up(s.body_len, ZCHUNK));
+      nchunks += s.nchunks;
+      nsegs++;
+    }
+  }
+  int launches = 0;
+  uint64_t total = 0;
+  if (nchunks) {
+    z_segs.ensure((size_t)P * sizeof(ZSeg));
+    TG_CUDA(cudaMemcpyAsync(z_segs.p, hs, (size_t)P * sizeof(ZSeg), cudaMemcpyHostToDevice, st));
+    z_slots.ensure((size_t)nchunks * ZSLOT);
+    z_csize.ensure((size_t)nchunks * 4);
+    z_cadler.ensure((size_t)nchunks * 4);
+    z_coff.ensure(((size_t)nchunks + 2) * 8);
+    static bool attr[64] = {};   // the attribute is per device
+    if (!attr[conf.device & 63]) {
+      TG_CUDA(cudaFuncSetAttribute(k_zdeflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZShared)));
+      attr[conf.device & 63] = true;
+    }
+    k_zdeflate<<<nchunks, ZLANES, sizeof(ZShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
+                                                        z_csize.as<uint32_t>(), z_cadler.as<uint32_t>());
+    const uint32_t nblk = (uint32_t)div_up(nchunks, SCAN_TILE);
+    blk.ensure(((size_t)nblk + 2) * 8);
+    k_sum_u32_blocks<<<nblk, SCAN_THREADS, 0, st>>>(z_csize.as<uint32_t>(), nchunks, blk.as<uint64_t>());
+    k_scan_block_sums<<<1, 1024, 0, st>>>(blk.as<uint64_t>(), nblk);
+    k_scan_u32_apply<<<nblk, SCAN_THREADS, 0, st>>>(z_csize.as<uint32_t>(), nchunks, blk.as<uint64_t>(), z_coff.as<uint64_t>());
+    k_zseg_layout<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_coff.as<uint64_t>());
+    launches += 5;
+    TG_CUDA(cudaGetLastError());
+    TG_CUDA(cudaMemcpyAsync(hs, z_segs.p, (size_t)P * sizeof(ZSeg), cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(hs) + (size_t)P * sizeof(ZSeg), z_coff.as<uint64_t>() + nchunks, 8,
+                            cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaStreamSynchronize(st));
+    uint64_t cbytes;
+    memcpy(&cbytes, reinterpret_cast<uint8_t *>(hs) + (size_t)P * sizeof(ZSeg), 8);
+    total = cbytes + 14 * nsegs;
+    TG_CHECK(total <= out_cap, TEZGPU_E_NOMEM, "output buffer too small for the compressed file.out");
+    // checksums of the chunks (k_crc_pieces, one piece per chunk), placed in their segments and folded per segment
+    const CrcTables *d_crc = DeviceConstants::get(conf.device).d_crc;
+    z_descs.ensure((size_t)nchunks * sizeof(SegDesc));
+    z_pstart.ensure(((size_t)nchunks + 1) * 4);
+    z_tc.ensure((size_t)nchunks * sizeof(TileCrc));
+    z_crc.ensure((size_t)P * 4);
+    TG_CUDA(cudaMemsetAsync(z_crc.p, 0, (size_t)P * 4, st));
+    k_zchunk_descs<SegDesc><<<(uint32_t)div_up((uint64_t)nchunks + 1, 256), 256, 0, st>>>(z_csize.as<uint32_t>(), nchunks, z_descs.as<SegDesc>(),
+                                                                                       z_pstart.as<uint32_t>());
+    k_crc_pieces<<<nchunks, CRCV_THREADS, 0, st>>>(z_slots.as<uint8_t>(), z_descs.as<SegDesc>(), z_pstart.as<uint32_t>(), nchunks, d_crc,
+                                                   z_tc.as<TileCrc>());
+    k_zcrc_place<TileCrc><<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, z_segs.as<ZSeg>(), (uint32_t)P,
+                                                                         z_coff.as<uint64_t>());
+    k_crc_combine<<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, d_crc, z_crc.as<uint32_t>());
+    k_zpack<<<nchunks, 256, 0, st>>>(z_slots.as<uint8_t>(), z_csize.as<uint32_t>(), z_coff.as<uint64_t>(), z_segs.as<ZSeg>(), (uint32_t)P, d_out);
+    k_zfinish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_cadler.as<uint32_t>(), z_csize.as<uint32_t>(),
+                                                       z_crc.as<uint32_t>(), d_crc, d_out);
+    launches += 6;
+    TG_CUDA(cudaGetLastError());
+  }
+  z_timer.mark(st);
+  TG_CUDA(cudaStreamSynchronize(st));
+  if (out_len) *out_len = total;
+  if (index) {
+    for (int p = 0; p < P; p++) {
+      const int64_t start = raw_index[3 * p], raw = raw_index[3 * p + 1], part = raw_index[3 * p + 2];
+      const uint64_t zstart = nchunks ? hs[p].zstart : 0;
+      index[3 * p] = part > 0 ? (int64_t)zstart : (start == 0 ? 0 : (int64_t)zstart);
+      index[3 * p + 1] = raw;
+      index[3 * p + 2] = part > 0 ? (int64_t)hs[p].zlen : 0;
+    }
+  }
+  if (stats) {
+    stats->output_bytes_physical = (int64_t)total;
+    stats->file_out_bytes = (int64_t)total;
+    stats->ms_total += z_timer.ms(0, 1);
+    stats->kernel_launches += launches;
+  }
+}
+
+// Compressed segments (TIF\x01 with a codec set) are staged, their CRC checked (unless the transport verified it),
+// inflated into images TIF\x00 + body + 4 bytes that the merge reads as verified ordinary segments.  Every other segment
+// goes to open() unchanged, so errors keep naming the caller's segment index.
+inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg) {
+  if (!pipe.codec) { open(in, nseg); return; }
+  cudaStream_t st = pipe.stream;
+  TG_CUDA(cudaSetDevice(pipe.conf.device));
+  // which segments are compressed: the header flag byte
+  std::vector<uint8_t> hdr((size_t)nseg * 4, 0);
+  for (uint32_t s = 0; s < nseg; s++) {
+    if (!(in[s].flags & TEZGPU_SEG_HAS_HEADER) || in[s].len < 10 || !in[s].data) continue;
+    if (in[s].flags & TEZGPU_SEG_DEVICE) TG_CUDA(cudaMemcpyAsync(&hdr[4 * (size_t)s], in[s].data, 4, cudaMemcpyDeviceToHost, st));
+    else memcpy(&hdr[4 * (size_t)s], in[s].data, 4);
+  }
+  TG_CUDA(cudaStreamSynchronize(st));
+  std::vector<uint32_t> zs;
+  for (uint32_t s = 0; s < nseg; s++)
+    if (hdr[4 * s] == 'T' && hdr[4 * s + 1] == 'I' && hdr[4 * s + 2] == 'F' && hdr[4 * s + 3] == 1) zs.push_back(s);
+  if (zs.empty()) { open(in, nseg); return; }
+  TG_CHECK(raw_len, TEZGPU_E_INVALID, "segment " + std::to_string(zs[0]) + " is compressed: its raw length is required");
+  const uint32_t nz = (uint32_t)zs.size();
+  uint64_t in_bytes = 0, img_bytes = 0;
+  std::vector<uint64_t> in_off(nz), img_off(nz);
+  // device segments the transport verified are inflated in place; the others are staged for the checksum kernels
+  auto in_place = [&](const tezgpu_segment &sg) {
+    return (sg.flags & TEZGPU_SEG_DEVICE) && (sg.flags & TEZGPU_SEG_VERIFIED);
+  };
+  for (uint32_t i = 0; i < nz; i++) {
+    const uint32_t s = zs[i];
+    TG_CHECK(raw_len[s] >= 6 && raw_len[s] < (1ll << 40), TEZGPU_E_INVALID,
+             "segment " + std::to_string(s) + ": raw length " + std::to_string(raw_len[s]) + " is not a valid IFile rawLength");
+    in_off[i] = in_bytes;
+    if (!in_place(in[s])) in_bytes = align_up(in_bytes + in[s].len, 16);
+    img_off[i] = img_bytes;
+    img_bytes = align_up(img_bytes + (uint64_t)raw_len[s] + 4, 16);
+  }
+  z_in.ensure(in_bytes + 64);
+  z_img.ensure(img_bytes + 64);
+  std::vector<SegDesc> sd(nz);
+  std::vector<ZInSeg> zi(nz);
+  for (uint32_t i = 0; i < nz; i++) {
+    const tezgpu_segment &sg = in[zs[i]];
+    const bool inplace = in_place(sg);
+    if (!inplace)
+      TG_CUDA(cudaMemcpyAsync(z_in.as<uint8_t>() + in_off[i], sg.data, sg.len,
+                              (sg.flags & TEZGPU_SEG_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+    sd[i].off = in_off[i];
+    sd[i].len = sg.len;
+    sd[i].body0 = 4;
+    sd[i].body_end = sg.len - 4;
+    sd[i].has_header = 1u | ((sg.flags & TEZGPU_SEG_VERIFIED) ? 2u : 0u);
+    sd[i].partition = 0;
+    zi[i].src = inplace ? static_cast<const uint8_t *>(sg.data) : z_in.as<uint8_t>() + in_off[i];
+    zi[i].len = sg.len;
+    zi[i].dst = z_img.as<uint8_t>() + img_off[i];
+    zi[i].body = (uint64_t)raw_len[zs[i]] - 4;
+  }
+  // checksums of the compressed bytes: the open() machinery over the staged segments
+  std::vector<uint32_t> piece_start(nz + 1);
+  uint32_t np = 0;
+  for (uint32_t i = 0; i < nz; i++) {
+    piece_start[i] = np;
+    if (sd[i].has_header == 1u) np += (uint32_t)div_up(sd[i].body_end - sd[i].body0, CRC_PIECE);
+  }
+  piece_start[nz] = np;
+  z_descs.ensure((size_t)nz * sizeof(SegDesc));
+  z_insegs.ensure((size_t)nz * sizeof(ZInSeg));
+  z_pstart.ensure(((size_t)nz + 1) * 4);
+  z_status.ensure((size_t)nz * 4 + 16);
+  z_flag.ensure(16);
+  TG_CUDA(cudaMemcpyAsync(z_descs.p, sd.data(), (size_t)nz * sizeof(SegDesc), cudaMemcpyHostToDevice, st));
+  TG_CUDA(cudaMemcpyAsync(z_insegs.p, zi.data(), (size_t)nz * sizeof(ZInSeg), cudaMemcpyHostToDevice, st));
+  TG_CUDA(cudaMemcpyAsync(z_pstart.p, piece_start.data(), ((size_t)nz + 1) * 4, cudaMemcpyHostToDevice, st));
+  TG_CUDA(cudaMemsetAsync(z_flag.p, 0, 16, st));
+  const CrcTables *d_crc = DeviceConstants::get(pipe.conf.device).d_crc;
+  if (np) {
+    z_tc.ensure((size_t)np * sizeof(TileCrc));
+    z_crc.ensure((size_t)nz * 4);
+    TG_CUDA(cudaMemsetAsync(z_crc.p, 0, (size_t)nz * 4, st));
+    k_crc_pieces<<<np, CRCV_THREADS, 0, st>>>(z_in.as<uint8_t>(), z_descs.as<SegDesc>(), z_pstart.as<uint32_t>(), nz, d_crc, z_tc.as<TileCrc>());
+    k_crc_combine<<<(uint32_t)div_up(np, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), np, d_crc, z_crc.as<uint32_t>());
+    k_crc_check<<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_in.as<uint8_t>(), z_descs.as<SegDesc>(), nz, z_crc.as<uint32_t>(), d_crc, z_flag.as<int>());
+    launches += 3;
+  }
+  k_zinflate<<<(uint32_t)div_up(nz, ZINF_WARPS), ZINF_WARPS * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_status.as<int32_t>());
+  launches++;
+  TG_CUDA(cudaGetLastError());
+  std::vector<int32_t> status(nz);
+  int bad_crc = 0;
+  TG_CUDA(cudaMemcpyAsync(status.data(), z_status.p, (size_t)nz * 4, cudaMemcpyDeviceToHost, st));
+  TG_CUDA(cudaMemcpyAsync(&bad_crc, z_flag.p, 4, cudaMemcpyDeviceToHost, st));
+  TG_CUDA(cudaStreamSynchronize(st));
+  TG_CHECK(bad_crc == 0, TEZGPU_E_FORMAT, "IFile checksum mismatch in segment " + std::to_string(bad_crc ? zs[bad_crc - 1] : 0));
+  for (uint32_t i = 0; i < nz; i++)
+    TG_CHECK(status[i] == Z_OK, TEZGPU_E_FORMAT,
+             std::string("compressed segment ") + std::to_string(zs[i]) + ": " + z_err_name(status[i]));
+  std::vector<tezgpu_segment> segs2(in, in + nseg);
+  for (uint32_t i = 0; i < nz; i++) {
+    tezgpu_segment &sg = segs2[zs[i]];
+    sg.data = zi[i].dst;
+    sg.len = (uint64_t)raw_len[zs[i]] + 4;
+    sg.flags = TEZGPU_SEG_HAS_HEADER | TEZGPU_SEG_DEVICE | TEZGPU_SEG_VERIFIED;
+  }
+  open(segs2.data(), nseg);
+}
+
+// host run of the device writer over one body: 78 01, the chunks, Adler-32 (tezgpu_debug_deflate_emulate)
+static inline std::vector<uint8_t> z_deflate_host(const uint8_t *body, uint64_t len) {
+  std::vector<uint8_t> out = {0x78, 0x01};
+  ZShared *sh = new ZShared();
+  std::vector<uint8_t> slot(ZSLOT);
+  const uint64_t nch = std::max<uint64_t>(1, div_up(len, ZCHUNK));
+  uint32_t adler = 1;
+  for (uint64_t k = 0; k < nch; k++) {
+    const uint32_t clen = (uint32_t)std::min<uint64_t>(ZCHUNK, len - k * ZCHUNK);
+    z_deflate_chunk_host(*sh, body + k * ZCHUNK, clen, k + 1 == nch, slot.data());
+    out.insert(out.end(), slot.begin(), slot.begin() + sh->bytes);
+    adler = z_adler_combine(adler, sh->adler, clen);
+  }
+  delete sh;
+  for (int b = 3; b >= 0; b--) out.push_back((uint8_t)(adler >> (8 * b)));
+  return out;
+}
+
+}  // namespace tezgpu

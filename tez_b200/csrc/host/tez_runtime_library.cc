@@ -65,6 +65,8 @@ static const char *K_EMPTY_PARTITIONS = "tez.runtime.empty.partitions.info-via-e
 static const char *K_FINAL_MERGE = "tez.runtime.enable.final-merge.in.output";  // :555-557 default true
 static const char *K_REPORT_STATS = "tez.runtime.report.partition.stats";       // :195-198 default memory_optimized
 static const char *K_COMPRESS = "tez.runtime.compress";
+static const char *K_COMPRESS_CODEC = "tez.runtime.compress.codec";
+static const char *DEFAULT_CODEC = "org.apache.hadoop.io.compress.DefaultCodec";
 static const char *K_SERIALIZATIONS = "io.serializations";
 static const char *K_VALUE_CLASS = "tez.runtime.value.class";
 static const char *K_COMBINER_CLASS = "tez.runtime.combiner.class";
@@ -187,6 +189,18 @@ static std::vector<uint8_t> roaring_serialize(const std::vector<uint32_t> &vals)
   return o;
 }
 
+// tez.runtime.compress / tez.runtime.compress.codec (IFile.Writer / Reader via CodecUtils.getCodec): DefaultCodec runs on
+// the device, any other class is refused by name.  Deviation from Tez: with compression on and no codec named, Tez uses
+// DefaultCodec; here that configuration keeps being refused (DESIGN.md 9).
+static int codec_for(const Configuration &conf) {
+  if (!conf.getBoolean(K_COMPRESS, false)) return TEZGPU_CODEC_NONE;
+  const std::string codec = conf.get(K_COMPRESS_CODEC, "");
+  RT_CHECK(!codec.empty(), TEZGPU_E_UNSUPPORTED, "tez.runtime.compress=true: IFile codecs are not supported on the device path yet");
+  RT_CHECK(codec == DEFAULT_CODEC, TEZGPU_E_UNSUPPORTED,
+           std::string(K_COMPRESS_CODEC) + "=" + codec + ": only " + DEFAULT_CODEC + " is supported on the device path");
+  return TEZGPU_CODEC_DEFAULT;
+}
+
 // ================================================================================================ output side
 // GpuSorter: the ExternalSorter seam (SORT/ExternalSorter.java:74-92,281-288) backed by tezgpu_sorter.  Records are
 // batched on the host and handed to the device; when the collected bytes reach the granted sort memory the device
@@ -214,6 +228,7 @@ struct GpuSorter {
   int last_spill_rle = 0;                // merger.needsRLE() of the most recent spill's SpanMerger (:599,805,814)
   int combiner = TEZGPU_COMBINE_NONE;    // runs on every spill, and on the final merge from min_spills spills on (:601-609,815-820)
   int min_spills = 3;
+  int codec = TEZGPU_CODEC_NONE;         // every spill is compressed; the final merge reads and writes through it
   std::map<std::string, int64_t> &counters;
 
   GpuSorter(const tezgpu_conf &c, int64_t mem, bool fm, const std::string &wd, const std::string &u, std::map<std::string, int64_t> &ctr)
@@ -225,6 +240,10 @@ struct GpuSorter {
     gpu_check(tezgpu_sorter_set_combiner(h, c));
     combiner = c;
     min_spills = min_spills_for_combine;
+  }
+  void set_codec(int c) {
+    gpu_check(tezgpu_sorter_set_codec(h, c));
+    codec = c;
   }
   // MRCombiner's COMBINE_INPUT_RECORDS / COMBINE_OUTPUT_RECORDS of one combined write
   void count_combine(const tezgpu_stats &st) {
@@ -321,6 +340,7 @@ struct GpuSorter {
     // final merge across spills, every partition at once on the device (:774-836)
     std::vector<std::vector<uint8_t>> bytes(num_spills);
     std::vector<tezgpu_segment> segs;
+    std::vector<int64_t> raws;   // rawLength of every segment (the compressed ones need it)
     for (int s = 0; s < num_spills; s++) {
       bytes[s] = read_file(spill_files[s]);
       counters["ADDITIONAL_SPILLS_BYTES_READ"] += (int64_t)bytes[s].size();
@@ -333,13 +353,14 @@ struct GpuSorter {
           sg.flags = TEZGPU_SEG_HAS_HEADER;
           sg.partition = (uint32_t)p;
           segs.push_back(sg);
+          raws.push_back(raw);
         }
       }
     }
     tezgpu_conf mc = gc;
     mc.fixed_key_len = mc.fixed_val_len = 0;
     tezgpu_merger *m = nullptr;
-    gpu_check(tezgpu_merge_open(&mc, segs.data(), (uint32_t)segs.size(), &m));
+    gpu_check(tezgpu_merge_open_codec(&mc, segs.data(), raws.data(), (uint32_t)segs.size(), codec, &m));
     final_idx.assign((size_t)P * 3, 0);
     tezgpu_stats st;
     // TezMerger.merge(..., checkForSameKeys = merger.needsRLE()) into Writer(..., rle = merger.needsRLE()), `merger`
@@ -402,7 +423,7 @@ struct Output {
     std::transform(sc.begin(), sc.end(), sc.begin(), ::toupper);
     RT_CHECK(sc == "PIPELINED" || sc == "LEGACY", TEZGPU_E_INVALID,
              "Invalid sorter class specified in config, propertyName=" + std::string(K_SORTER_CLASS) + ", value=" + sc + ", validValues=[LEGACY, PIPELINED]");
-    RT_CHECK(!conf.getBoolean(K_COMPRESS, false), TEZGPU_E_UNSUPPORTED, "tez.runtime.compress=true: IFile codecs are not supported on the device path yet");
+    const int codec = codec_for(conf);
     tezgpu_conf gc;
     memset(&gc, 0, sizeof(gc));
     gc.abi_version = TEZGPU_ABI_VERSION;
@@ -417,6 +438,7 @@ struct Output {
     gc.mem_budget_bytes = (uint64_t)granted;
     sorter = new GpuSorter(gc, granted > 0 ? granted : requested, final_merge, work_dir, uid, counters);
     if (const int c = combiner_for(conf)) sorter->set_combiner(c, (int)conf.getInt(K_COMBINE_MIN_SPILLS, 3));
+    if (codec) sorter->set_codec(codec);
     started = true;
   }
   void write(const uint8_t *k, uint32_t kl, const uint8_t *v, uint32_t vl, int32_t partition) {
@@ -514,6 +536,7 @@ struct Input {
   bool initialized = false, started = false, ready = false;
   std::map<std::string, int64_t> counters;
   std::vector<std::vector<uint8_t>> seg_bytes;
+  std::vector<int64_t> seg_raw;   // rawLength of each fetched segment (index / ShuffleHeader)
   // per source: spill ids seen and the id carried by the event with last_event_flag (pipelined shuffle; the reference's
   // ShuffleScheduler tracks the same per input identifier: eventsProcessed / finalEventId, OG/ShuffleScheduler.java:540-600); spill id -1 = the single
   // event of a producer that ran its final merge
@@ -522,6 +545,7 @@ struct Input {
   int num_delivered = 0;
   tezgpu_merger *merger = nullptr;
   int cmp = 0;
+  int codec = TEZGPU_CODEC_NONE;
   // iterator state (RL/common/ValuesIterator.java:91-201)
   std::vector<uint8_t> batch, next_batch_buf;
   std::vector<tezgpu_kv_index> idx;
@@ -538,6 +562,7 @@ struct Input {
     double pct = conf.getFloat("tez.runtime.shuffle.fetch.buffer.percent", 0.9);
     requested = (int64_t)(pct * (double)task_memory);
     cmp = comparator_for(conf);
+    codec = codec_for(conf);
     initialized = true;
   }
   void start() {
@@ -581,6 +606,7 @@ struct Input {
     int64_t start = be64((size_t)partition * 24), raw = be64((size_t)partition * 24 + 8), part = be64((size_t)partition * 24 + 16);
     if (!(raw > 6)) { counters["NUM_SKIPPED_INPUTS"]++; return; }  // !hasData
     seg_bytes.push_back(read_file(file_out, (uint64_t)start, part));
+    seg_raw.push_back(raw);
     counters["NUM_SHUFFLED_INPUTS"]++;
     counters["SHUFFLE_BYTES"] += part;
     counters["SHUFFLE_BYTES_DECOMPRESSED"] += raw;
@@ -605,9 +631,11 @@ struct Input {
       segs[i].flags = TEZGPU_SEG_HAS_HEADER;
       segs[i].partition = 0;
     }
-    gpu_check(tezgpu_merge_open(&gc, segs.data(), (uint32_t)segs.size(), &merger));  // MergeManager.finalMerge -> TezMerger.merge
+    // MergeManager.finalMerge -> TezMerger.merge; compressed segments are inflated with their index rawLength
+    gpu_check(tezgpu_merge_open_codec(&gc, segs.data(), seg_raw.data(), (uint32_t)segs.size(), codec, &merger));
     counters["MERGED_MAP_OUTPUTS"] += (int64_t)segs.size();
     seg_bytes.clear();
+    seg_raw.clear();
     batch.resize(8u << 20);
     idx.resize(1u << 16);
     ready = true;

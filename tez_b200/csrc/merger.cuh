@@ -774,13 +774,19 @@ class Merger {
     launches += 2;
   }
 
-  uint64_t output_bound() const { return SortPipeline::output_bound(n, kv_bytes, pipe.conf.num_partitions) + 16; }
+  uint64_t raw_output_bound() const { return SortPipeline::output_bound(n, kv_bytes, pipe.conf.num_partitions) + 16; }
+  uint64_t output_bound() const {
+    return pipe.codec ? SortPipeline::codec_bound(raw_output_bound(), pipe.conf.num_partitions) : raw_output_bound();
+  }
+
+  // ---- codec (codec.cuh): compressed segments are checked, inflated into z_img and merged as ordinary segments
+  DeviceBuffer z_in, z_img, z_insegs, z_status, z_descs, z_pstart, z_tc, z_crc, z_flag;
+  void open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg);
 
   // the writer behind write_*: TezMerger.writeFile semantics, or -- with a combiner -- the combined records, which carry
   // no segment tags and unique keys (merge mode and the plain writer then write the same bytes)
   void emit(int writer_rle, uint8_t *d_out_buf, uint64_t cap, uint64_t *out_len, int64_t *index, tezgpu_stats *st) {
-    if (pipe.combiner) pipe.emit_combined(writer_rle ? 1 : 0, d_out_buf, cap, out_len, index, st);
-    else pipe.emit_phase(writer_rle ? 1 : 0, true, d_out_buf, cap, out_len, index, st);
+    pipe.emit_out(writer_rle ? 1 : 0, true, raw_output_bound(), d_out_buf, cap, out_len, index, st);
   }
 
   // TezMerger.writeFile: one IFile segment, equal adjacent keys written through IFile.REPEAT_KEY

@@ -9,6 +9,7 @@
 #include "../../include/tezgpu.h"
 #include "device_util.h"
 #include "combine.cuh"
+#include "deflate.cuh"
 #include "emit_pipe_u.cuh"
 #include "sorter_kernels.cuh"
 
@@ -225,14 +226,44 @@ class SortPipeline {
   }
 
   void run(Records rec, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index, tezgpu_stats *stats) {
+    const uint64_t raw_bound = output_bound(rec.n, rec.fixed ? (uint64_t)rec.n * (rec.klen + rec.vlen) : rec.kv_bytes, conf.num_partitions);
     sort_phase(rec);
     int rle;
     if (conf.rle_policy == TEZGPU_RLE_ON) rle = 1;
     else if (conf.rle_policy == TEZGPU_RLE_OFF) rle = 0;
     else rle = (conf.sorter_impl == 1) ? 0 : ((double)state.dup_count > 0.1 * (double)rec.n);
     if (conf.sorter_impl == TEZGPU_SORTER_UNORDERED) rle = 0;   // Writer(..., codec, null, null): no run-length encoding (:1092)
-    if (combiner) emit_combined(rle, d_out, out_cap, out_len, index, stats);
-    else emit_phase(rle, false, d_out, out_cap, out_len, index, stats);
+    emit_out(rle, false, raw_bound, d_out, out_cap, out_len, index, stats);
+  }
+
+  // ---- codec (deflate.cuh, codec.cuh): with TEZGPU_CODEC_DEFAULT the emit writes the uncompressed file into z_img and
+  // compress_image turns every segment into a zlib-compressed one in d_out
+  int codec = TEZGPU_CODEC_NONE;
+  DeviceBuffer z_img, z_slots, z_csize, z_cadler, z_coff, z_segs, z_descs, z_pstart, z_tc, z_crc;
+  PinnedBuffer z_host;
+  EventTimer z_timer;
+  // worst case of the compressed file given the uncompressed file's bound: every chunk stored
+  static uint64_t codec_bound(uint64_t raw_bound, int P) { return raw_bound + 5 * (raw_bound / ZCHUNK + (uint64_t)P + 1) + 11ull * P + 64; }
+  void compress_image(const int64_t *raw_index, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index, tezgpu_stats *stats);
+
+  // the emit of the sorted (merged) records: combined or not, compressed or not.  raw_bound bounds the uncompressed file.
+  void emit_out(int rle, bool merge_mode, uint64_t raw_bound, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index,
+                tezgpu_stats *stats) {
+    if (!codec) {
+      if (combiner) emit_combined(rle, d_out, out_cap, out_len, index, stats);
+      else emit_phase(rle, merge_mode, d_out, out_cap, out_len, index, stats);
+      return;
+    }
+    const int P = conf.num_partitions;
+    z_img.ensure(raw_bound + 64);
+    std::vector<int64_t> raw_index((size_t)P * 3, 0);
+    uint64_t raw_len = 0;
+    tezgpu_stats st;
+    memset(&st, 0, sizeof(st));
+    if (combiner) emit_combined(rle, z_img.as<uint8_t>(), z_img.cap, &raw_len, raw_index.data(), &st);
+    else emit_phase(rle, merge_mode, z_img.as<uint8_t>(), z_img.cap, &raw_len, raw_index.data(), &st);
+    compress_image(raw_index.data(), d_out, out_cap, out_len, index, &st);
+    if (stats) *stats = st;
   }
 
   // partition + sort: stage, radix sort of (sort word, index), tie refinement.  Leaves K / order / same / counts.

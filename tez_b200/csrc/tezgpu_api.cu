@@ -9,6 +9,7 @@
 #include <string>
 
 #include "../../include/tezgpu.h"
+#include "codec.cuh"
 #include "merger.cuh"
 #include "sorter.cuh"
 #include "peer_fetch.cuh"
@@ -241,12 +242,17 @@ int32_t tezgpu_sorter_collect_fixed(tezgpu_sorter *h, const uint8_t *kv, const i
   TG_API_END
 }
 
-uint64_t tezgpu_sorter_output_bound(const tezgpu_sorter *h) {
-  if (!h) return 0;
+static uint64_t sorter_raw_bound(const tezgpu_sorter *h) {
   if (h->fixed && h->pipe.conf.rle_policy == TEZGPU_RLE_OFF)  // exact: n * (vint(k) + vint(v) + k + v) + 10 bytes per segment
     return h->n * ((uint64_t)vint_size_u32(h->klen) + vint_size_u32(h->vlen) + h->klen + h->vlen) +
            10ull * h->pipe.conf.num_partitions + 64;
   return SortPipeline::output_bound(h->n, h->kv_bytes, h->pipe.conf.num_partitions);
+}
+
+uint64_t tezgpu_sorter_output_bound(const tezgpu_sorter *h) {
+  if (!h) return 0;
+  const uint64_t raw = sorter_raw_bound(h);
+  return h->pipe.codec ? SortPipeline::codec_bound(raw, h->pipe.conf.num_partitions) : raw;
 }
 
 static void sorter_run(tezgpu_sorter *h, uint8_t *host_out, uint64_t out_cap, uint64_t *out_len, int64_t *index,
@@ -341,6 +347,40 @@ int32_t tezgpu_sorter_set_combiner(tezgpu_sorter *h, int32_t combiner) {
            "fixed_val_len " + std::to_string(h->vlen) + " is not the combiner's value width");
   TG_CHECK(h->n == 0 && !h->flushed, TEZGPU_E_STATE, "set the combiner before the first collect (or after a reset)");
   h->pipe.combiner = combiner;
+  TG_API_END
+}
+
+int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec) {
+  TG_API_BEGIN
+  TG_CHECK(h, TEZGPU_E_INVALID, "null handle");
+  TG_CHECK(codec == TEZGPU_CODEC_NONE || codec == TEZGPU_CODEC_DEFAULT, TEZGPU_E_UNSUPPORTED,
+           "codec " + std::to_string(codec) + " is not on the device (DefaultCodec only)");
+  TG_CHECK(h->n == 0 && !h->flushed, TEZGPU_E_STATE, "set the codec before the first collect (or after a reset)");
+  h->pipe.codec = codec;
+  TG_API_END
+}
+
+int32_t tezgpu_debug_deflate_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len) {
+  TG_API_BEGIN
+  TG_CHECK((body || len == 0) && out && out_len, TEZGPU_E_INVALID, "null argument");
+  const std::vector<uint8_t> z = z_deflate_host(body, len);
+  *out_len = z.size();
+  TG_CHECK(z.size() <= cap, TEZGPU_E_NOMEM, "output buffer too small");
+  memcpy(out, z.data(), z.size());
+  TG_API_END
+}
+
+int32_t tezgpu_debug_inflate_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
+                                     uint64_t *out_len) {
+  TG_API_BEGIN
+  TG_CHECK((z || len == 0) && (out || body_len == 0) && out_len, TEZGPU_E_INVALID, "null argument");
+  TG_CHECK(body_len <= cap, TEZGPU_E_INVALID, "output buffer smaller than body_len");
+  ZInflateWork *w = new ZInflateWork();
+  uint64_t got = 0;
+  const int32_t rc = z_inflate(z, len, out, body_len, &got, *w);
+  delete w;
+  *out_len = got;
+  TG_CHECK(rc == Z_OK, TEZGPU_E_FORMAT, std::string("compressed segment 0: ") + z_err_name(rc));
   TG_API_END
 }
 

@@ -33,24 +33,30 @@ def make_conf(num_partitions, comparator=CMP_BYTES, partitioner=PART_HASH, rle_p
 
 
 class GpuSorter:
-    def __init__(self, num_partitions, combiner=COMBINE_NONE, **kw):
+    def __init__(self, num_partitions, combiner=COMBINE_NONE, codec=CODEC_NONE, **kw):
         """combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG runs MRCombiner with IntSumReducer / LongSumReducer on every
-        flush (tezgpu_sorter_set_combiner)."""
+        flush (tezgpu_sorter_set_combiner).  codec: CODEC_DEFAULT writes zlib-compressed segments (tezgpu_sorter_set_codec)."""
         self.L = _lib.load()
         self.conf = make_conf(num_partitions, **kw)
         self.P = num_partitions
         self.h = C.c_void_p()
         check(self.L.tezgpu_sorter_create(C.byref(self.conf), C.byref(self.h)))
-        if combiner:
-            try:
+        try:
+            if combiner:
                 self.set_combiner(combiner)
-            except Exception:
-                self.close()
-                raise
+            if codec:
+                self.set_codec(codec)
+        except Exception:
+            self.close()
+            raise
 
     def set_combiner(self, combiner):
         """Before the first collect (or after reset); survives reset."""
         check(self.L.tezgpu_sorter_set_combiner(self.h, combiner))
+
+    def set_codec(self, codec):
+        """CODEC_NONE / CODEC_DEFAULT; before the first collect (or after reset); survives reset."""
+        check(self.L.tezgpu_sorter_set_codec(self.h, codec))
 
     def close(self):
         if self.h:
@@ -128,11 +134,14 @@ class GpuSorter:
 
 class GpuMerger:
     def __init__(self, segments, comparator=CMP_BYTES, device=0, has_header=True, device_ptrs=False, fixed=None,
-                 partitions=None, num_partitions=1, send_empty=True, verified=None, combiner=COMBINE_NONE):
+                 partitions=None, num_partitions=1, send_empty=True, verified=None, combiner=COMBINE_NONE,
+                 codec=CODEC_NONE, raw_lens=None):
         """segments: list of bytes / uint8 arrays (host) or (ptr, len) tuples when device_ptrs.
         verified: optional per-segment booleans -- the transport already checked that segment's checksum
         (TEZGPU_SEG_VERIFIED: fetch_segments_verified), the merge does not read it again to verify.
-        combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG combines the merged stream in write_* (tezgpu_merge_set_combiner)."""
+        combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG combines the merged stream in write_* (tezgpu_merge_set_combiner).
+        codec: CODEC_DEFAULT reads compressed (TIF\\x01) segments and writes compressed output (tezgpu_merge_open_codec);
+        raw_lens: per-segment rawLength, required for the compressed segments."""
         self.L = _lib.load()
         self.conf = make_conf(num_partitions, comparator=comparator, partitioner=PART_GIVEN, device=device, fixed=fixed,
                               send_empty=send_empty)
@@ -140,7 +149,12 @@ class GpuMerger:
         self._has_header, self._device_ptrs = has_header, device_ptrs
         arr = self._segments(segments, partitions, verified)
         self.h = C.c_void_p()
-        check(self.L.tezgpu_merge_open(C.byref(self.conf), arr, len(segments), C.byref(self.h)))
+        if codec:
+            check(self.L.tezgpu_merge_open_codec(C.byref(self.conf), arr, _ptr(self._raw(raw_lens)), len(segments), codec,
+                                                 C.byref(self.h)))
+        else:
+            check(self.L.tezgpu_merge_open(C.byref(self.conf), arr, len(segments), C.byref(self.h)))
+        self.codec = codec
         if combiner:
             try:
                 self.set_combiner(combiner)
@@ -179,10 +193,17 @@ class GpuMerger:
             arr[i].partition = 0 if partitions is None else int(partitions[i])
         return arr
 
-    def reopen(self, segments, partitions=None, verified=None):
+    def _raw(self, raw_lens):
+        self._raw_keep = None if raw_lens is None else np.ascontiguousarray(raw_lens, dtype=np.int64)
+        return self._raw_keep
+
+    def reopen(self, segments, partitions=None, verified=None, raw_lens=None):
         """New merge through the same handle (device allocations are kept)."""
         arr = self._segments(segments, partitions, verified)
-        check(self.L.tezgpu_merge_reopen(self.h, arr, len(segments)))
+        if self.codec:
+            check(self.L.tezgpu_merge_reopen_codec(self.h, arr, _ptr(self._raw(raw_lens)), len(segments)))
+        else:
+            check(self.L.tezgpu_merge_reopen(self.h, arr, len(segments)))
 
     def close(self):
         if self.h:

@@ -1,0 +1,176 @@
+"""DefaultCodec cost on the device: one JSON line per case, codec and no-codec runs alternating in one process.
+
+  1. config-2 map side: 1e8 random 80-byte records, P = 64, sort_device_fixed (the stored path)
+  2. compressible map side: Text words drawn from a Zipf law with IntWritable 1 values, sort_device_fixed
+  3. reduce side: config-3 segments compressed on the host with zlib level 1, reopen + write_ifile_device
+  4. e2e through host buffers: collect_batch + flush_to_memory of the case-2 records
+
+Times: host clock around fully synchronised library calls.  The card name and power limit are read in the same run.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+import zlib
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from oracle import tez_oracle as O  # noqa: E402
+import tez_b200 as T  # noqa: E402
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 else "unknown"
+
+
+def zcap(raw, P):
+    return raw + 5 * (raw // 32768 + P + 1) + 11 * P + 64
+
+
+def timed(fn):
+    torch.cuda.synchronize()
+    t = time.perf_counter()
+    r = fn()
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t) * 1e3, r
+
+
+def words_kv(n, seed=7):
+    """n records of an 8-byte Text key (vint 7, 'w', 6 digits of a Zipf-drawn word id) and IntWritable 1"""
+    rng = np.random.default_rng(seed)
+    ids = np.minimum(rng.zipf(1.2, n), 999999)
+    rec = np.empty((n, 12), dtype=np.uint8)
+    rec[:, 0] = 7
+    rec[:, 1] = ord("w")
+    for d in range(6):
+        rec[:, 7 - d] = ord("0") + (ids // 10 ** d) % 10
+    rec[:, 8:11] = 0
+    rec[:, 11] = 1
+    return rec.reshape(-1)
+
+
+def map_side(name, kv, kl, vl, cmp_kind, P, runs, out):
+    n = kv.size // (kl + vl)
+    d_kv = torch.from_numpy(kv).cuda()
+    raw_cap = n * (kl + vl + 2) + 10 * P + 64
+    d_out = torch.empty(zcap(raw_cap, P), dtype=torch.uint8, device="cuda")
+    res = {0: [], 1: []}
+    lens = {}
+    sorters = {c: T.GpuSorter(P, comparator=cmp_kind, fixed=(kl, vl), codec=c) for c in (0, T.CODEC_DEFAULT)}
+    for r in range(runs + 1):
+        for c, s in sorters.items():
+            ms, (ln, index, st) = timed(lambda: s.sort_device_fixed(d_kv.data_ptr(), n, d_out.data_ptr(), d_out.numel()))
+            if r:
+                res[c].append(ms)
+            lens[c] = (ln, index)
+    raw = lens[0][0]
+    zlen, zindex = lens[T.CODEC_DEFAULT]
+    line = dict(case=name, records=n, partitions=P, raw_bytes=raw, compressed_bytes=zlen, ratio=round(zlen / raw, 4),
+                ms_no_codec=round(min(res[0]), 2), ms_codec=round(min(res[T.CODEC_DEFAULT]), 2),
+                ms_runs_no_codec=[round(x, 2) for x in res[0]], ms_runs_codec=[round(x, 2) for x in res[T.CODEC_DEFAULT]])
+    extra = line["ms_codec"] - line["ms_no_codec"]
+    line["compress_gbps_derived"] = round(raw / extra / 1e6, 2) if extra > 0 else None
+    if name == "compressible":
+        # zlib level 1 on the same bodies (the first 8 partitions)
+        host = d_out[:zlen].cpu().numpy().tobytes()
+        zsum = rsum = 0
+        for p in range(8):
+            s0, rl, pl = (int(x) for x in zindex[p])
+            body = zlib.decompress(host[s0 + 4:s0 + pl - 4])
+            zsum += pl - 8
+            rsum += len(zlib.compress(body, 1))
+        line["ratio_to_zlib1"] = round(zsum / rsum, 4)
+    for s in sorters.values():
+        s.close()
+    del d_kv, d_out
+    torch.cuda.empty_cache()
+    out.append(line)
+
+
+def reduce_side(nseg, seg_bytes, runs, out):
+    plain, _ = O.gen_c3_segments(nseg, seg_bytes, seed=3, threads=16)
+    plain = [p.tobytes() for p in plain]
+    zsegs, raws = [], []
+    for p in plain:
+        z = zlib.compress(p[4:-4], 1)
+        zsegs.append(b"TIF\x01" + z + zlib.crc32(z).to_bytes(4, "big"))
+        raws.append(len(p) - 4)
+    mz = T.GpuMerger(zsegs, comparator=T.CMP_TEXT, codec=T.CODEC_DEFAULT, raw_lens=raws)
+    mp = T.GpuMerger(plain, comparator=T.CMP_TEXT)
+    cap = max(mz.output_bound(), mp.output_bound())
+    d_out = torch.empty(cap, dtype=torch.uint8, device="cuda")
+    res = {0: [], 1: []}
+    for r in range(runs + 1):
+        for c, m, segs in ((0, mp, plain), (1, mz, zsegs)):
+            def step():
+                if c:
+                    m.reopen(segs, raw_lens=raws)
+                else:
+                    m.reopen(segs)
+                return m.write_ifile_device(d_out.data_ptr(), cap)
+            ms, (raw, part, st) = timed(step)
+            if r:
+                res[c].append(ms)
+    raw_total, z_total = sum(len(p) for p in plain), sum(len(z) for z in zsegs)
+    line = dict(case="reduce_c3_zlib1", segments=nseg, raw_bytes=raw_total, compressed_in_bytes=z_total,
+                ms_plain=round(min(res[0]), 2), ms_codec=round(min(res[1]), 2),
+                ms_runs_plain=[round(x, 2) for x in res[0]], ms_runs_codec=[round(x, 2) for x in res[1]],
+                note="codec: reads compressed segments and writes a compressed merged segment")
+    out.append(line)
+    mz.close()
+    mp.close()
+
+
+def e2e(kv, kl, vl, cmp_kind, P, runs, out):
+    """collect_batch (variable-width API, one batch) + flush_to_memory"""
+    n = kv.size // (kl + vl)
+    stride = kl + vl
+    key_off = (np.arange(n, dtype=np.uint64) * stride).astype(np.uint32)
+    val_off = key_off + np.uint32(kl)
+    val_len = np.full(n, vl, dtype=np.uint32)
+    res = {0: [], 1: []}
+    moved = {}
+    for r in range(runs + 1):
+        for c in (0, T.CODEC_DEFAULT):
+            with T.GpuSorter(P, comparator=cmp_kind, codec=c) as s:
+                def step():
+                    s.collect(kv, key_off, val_off, val_len)
+                    return s.flush_to_memory()
+                ms, (o, _, _, _) = timed(step)
+            if r:
+                res[c].append(ms)
+            moved[c] = len(o)
+    out.append(dict(case="e2e_host_buffers", api="collect_batch + flush_to_memory", records=n, kv_bytes=kv.size,
+                    down_bytes_no_codec=moved[0], down_bytes_codec=moved[1], ms_no_codec=round(min(res[0]), 1),
+                    ms_codec=round(min(res[1]), 1), kv_gbps_no_codec=round(kv.size / min(res[0]) / 1e6, 2),
+                    kv_gbps_codec=round(kv.size / min(res[1]) / 1e6, 2)))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--runs", type=int, default=3)
+    ap.add_argument("--c2-records", type=int, default=10 ** 8)
+    ap.add_argument("--words-records", type=int, default=90 * 10 ** 6)
+    ap.add_argument("--c3-segments", type=int, default=256)
+    ap.add_argument("--c3-seg-bytes", type=int, default=1 << 22)
+    a = ap.parse_args()
+    dev = card()
+    out = []
+    map_side("config2_stored", O.gen_c2(0, a.c2_records, seed=2, threads=16), 16, 64, T.CMP_BYTES, 64, a.runs, out)
+    words = words_kv(a.words_records)
+    map_side("compressible", words, 8, 4, T.CMP_TEXT, 64, a.runs, out)
+    reduce_side(a.c3_segments, a.c3_seg_bytes, a.runs, out)
+    e2e(words[:12 * (a.words_records // 4)], 8, 4, T.CMP_TEXT, 64, a.runs, out)
+    for line in out:
+        line["device"] = dev
+        print(json.dumps(line), flush=True)
+
+
+if __name__ == "__main__":
+    main()
