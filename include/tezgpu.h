@@ -344,6 +344,15 @@ int32_t tezgpu_debug_deflate_emulate(const uint8_t *body, uint64_t len, uint8_t 
 int32_t tezgpu_debug_inflate_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
                                      uint64_t *out_len);
 
+/* diagnostics: the 32-bit sort words the variable-width map side gives n keys (key i = kv[key_off[i] ..
+ * key_off[i] + key_len[i])), computed on the host with the device's code: the alphabet table built from the byte values
+ * that occur, then every key's word.  partition: given partition ids, or NULL for the HashPartitioner.  use_sym = 0
+ * forces the raw 4-byte prefix (TEZGPU_NO_SYM=1).  npos: content positions the alphabet table packs; sym_used: 1 when
+ * the words are packed ranks (the table packs more positions than the raw prefix holds), 0 for the raw prefix. */
+int32_t tezgpu_debug_sort_words_emulate(const uint8_t *kv, const uint64_t *key_off, const uint32_t *key_len, uint32_t n,
+                                        int32_t comparator, int32_t num_partitions, const int32_t *partition,
+                                        int32_t use_sym, uint32_t *words, uint32_t *npos, int32_t *sym_used);
+
 #ifdef __cplusplus
 }
 #endif

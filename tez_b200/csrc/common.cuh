@@ -36,6 +36,7 @@ static inline uint64_t align_up(uint64_t a, uint64_t b) { return div_up(a, b) * 
 enum { CMP_BYTES = 0, CMP_TEXT = 1, CMP_BYTESWRITABLE = 2, CMP_INT = 3, CMP_LONG = 4 };
 
 // -------------------------------------------------------------------------------------------- device helpers
+// (the key helpers are __host__ __device__: tezgpu_debug_sort_words_emulate runs the sort word build on the host)
 // hadoop WritableUtils.decodeVIntSize on the first byte
 __host__ __device__ __forceinline__ int vint_decode_size(uint8_t first) {
   int v = (int)(int8_t)first;
@@ -61,7 +62,7 @@ __host__ __device__ __forceinline__ uint8_t vint_byte_u32(uint32_t v, int b) {
 }
 
 // bytes of key content to skip before comparing / hashing (Text: vint prefix, BytesWritable: 4-byte length)
-__device__ __forceinline__ uint32_t key_content_skip(int cmp, const uint8_t *key, uint32_t klen) {
+__host__ __device__ __forceinline__ uint32_t key_content_skip(int cmp, const uint8_t *key, uint32_t klen) {
   if (klen == 0) return 0;
   if (cmp == CMP_TEXT) {
     uint32_t s = (uint32_t)vint_decode_size(key[0]);
@@ -73,21 +74,21 @@ __device__ __forceinline__ uint32_t key_content_skip(int cmp, const uint8_t *key
 
 // normalised content byte i: unsigned lexicographic order over these bytes == comparator order
 // (IntWritable / LongWritable: two's complement big-endian => flip the sign bit of byte 0)
-__device__ __forceinline__ uint32_t norm_byte(int cmp, const uint8_t *content, uint32_t i) {
+__host__ __device__ __forceinline__ uint32_t norm_byte(int cmp, const uint8_t *content, uint32_t i) {
   uint32_t b = content[i];
   if (i == 0 && (cmp == CMP_INT || cmp == CMP_LONG)) b ^= 0x80u;
   return b;
 }
 
 // WritableComparator.hashBytes
-__device__ __forceinline__ int32_t hash_bytes_dev(const uint8_t *p, uint32_t n) {
+__host__ __device__ __forceinline__ int32_t hash_bytes_dev(const uint8_t *p, uint32_t n) {
   uint32_t h = 1;
   for (uint32_t i = 0; i < n; i++) h = 31u * h + (uint32_t)(int32_t)(int8_t)p[i];
   return (int32_t)h;
 }
 
 // key.hashCode() for the supported key classes
-__device__ __forceinline__ int32_t key_hash_dev(int cmp, const uint8_t *key, uint32_t klen) {
+__host__ __device__ __forceinline__ int32_t key_hash_dev(int cmp, const uint8_t *key, uint32_t klen) {
   if (cmp == CMP_INT && klen >= 4)
     return (int32_t)(((uint32_t)key[0] << 24) | ((uint32_t)key[1] << 16) | ((uint32_t)key[2] << 8) | key[3]);
   if (cmp == CMP_LONG && klen >= 8) {

@@ -318,24 +318,8 @@ class SortPipeline {
       TG_CUDA(cudaMemcpyAsync(hs, sym_sets.p, sizeof(hs), cudaMemcpyDeviceToHost, stream));
       TG_CUDA(cudaStreamSynchronize(stream));
       SymTable *t = new SymTable();
-      memset(t, 0, sizeof(*t));
-      const uint32_t avail = 32u - (uint32_t)pbits;
-      uint32_t used = 0, np = 0;
-      for (; np < (uint32_t)SYM_MAX_POS; np++) {
-        uint32_t cnt = 0;
-        for (int w = 0; w < 8; w++) cnt += (uint32_t)__builtin_popcount(hs[np * 8 + w]);
-        if (cnt == 0) break;                       // no key is this long
-        uint32_t bits = 0;
-        while ((1u << bits) < cnt + 1) bits++;     // ranks 1..cnt, 0 = the key ended
-        if (used + bits > avail) break;
-        used += bits;
-        t->shift[np] = (uint8_t)(avail - used);
-        uint32_t rk = 0;
-        for (uint32_t b = 0; b < 256; b++)
-          if ((hs[np * 8 + (b >> 5)] >> (b & 31u)) & 1u) t->rank[np][b] = (uint8_t)(++rk);
-      }
-      t->npos = np;
-      if (np > avail / 8) {                        // packs more positions than the raw bytes would
+      const uint32_t np = sym_table_build(hs, pbits, t);
+      if (sym_table_pays(np, pbits)) {             // packs more positions than the raw bytes would
         TG_CUDA(cudaMemcpyAsync(sym_tab.p, t, sizeof(SymTable), cudaMemcpyHostToDevice, stream));
         TG_CUDA(cudaStreamSynchronize(stream));
         rec.sym = sym_tab.as<SymTable>();

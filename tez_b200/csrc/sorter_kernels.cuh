@@ -57,13 +57,39 @@ __device__ __forceinline__ uint64_t run_record_off_p(const RunTable &t, uint32_t
 // records WHICH byte values occur at each of the first SYM_MAX_POS content positions; position q then needs only
 // ceil(log2(#values + 1)) bits (rank 0 = "key ended before q", so a proper prefix still sorts first), and as many
 // positions as fit are packed, most significant first.  Order-preserving by construction (ranks follow byte order per
-// position), exact for any input; lower-case words get 6 characters into 30 bits instead of 3-4.
+// position), exact for any input; lower-case words get 6 characters into 30 bits instead of 3-4.  A position where all
+// 256 byte values occur needs ranks 1..256, i.e. 9 bits and a rank wider than a byte.
 constexpr int SYM_MAX_POS = 16;
 struct SymTable {
-  uint8_t rank[SYM_MAX_POS][256];  // 1 + number of occurring byte values below b (0 for values that never occur)
-  uint8_t shift[SYM_MAX_POS];      // left shift of position q's rank inside the (32 - pbits)-bit field
-  uint32_t npos;                   // positions packed; equal sort words <=> equal first npos content bytes (or both ended)
+  uint16_t rank[SYM_MAX_POS][256];  // 1 + number of occurring byte values below b (0 for values that never occur)
+  uint8_t shift[SYM_MAX_POS];       // left shift of position q's rank inside the (32 - pbits)-bit field
+  uint32_t npos;                    // positions packed; equal sort words <=> equal first npos content bytes (or both ended)
 };
+
+// Host: the table from k_symbols' occurrence sets (sets[q * 8 + (b >> 5)] bit (b & 31) = byte value b occurs at content
+// position q).  Packs positions while their ranks fit the (32 - pbits)-bit field and returns how many it packed; the sort
+// uses the table only when that is more than the (32 - pbits) / 8 positions the raw prefix holds.
+static inline uint32_t sym_table_build(const uint32_t *sets, int pbits, SymTable *t) {
+  memset(t, 0, sizeof(*t));
+  const uint32_t avail = 32u - (uint32_t)pbits;
+  uint32_t used = 0, np = 0;
+  for (; np < (uint32_t)SYM_MAX_POS; np++) {
+    uint32_t cnt = 0;
+    for (int w = 0; w < 8; w++) cnt += (uint32_t)__builtin_popcount(sets[np * 8 + w]);
+    if (cnt == 0) break;                       // no key is this long
+    uint32_t bits = 0;
+    while ((1u << bits) < cnt + 1) bits++;     // ranks 1..cnt, 0 = the key ended
+    if (used + bits > avail) break;
+    used += bits;
+    t->shift[np] = (uint8_t)(avail - used);
+    uint32_t rk = 0;
+    for (uint32_t b = 0; b < 256; b++)
+      if ((sets[np * 8 + (b >> 5)] >> (b & 31u)) & 1u) t->rank[np][b] = (uint16_t)(++rk);
+  }
+  t->npos = np;
+  return np;
+}
+static inline bool sym_table_pays(uint32_t npos, int pbits) { return npos > (32u - (uint32_t)pbits) / 8u; }
 
 // Collected records as they sit in HBM (the analogue of PipelinedSorter's kvbuffer + kvmeta, :957-959)
 struct Records {
@@ -115,9 +141,41 @@ __device__ __forceinline__ uint32_t record_tag(const Records &r, uint32_t i) {
 }
 
 // ------------------------------------------------------------------------------------------------ stage
-// One thread per record: partition id (HashPartitioner or given), first four normalised key bytes, sort word
-//   K = partition << (32 - pbits) | prefix >> pbits,
-// and the digit histograms of all four radix passes (so the sort never re-reads the keys for counting).
+// K = partition << (32 - pbits) | prefix >> pbits.  bad: the partition lies outside [0, num_partitions) (it is replaced
+// by 0).  Unordered: the word is the partition alone.
+__host__ __device__ __forceinline__ uint32_t compose_sort_word(const Records &r, int32_t p, uint32_t prefix, bool &bad) {
+  bad = p < 0 || p >= r.num_partitions;
+  if (bad) p = 0;
+  if (r.unordered) prefix = 0;
+  return r.pbits ? (((uint32_t)p << (32 - r.pbits)) | (prefix >> r.pbits)) : prefix;
+}
+
+// Sort word of one record with its key at `key` (every path of k_stage but the 16-byte fast one; the host emulation
+// tezgpu_debug_sort_words_emulate runs the same code): partition id (HashPartitioner, else `given`) and prefix = the
+// first normalised content bytes or the packed SymTable ranks.
+__host__ __device__ __forceinline__ uint32_t stage_sort_word(const Records &r, const uint8_t *key, uint32_t klen,
+                                                             int32_t given, bool &bad) {
+  const uint32_t skip = key_content_skip(r.cmp, key, klen);
+  const uint8_t *content = key + skip;
+  const uint32_t clen = klen - skip;
+  uint32_t prefix = 0;
+  if (r.sym) {   // packed ranks: already a (32 - pbits)-bit value, shifted up so that the common `>> pbits` below fits
+    const SymTable *__restrict__ st = r.sym;
+    const uint32_t np = st->npos;
+    for (uint32_t q = 0; q < np && q < clen; q++) prefix |= (uint32_t)st->rank[q][norm_byte(r.cmp, content, q)] << st->shift[q];
+    prefix <<= r.pbits;
+  } else {
+#pragma unroll
+    for (uint32_t b = 0; b < 4; b++) prefix = (prefix << 8) | (b < clen ? norm_byte(r.cmp, content, b) : 0u);
+  }
+  const int32_t p = r.hash_partition
+                        ? (int32_t)((uint32_t)(key_hash_dev(r.cmp, key, klen) & 0x7fffffff) % (uint32_t)r.num_partitions)
+                        : given;
+  return compose_sort_word(r, p, prefix, bad);
+}
+
+// One thread per record: its sort word (stage_sort_word, or inline for 16-byte fixed keys) and the digit histograms of
+// all four radix passes (so the sort never re-reads the keys for counting).
 template <bool FAST16>
 __global__ void __launch_bounds__(256) k_stage(Records r, uint32_t *__restrict__ keys_out, uint32_t *__restrict__ hist,
                                                int *__restrict__ error_flag) {
@@ -126,12 +184,13 @@ __global__ void __launch_bounds__(256) k_stage(Records r, uint32_t *__restrict__
   __syncthreads();
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += stride) {
-    uint32_t prefix;
-    int32_t p;
+    uint32_t K;
+    bool bad;
     if (FAST16) {
       // fixed 16-byte keys on a 16-byte aligned stride (config C2): one 128-bit load per record
       const uint4 kq = *reinterpret_cast<const uint4 *>(r.kv + (uint64_t)i * (r.klen + r.vlen));
-      prefix = __byte_perm(kq.x, 0, 0x0123);
+      const uint32_t prefix = __byte_perm(kq.x, 0, 0x0123);
+      int32_t p;
       if (r.hash_partition) {
         uint32_t h = 1;
         const uint32_t w[4] = {kq.x, kq.y, kq.z, kq.w};
@@ -141,6 +200,7 @@ __global__ void __launch_bounds__(256) k_stage(Records r, uint32_t *__restrict__
       } else {
         p = r.partition ? r.partition[i] : 0;
       }
+      K = compose_sort_word(r, p, prefix, bad);
     } else {
       uint64_t koff;
       uint32_t klen, vlen;
@@ -165,29 +225,10 @@ __global__ void __launch_bounds__(256) k_stage(Records r, uint32_t *__restrict__
       } else {
         record_lookup(r, i, koff, klen, vlen);
       }
-      const uint8_t *key = r.kv + koff;
-      uint32_t skip = key_content_skip(r.cmp, key, klen);
-      const uint8_t *content = key + skip;
-      uint32_t clen = klen - skip;
-      prefix = 0;
-      if (r.sym) {   // packed ranks: already a (32 - pbits)-bit value, shifted up so that the common `>> pbits` below fits
-        const SymTable *__restrict__ st = r.sym;
-        const uint32_t np = st->npos;
-        for (uint32_t q = 0; q < np && q < clen; q++) prefix |= (uint32_t)st->rank[q][norm_byte(r.cmp, content, q)] << st->shift[q];
-        prefix <<= r.pbits;
-      } else {
-#pragma unroll
-        for (uint32_t b = 0; b < 4; b++) prefix = (prefix << 8) | (b < clen ? norm_byte(r.cmp, content, b) : 0u);
-      }
-      p = r.hash_partition ? (int32_t)((uint32_t)(key_hash_dev(r.cmp, key, klen) & 0x7fffffff) % (uint32_t)r.num_partitions)
-                           : ((r.fixed && r.use_runs) ? run_part : (r.partition ? r.partition[i] : 0));
+      const int32_t given = r.hash_partition ? 0 : ((r.fixed && r.use_runs) ? run_part : (r.partition ? r.partition[i] : 0));
+      K = stage_sort_word(r, r.kv + koff, klen, given, bad);
     }
-    if (p < 0 || p >= r.num_partitions) {
-      atomicOr(error_flag, 1);  // "Illegal partition" (PipelinedSorter.java:410-413)
-      p = 0;
-    }
-    if (r.unordered) prefix = 0;
-    uint32_t K = r.pbits ? (((uint32_t)p << (32 - r.pbits)) | (prefix >> r.pbits)) : prefix;
+    if (bad) atomicOr(error_flag, 1);  // "Illegal partition" (PipelinedSorter.java:410-413)
     keys_out[r.unordered ? r.n - 1u - i : i] = K;
 #pragma unroll
     for (int q = 0; q < 4; q++) atomicAdd(&s_hist[q * RADIX + ((K >> (8 * q)) & 0xFF)], 1u);

@@ -384,6 +384,44 @@ int32_t tezgpu_debug_inflate_emulate(const uint8_t *z, uint64_t len, uint64_t bo
   TG_API_END
 }
 
+int32_t tezgpu_debug_sort_words_emulate(const uint8_t *kv, const uint64_t *key_off, const uint32_t *key_len, uint32_t n,
+                                        int32_t comparator, int32_t num_partitions, const int32_t *partition,
+                                        int32_t use_sym, uint32_t *words, uint32_t *npos, int32_t *sym_used) {
+  TG_API_BEGIN
+  TG_CHECK((kv || n == 0) && ((key_off && key_len) || n == 0) && (words || n == 0) && npos && sym_used, TEZGPU_E_INVALID,
+           "null argument");
+  TG_CHECK(comparator >= TEZGPU_CMP_BYTES && comparator <= TEZGPU_CMP_LONG, TEZGPU_E_UNSUPPORTED, "unknown comparator");
+  const int pbits = partition_bits(num_partitions);
+  TG_CHECK(num_partitions >= 1 && pbits <= 31, TEZGPU_E_INVALID, "num_partitions out of range");
+  Records r;
+  memset(&r, 0, sizeof(r));
+  r.kv = kv;
+  r.n = n;
+  r.cmp = comparator;
+  r.hash_partition = partition == nullptr;
+  r.num_partitions = num_partitions;
+  r.pbits = pbits;
+  // k_symbols: which normalised byte values occur at each of the first SYM_MAX_POS content positions
+  uint32_t sets[SYM_MAX_POS * 8] = {0};
+  for (uint32_t i = 0; i < n; i++) {
+    const uint8_t *key = kv + key_off[i];
+    const uint32_t skip = key_content_skip(comparator, key, key_len[i]);
+    for (uint32_t q = 0; q < (uint32_t)SYM_MAX_POS && q < key_len[i] - skip; q++) {
+      const uint32_t b = norm_byte(comparator, key + skip, q);
+      sets[q * 8 + (b >> 5)] |= 1u << (b & 31u);
+    }
+  }
+  SymTable *t = new SymTable();
+  *npos = n ? sym_table_build(sets, pbits, t) : 0;
+  *sym_used = (n && use_sym && sym_table_pays(*npos, pbits)) ? 1 : 0;
+  r.sym = *sym_used ? t : nullptr;
+  bool bad = false;
+  for (uint32_t i = 0; i < n && !bad; i++) words[i] = stage_sort_word(r, kv + key_off[i], key_len[i], partition ? partition[i] : 0, bad);
+  delete t;
+  TG_CHECK(!bad, TEZGPU_E_INVALID, "Illegal partition (outside [0, numPartitions))");
+  TG_API_END
+}
+
 // ------------------------------------------------------------------------------------------------ NVLink peer fetch
 int32_t tezgpu_peer_alloc(int32_t device, uint64_t bytes, void **dptr, uint8_t *handle_out) {
   TG_API_BEGIN
