@@ -113,9 +113,18 @@ typedef struct tezgpu_merger tezgpu_merger;
 /* Codec of the IFile segments (tez.runtime.compress / tez.runtime.compress.codec, SORT/IFile.java:351-420): with
  * DEFAULT (org.apache.hadoop.io.compress.DefaultCodec, RL/common/ConfigUtils.java:44-66) a segment is 'T','I','F',1, one
  * zlib stream (RFC 1950) of the uncompressed body, and the CRC-32 of the compressed bytes; its index triple keeps the
- * uncompressed rawLength and has the compressed segment length as partLength.  Other codecs are not on the device. */
+ * uncompressed rawLength and has the compressed segment length as partLength.  With LZ4
+ * (org.apache.hadoop.io.compress.Lz4Codec) the stream between header and CRC is Hadoop's BlockCompressorStream
+ * framing: blocks of a big-endian int32 raw length and one or more chunks, each a big-endian int32 compressed length
+ * and one raw LZ4 block.  The device writes blocks of TEZGPU_LZ4_BLOCK_BYTES raw bytes (the last one shorter), one
+ * chunk each, no chunk longer than TEZGPU_LZ4_CHUNK_BOUND; a Java reader needs io.compression.codec.lz4.buffersize of
+ * at least that.  The device reader takes chunks that decode to at most 262,144 bytes (the default buffersize).
+ * Other codecs are not on the device. */
 #define TEZGPU_CODEC_NONE 0
 #define TEZGPU_CODEC_DEFAULT 1
+#define TEZGPU_CODEC_LZ4 2
+#define TEZGPU_LZ4_BLOCK_BYTES 65024
+#define TEZGPU_LZ4_CHUNK_BOUND (TEZGPU_LZ4_BLOCK_BYTES + TEZGPU_LZ4_BLOCK_BYTES / 255 + 16) /* LZ4_compressBound */
 
 const char *tezgpu_last_error(void);
 int32_t tezgpu_abi_version(void);
@@ -176,7 +185,7 @@ int32_t tezgpu_sorter_set_combiner(tezgpu_sorter *h, int32_t combiner);
 /* writes every segment through the codec (TEZGPU_CODEC_*) in flush, flush_to_memory and sort_device_fixed, after the
  * combiner when one is set; unordered handles too (UnorderedPartitionedKVWriter writes through the codec).  Call before
  * the first collect (or right after a reset); survives reset.  With a codec, tezgpu_sorter_output_bound includes the
- * worst case (every 32 KiB chunk stored), stats.output_bytes_physical / file_out_bytes count compressed bytes,
+ * worst case (every 32 KiB zlib chunk stored; every LZ4 block all literals), stats.output_bytes_physical / file_out_bytes count compressed bytes,
  * output_bytes_with_overhead is still the sum of rawLength, and ms_total includes the compression (ms_emit does not).
  * TEZGPU_E_UNSUPPORTED for any other codec. */
 int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec);
@@ -214,7 +223,8 @@ int32_t tezgpu_merge_reopen(tezgpu_merger *m, const tezgpu_segment *segs, uint32
  * ShuffleHeader uncompressedLength): required for segments whose header flag is 1 (TEZGPU_E_INVALID without it), ignored
  * for the others; raw_len may be NULL when none is compressed.  Compressed and uncompressed segments may be mixed.  A
  * compressed segment's CRC is checked on the compressed bytes (unless TEZGPU_SEG_VERIFIED), its body must inflate to
- * exactly raw_len[i] - 4 bytes (one or more complete zlib streams), else TEZGPU_E_FORMAT naming the segment.  Every
+ * exactly raw_len[i] - 4 bytes (DEFAULT: one or more complete zlib streams; LZ4: blocks of raw length > 0 whose chunks decode to
+ * exactly that length, adding up to raw_len[i] - 4, nothing after the last block), else TEZGPU_E_FORMAT naming the segment.  Every
  * tezgpu_merge_write_* of the handle writes through the same codec (PipelinedSorter's final merge, :774-836).
  * TEZGPU_CODEC_NONE behaves exactly like open / reopen. */
 int32_t tezgpu_merge_open_codec(const tezgpu_conf *conf, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg,
@@ -343,6 +353,11 @@ uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks);
 int32_t tezgpu_debug_deflate_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len);
 int32_t tezgpu_debug_inflate_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
                                      uint64_t *out_len);
+/* the same for TEZGPU_CODEC_LZ4: lz4_compress gives the block stream the device writes for one body; lz4_decompress runs
+ * the device reader's exact (serial) path over a stream that must yield exactly body_len bytes. */
+int32_t tezgpu_debug_lz4_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len);
+int32_t tezgpu_debug_lz4_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
+                                            uint64_t *out_len);
 
 /* diagnostics: the 32-bit sort words the variable-width map side gives n keys (key i = kv[key_off[i] ..
  * key_off[i] + key_len[i])), computed on the host with the device's code: the alphabet table built from the byte values

@@ -1,18 +1,27 @@
-// codec.cuh -- DefaultCodec on both sides of the shuffle: the compress phase behind every emit (SortPipeline) and the
-// inflate step in front of every merge open (Merger).  Formats and kernels: deflate.cuh, inflate.cuh.
+// codec.cuh -- DefaultCodec and Lz4Codec on both sides of the shuffle: the compress phase behind every emit
+// (SortPipeline) and the decompress step in front of every merge open (Merger).  Formats and kernels: deflate.cuh,
+// inflate.cuh (DefaultCodec), lz4.cuh (Lz4Codec).  The two codecs share the chunk layout, the size scan, the pack and
+// the checksum kernels; only the chunk kernels and the segment finish differ.
 #pragma once
 #include "inflate.cuh"
+#include "lz4.cuh"
 #include "merger.cuh"
 
 namespace tezgpu {
 
 // The uncompressed file is in z_img with its index raw_index (start, rawLength, partLength per partition).  Every
-// partition that has a segment gets a compressed one: TIF\x01, the zlib stream of the same body, CRC-32 of the stream.
-// index receives (start, the same rawLength, compressed length).  One host round trip (the compressed layout).
+// partition that has a segment gets a compressed one: TIF\x01, the codec stream of the same body (zlib, or LZ4 blocks),
+// CRC-32 of the stream.  index receives (start, the same rawLength, compressed length).  One host round trip (the
+// compressed layout).
 inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len,
                                          int64_t *index, tezgpu_stats *stats) {
   const int P = conf.num_partitions;
   cudaStream_t st = stream;
+  // zlib: 32 KiB chunks, framed by TIF\x01 78 01 | chunks | Adler-32 CRC; LZ4: blocks of one chunk each (their 8 header
+  // bytes in the slot), framed by TIF\x01 | blocks | CRC
+  const bool lz4 = codec == TEZGPU_CODEC_LZ4;
+  const uint64_t chunk = lz4 ? L4_BLOCK : ZCHUNK;
+  const uint32_t slot = lz4 ? L4_SLOT : ZSLOT, frame = lz4 ? 8 : 14, head = lz4 ? 4 : 6, tail = lz4 ? 0 : 4;
   z_timer.reset();
   z_timer.mark(st);
   z_host.ensure((size_t)P * sizeof(ZSeg) + 64);
@@ -28,7 +37,7 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     if (part > 0) {
       s.body_off = (uint64_t)start + 4;
       s.body_len = (uint64_t)part - 8;
-      s.nchunks = (uint32_t)std::max<uint64_t>(1, div_up(s.body_len, ZCHUNK));
+      s.nchunks = (uint32_t)std::max<uint64_t>(1, div_up(s.body_len, chunk));
       nchunks += s.nchunks;
       nsegs++;
     }
@@ -38,23 +47,29 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
   if (nchunks) {
     z_segs.ensure((size_t)P * sizeof(ZSeg));
     TG_CUDA(cudaMemcpyAsync(z_segs.p, hs, (size_t)P * sizeof(ZSeg), cudaMemcpyHostToDevice, st));
-    z_slots.ensure((size_t)nchunks * ZSLOT);
+    z_slots.ensure((size_t)nchunks * slot);
     z_csize.ensure((size_t)nchunks * 4);
-    z_cadler.ensure((size_t)nchunks * 4);
     z_coff.ensure(((size_t)nchunks + 2) * 8);
-    static bool attr[64] = {};   // the attribute is per device
-    if (!attr[conf.device & 63]) {
-      TG_CUDA(cudaFuncSetAttribute(k_zdeflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZShared)));
-      attr[conf.device & 63] = true;
+    static bool attr[2][64] = {};   // the attribute is per device
+    if (!attr[lz4][conf.device & 63]) {
+      if (lz4) TG_CUDA(cudaFuncSetAttribute(k_l4compress, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(L4Shared)));
+      else TG_CUDA(cudaFuncSetAttribute(k_zdeflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZShared)));
+      attr[lz4][conf.device & 63] = true;
     }
-    k_zdeflate<<<nchunks, ZLANES, sizeof(ZShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
-                                                        z_csize.as<uint32_t>(), z_cadler.as<uint32_t>());
+    if (lz4) {
+      k_l4compress<<<nchunks, L4_LANES, sizeof(L4Shared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
+                                                               z_csize.as<uint32_t>());
+    } else {
+      z_cadler.ensure((size_t)nchunks * 4);
+      k_zdeflate<<<nchunks, ZLANES, sizeof(ZShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
+                                                          z_csize.as<uint32_t>(), z_cadler.as<uint32_t>());
+    }
     const uint32_t nblk = (uint32_t)div_up(nchunks, SCAN_TILE);
     blk.ensure(((size_t)nblk + 2) * 8);
     k_sum_u32_blocks<<<nblk, SCAN_THREADS, 0, st>>>(z_csize.as<uint32_t>(), nchunks, blk.as<uint64_t>());
     k_scan_block_sums<<<1, 1024, 0, st>>>(blk.as<uint64_t>(), nblk);
     k_scan_u32_apply<<<nblk, SCAN_THREADS, 0, st>>>(z_csize.as<uint32_t>(), nchunks, blk.as<uint64_t>(), z_coff.as<uint64_t>());
-    k_zseg_layout<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_coff.as<uint64_t>());
+    k_zseg_layout<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_coff.as<uint64_t>(), frame);
     launches += 5;
     TG_CUDA(cudaGetLastError());
     TG_CUDA(cudaMemcpyAsync(hs, z_segs.p, (size_t)P * sizeof(ZSeg), cudaMemcpyDeviceToHost, st));
@@ -63,7 +78,7 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     TG_CUDA(cudaStreamSynchronize(st));
     uint64_t cbytes;
     memcpy(&cbytes, reinterpret_cast<uint8_t *>(hs) + (size_t)P * sizeof(ZSeg), 8);
-    total = cbytes + 14 * nsegs;
+    total = cbytes + frame * nsegs;
     TG_CHECK(total <= out_cap, TEZGPU_E_NOMEM, "output buffer too small for the compressed file.out");
     // checksums of the chunks (k_crc_pieces, one piece per chunk), placed in their segments and folded per segment
     const CrcTables *d_crc = DeviceConstants::get(conf.device).d_crc;
@@ -72,16 +87,20 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     z_tc.ensure((size_t)nchunks * sizeof(TileCrc));
     z_crc.ensure((size_t)P * 4);
     TG_CUDA(cudaMemsetAsync(z_crc.p, 0, (size_t)P * 4, st));
-    k_zchunk_descs<SegDesc><<<(uint32_t)div_up((uint64_t)nchunks + 1, 256), 256, 0, st>>>(z_csize.as<uint32_t>(), nchunks, z_descs.as<SegDesc>(),
-                                                                                       z_pstart.as<uint32_t>());
+    k_zchunk_descs<SegDesc><<<(uint32_t)div_up((uint64_t)nchunks + 1, 256), 256, 0, st>>>(z_csize.as<uint32_t>(), nchunks, slot,
+                                                                                       z_descs.as<SegDesc>(), z_pstart.as<uint32_t>());
     k_crc_pieces<<<nchunks, CRCV_THREADS, 0, st>>>(z_slots.as<uint8_t>(), z_descs.as<SegDesc>(), z_pstart.as<uint32_t>(), nchunks, d_crc,
                                                    z_tc.as<TileCrc>());
     k_zcrc_place<TileCrc><<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, z_segs.as<ZSeg>(), (uint32_t)P,
-                                                                         z_coff.as<uint64_t>());
+                                                                         z_coff.as<uint64_t>(), tail);
     k_crc_combine<<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, d_crc, z_crc.as<uint32_t>());
-    k_zpack<<<nchunks, 256, 0, st>>>(z_slots.as<uint8_t>(), z_csize.as<uint32_t>(), z_coff.as<uint64_t>(), z_segs.as<ZSeg>(), (uint32_t)P, d_out);
-    k_zfinish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_cadler.as<uint32_t>(), z_csize.as<uint32_t>(),
-                                                       z_crc.as<uint32_t>(), d_crc, d_out);
+    k_zpack<<<nchunks, 256, 0, st>>>(z_slots.as<uint8_t>(), z_csize.as<uint32_t>(), z_coff.as<uint64_t>(), z_segs.as<ZSeg>(), (uint32_t)P,
+                                     slot, head, d_out);
+    if (lz4)
+      k_l4finish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_crc.as<uint32_t>(), d_crc, d_out);
+    else
+      k_zfinish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_cadler.as<uint32_t>(), z_csize.as<uint32_t>(),
+                                                         z_crc.as<uint32_t>(), d_crc, d_out);
     launches += 6;
     TG_CUDA(cudaGetLastError());
   }
@@ -106,7 +125,9 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
 }
 
 // Compressed segments (TIF\x01 with a codec set) are staged, their CRC checked (unless the transport verified it),
-// inflated into images TIF\x00 + body + 4 bytes that the merge reads as verified ordinary segments.  Every other segment
+// decompressed into images TIF\x00 + body + 4 bytes that the merge reads as verified ordinary segments.  zlib: one warp
+// per segment.  LZ4: one thread per segment walks the block headers (one host round trip for the block count), one warp
+// per block decodes, and a segment the block pass could not take is decoded again serially by one warp.  Every other segment
 // goes to open() unchanged, so errors keep naming the caller's segment index.
 inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg) {
   if (!pipe.codec) { open(in, nseg); return; }
@@ -189,7 +210,34 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
     k_crc_check<<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_in.as<uint8_t>(), z_descs.as<SegDesc>(), nz, z_crc.as<uint32_t>(), d_crc, z_flag.as<int>());
     launches += 3;
   }
-  k_zinflate<<<(uint32_t)div_up(nz, ZINF_WARPS), ZINF_WARPS * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_status.as<int32_t>());
+  const bool lz4 = pipe.codec == TEZGPU_CODEC_LZ4;
+  if (lz4) {
+    z_nblk.ensure((size_t)nz * 4);
+    z_slow.ensure((size_t)nz * 4);
+    TG_CUDA(cudaMemsetAsync(z_slow.p, 0, (size_t)nz * 4, st));
+    k_l4walk<0><<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), nullptr, nullptr);
+    launches++;
+    TG_CUDA(cudaGetLastError());
+    std::vector<uint32_t> nblk(nz), base(nz);
+    TG_CUDA(cudaMemcpyAsync(nblk.data(), z_nblk.p, (size_t)nz * 4, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaStreamSynchronize(st));
+    uint64_t nb = 0;
+    for (uint32_t i = 0; i < nz; i++) { base[i] = (uint32_t)nb; nb += nblk[i]; }
+    TG_CHECK(nb < (1ull << 32), TEZGPU_E_INVALID, "too many LZ4 blocks in one merge");
+    if (nb) {
+      z_base.ensure((size_t)nz * 4);
+      z_blks.ensure((size_t)nb * sizeof(L4Blk));
+      TG_CUDA(cudaMemcpyAsync(z_base.p, base.data(), (size_t)nz * 4, cudaMemcpyHostToDevice, st));
+      k_l4walk<1><<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), z_base.as<uint32_t>(),
+                                                            z_blks.as<L4Blk>());
+      k_l4blocks<<<(uint32_t)div_up(nb, L4DEC_WARPS), L4DEC_WARPS * 32, 0, st>>>(z_blks.as<L4Blk>(), (uint32_t)nb, z_slow.as<int32_t>());
+      launches += 2;
+    }
+    k_l4serial<<<(uint32_t)div_up(nz, L4DEC_WARPS), L4DEC_WARPS * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(),
+                                                                              z_slow.as<int32_t>(), z_status.as<int32_t>());
+  } else {
+    k_zinflate<<<(uint32_t)div_up(nz, ZINF_WARPS), ZINF_WARPS * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_status.as<int32_t>());
+  }
   launches++;
   TG_CUDA(cudaGetLastError());
   std::vector<int32_t> status(nz);
@@ -200,7 +248,7 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
   TG_CHECK(bad_crc == 0, TEZGPU_E_FORMAT, "IFile checksum mismatch in segment " + std::to_string(bad_crc ? zs[bad_crc - 1] : 0));
   for (uint32_t i = 0; i < nz; i++)
     TG_CHECK(status[i] == Z_OK, TEZGPU_E_FORMAT,
-             std::string("compressed segment ") + std::to_string(zs[i]) + ": " + z_err_name(status[i]));
+             std::string("compressed segment ") + std::to_string(zs[i]) + ": " + (lz4 ? l4_err_name(status[i]) : z_err_name(status[i])));
   std::vector<tezgpu_segment> segs2(in, in + nseg);
   for (uint32_t i = 0; i < nz; i++) {
     tezgpu_segment &sg = segs2[zs[i]];
@@ -227,6 +275,13 @@ static inline std::vector<uint8_t> z_deflate_host(const uint8_t *body, uint64_t 
   delete sh;
   for (int b = 3; b >= 0; b--) out.push_back((uint8_t)(adler >> (8 * b)));
   return out;
+}
+
+// worst case of the compressed file given the uncompressed file's bound.  zlib: every chunk stored.  LZ4: every block
+// all literals (one token, (n - 15) / 255 + 1 length bytes) plus its 8 header bytes.
+inline uint64_t SortPipeline::codec_bound(int codec, uint64_t raw_bound, int P) {
+  if (codec == TEZGPU_CODEC_LZ4) return raw_bound + raw_bound / 255 + 10 * (raw_bound / L4_BLOCK + (uint64_t)P + 1) + 64;
+  return raw_bound + 5 * (raw_bound / ZCHUNK + (uint64_t)P + 1) + 11ull * P + 64;
 }
 
 }  // namespace tezgpu

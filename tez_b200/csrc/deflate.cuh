@@ -518,16 +518,16 @@ __global__ void __launch_bounds__(ZLANES)
   if (tid == 0) { csize[c] = sh.bytes; cadler[c] = sh.adler; }
 }
 
-// chunk descriptors for k_crc_pieces (one piece per chunk: a chunk is < CRC_PIECE bytes)
+// chunk descriptors for k_crc_pieces (one piece per chunk: a chunk is < CRC_PIECE bytes); slot: bytes per chunk slot
 template <typename SegDescT>
-__global__ void k_zchunk_descs(const uint32_t *__restrict__ csize, uint32_t nchunks, SegDescT *__restrict__ descs,
+__global__ void k_zchunk_descs(const uint32_t *__restrict__ csize, uint32_t nchunks, uint32_t slot, SegDescT *__restrict__ descs,
                                uint32_t *__restrict__ piece_start) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c > nchunks) return;
   piece_start[c] = c;
   if (c == nchunks) return;
   SegDescT d;
-  d.off = (uint64_t)c * ZSLOT;
+  d.off = (uint64_t)c * slot;
   d.len = csize[c] + 4;
   d.body0 = 0;
   d.body_end = csize[c];
@@ -536,34 +536,35 @@ __global__ void k_zchunk_descs(const uint32_t *__restrict__ csize, uint32_t nchu
   descs[c] = d;
 }
 
-// per partition: file offset and length of its compressed segment
-__global__ void k_zseg_layout(ZSeg *__restrict__ segs, uint32_t P, const uint64_t *__restrict__ coff) {
+// per partition: file offset and length of its compressed segment; frame: bytes of a segment outside its chunks
+__global__ void k_zseg_layout(ZSeg *__restrict__ segs, uint32_t P, const uint64_t *__restrict__ coff, uint32_t frame) {
   const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= P) return;
   ZSeg &s = segs[p];
-  s.zstart = coff[s.chunk0] + 14 * s.rank;
-  s.zlen = s.nchunks ? coff[s.chunk0 + s.nchunks] - coff[s.chunk0] + 14 : 0;
+  s.zstart = coff[s.chunk0] + frame * s.rank;
+  s.zlen = s.nchunks ? coff[s.chunk0 + s.nchunks] - coff[s.chunk0] + frame : 0;
 }
 
-// chunk checksums -> positions in their segment's checksummed bytes (zlib header, chunks, Adler-32)
+// chunk checksums -> positions in their segment's checksummed bytes (zlib: header, chunks, Adler-32; LZ4: the chunks);
+// tail: checksummed bytes after the last chunk
 template <typename TileCrcT>
 __global__ void k_zcrc_place(TileCrcT *__restrict__ tc, uint32_t nchunks, const ZSeg *__restrict__ segs, uint32_t P,
-                             const uint64_t *__restrict__ coff) {
+                             const uint64_t *__restrict__ coff, uint32_t tail) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= nchunks) return;
   const uint32_t p = z_chunk_part(segs, P, c);
   const ZSeg s = segs[p];
   tc[c].p = p;
-  tc[c].after = coff[s.chunk0 + s.nchunks] - coff[c + 1] + 4;
+  tc[c].after = coff[s.chunk0 + s.nchunks] - coff[c + 1] + tail;
 }
 
-// one CTA per chunk: the chunk's bytes into the file
+// one CTA per chunk: the chunk's bytes into the file (slot: bytes per chunk slot; head: segment bytes before the chunks)
 __global__ void k_zpack(const uint8_t *__restrict__ slots, const uint32_t *__restrict__ csize, const uint64_t *__restrict__ coff,
-                        const ZSeg *__restrict__ segs, uint32_t P, uint8_t *__restrict__ out) {
+                        const ZSeg *__restrict__ segs, uint32_t P, uint32_t slot, uint32_t head, uint8_t *__restrict__ out) {
   const uint32_t c = blockIdx.x;
   const ZSeg s = segs[z_chunk_part(segs, P, c)];
-  uint8_t *dst = out + s.zstart + 6 + (coff[c] - coff[s.chunk0]);
-  const uint8_t *src = slots + (uint64_t)c * ZSLOT;
+  uint8_t *dst = out + s.zstart + head + (coff[c] - coff[s.chunk0]);
+  const uint8_t *src = slots + (uint64_t)c * slot;
   const uint32_t n = csize[c];
   for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
 }

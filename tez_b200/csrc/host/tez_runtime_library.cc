@@ -67,6 +67,8 @@ static const char *K_REPORT_STATS = "tez.runtime.report.partition.stats";       
 static const char *K_COMPRESS = "tez.runtime.compress";
 static const char *K_COMPRESS_CODEC = "tez.runtime.compress.codec";
 static const char *DEFAULT_CODEC = "org.apache.hadoop.io.compress.DefaultCodec";
+static const char *LZ4_CODEC = "org.apache.hadoop.io.compress.Lz4Codec";
+static const char *K_LZ4_BUFFERSIZE = "io.compression.codec.lz4.buffersize";   // CommonConfigurationKeys, default 256 KiB
 static const char *K_SERIALIZATIONS = "io.serializations";
 static const char *K_VALUE_CLASS = "tez.runtime.value.class";
 static const char *K_COMBINER_CLASS = "tez.runtime.combiner.class";
@@ -189,15 +191,26 @@ static std::vector<uint8_t> roaring_serialize(const std::vector<uint32_t> &vals)
   return o;
 }
 
-// tez.runtime.compress / tez.runtime.compress.codec (IFile.Writer / Reader via CodecUtils.getCodec): DefaultCodec runs on
-// the device, any other class is refused by name.  Deviation from Tez: with compression on and no codec named, Tez uses
-// DefaultCodec; here that configuration keeps being refused (DESIGN.md 9).
+// tez.runtime.compress / tez.runtime.compress.codec (IFile.Writer / Reader via CodecUtils.getCodec): DefaultCodec and
+// Lz4Codec run on the device, any other class is refused by name.  Deviation from Tez: with compression on and no codec
+// named, Tez uses DefaultCodec; here that configuration keeps being refused (DESIGN.md 9).  Lz4Codec: Java's
+// Lz4Decompressor decodes each chunk into a buffer of io.compression.codec.lz4.buffersize bytes, so a buffer smaller
+// than the device writer's worst-case chunk (TEZGPU_LZ4_CHUNK_BOUND) could not read the device's output, and Java
+// writers with a buffer over 262,144 bytes write chunks the device reader refuses: both are refused by key name.
 static int codec_for(const Configuration &conf) {
   if (!conf.getBoolean(K_COMPRESS, false)) return TEZGPU_CODEC_NONE;
   const std::string codec = conf.get(K_COMPRESS_CODEC, "");
   RT_CHECK(!codec.empty(), TEZGPU_E_UNSUPPORTED, "tez.runtime.compress=true: IFile codecs are not supported on the device path yet");
+  if (codec == LZ4_CODEC) {
+    const long buf = conf.getInt(K_LZ4_BUFFERSIZE, 256 * 1024);
+    RT_CHECK(buf >= TEZGPU_LZ4_CHUNK_BOUND && buf <= 256 * 1024, TEZGPU_E_UNSUPPORTED,
+             std::string(K_LZ4_BUFFERSIZE) + "=" + std::to_string(buf) + ": the device path needs " +
+                 std::to_string(TEZGPU_LZ4_CHUNK_BOUND) + " to 262144 bytes with " + LZ4_CODEC);
+    return TEZGPU_CODEC_LZ4;
+  }
   RT_CHECK(codec == DEFAULT_CODEC, TEZGPU_E_UNSUPPORTED,
-           std::string(K_COMPRESS_CODEC) + "=" + codec + ": only " + DEFAULT_CODEC + " is supported on the device path");
+           std::string(K_COMPRESS_CODEC) + "=" + codec + ": only " + DEFAULT_CODEC + " and " + LZ4_CODEC +
+               " are supported on the device path");
   return TEZGPU_CODEC_DEFAULT;
 }
 

@@ -776,11 +776,12 @@ class Merger {
 
   uint64_t raw_output_bound() const { return SortPipeline::output_bound(n, kv_bytes, pipe.conf.num_partitions) + 16; }
   uint64_t output_bound() const {
-    return pipe.codec ? SortPipeline::codec_bound(raw_output_bound(), pipe.conf.num_partitions) : raw_output_bound();
+    return pipe.codec ? SortPipeline::codec_bound(pipe.codec, raw_output_bound(), pipe.conf.num_partitions) : raw_output_bound();
   }
 
-  // ---- codec (codec.cuh): compressed segments are checked, inflated into z_img and merged as ordinary segments
+  // ---- codec (codec.cuh): compressed segments are checked, decompressed into z_img and merged as ordinary segments
   DeviceBuffer z_in, z_img, z_insegs, z_status, z_descs, z_pstart, z_tc, z_crc, z_flag;
+  DeviceBuffer z_nblk, z_base, z_blks, z_slow;   // LZ4: blocks per segment, their first index, the blocks, serial-path flags
   void open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg);
 
   // the writer behind write_*: TezMerger.writeFile semantics, or -- with a combiner -- the combined records, which carry

@@ -236,14 +236,14 @@ class SortPipeline {
     emit_out(rle, false, raw_bound, d_out, out_cap, out_len, index, stats);
   }
 
-  // ---- codec (deflate.cuh, codec.cuh): with TEZGPU_CODEC_DEFAULT the emit writes the uncompressed file into z_img and
-  // compress_image turns every segment into a zlib-compressed one in d_out
+  // ---- codec (deflate.cuh, lz4.cuh, codec.cuh): with a codec the emit writes the uncompressed file into z_img and
+  // compress_image turns every segment into a compressed one (zlib or LZ4) in d_out
   int codec = TEZGPU_CODEC_NONE;
   DeviceBuffer z_img, z_slots, z_csize, z_cadler, z_coff, z_segs, z_descs, z_pstart, z_tc, z_crc;
   PinnedBuffer z_host;
   EventTimer z_timer;
-  // worst case of the compressed file given the uncompressed file's bound: every chunk stored
-  static uint64_t codec_bound(uint64_t raw_bound, int P) { return raw_bound + 5 * (raw_bound / ZCHUNK + (uint64_t)P + 1) + 11ull * P + 64; }
+  // worst case of the compressed file given the uncompressed file's bound (codec.cuh)
+  static uint64_t codec_bound(int codec, uint64_t raw_bound, int P);
   void compress_image(const int64_t *raw_index, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index, tezgpu_stats *stats);
 
   // the emit of the sorted (merged) records: combined or not, compressed or not.  raw_bound bounds the uncompressed file.

@@ -252,7 +252,7 @@ static uint64_t sorter_raw_bound(const tezgpu_sorter *h) {
 uint64_t tezgpu_sorter_output_bound(const tezgpu_sorter *h) {
   if (!h) return 0;
   const uint64_t raw = sorter_raw_bound(h);
-  return h->pipe.codec ? SortPipeline::codec_bound(raw, h->pipe.conf.num_partitions) : raw;
+  return h->pipe.codec ? SortPipeline::codec_bound(h->pipe.codec, raw, h->pipe.conf.num_partitions) : raw;
 }
 
 static void sorter_run(tezgpu_sorter *h, uint8_t *host_out, uint64_t out_cap, uint64_t *out_len, int64_t *index,
@@ -353,8 +353,8 @@ int32_t tezgpu_sorter_set_combiner(tezgpu_sorter *h, int32_t combiner) {
 int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec) {
   TG_API_BEGIN
   TG_CHECK(h, TEZGPU_E_INVALID, "null handle");
-  TG_CHECK(codec == TEZGPU_CODEC_NONE || codec == TEZGPU_CODEC_DEFAULT, TEZGPU_E_UNSUPPORTED,
-           "codec " + std::to_string(codec) + " is not on the device (DefaultCodec only)");
+  TG_CHECK(codec == TEZGPU_CODEC_NONE || codec == TEZGPU_CODEC_DEFAULT || codec == TEZGPU_CODEC_LZ4, TEZGPU_E_UNSUPPORTED,
+           "codec " + std::to_string(codec) + " is not on the device (DefaultCodec and Lz4Codec only)");
   TG_CHECK(h->n == 0 && !h->flushed, TEZGPU_E_STATE, "set the codec before the first collect (or after a reset)");
   h->pipe.codec = codec;
   TG_API_END
@@ -381,6 +381,28 @@ int32_t tezgpu_debug_inflate_emulate(const uint8_t *z, uint64_t len, uint64_t bo
   delete w;
   *out_len = got;
   TG_CHECK(rc == Z_OK, TEZGPU_E_FORMAT, std::string("compressed segment 0: ") + z_err_name(rc));
+  TG_API_END
+}
+
+int32_t tezgpu_debug_lz4_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len) {
+  TG_API_BEGIN
+  TG_CHECK((body || len == 0) && out && out_len, TEZGPU_E_INVALID, "null argument");
+  const std::vector<uint8_t> z = l4_compress_host(body, len);
+  *out_len = z.size();
+  TG_CHECK(z.size() <= cap, TEZGPU_E_NOMEM, "output buffer too small");
+  memcpy(out, z.data(), z.size());
+  TG_API_END
+}
+
+int32_t tezgpu_debug_lz4_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
+                                            uint64_t *out_len) {
+  TG_API_BEGIN
+  TG_CHECK((z || len == 0) && (out || body_len == 0) && out_len, TEZGPU_E_INVALID, "null argument");
+  TG_CHECK(body_len <= cap, TEZGPU_E_INVALID, "output buffer smaller than body_len");
+  uint64_t got = 0;
+  const int32_t rc = l4_decompress(z, len, out, body_len, &got);
+  *out_len = got;
+  TG_CHECK(rc == L4_OK, TEZGPU_E_FORMAT, std::string("compressed segment 0: ") + l4_err_name(rc));
   TG_API_END
 }
 

@@ -1,19 +1,23 @@
-"""DefaultCodec cost on the device: one JSON line per case, codec and no-codec runs alternating in one process.
+"""DefaultCodec and Lz4Codec cost on the device: one JSON line per case, no-codec, zlib and LZ4 runs alternating in one
+process (the *_lz4 fields are Lz4Codec's).
 
-  1. config-2 map side: 1e8 random 80-byte records, P = 64, sort_device_fixed (the stored path)
+  1. config-2 map side: 1e8 random 80-byte records, P = 64, sort_device_fixed (the stored / all-literal path)
   2. compressible map side: Text words drawn from a Zipf law with IntWritable 1 values, sort_device_fixed
-  3. reduce side: config-3 segments compressed on the host with zlib level 1, reopen + write_ifile_device
+  3. reduce side: config-3 segments compressed on the host (zlib level 1; LZ4 by the device writer's host emulation),
+     reopen + write_ifile_device
   4. e2e through host buffers: collect_batch + flush_to_memory of the case-2 records
 
 Times: host clock around fully synchronised library calls.  The card name and power limit are read in the same run.
 """
 import argparse
+import ctypes as C
 import json
 import os
 import subprocess
 import sys
 import time
 import zlib
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
@@ -30,7 +34,21 @@ def card():
 
 
 def zcap(raw, P):
-    return raw + 5 * (raw // 32768 + P + 1) + 11 * P + 64
+    """room for the zlib (every chunk stored) and the LZ4 (every block all literals) worst case"""
+    return raw + raw // 255 + 10 * (raw // 32768 + P + 1) + 11 * P + 64
+
+
+CODECS = (0, T.CODEC_LZ4, T.CODEC_DEFAULT)   # zlib last: the compressible case reads its output back
+
+
+def lz4_stream(body):
+    """the device writer's LZ4 stream of one body, run on the host (tezgpu_debug_lz4_compress_emulate)"""
+    L = T._lib.load()
+    cap = len(body) + len(body) // 255 + 10 * (len(body) // T.LZ4_BLOCK_BYTES + 2) + 64
+    out = (C.c_uint8 * cap)()
+    n = C.c_uint64()
+    T._lib.check(L.tezgpu_debug_lz4_compress_emulate(body, len(body), out, cap, C.byref(n)))
+    return bytes(out[:n.value])
 
 
 def timed(fn):
@@ -60,9 +78,9 @@ def map_side(name, kv, kl, vl, cmp_kind, P, runs, out):
     d_kv = torch.from_numpy(kv).cuda()
     raw_cap = n * (kl + vl + 2) + 10 * P + 64
     d_out = torch.empty(zcap(raw_cap, P), dtype=torch.uint8, device="cuda")
-    res = {0: [], 1: []}
+    res = {c: [] for c in CODECS}
     lens = {}
-    sorters = {c: T.GpuSorter(P, comparator=cmp_kind, fixed=(kl, vl), codec=c) for c in (0, T.CODEC_DEFAULT)}
+    sorters = {c: T.GpuSorter(P, comparator=cmp_kind, fixed=(kl, vl), codec=c) for c in CODECS}
     for r in range(runs + 1):
         for c, s in sorters.items():
             ms, (ln, index, st) = timed(lambda: s.sort_device_fixed(d_kv.data_ptr(), n, d_out.data_ptr(), d_out.numel()))
@@ -76,6 +94,11 @@ def map_side(name, kv, kl, vl, cmp_kind, P, runs, out):
                 ms_runs_no_codec=[round(x, 2) for x in res[0]], ms_runs_codec=[round(x, 2) for x in res[T.CODEC_DEFAULT]])
     extra = line["ms_codec"] - line["ms_no_codec"]
     line["compress_gbps_derived"] = round(raw / extra / 1e6, 2) if extra > 0 else None
+    llen = lens[T.CODEC_LZ4][0]
+    line.update(compressed_bytes_lz4=llen, ratio_lz4=round(llen / raw, 4), ms_lz4=round(min(res[T.CODEC_LZ4]), 2),
+                ms_runs_lz4=[round(x, 2) for x in res[T.CODEC_LZ4]])
+    extra = line["ms_lz4"] - line["ms_no_codec"]
+    line["compress_gbps_derived_lz4"] = round(raw / extra / 1e6, 2) if extra > 0 else None
     if name == "compressible":
         # zlib level 1 on the same bodies (the first 8 partitions)
         host = d_out[:zlen].cpu().numpy().tobytes()
@@ -101,13 +124,16 @@ def reduce_side(nseg, seg_bytes, runs, out):
         z = zlib.compress(p[4:-4], 1)
         zsegs.append(b"TIF\x01" + z + zlib.crc32(z).to_bytes(4, "big"))
         raws.append(len(p) - 4)
+    with ThreadPoolExecutor(16) as ex:
+        lsegs = [b"TIF\x01" + z + zlib.crc32(z).to_bytes(4, "big") for z in ex.map(lambda p: lz4_stream(p[4:-4]), plain)]
     mz = T.GpuMerger(zsegs, comparator=T.CMP_TEXT, codec=T.CODEC_DEFAULT, raw_lens=raws)
+    ml = T.GpuMerger(lsegs, comparator=T.CMP_TEXT, codec=T.CODEC_LZ4, raw_lens=raws)
     mp = T.GpuMerger(plain, comparator=T.CMP_TEXT)
-    cap = max(mz.output_bound(), mp.output_bound())
+    cap = max(mz.output_bound(), ml.output_bound(), mp.output_bound())
     d_out = torch.empty(cap, dtype=torch.uint8, device="cuda")
-    res = {0: [], 1: []}
+    res = {c: [] for c in CODECS}
     for r in range(runs + 1):
-        for c, m, segs in ((0, mp, plain), (1, mz, zsegs)):
+        for c, m, segs in ((0, mp, plain), (T.CODEC_DEFAULT, mz, zsegs), (T.CODEC_LZ4, ml, lsegs)):
             def step():
                 if c:
                     m.reopen(segs, raw_lens=raws)
@@ -121,9 +147,12 @@ def reduce_side(nseg, seg_bytes, runs, out):
     line = dict(case="reduce_c3_zlib1", segments=nseg, raw_bytes=raw_total, compressed_in_bytes=z_total,
                 ms_plain=round(min(res[0]), 2), ms_codec=round(min(res[1]), 2),
                 ms_runs_plain=[round(x, 2) for x in res[0]], ms_runs_codec=[round(x, 2) for x in res[1]],
+                compressed_in_bytes_lz4=sum(len(z) for z in lsegs), ms_lz4=round(min(res[T.CODEC_LZ4]), 2),
+                ms_runs_lz4=[round(x, 2) for x in res[T.CODEC_LZ4]],
                 note="codec: reads compressed segments and writes a compressed merged segment")
     out.append(line)
     mz.close()
+    ml.close()
     mp.close()
 
 
@@ -134,10 +163,10 @@ def e2e(kv, kl, vl, cmp_kind, P, runs, out):
     key_off = (np.arange(n, dtype=np.uint64) * stride).astype(np.uint32)
     val_off = key_off + np.uint32(kl)
     val_len = np.full(n, vl, dtype=np.uint32)
-    res = {0: [], 1: []}
+    res = {c: [] for c in CODECS}
     moved = {}
     for r in range(runs + 1):
-        for c in (0, T.CODEC_DEFAULT):
+        for c in CODECS:
             with T.GpuSorter(P, comparator=cmp_kind, codec=c) as s:
                 def step():
                     s.collect(kv, key_off, val_off, val_len)
@@ -149,7 +178,8 @@ def e2e(kv, kl, vl, cmp_kind, P, runs, out):
     out.append(dict(case="e2e_host_buffers", api="collect_batch + flush_to_memory", records=n, kv_bytes=kv.size,
                     down_bytes_no_codec=moved[0], down_bytes_codec=moved[1], ms_no_codec=round(min(res[0]), 1),
                     ms_codec=round(min(res[1]), 1), kv_gbps_no_codec=round(kv.size / min(res[0]) / 1e6, 2),
-                    kv_gbps_codec=round(kv.size / min(res[1]) / 1e6, 2)))
+                    kv_gbps_codec=round(kv.size / min(res[1]) / 1e6, 2), down_bytes_lz4=moved[T.CODEC_LZ4],
+                    ms_lz4=round(min(res[T.CODEC_LZ4]), 1), kv_gbps_lz4=round(kv.size / min(res[T.CODEC_LZ4]) / 1e6, 2)))
 
 
 def main():
