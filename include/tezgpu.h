@@ -119,12 +119,19 @@ typedef struct tezgpu_merger tezgpu_merger;
  * and one raw LZ4 block.  The device writes blocks of TEZGPU_LZ4_BLOCK_BYTES raw bytes (the last one shorter), one
  * chunk each, no chunk longer than TEZGPU_LZ4_CHUNK_BOUND; a Java reader needs io.compression.codec.lz4.buffersize of
  * at least that.  The device reader takes chunks that decode to at most 262,144 bytes (the default buffersize).
+ * With ZSTD (org.apache.hadoop.io.compress.ZStandardCodec) the stream is one or more Zstandard frames (RFC 8878).  The
+ * device writes one frame per TEZGPU_ZSTD_BLOCK_BYTES raw bytes (the last one shorter): Single_Segment with
+ * Frame_Content_Size, one block, no checksum, at most TEZGPU_ZSTD_FRAME_BOUND bytes.  The device reader takes what
+ * libzstd's default streaming decoder takes (windows up to 2^27), except dictionaries.
  * Other codecs are not on the device. */
 #define TEZGPU_CODEC_NONE 0
 #define TEZGPU_CODEC_DEFAULT 1
 #define TEZGPU_CODEC_LZ4 2
 #define TEZGPU_LZ4_BLOCK_BYTES 65024
 #define TEZGPU_LZ4_CHUNK_BOUND (TEZGPU_LZ4_BLOCK_BYTES + TEZGPU_LZ4_BLOCK_BYTES / 255 + 16) /* LZ4_compressBound */
+#define TEZGPU_CODEC_ZSTD 3
+#define TEZGPU_ZSTD_BLOCK_BYTES 65024
+#define TEZGPU_ZSTD_FRAME_BOUND (TEZGPU_ZSTD_BLOCK_BYTES + 10) /* a raw frame: magic, descriptor, 2-byte size, block header */
 
 const char *tezgpu_last_error(void);
 int32_t tezgpu_abi_version(void);
@@ -185,7 +192,7 @@ int32_t tezgpu_sorter_set_combiner(tezgpu_sorter *h, int32_t combiner);
 /* writes every segment through the codec (TEZGPU_CODEC_*) in flush, flush_to_memory and sort_device_fixed, after the
  * combiner when one is set; unordered handles too (UnorderedPartitionedKVWriter writes through the codec).  Call before
  * the first collect (or right after a reset); survives reset.  With a codec, tezgpu_sorter_output_bound includes the
- * worst case (every 32 KiB zlib chunk stored; every LZ4 block all literals), stats.output_bytes_physical / file_out_bytes count compressed bytes,
+ * worst case (every 32 KiB zlib chunk stored; every LZ4 block all literals; every zstd frame raw), stats.output_bytes_physical / file_out_bytes count compressed bytes,
  * output_bytes_with_overhead is still the sum of rawLength, and ms_total includes the compression (ms_emit does not).
  * TEZGPU_E_UNSUPPORTED for any other codec. */
 int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec);
@@ -224,7 +231,8 @@ int32_t tezgpu_merge_reopen(tezgpu_merger *m, const tezgpu_segment *segs, uint32
  * for the others; raw_len may be NULL when none is compressed.  Compressed and uncompressed segments may be mixed.  A
  * compressed segment's CRC is checked on the compressed bytes (unless TEZGPU_SEG_VERIFIED), its body must inflate to
  * exactly raw_len[i] - 4 bytes (DEFAULT: one or more complete zlib streams; LZ4: blocks of raw length > 0 whose chunks decode to
- * exactly that length, adding up to raw_len[i] - 4, nothing after the last block), else TEZGPU_E_FORMAT naming the segment.  Every
+ * exactly that length, adding up to raw_len[i] - 4, nothing after the last block; ZSTD: frames and skippable frames whose
+ * content adds up to raw_len[i] - 4, nothing after the last one), else TEZGPU_E_FORMAT naming the segment.  Every
  * tezgpu_merge_write_* of the handle writes through the same codec (PipelinedSorter's final merge, :774-836).
  * TEZGPU_CODEC_NONE behaves exactly like open / reopen. */
 int32_t tezgpu_merge_open_codec(const tezgpu_conf *conf, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg,
@@ -358,6 +366,11 @@ int32_t tezgpu_debug_inflate_emulate(const uint8_t *z, uint64_t len, uint64_t bo
 int32_t tezgpu_debug_lz4_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len);
 int32_t tezgpu_debug_lz4_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
                                             uint64_t *out_len);
+/* the same for TEZGPU_CODEC_ZSTD: zstd_compress gives the frames the device writes for one body; zstd_decompress runs
+ * the device reader's exact (serial) path over a stream that must yield exactly body_len bytes. */
+int32_t tezgpu_debug_zstd_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len);
+int32_t tezgpu_debug_zstd_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
+                                             uint64_t *out_len);
 
 /* diagnostics: the 32-bit sort words the variable-width map side gives n keys (key i = kv[key_off[i] ..
  * key_off[i] + key_len[i])), computed on the host with the device's code: the alphabet table built from the byte values

@@ -46,7 +46,7 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
   /**
    * @param rawLengths rawLength of every segment (TezIndexRecord, or the ShuffleHeader's uncompressedLength); required
    *                   for the compressed ones ('T','I','F',1), may be null when none is compressed
-   * @param codec      GpuSorter.codecId(CodecUtils.getCodec(conf)): CODEC_DEFAULT / CODEC_LZ4 decompresses compressed segments on the
+   * @param codec      GpuSorter.codecId(CodecUtils.getCodec(conf)): CODEC_DEFAULT / CODEC_LZ4 / CODEC_ZSTD decompresses compressed segments on the
    *                   device, and writeFile then writes a compressed segment
    */
   public GpuMergeIterator(long[] addresses, long[] lengths, int[] flags, long[] rawLengths, int codec, int comparator,
@@ -101,7 +101,7 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
       boolean sendEmptyPartitionDetails, boolean checkForSameKeys, boolean writerRle, int codec, String out, String index)
       throws IOException {
     // tezgpu_merge_open_codec(P, the spills' rawLengths, codec) + set_check_for_same_keys + tezgpu_merge_write_partitions:
-    // with CODEC_DEFAULT or CODEC_LZ4 the compressed spills are read and file.out is written compressed
+    // with CODEC_DEFAULT, CODEC_LZ4 or CODEC_ZSTD the compressed spills are read and file.out is written compressed
     nativeMergeSpills(spillFiles, spillIndexFiles, partitions, comparator, sendEmptyPartitionDetails, checkForSameKeys,
         writerRle, codec, out, index);
   }

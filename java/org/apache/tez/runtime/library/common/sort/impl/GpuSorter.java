@@ -24,6 +24,7 @@ import org.apache.hadoop.io.Text;
 import org.apache.hadoop.io.compress.CompressionCodec;
 import org.apache.hadoop.io.compress.DefaultCodec;
 import org.apache.hadoop.io.compress.Lz4Codec;
+import org.apache.hadoop.io.compress.ZStandardCodec;
 import org.apache.tez.runtime.api.OutputContext;
 import org.apache.tez.runtime.library.common.comparator.TezBytesComparator;
 import org.apache.tez.runtime.library.partitioner.HashPartitioner;
@@ -38,7 +39,7 @@ public class GpuSorter extends ExternalSorter {
   static final int CMP_BYTES = 0, CMP_TEXT = 1, CMP_BYTESWRITABLE = 2, CMP_INT = 3, CMP_LONG = 4;
   static final int PART_GIVEN = 0, PART_HASH = 1;
   static final int COMBINE_NONE = 0, COMBINE_SUM_INT = 1, COMBINE_SUM_LONG = 2;
-  static final int CODEC_NONE = 0, CODEC_DEFAULT = 1, CODEC_LZ4 = 2;
+  static final int CODEC_NONE = 0, CODEC_DEFAULT = 1, CODEC_LZ4 = 2, CODEC_ZSTD = 3;
   private static final int BATCH_BYTES = 32 << 20;
   private static final int BATCH_RECORDS = 1 << 20;
 
@@ -71,19 +72,20 @@ public class GpuSorter extends ExternalSorter {
   }
 
   /**
-   * The device writes and reads DefaultCodec (zlib) and Lz4Codec segments only.  The class must be one of them itself:
+   * The device writes and reads DefaultCodec (zlib), Lz4Codec and ZStandardCodec segments only.  The class must be one of them itself:
    * GzipCodec extends DefaultCodec but writes gzip members, so an instanceof test would be wrong.  Lz4Codec's
    * io.compression.codec.lz4.buffersize must lie in [TEZGPU_LZ4_CHUNK_BOUND, 262144] (tezgpu.h), as the plugin mirror
    * checks: Java readers decode the device's chunks into a buffer of that size, and the device reader takes chunks of
-   * at most 262,144 bytes.
+   * at most 262,144 bytes.  ZStandardCodec's io.compression.codec.zstd.level has no effect on the device writer.
    */
   static int codecId(CompressionCodec codec) throws IOException {
     if (codec == null) return CODEC_NONE;
     if (codec.getClass() == DefaultCodec.class) return CODEC_DEFAULT;
     if (codec.getClass() == Lz4Codec.class) return CODEC_LZ4;
+    if (codec.getClass() == ZStandardCodec.class) return CODEC_ZSTD;
     throw new IOException("tez.runtime.compress.codec=" + codec.getClass().getName()
-        + ": only org.apache.hadoop.io.compress.DefaultCodec and org.apache.hadoop.io.compress.Lz4Codec are supported"
-        + " on the device path");
+        + ": only org.apache.hadoop.io.compress.DefaultCodec, org.apache.hadoop.io.compress.Lz4Codec and"
+        + " org.apache.hadoop.io.compress.ZStandardCodec are supported on the device path");
   }
 
   /**

@@ -88,7 +88,7 @@ JNIEXPORT void JNICALL SORTER(nativeSetCombiner)(JNIEnv *env, jclass cls, jlong 
   failed(env, tezgpu_sorter_set_combiner((tezgpu_sorter *)(intptr_t)h, combiner));
 }
 
-/* ExternalSorter.codec when it is DefaultCodec or Lz4Codec itself (TEZGPU_CODEC_*; GpuSorter.codecId) */
+/* ExternalSorter.codec when it is DefaultCodec, Lz4Codec or ZStandardCodec itself (TEZGPU_CODEC_*; GpuSorter.codecId) */
 JNIEXPORT void JNICALL SORTER(nativeSetCodec)(JNIEnv *env, jclass cls, jlong h, jint codec) {
   (void)cls;
   failed(env, tezgpu_sorter_set_codec((tezgpu_sorter *)(intptr_t)h, codec));

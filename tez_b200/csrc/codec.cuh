@@ -1,10 +1,11 @@
-// codec.cuh -- DefaultCodec and Lz4Codec on both sides of the shuffle: the compress phase behind every emit
-// (SortPipeline) and the decompress step in front of every merge open (Merger).  Formats and kernels: deflate.cuh,
-// inflate.cuh (DefaultCodec), lz4.cuh (Lz4Codec).  The two codecs share the chunk layout, the size scan, the pack and
-// the checksum kernels; only the chunk kernels and the segment finish differ.
+// codec.cuh -- DefaultCodec, Lz4Codec and ZStandardCodec on both sides of the shuffle: the compress phase behind every
+// emit (SortPipeline) and the decompress step in front of every merge open (Merger).  Formats and kernels: deflate.cuh,
+// inflate.cuh (DefaultCodec), lz4.cuh (Lz4Codec), zstd.cuh (ZStandardCodec).  The codecs share the chunk layout, the
+// size scan, the pack and the checksum kernels; only the chunk kernels and the segment finish differ.
 #pragma once
 #include "inflate.cuh"
 #include "lz4.cuh"
+#include "zstd.cuh"
 #include "merger.cuh"
 
 namespace tezgpu {
@@ -18,10 +19,10 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
   const int P = conf.num_partitions;
   cudaStream_t st = stream;
   // zlib: 32 KiB chunks, framed by TIF\x01 78 01 | chunks | Adler-32 CRC; LZ4: blocks of one chunk each (their 8 header
-  // bytes in the slot), framed by TIF\x01 | blocks | CRC
-  const bool lz4 = codec == TEZGPU_CODEC_LZ4;
-  const uint64_t chunk = lz4 ? L4_BLOCK : ZCHUNK;
-  const uint32_t slot = lz4 ? L4_SLOT : ZSLOT, frame = lz4 ? 8 : 14, head = lz4 ? 4 : 6, tail = lz4 ? 0 : 4;
+  // bytes in the slot), framed by TIF\x01 | blocks | CRC; zstd: one frame per chunk, framed by TIF\x01 | frames | CRC
+  const bool lz4 = codec == TEZGPU_CODEC_LZ4, zstd = codec == TEZGPU_CODEC_ZSTD, blocks = lz4 || zstd;
+  const uint64_t chunk = lz4 ? L4_BLOCK : zstd ? ZS_BLOCK : ZCHUNK;
+  const uint32_t slot = lz4 ? L4_SLOT : zstd ? ZS_SLOT : ZSLOT, frame = blocks ? 8 : 14, head = blocks ? 4 : 6, tail = blocks ? 0 : 4;
   z_timer.reset();
   z_timer.mark(st);
   z_host.ensure((size_t)P * sizeof(ZSeg) + 64);
@@ -50,13 +51,17 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     z_slots.ensure((size_t)nchunks * slot);
     z_csize.ensure((size_t)nchunks * 4);
     z_coff.ensure(((size_t)nchunks + 2) * 8);
-    static bool attr[2][64] = {};   // the attribute is per device
-    if (!attr[lz4][conf.device & 63]) {
+    static bool attr[4][64] = {};   // the attribute is per device
+    if (!attr[codec & 3][conf.device & 63]) {
       if (lz4) TG_CUDA(cudaFuncSetAttribute(k_l4compress, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(L4Shared)));
+      else if (zstd) TG_CUDA(cudaFuncSetAttribute(k_zscompress, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZsShared)));
       else TG_CUDA(cudaFuncSetAttribute(k_zdeflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZShared)));
-      attr[lz4][conf.device & 63] = true;
+      attr[codec & 3][conf.device & 63] = true;
     }
-    if (lz4) {
+    if (zstd) {
+      k_zscompress<<<nchunks, ZS_LANES, sizeof(ZsShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
+                                                               z_csize.as<uint32_t>());
+    } else if (lz4) {
       k_l4compress<<<nchunks, L4_LANES, sizeof(L4Shared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
                                                                z_csize.as<uint32_t>());
     } else {
@@ -96,7 +101,7 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     k_crc_combine<<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, d_crc, z_crc.as<uint32_t>());
     k_zpack<<<nchunks, 256, 0, st>>>(z_slots.as<uint8_t>(), z_csize.as<uint32_t>(), z_coff.as<uint64_t>(), z_segs.as<ZSeg>(), (uint32_t)P,
                                      slot, head, d_out);
-    if (lz4)
+    if (blocks)   // TIF\x01 and the CRC: LZ4 and zstd segments frame their stream alike
       k_l4finish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_crc.as<uint32_t>(), d_crc, d_out);
     else
       k_zfinish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_cadler.as<uint32_t>(), z_csize.as<uint32_t>(),
@@ -127,8 +132,9 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
 // Compressed segments (TIF\x01 with a codec set) are staged, their CRC checked (unless the transport verified it),
 // decompressed into images TIF\x00 + body + 4 bytes that the merge reads as verified ordinary segments.  zlib: one warp
 // per segment.  LZ4: one thread per segment walks the block headers (one host round trip for the block count), one warp
-// per block decodes, and a segment the block pass could not take is decoded again serially by one warp.  Every other segment
-// goes to open() unchanged, so errors keep naming the caller's segment index.
+// per block decodes, and a segment the block pass could not take is decoded again serially by one warp.  zstd: the same
+// shape with frames: a segment whose frames all carry Frame_Content_Size is decoded one warp per frame, any other one
+// warp per segment.  Every other segment goes to open() unchanged, so errors keep naming the caller's segment index.
 inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg) {
   if (!pipe.codec) { open(in, nseg); return; }
   cudaStream_t st = pipe.stream;
@@ -210,8 +216,32 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
     k_crc_check<<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_in.as<uint8_t>(), z_descs.as<SegDesc>(), nz, z_crc.as<uint32_t>(), d_crc, z_flag.as<int>());
     launches += 3;
   }
-  const bool lz4 = pipe.codec == TEZGPU_CODEC_LZ4;
-  if (lz4) {
+  const bool lz4 = pipe.codec == TEZGPU_CODEC_LZ4, zstd = pipe.codec == TEZGPU_CODEC_ZSTD;
+  if (zstd) {
+    z_nblk.ensure((size_t)nz * 4);
+    z_slow.ensure((size_t)nz * 4);
+    TG_CUDA(cudaMemsetAsync(z_slow.p, 0, (size_t)nz * 4, st));
+    k_zswalk<0><<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), nullptr, nullptr);
+    launches++;
+    TG_CUDA(cudaGetLastError());
+    std::vector<uint32_t> nfr(nz), base(nz);
+    TG_CUDA(cudaMemcpyAsync(nfr.data(), z_nblk.p, (size_t)nz * 4, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaStreamSynchronize(st));
+    uint64_t nf = 0;
+    for (uint32_t i = 0; i < nz; i++) { base[i] = (uint32_t)nf; nf += nfr[i]; }
+    TG_CHECK(nf < (1ull << 32), TEZGPU_E_INVALID, "too many zstd frames in one merge");
+    if (nf) {
+      z_base.ensure((size_t)nz * 4);
+      z_blks.ensure((size_t)nf * sizeof(ZsFrm));
+      TG_CUDA(cudaMemcpyAsync(z_base.p, base.data(), (size_t)nz * 4, cudaMemcpyHostToDevice, st));
+      k_zswalk<1><<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), z_base.as<uint32_t>(),
+                                                            z_blks.as<ZsFrm>());
+      k_zsframes<<<(uint32_t)div_up(nf, ZSD_WARPS), ZSD_WARPS * 32, 0, st>>>(z_blks.as<ZsFrm>(), (uint32_t)nf, z_slow.as<int32_t>());
+      launches += 2;
+    }
+    k_zsserial<<<(uint32_t)div_up(nz, ZSD_WARPS), ZSD_WARPS * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(),
+                                                                          z_slow.as<int32_t>(), z_status.as<int32_t>());
+  } else if (lz4) {
     z_nblk.ensure((size_t)nz * 4);
     z_slow.ensure((size_t)nz * 4);
     TG_CUDA(cudaMemsetAsync(z_slow.p, 0, (size_t)nz * 4, st));
@@ -248,7 +278,8 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
   TG_CHECK(bad_crc == 0, TEZGPU_E_FORMAT, "IFile checksum mismatch in segment " + std::to_string(bad_crc ? zs[bad_crc - 1] : 0));
   for (uint32_t i = 0; i < nz; i++)
     TG_CHECK(status[i] == Z_OK, TEZGPU_E_FORMAT,
-             std::string("compressed segment ") + std::to_string(zs[i]) + ": " + (lz4 ? l4_err_name(status[i]) : z_err_name(status[i])));
+             std::string("compressed segment ") + std::to_string(zs[i]) + ": " +
+                 (zstd ? zs_err_name(status[i]) : lz4 ? l4_err_name(status[i]) : z_err_name(status[i])));
   std::vector<tezgpu_segment> segs2(in, in + nseg);
   for (uint32_t i = 0; i < nz; i++) {
     tezgpu_segment &sg = segs2[zs[i]];
@@ -278,8 +309,10 @@ static inline std::vector<uint8_t> z_deflate_host(const uint8_t *body, uint64_t 
 }
 
 // worst case of the compressed file given the uncompressed file's bound.  zlib: every chunk stored.  LZ4: every block
-// all literals (one token, (n - 15) / 255 + 1 length bytes) plus its 8 header bytes.
+// all literals (one token, (n - 15) / 255 + 1 length bytes) plus its 8 header bytes.  zstd: every frame raw (10 bytes
+// of frame and block header).
 inline uint64_t SortPipeline::codec_bound(int codec, uint64_t raw_bound, int P) {
+  if (codec == TEZGPU_CODEC_ZSTD) return raw_bound + 10 * (raw_bound / ZS_BLOCK + (uint64_t)P + 1) + 64;
   if (codec == TEZGPU_CODEC_LZ4) return raw_bound + raw_bound / 255 + 10 * (raw_bound / L4_BLOCK + (uint64_t)P + 1) + 64;
   return raw_bound + 5 * (raw_bound / ZCHUNK + (uint64_t)P + 1) + 11ull * P + 64;
 }

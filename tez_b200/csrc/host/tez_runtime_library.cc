@@ -69,6 +69,7 @@ static const char *K_COMPRESS_CODEC = "tez.runtime.compress.codec";
 static const char *DEFAULT_CODEC = "org.apache.hadoop.io.compress.DefaultCodec";
 static const char *LZ4_CODEC = "org.apache.hadoop.io.compress.Lz4Codec";
 static const char *K_LZ4_BUFFERSIZE = "io.compression.codec.lz4.buffersize";   // CommonConfigurationKeys, default 256 KiB
+static const char *ZSTD_CODEC = "org.apache.hadoop.io.compress.ZStandardCodec";
 static const char *K_SERIALIZATIONS = "io.serializations";
 static const char *K_VALUE_CLASS = "tez.runtime.value.class";
 static const char *K_COMBINER_CLASS = "tez.runtime.combiner.class";
@@ -197,6 +198,8 @@ static std::vector<uint8_t> roaring_serialize(const std::vector<uint32_t> &vals)
 // Lz4Decompressor decodes each chunk into a buffer of io.compression.codec.lz4.buffersize bytes, so a buffer smaller
 // than the device writer's worst-case chunk (TEZGPU_LZ4_CHUNK_BOUND) could not read the device's output, and Java
 // writers with a buffer over 262,144 bytes write chunks the device reader refuses: both are refused by key name.
+// ZStandardCodec: io.compression.codec.zstd.level is accepted and has no effect on the device writer, which has one
+// parse; a Java reader reads its frames at any level (DESIGN.md 9).
 static int codec_for(const Configuration &conf) {
   if (!conf.getBoolean(K_COMPRESS, false)) return TEZGPU_CODEC_NONE;
   const std::string codec = conf.get(K_COMPRESS_CODEC, "");
@@ -208,8 +211,9 @@ static int codec_for(const Configuration &conf) {
                  std::to_string(TEZGPU_LZ4_CHUNK_BOUND) + " to 262144 bytes with " + LZ4_CODEC);
     return TEZGPU_CODEC_LZ4;
   }
+  if (codec == ZSTD_CODEC) return TEZGPU_CODEC_ZSTD;
   RT_CHECK(codec == DEFAULT_CODEC, TEZGPU_E_UNSUPPORTED,
-           std::string(K_COMPRESS_CODEC) + "=" + codec + ": only " + DEFAULT_CODEC + " and " + LZ4_CODEC +
+           std::string(K_COMPRESS_CODEC) + "=" + codec + ": only " + DEFAULT_CODEC + ", " + LZ4_CODEC + " and " + ZSTD_CODEC +
                " are supported on the device path");
   return TEZGPU_CODEC_DEFAULT;
 }

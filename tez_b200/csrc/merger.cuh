@@ -781,7 +781,7 @@ class Merger {
 
   // ---- codec (codec.cuh): compressed segments are checked, decompressed into z_img and merged as ordinary segments
   DeviceBuffer z_in, z_img, z_insegs, z_status, z_descs, z_pstart, z_tc, z_crc, z_flag;
-  DeviceBuffer z_nblk, z_base, z_blks, z_slow;   // LZ4: blocks per segment, their first index, the blocks, serial-path flags
+  DeviceBuffer z_nblk, z_base, z_blks, z_slow;   // LZ4 / zstd: blocks (frames) per segment, their first index, the units, serial-path flags
   void open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg);
 
   // the writer behind write_*: TezMerger.writeFile semantics, or -- with a combiner -- the combined records, which carry

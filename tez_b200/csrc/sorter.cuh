@@ -236,8 +236,8 @@ class SortPipeline {
     emit_out(rle, false, raw_bound, d_out, out_cap, out_len, index, stats);
   }
 
-  // ---- codec (deflate.cuh, lz4.cuh, codec.cuh): with a codec the emit writes the uncompressed file into z_img and
-  // compress_image turns every segment into a compressed one (zlib or LZ4) in d_out
+  // ---- codec (deflate.cuh, lz4.cuh, zstd.cuh, codec.cuh): with a codec the emit writes the uncompressed file into z_img
+  // and compress_image turns every segment into a compressed one (zlib, LZ4 or zstd) in d_out
   int codec = TEZGPU_CODEC_NONE;
   DeviceBuffer z_img, z_slots, z_csize, z_cadler, z_coff, z_segs, z_descs, z_pstart, z_tc, z_crc;
   PinnedBuffer z_host;

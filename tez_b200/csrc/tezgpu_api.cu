@@ -5,6 +5,7 @@
 #include <sys/stat.h>
 #include <unistd.h>
 
+#include <memory>
 #include <mutex>
 #include <string>
 
@@ -353,8 +354,8 @@ int32_t tezgpu_sorter_set_combiner(tezgpu_sorter *h, int32_t combiner) {
 int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec) {
   TG_API_BEGIN
   TG_CHECK(h, TEZGPU_E_INVALID, "null handle");
-  TG_CHECK(codec == TEZGPU_CODEC_NONE || codec == TEZGPU_CODEC_DEFAULT || codec == TEZGPU_CODEC_LZ4, TEZGPU_E_UNSUPPORTED,
-           "codec " + std::to_string(codec) + " is not on the device (DefaultCodec and Lz4Codec only)");
+  TG_CHECK(codec == TEZGPU_CODEC_NONE || codec == TEZGPU_CODEC_DEFAULT || codec == TEZGPU_CODEC_LZ4 || codec == TEZGPU_CODEC_ZSTD,
+           TEZGPU_E_UNSUPPORTED, "codec " + std::to_string(codec) + " is not on the device (DefaultCodec, Lz4Codec and ZStandardCodec only)");
   TG_CHECK(h->n == 0 && !h->flushed, TEZGPU_E_STATE, "set the codec before the first collect (or after a reset)");
   h->pipe.codec = codec;
   TG_API_END
@@ -403,6 +404,29 @@ int32_t tezgpu_debug_lz4_decompress_emulate(const uint8_t *z, uint64_t len, uint
   const int32_t rc = l4_decompress(z, len, out, body_len, &got);
   *out_len = got;
   TG_CHECK(rc == L4_OK, TEZGPU_E_FORMAT, std::string("compressed segment 0: ") + l4_err_name(rc));
+  TG_API_END
+}
+
+int32_t tezgpu_debug_zstd_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len) {
+  TG_API_BEGIN
+  TG_CHECK((body || len == 0) && out && out_len, TEZGPU_E_INVALID, "null argument");
+  const std::vector<uint8_t> z = zs_compress_host(body, len);
+  *out_len = z.size();
+  TG_CHECK(z.size() <= cap, TEZGPU_E_NOMEM, "output buffer too small");
+  memcpy(out, z.data(), z.size());
+  TG_API_END
+}
+
+int32_t tezgpu_debug_zstd_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
+                                             uint64_t *out_len) {
+  TG_API_BEGIN
+  TG_CHECK((z || len == 0) && (out || body_len == 0) && out_len, TEZGPU_E_INVALID, "null argument");
+  TG_CHECK(body_len <= cap, TEZGPU_E_INVALID, "output buffer smaller than body_len");
+  uint64_t got = 0;
+  std::unique_ptr<ZsDec> d(new ZsDec());
+  const int32_t rc = zs_decompress(z, len, out, body_len, &got, *d);
+  *out_len = got;
+  TG_CHECK(rc == ZS_OK, TEZGPU_E_FORMAT, std::string("compressed segment 0: ") + zs_err_name(rc));
   TG_API_END
 }
 

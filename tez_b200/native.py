@@ -36,7 +36,8 @@ class GpuSorter:
     def __init__(self, num_partitions, combiner=COMBINE_NONE, codec=CODEC_NONE, **kw):
         """combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG runs MRCombiner with IntSumReducer / LongSumReducer on every
         flush (tezgpu_sorter_set_combiner).  codec: CODEC_DEFAULT writes zlib-compressed segments, CODEC_LZ4 Lz4Codec
-        segments (blocks of LZ4_BLOCK_BYTES raw bytes, one chunk each) (tezgpu_sorter_set_codec)."""
+        segments (blocks of LZ4_BLOCK_BYTES raw bytes, one chunk each), CODEC_ZSTD ZStandardCodec segments (one frame per
+        ZSTD_BLOCK_BYTES raw bytes) (tezgpu_sorter_set_codec)."""
         self.L = _lib.load()
         self.conf = make_conf(num_partitions, **kw)
         self.P = num_partitions
@@ -56,7 +57,7 @@ class GpuSorter:
         check(self.L.tezgpu_sorter_set_combiner(self.h, combiner))
 
     def set_codec(self, codec):
-        """CODEC_NONE / CODEC_DEFAULT / CODEC_LZ4; before the first collect (or after reset); survives reset."""
+        """CODEC_NONE / CODEC_DEFAULT / CODEC_LZ4 / CODEC_ZSTD; before the first collect (or after reset); survives reset."""
         check(self.L.tezgpu_sorter_set_codec(self.h, codec))
 
     def close(self):
@@ -141,7 +142,7 @@ class GpuMerger:
         verified: optional per-segment booleans -- the transport already checked that segment's checksum
         (TEZGPU_SEG_VERIFIED: fetch_segments_verified), the merge does not read it again to verify.
         combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG combines the merged stream in write_* (tezgpu_merge_set_combiner).
-        codec: CODEC_DEFAULT (zlib) or CODEC_LZ4 (Lz4Codec) reads compressed (TIF\\x01) segments of that codec and writes
+        codec: CODEC_DEFAULT (zlib), CODEC_LZ4 (Lz4Codec) or CODEC_ZSTD (ZStandardCodec) reads compressed (TIF\\x01) segments of that codec and writes
         compressed output (tezgpu_merge_open_codec); raw_lens: per-segment rawLength, required for the compressed
         segments."""
         self.L = _lib.load()

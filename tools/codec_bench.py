@@ -1,10 +1,11 @@
-"""DefaultCodec and Lz4Codec cost on the device: one JSON line per case, no-codec, zlib and LZ4 runs alternating in one
-process (the *_lz4 fields are Lz4Codec's).
+"""DefaultCodec, Lz4Codec and ZStandardCodec cost on the device: one JSON line per case, no-codec, zlib, LZ4 and zstd runs
+alternating in one process (the *_lz4 fields are Lz4Codec's, the *_zstd fields ZStandardCodec's).
 
   1. config-2 map side: 1e8 random 80-byte records, P = 64, sort_device_fixed (the stored / all-literal path)
   2. compressible map side: Text words drawn from a Zipf law with IntWritable 1 values, sort_device_fixed
-  3. reduce side: config-3 segments compressed on the host (zlib level 1; LZ4 by the device writer's host emulation),
-     reopen + write_ifile_device
+  3. reduce side: config-3 segments compressed on the host (zlib level 1; LZ4 and zstd by the device writers' host
+     emulations, zstd's frames taking the one-warp-per-frame path; zstd also as libzstd level-3 one-frame streams
+     without content size, the one-warp-per-segment path, where libzstd can be loaded), reopen + write_ifile_device
   4. e2e through host buffers: collect_batch + flush_to_memory of the case-2 records
 
 Times: host clock around fully synchronised library calls.  The card name and power limit are read in the same run.
@@ -34,11 +35,11 @@ def card():
 
 
 def zcap(raw, P):
-    """room for the zlib (every chunk stored) and the LZ4 (every block all literals) worst case"""
+    """room for the zlib (every chunk stored), the LZ4 (every block all literals) and the zstd (every frame raw) worst case"""
     return raw + raw // 255 + 10 * (raw // 32768 + P + 1) + 11 * P + 64
 
 
-CODECS = (0, T.CODEC_LZ4, T.CODEC_DEFAULT)   # zlib last: the compressible case reads its output back
+CODECS = (0, T.CODEC_LZ4, T.CODEC_ZSTD, T.CODEC_DEFAULT)   # zlib last: the compressible case reads its output back
 
 
 def lz4_stream(body):
@@ -49,6 +50,37 @@ def lz4_stream(body):
     n = C.c_uint64()
     T._lib.check(L.tezgpu_debug_lz4_compress_emulate(body, len(body), out, cap, C.byref(n)))
     return bytes(out[:n.value])
+
+
+def zstd_stream(body):
+    """the device writer's zstd frames of one body, run on the host (tezgpu_debug_zstd_compress_emulate)"""
+    L = T._lib.load()
+    cap = len(body) + 10 * (len(body) // T.ZSTD_BLOCK_BYTES + 2) + 64
+    out = (C.c_uint8 * cap)()
+    n = C.c_uint64()
+    T._lib.check(L.tezgpu_debug_zstd_compress_emulate(body, len(body), out, cap, C.byref(n)))
+    return bytes(out[:n.value])
+
+
+def libzstd_level3(body):
+    """libzstd level 3, one frame without Frame_Content_Size (ZSTD_c_contentSizeFlag 0), or None without libzstd"""
+    try:
+        L = C.CDLL("libzstd.so.1")
+    except OSError:
+        return None
+    L.ZSTD_createCCtx.restype = C.c_void_p
+    L.ZSTD_compress2.restype = L.ZSTD_compressBound.restype = C.c_size_t
+    L.ZSTD_compress2.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    L.ZSTD_CCtx_setParameter.argtypes = [C.c_void_p, C.c_int, C.c_int]
+    L.ZSTD_freeCCtx.argtypes = [C.c_void_p]
+    cctx = L.ZSTD_createCCtx()
+    L.ZSTD_CCtx_setParameter(cctx, 100, 3)
+    L.ZSTD_CCtx_setParameter(cctx, 200, 0)
+    cap = L.ZSTD_compressBound(C.c_size_t(len(body)))
+    out = C.create_string_buffer(cap)
+    n = L.ZSTD_compress2(cctx, out, cap, body, len(body))
+    L.ZSTD_freeCCtx(cctx)
+    return out.raw[:n]
 
 
 def timed(fn):
@@ -99,6 +131,11 @@ def map_side(name, kv, kl, vl, cmp_kind, P, runs, out):
                 ms_runs_lz4=[round(x, 2) for x in res[T.CODEC_LZ4]])
     extra = line["ms_lz4"] - line["ms_no_codec"]
     line["compress_gbps_derived_lz4"] = round(raw / extra / 1e6, 2) if extra > 0 else None
+    slen = lens[T.CODEC_ZSTD][0]
+    line.update(compressed_bytes_zstd=slen, ratio_zstd=round(slen / raw, 4), ms_zstd=round(min(res[T.CODEC_ZSTD]), 2),
+                ms_runs_zstd=[round(x, 2) for x in res[T.CODEC_ZSTD]])
+    extra = line["ms_zstd"] - line["ms_no_codec"]
+    line["compress_gbps_derived_zstd"] = round(raw / extra / 1e6, 2) if extra > 0 else None
     if name == "compressible":
         # zlib level 1 on the same bodies (the first 8 partitions)
         host = d_out[:zlen].cpu().numpy().tobytes()
@@ -126,14 +163,23 @@ def reduce_side(nseg, seg_bytes, runs, out):
         raws.append(len(p) - 4)
     with ThreadPoolExecutor(16) as ex:
         lsegs = [b"TIF\x01" + z + zlib.crc32(z).to_bytes(4, "big") for z in ex.map(lambda p: lz4_stream(p[4:-4]), plain)]
+        ssegs = [b"TIF\x01" + z + zlib.crc32(z).to_bytes(4, "big") for z in ex.map(lambda p: zstd_stream(p[4:-4]), plain)]
+        jz = list(ex.map(lambda p: libzstd_level3(p[4:-4]), plain))
+    jsegs = None if jz[0] is None else [b"TIF\x01" + z + zlib.crc32(z).to_bytes(4, "big") for z in jz]
+    if jsegs is None:
+        print("note: libzstd cannot be loaded; the zstd one-warp-per-segment (libzstd level 3) arm is skipped", file=sys.stderr)
     mz = T.GpuMerger(zsegs, comparator=T.CMP_TEXT, codec=T.CODEC_DEFAULT, raw_lens=raws)
     ml = T.GpuMerger(lsegs, comparator=T.CMP_TEXT, codec=T.CODEC_LZ4, raw_lens=raws)
+    ms_ = T.GpuMerger(ssegs, comparator=T.CMP_TEXT, codec=T.CODEC_ZSTD, raw_lens=raws)
     mp = T.GpuMerger(plain, comparator=T.CMP_TEXT)
-    cap = max(mz.output_bound(), ml.output_bound(), mp.output_bound())
+    cap = max(mz.output_bound(), ml.output_bound(), ms_.output_bound(), mp.output_bound())
     d_out = torch.empty(cap, dtype=torch.uint8, device="cuda")
-    res = {c: [] for c in CODECS}
+    res = {c: [] for c in CODECS + ("java",)}
+    arms = [(0, mp, plain), (T.CODEC_DEFAULT, mz, zsegs), (T.CODEC_LZ4, ml, lsegs), (T.CODEC_ZSTD, ms_, ssegs)]
+    if jsegs is not None:
+        arms.append(("java", ms_, jsegs))
     for r in range(runs + 1):
-        for c, m, segs in ((0, mp, plain), (T.CODEC_DEFAULT, mz, zsegs), (T.CODEC_LZ4, ml, lsegs)):
+        for c, m, segs in arms:
             def step():
                 if c:
                     m.reopen(segs, raw_lens=raws)
@@ -149,10 +195,16 @@ def reduce_side(nseg, seg_bytes, runs, out):
                 ms_runs_plain=[round(x, 2) for x in res[0]], ms_runs_codec=[round(x, 2) for x in res[1]],
                 compressed_in_bytes_lz4=sum(len(z) for z in lsegs), ms_lz4=round(min(res[T.CODEC_LZ4]), 2),
                 ms_runs_lz4=[round(x, 2) for x in res[T.CODEC_LZ4]],
+                compressed_in_bytes_zstd=sum(len(z) for z in ssegs), ms_zstd=round(min(res[T.CODEC_ZSTD]), 2),
+                ms_runs_zstd=[round(x, 2) for x in res[T.CODEC_ZSTD]],
                 note="codec: reads compressed segments and writes a compressed merged segment")
+    if jsegs is not None:
+        line.update(compressed_in_bytes_zstd_libzstd3=sum(len(z) for z in jsegs), ms_zstd_libzstd3=round(min(res["java"]), 2),
+                    ms_runs_zstd_libzstd3=[round(x, 2) for x in res["java"]])
     out.append(line)
     mz.close()
     ml.close()
+    ms_.close()
     mp.close()
 
 
@@ -179,7 +231,9 @@ def e2e(kv, kl, vl, cmp_kind, P, runs, out):
                     down_bytes_no_codec=moved[0], down_bytes_codec=moved[1], ms_no_codec=round(min(res[0]), 1),
                     ms_codec=round(min(res[1]), 1), kv_gbps_no_codec=round(kv.size / min(res[0]) / 1e6, 2),
                     kv_gbps_codec=round(kv.size / min(res[1]) / 1e6, 2), down_bytes_lz4=moved[T.CODEC_LZ4],
-                    ms_lz4=round(min(res[T.CODEC_LZ4]), 1), kv_gbps_lz4=round(kv.size / min(res[T.CODEC_LZ4]) / 1e6, 2)))
+                    ms_lz4=round(min(res[T.CODEC_LZ4]), 1), kv_gbps_lz4=round(kv.size / min(res[T.CODEC_LZ4]) / 1e6, 2),
+                    down_bytes_zstd=moved[T.CODEC_ZSTD], ms_zstd=round(min(res[T.CODEC_ZSTD]), 1),
+                    kv_gbps_zstd=round(kv.size / min(res[T.CODEC_ZSTD]) / 1e6, 2)))
 
 
 def main():
