@@ -36,6 +36,17 @@ const char *tezrt_last_error(void);
 int32_t tezrt_output_create(const char *conf, const char *work_dir, const char *unique_id, const char *dest_vertex,
                             const char *host, int32_t shuffle_port, int64_t task_memory, int32_t num_physical_outputs,
                             int32_t device, tezrt_output **out);
+/* `new UnorderedPartitionedKVOutput(outputContext, numPhysicalOutputs)` (partitioned = 1) or
+ * `new UnorderedKVOutput(outputContext, numPhysicalOutputs)` (partitioned = 0: one writer partition,
+ * RL/output/UnorderedKVOutput.java:107): the same output with the writer in TEZGPU_SORTER_UNORDERED mode
+ * (RL/common/writers/UnorderedPartitionedKVWriter.java).  Every other tezrt_output_* call works on the handle.
+ * initialize() requests tez.runtime.unordered.output.buffer.size-mb (> 0, :705-716); no combiner runs; close() writes
+ * a single spill directly, concatenates several per partition with tezgpu_concat_open (current buffer first, then the
+ * spills in order: mergeAll :1058-1144), or -- final merge off or tez.runtime.pipelined-shuffle.enabled -- sends one
+ * event per spill with spill id and last-event flag (finalSpill :966-1006). */
+int32_t tezrt_output_create_unordered(const char *conf, const char *work_dir, const char *unique_id, const char *dest_vertex,
+                                      const char *host, int32_t shuffle_port, int64_t task_memory,
+                                      int32_t num_physical_outputs, int32_t partitioned, int32_t device, tezrt_output **out);
 /* initialize(): reads the configuration, requests the sort memory (requested = bytes passed to requestInitialMemory) */
 int32_t tezrt_output_initialize(tezrt_output *o, int64_t *requested_memory);
 /* MemoryUpdateCallback.memoryAssigned (the MemoryDistributor may grant less than requested) */
@@ -79,6 +90,14 @@ int32_t tezrt_input_wait_ready(tezrt_input *in);
 int32_t tezrt_input_next(tezrt_input *in, const uint8_t **key, uint32_t *klen);
 /* getCurrentValues() iteration: 1 and the next value of the current key, 0 when the group is exhausted */
 int32_t tezrt_input_next_value(tezrt_input *in, const uint8_t **val, uint32_t *vlen);
+/* ---- `new UnorderedKVInput(inputContext, numPhysicalInputs)` (RL/input/UnorderedKVInput.java): inputs are delivered
+ * with tezrt_input_add_local_output / _add_local_spill; the first tezrt_input_next_kv (all inputs delivered) reads them
+ * through tezgpu_concat_open in delivery order, the spills of one source in spill-id order (UnorderedKVReader reads
+ * them in fetch-completion order, :119-230). */
+int32_t tezrt_input_create_unordered(const char *conf, const char *work_dir, const char *unique_id, int64_t task_memory,
+                                     int32_t num_physical_inputs, int32_t device, tezrt_input **out);
+/* KeyValueReader.next() + getCurrentKey() / getCurrentValue(): 1 and the next record, 0 at the end */
+int32_t tezrt_input_next_kv(tezrt_input *in, const uint8_t **key, uint32_t *klen, const uint8_t **val, uint32_t *vlen);
 int64_t tezrt_input_counter(tezrt_input *in, const char *name);
 int32_t tezrt_input_destroy(tezrt_input *in);
 

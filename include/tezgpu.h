@@ -238,6 +238,26 @@ int32_t tezgpu_merge_reopen(tezgpu_merger *m, const tezgpu_segment *segs, uint32
 int32_t tezgpu_merge_open_codec(const tezgpu_conf *conf, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg,
                                 int32_t codec, tezgpu_merger **out);
 int32_t tezgpu_merge_reopen_codec(tezgpu_merger *m, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg);
+/* UnorderedPartitionedKVWriter.mergeAll (RL/common/writers/UnorderedPartitionedKVWriter.java:1058-1144) and
+ * UnorderedKVReader (RL/common/readers/UnorderedKVReader.java:119-230): records leave in (segment, position) order; no
+ * key order, no comparator.  codec and raw_len as for tezgpu_merge_open_codec (compressed and plain segments may be
+ * mixed).  Every segment's header and checksum are checked (the checksum unless TEZGPU_SEG_VERIFIED) and its body must
+ * end in the FF FF EOF marker, else TEZGPU_E_FORMAT naming the segment.
+ *   write_partitions* / write_ifile*: partition p's segment is the records of p's input segments, concatenated in the
+ *     order of segs, written with rle = 0 (any other rle: TEZGPU_E_INVALID); a partition without records gets no bytes
+ *     and an all-zero index triple (:1087-1091); with a codec the output is compressed like a merge's.  The write copies
+ *     each input's record bytes as they are and derives the output checksum from the input checksums: nothing is parsed
+ *     (tezgpu_merge_parse_info: mode 3).  It differs from mergeAll, which re-encodes every record, only for inputs that
+ *     writer never produces: REPEAT_KEY markers are carried over (the output still reads back as the same records) and
+ *     so are non-canonical vints.  stats.output_records / spilled_records / output_bytes stay 0: the write counts no
+ *     records (tezgpu_merge_counts does).
+ *   next_batch: the records in (segment, position) order, same_key = 0; the first call (or tezgpu_merge_counts) parses.
+ *     With num_partitions > 1 the segments are taken partition by partition (stable: inside a partition in the order
+ *     of segs), as the writes lay them out; segs listed partition-major keep exactly their order.
+ *   tezgpu_merge_set_combiner and tezgpu_merge_set_check_for_same_keys fail with TEZGPU_E_STATE; reopen / reopen_codec
+ *   keep the handle's mode. */
+int32_t tezgpu_concat_open(const tezgpu_conf *conf, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg,
+                           int32_t codec, tezgpu_merger **out);
 /* MergeQueue's checkForSameKeys constructor argument (SORT/TezMerger.java:560-573; default true like the reference's
  * other constructors, :519).  When 0, isSameKey() -- and therefore REPEAT_KEY in tezgpu_merge_write_* -- is reported
  * only for records that were run-length encoded in their input segment, never across segment boundaries
@@ -251,7 +271,8 @@ int32_t tezgpu_merge_set_combiner(tezgpu_merger *m, int32_t combiner);
 /* total records / key+value bytes of the merged stream */
 /* diagnostics: how the last open / reopen located the records -- mode 0: fixed framing, records addressed in place
  * (no parse); 1: parallel window parser (by_hand = windows whose guessed entry was wrong and that the chase walked
- * itself); 2: sequential walker (one lane per segment: taken when the window parser meets a malformed record) */
+ * itself); 2: sequential walker (one lane per segment: taken when the window parser meets a malformed record);
+ * 3: not parsed: concatenated (tezgpu_concat_open before its first next_batch / counts) */
 int32_t tezgpu_merge_parse_info(tezgpu_merger *m, int32_t *mode, int32_t *by_hand);
 int32_t tezgpu_merge_counts(tezgpu_merger *m, uint64_t *records, uint64_t *kv_bytes);
 /* replaces the next()/getKey()/getValue()/isSameKey() loop: fills up to idx_cap records (key||value bytes appended to
@@ -354,6 +375,11 @@ uint32_t tezgpu_debug_chunk_fold_emulate(const uint8_t *data, uint32_t nchunks, 
 
 /* diagnostics: host-side run of the per-thread-run CRC fold of the packed fixed-width emit kernel (nchunks <= 1280) */
 uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks);
+
+/* diagnostics: the checksum algebra of tezgpu_concat_open on the host: bodies[i] (lens[i] bytes, ending in FF FF) are
+ * the input bodies; each one's CRC-32 becomes the remainder of its record bytes, those are folded with crc(A||B), and
+ * the EOF marker is appended.  *crc = the CRC-32 of the concatenated record bytes followed by FF FF. */
+int32_t tezgpu_debug_crc_concat_emulate(const uint8_t *const *bodies, const uint64_t *lens, uint32_t n, uint32_t *crc);
 
 /* diagnostics: the device codec run on the host with the same code.  deflate: the zlib stream the device writes for one
  * segment body (a compressed segment is TIF\x01 + this + CRC-32).  inflate: decodes a compressed segment body (the bytes

@@ -56,6 +56,28 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
     if (!checkForSameKeys) nativeSetCheckForSameKeys(handle, false);
   }
 
+  private GpuMergeIterator(long handle) {
+    this.handle = handle;
+  }
+
+  /**
+   * UnorderedPartitionedKVWriter.mergeAll (UnorderedPartitionedKVWriter.java:1058-1144) and UnorderedKVReader
+   * (UnorderedKVReader.java:119-230): the segments concatenated, records in (segment, position) order, no comparator,
+   * isSameKey() always false (tezgpu_concat_open).  partitions may be null for one partition.
+   */
+  public static GpuMergeIterator concat(long[] addresses, long[] lengths, int[] flags, int[] partitions, int numPartitions,
+      long[] rawLengths, int codec) throws IOException {
+    return new GpuMergeIterator(nativeConcatOpen(addresses, lengths, flags, partitions, numPartitions, rawLengths, codec,
+        Integer.parseInt(System.getenv().getOrDefault("TEZGPU_DEVICE", "0"))));
+  }
+
+  /** file.out + file.out.index of every partition (tezgpu_merge_write_partitions); returns the 3 * P index triples. */
+  public long[] writePartitions(String out, String index, int numPartitions, boolean writerRle) throws IOException {
+    final long[] idx = new long[3 * numPartitions];
+    nativeWritePartitions(handle, out, index, writerRle, idx);
+    return idx;
+  }
+
   /**
    * Combines the merged stream in writeIFile (PipelinedSorter's final merge from tez.runtime.combine.min.spills spills
    * on, PipelinedSorter.java:815-820); next() then fails: a combining merge has no record iterator.
@@ -108,6 +130,12 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
 
   private static native long nativeOpen(long[] addresses, long[] lengths, int[] flags, int[] partitions, int numPartitions,
       long[] rawLengths, int codec, int comparator, int device) throws IOException;
+  /** native address of a direct buffer (GetDirectBufferAddress), for the segment tables of the open calls */
+  static native long nativeAddress(ByteBuffer direct);
+  private static native long nativeConcatOpen(long[] addresses, long[] lengths, int[] flags, int[] partitions,
+      int numPartitions, long[] rawLengths, int codec, int device) throws IOException;
+  private static native void nativeWritePartitions(long h, String out, String index, boolean rle, long[] idx)
+      throws IOException;
   private static native void nativeSetCheckForSameKeys(long h, boolean on) throws IOException;
   private static native void nativeSetCombiner(long h, int combiner) throws IOException;
   private static native int nativeNextBatch(long h, ByteBuffer out, int cap, IntBuffer idx, int idxCap) throws IOException;

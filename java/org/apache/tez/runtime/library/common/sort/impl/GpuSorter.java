@@ -40,6 +40,7 @@ public class GpuSorter extends ExternalSorter {
   static final int PART_GIVEN = 0, PART_HASH = 1;
   static final int COMBINE_NONE = 0, COMBINE_SUM_INT = 1, COMBINE_SUM_LONG = 2;
   static final int CODEC_NONE = 0, CODEC_DEFAULT = 1, CODEC_LZ4 = 2, CODEC_ZSTD = 3;
+  static final int SORTER_UNORDERED = 2;
   private static final int BATCH_BYTES = 32 << 20;
   private static final int BATCH_RECORDS = 1 << 20;
 
@@ -52,6 +53,7 @@ public class GpuSorter extends ExternalSorter {
   private int n;
   private long collectedBytes;
   private boolean lastSpillRle;
+  private final boolean unordered;
 
   private static IntBuffer direct(int ints) {
     return ByteBuffer.allocateDirect(4 * ints).order(ByteOrder.nativeOrder()).asIntBuffer();
@@ -59,11 +61,21 @@ public class GpuSorter extends ExternalSorter {
 
   public GpuSorter(OutputContext outputContext, Configuration conf, int numOutputs, long initialMemoryAvailable)
       throws IOException {
+    this(outputContext, conf, numOutputs, initialMemoryAvailable, false);
+  }
+
+  /**
+   * unordered: the writer behind UnorderedPartitionedKVOutput / UnorderedKVOutput (UnorderedPartitionedKVWriter): records
+   * are only partitioned, no combiner runs, and the final merge over spills concatenates them (concatSpills).
+   */
+  public GpuSorter(OutputContext outputContext, Configuration conf, int numOutputs, long initialMemoryAvailable,
+      boolean unordered) throws IOException {
     super(outputContext, conf, numOutputs, initialMemoryAvailable);
+    this.unordered = unordered;
     deviceHash = partitioner instanceof HashPartitioner;
-    handle = nativeCreate(numOutputs, comparatorId(comparator, conf), deviceHash ? PART_HASH : PART_GIVEN,
+    handle = nativeCreate(numOutputs, unordered ? CMP_BYTES : comparatorId(comparator, conf), deviceHash ? PART_HASH : PART_GIVEN,
         sendEmptyPartitionDetails, initialMemoryAvailable, /* CUDA ordinal, from the container's environment */
-        Integer.parseInt(System.getenv().getOrDefault("TEZGPU_DEVICE", "0")));
+        Integer.parseInt(System.getenv().getOrDefault("TEZGPU_DEVICE", "0")), unordered ? SORTER_UNORDERED : 0);
     keySerializer.open(sink);
     valSerializer.open(sink);
     // ExternalSorter.codec = CodecUtils.getCodec(conf): every spill and the final merge write through it
@@ -171,6 +183,11 @@ public class GpuSorter extends ExternalSorter {
     // checkForSameKeys and the writer's rle are both needsRLE() of the LAST spill (:797-814)
     finalOutputFile = mapOutputFile.getOutputFileForWrite(0);
     finalIndexFile = mapOutputFile.getOutputIndexFileForWrite(0);
+    if (unordered) {
+      concatSpills(finalOutputFile.toString(), finalIndexFile.toString());
+      numShuffleChunks.setValue(1);
+      return;
+    }
     GpuMergeIterator.mergeSpillsToFile(spillFilePaths(), spillIndexPaths(), partitions,
         comparatorId(comparator, conf), sendEmptyPartitionDetails, lastSpillRle, lastSpillRle, codecId(codec),
         finalOutputFile.toString(), finalIndexFile.toString());
@@ -184,6 +201,49 @@ public class GpuSorter extends ExternalSorter {
     handle = 0;
   }
 
+  /**
+   * UnorderedPartitionedKVWriter.mergeAll (UnorderedPartitionedKVWriter.java:1058-1144) on the device: per partition the
+   * current buffer (the spill flush() forced last) and then the spills in order, concatenated without run-length
+   * encoding (tezgpu_concat_open + tezgpu_merge_write_partitions).  Partitions without records get no bytes and an
+   * all-zero index entry.
+   */
+  private void concatSpills(String out, String index) throws IOException {
+    final String[] files = spillFilePaths(), indexFiles = spillIndexPaths();
+    final int s0 = numSpills;
+    final ByteBuffer[] bytes = new ByteBuffer[s0];
+    final TezSpillRecord[] records = new TezSpillRecord[s0];
+    int nseg = 0;
+    for (int s = 0; s < s0; s++) {
+      try (java.nio.channels.FileChannel ch = java.nio.channels.FileChannel.open(java.nio.file.Paths.get(files[s]))) {
+        bytes[s] = ByteBuffer.allocateDirect((int) ch.size());
+        while (bytes[s].hasRemaining() && ch.read(bytes[s]) >= 0) { }
+      }
+      records[s] = new TezSpillRecord(new org.apache.hadoop.fs.Path(indexFiles[s]), conf);
+      for (int p = 0; p < partitions; p++) if (records[s].getIndex(p).getPartLength() > 0) nseg++;
+    }
+    final long[] addresses = new long[nseg], lengths = new long[nseg], raws = new long[nseg];
+    final int[] flags = new int[nseg], parts = new int[nseg];
+    int i = 0;
+    for (int p = 0; p < partitions; p++) {
+      for (int k = 0; k < s0; k++) {
+        final int s = k == 0 ? s0 - 1 : k - 1;
+        final TezIndexRecord r = records[s].getIndex(p);
+        if (r.getPartLength() == 0) continue;   // "Skip empty partitions within a spill" (:1108-1111)
+        addresses[i] = GpuMergeIterator.nativeAddress(bytes[s]) + r.getStartOffset();
+        lengths[i] = r.getPartLength();
+        raws[i] = r.getRawLength();
+        flags[i] = GpuMergeIterator.SEG_HAS_HEADER;
+        parts[i++] = p;
+      }
+    }
+    final GpuMergeIterator m = GpuMergeIterator.concat(addresses, lengths, flags, parts, partitions, raws, codecId(codec));
+    try {
+      m.writePartitions(out, index, partitions, false);
+    } finally {
+      m.close();
+    }
+  }
+
   // helpers a maintainer wires to the reference's own code (names as in PipelinedSorter)
   private void finishSingleSpillOrPipelined() throws IOException { /* PipelinedSorter.flush :730-772 */ }
   private String[] spillFilePaths() { return new String[numSpills]; }
@@ -191,7 +251,7 @@ public class GpuSorter extends ExternalSorter {
 
   // every native failure surfaces as IOException(tezgpu_last_error()), like the reference's own failures
   private static native long nativeCreate(int partitions, int comparator, int partitioner, boolean sendEmpty, long memory,
-      int device) throws IOException;
+      int device, int sorterImpl) throws IOException;
   private static native void nativeCollect(long h, ByteBuffer kv, int bytes, IntBuffer keyOff, IntBuffer valOff,
       IntBuffer valLen, IntBuffer partition, int n) throws IOException;
   /** counters: [0] OUTPUT_BYTES_WITH_OVERHEAD [1] OUTPUT_BYTES_PHYSICAL [2] SPILLED_RECORDS [3] OUTPUT_RECORDS

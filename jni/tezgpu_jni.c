@@ -30,8 +30,9 @@ static int failed(JNIEnv *env, int32_t rc) {
 static void *addr(JNIEnv *env, jobject buf) { return buf ? (*env)->GetDirectBufferAddress(env, buf) : NULL; }
 
 /* ------------------------------------------------------------------------------------------------ GpuSorter */
+/* sorter_impl: 0 PipelinedSorter, TEZGPU_SORTER_UNORDERED for UnorderedPartitionedKVWriter */
 JNIEXPORT jlong JNICALL SORTER(nativeCreate)(JNIEnv *env, jclass cls, jint partitions, jint comparator, jint partitioner,
-                                             jboolean send_empty, jlong memory, jint device) {
+                                             jboolean send_empty, jlong memory, jint device, jint sorter_impl) {
   (void)cls;
   tezgpu_conf c;
   memset(&c, 0, sizeof(c));
@@ -43,6 +44,7 @@ JNIEXPORT jlong JNICALL SORTER(nativeCreate)(JNIEnv *env, jclass cls, jint parti
   c.rle_policy = TEZGPU_RLE_AUTO;
   c.send_empty_partition_details = send_empty ? 1 : 0;
   c.mem_budget_bytes = (uint64_t)memory;
+  c.sorter_impl = sorter_impl;
   tezgpu_sorter *h = NULL;
   if (failed(env, tezgpu_sorter_create(&c, &h))) return 0;
   return (jlong)(intptr_t)h;
@@ -100,10 +102,9 @@ JNIEXPORT void JNICALL SORTER(nativeDestroy)(JNIEnv *env, jclass cls, jlong h) {
 }
 
 /* ------------------------------------------------------------------------------------------------ GpuMergeIterator */
-JNIEXPORT jlong JNICALL MERGER(nativeOpen)(JNIEnv *env, jclass cls, jlongArray addresses, jlongArray lengths, jintArray flags,
-                                           jintArray partitions, jint num_partitions, jlongArray raw_lengths, jint codec,
-                                           jint comparator, jint device) {
-  (void)cls;
+/* the segment table of nativeOpen / nativeConcatOpen; concat != 0: tezgpu_concat_open, else tezgpu_merge_open_codec */
+static jlong open_merger(JNIEnv *env, jlongArray addresses, jlongArray lengths, jintArray flags, jintArray partitions,
+                         jint num_partitions, jlongArray raw_lengths, jint codec, jint comparator, jint device, int concat) {
   jsize n = (*env)->GetArrayLength(env, addresses);
   jlong *a = (*env)->GetLongArrayElements(env, addresses, NULL), *l = (*env)->GetLongArrayElements(env, lengths, NULL);
   jint *f = (*env)->GetIntArrayElements(env, flags, NULL);
@@ -126,7 +127,8 @@ JNIEXPORT jlong JNICALL MERGER(nativeOpen)(JNIEnv *env, jclass cls, jlongArray a
   c.send_empty_partition_details = 1;
   tezgpu_merger *m = NULL;
   /* rawLength of every segment: required for the compressed ones (jlong and int64_t are both 64-bit) */
-  int32_t rc = tezgpu_merge_open_codec(&c, segs, (const int64_t *)r, (uint32_t)n, codec, &m);
+  int32_t rc = concat ? tezgpu_concat_open(&c, segs, (const int64_t *)r, (uint32_t)n, codec, &m)
+                      : tezgpu_merge_open_codec(&c, segs, (const int64_t *)r, (uint32_t)n, codec, &m);
   free(segs);
   if (r) (*env)->ReleaseLongArrayElements(env, raw_lengths, r, JNI_ABORT);
   (*env)->ReleaseLongArrayElements(env, addresses, a, JNI_ABORT);
@@ -135,6 +137,39 @@ JNIEXPORT jlong JNICALL MERGER(nativeOpen)(JNIEnv *env, jclass cls, jlongArray a
   if (p) (*env)->ReleaseIntArrayElements(env, partitions, p, JNI_ABORT);
   if (failed(env, rc)) return 0;
   return (jlong)(intptr_t)m;
+}
+
+JNIEXPORT jlong JNICALL MERGER(nativeOpen)(JNIEnv *env, jclass cls, jlongArray addresses, jlongArray lengths, jintArray flags,
+                                           jintArray partitions, jint num_partitions, jlongArray raw_lengths, jint codec,
+                                           jint comparator, jint device) {
+  (void)cls;
+  return open_merger(env, addresses, lengths, flags, partitions, num_partitions, raw_lengths, codec, comparator, device, 0);
+}
+
+/* UnorderedPartitionedKVWriter.mergeAll / UnorderedKVReader: records in (segment, position) order, no comparator */
+JNIEXPORT jlong JNICALL MERGER(nativeConcatOpen)(JNIEnv *env, jclass cls, jlongArray addresses, jlongArray lengths,
+                                                 jintArray flags, jintArray partitions, jint num_partitions,
+                                                 jlongArray raw_lengths, jint codec, jint device) {
+  (void)cls;
+  return open_merger(env, addresses, lengths, flags, partitions, num_partitions, raw_lengths, codec, TEZGPU_CMP_BYTES, device, 1);
+}
+
+JNIEXPORT jlong JNICALL MERGER(nativeAddress)(JNIEnv *env, jclass cls, jobject buf) {
+  (void)cls;
+  return (jlong)(intptr_t)addr(env, buf);
+}
+
+/* file.out + file.out.index of all partitions (tezgpu_merge_write_partitions); index receives the 3 * P triples */
+JNIEXPORT void JNICALL MERGER(nativeWritePartitions)(JNIEnv *env, jclass cls, jlong h, jstring out, jstring index_path,
+                                                     jboolean rle, jlongArray index) {
+  (void)cls;
+  const char *o = (*env)->GetStringUTFChars(env, out, NULL), *ip = (*env)->GetStringUTFChars(env, index_path, NULL);
+  jlong *idx = (*env)->GetLongArrayElements(env, index, NULL);
+  int32_t rc = tezgpu_merge_write_partitions((tezgpu_merger *)(intptr_t)h, o, ip, rle ? 1 : 0, (int64_t *)idx, NULL);
+  (*env)->ReleaseLongArrayElements(env, index, idx, rc == TEZGPU_OK ? 0 : JNI_ABORT);
+  (*env)->ReleaseStringUTFChars(env, out, o);
+  (*env)->ReleaseStringUTFChars(env, index_path, ip);
+  failed(env, rc);
 }
 
 JNIEXPORT void JNICALL MERGER(nativeSetCheckForSameKeys)(JNIEnv *env, jclass cls, jlong h, jboolean on) {

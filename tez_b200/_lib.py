@@ -85,6 +85,8 @@ SYMBOLS = [
     ("tezgpu_merge_reopen", C.c_int32, [_V, _P(Segment), C.c_uint32]),
     ("tezgpu_merge_open_codec", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, _P(_V)]),
     ("tezgpu_merge_reopen_codec", C.c_int32, [_V, _P(Segment), _V, C.c_uint32]),
+    ("tezgpu_concat_open", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, _P(_V)]),
+    ("tezgpu_debug_crc_concat_emulate", C.c_int32, [_V, _V, C.c_uint32, _P(C.c_uint32)]),
     ("tezgpu_merge_set_check_for_same_keys", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_merge_set_combiner", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_merge_parse_info", C.c_int32, [_V, _V, _V]),
@@ -108,6 +110,8 @@ SYMBOLS = [
 RT_SYMBOLS = [
     ("tezrt_last_error", C.c_char_p, []),
     ("tezrt_output_create", C.c_int32, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, _P(_V)]),
+    ("tezrt_output_create_unordered", C.c_int32, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int32, C.c_int64,
+                                                  C.c_int32, C.c_int32, C.c_int32, _P(_V)]),
     ("tezrt_output_initialize", C.c_int32, [_V, _P(C.c_int64)]),
     ("tezrt_output_memory_assigned", C.c_int32, [_V, C.c_int64]),
     ("tezrt_output_start", C.c_int32, [_V]),
@@ -120,6 +124,8 @@ RT_SYMBOLS = [
     ("tezrt_output_index_file", C.c_char_p, [_V]),
     ("tezrt_output_destroy", C.c_int32, [_V]),
     ("tezrt_input_create", C.c_int32, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_int64, C.c_int32, C.c_int32, _P(_V)]),
+    ("tezrt_input_create_unordered", C.c_int32, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_int64, C.c_int32, C.c_int32, _P(_V)]),
+    ("tezrt_input_next_kv", C.c_int32, [_V, _P(_V), _P(C.c_uint32), _P(_V), _P(C.c_uint32)]),
     ("tezrt_input_initialize", C.c_int32, [_V, _P(C.c_int64)]),
     ("tezrt_input_start", C.c_int32, [_V]),
     ("tezrt_input_add_local_output", C.c_int32, [_V, C.c_int32, C.c_char_p, C.c_char_p, C.c_int32, C.c_int32]),

@@ -285,7 +285,7 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
     tezgpu_segment &sg = segs2[zs[i]];
     sg.data = zi[i].dst;
     sg.len = (uint64_t)raw_len[zs[i]] + 4;
-    sg.flags = TEZGPU_SEG_HAS_HEADER | TEZGPU_SEG_DEVICE | TEZGPU_SEG_VERIFIED;
+    sg.flags = TEZGPU_SEG_HAS_HEADER | TEZGPU_SEG_DEVICE | TEZGPU_SEG_VERIFIED | SEG_DECODED;
   }
   open(segs2.data(), nseg);
 }

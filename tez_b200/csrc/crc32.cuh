@@ -38,6 +38,8 @@ struct CrcTables {
   uint32_t pow0[4096];      // x^(8*a)
   uint32_t pow1[4096];      // x^(8*4096*a)
   uint32_t pow2[4096];      // x^(8*2^24*a)
+  uint32_t eof_raw;         // raw remainder of the IFile EOF markers FF FF
+  uint32_t xinv16;          // x^(-16): strips the EOF markers off the raw remainder of a body (concat.cuh)
 };
 
 static inline uint32_t crc_host_xpow8(uint64_t nbytes) {
@@ -102,6 +104,9 @@ static inline void crc_build_tables(CrcTables &t, int stride_words) {
     t.pow1[a] = crc_multmodp(t.pow1[a - 1], s1);
     t.pow2[a] = crc_multmodp(t.pow2[a - 1], s2);
   }
+  t.eof_raw = 0;
+  for (int k = 0; k < 2; k++) t.eof_raw = t.slice[0][(t.eof_raw ^ 0xFFu) & 0xFF] ^ (t.eof_raw >> 8);
+  t.xinv16 = crc_host_xpow_bits_inv(16);
 }
 
 // ---------------------------------------------------------------------------------------------- warp-resident maps

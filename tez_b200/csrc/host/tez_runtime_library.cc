@@ -74,6 +74,8 @@ static const char *K_SERIALIZATIONS = "io.serializations";
 static const char *K_VALUE_CLASS = "tez.runtime.value.class";
 static const char *K_COMBINER_CLASS = "tez.runtime.combiner.class";
 static const char *K_COMBINE_MIN_SPILLS = "tez.runtime.combine.min.spills";  // TezRuntimeConfiguration:128-130 default 3
+static const char *K_UNORDERED_BUFFER_MB = "tez.runtime.unordered.output.buffer.size-mb";  // :204-206 default 100
+static const char *K_PIPELINED_SHUFFLE = "tez.runtime.pipelined-shuffle.enabled";           // default false
 
 static bool ends_with(const std::string &s, const char *suf) {
   size_t n = strlen(suf);
@@ -303,7 +305,9 @@ struct GpuSorter {
     }
   }
 
-  void spill() {
+  // last: the spill flush() forces, i.e. the unordered writer's current buffer, whose records
+  // UnorderedPartitionedKVWriter does not count as spilled (finalSpill passes no counter, :985)
+  void spill(bool last = false) {
     std::string dir = spill_dir(num_spills);
     mkdirs(dir);
     std::string f = dir + "/file.out", fi = f + ".index";
@@ -315,7 +319,7 @@ struct GpuSorter {
     if (!final_merge) counters["OUTPUT_BYTES_WITH_OVERHEAD"] += st.output_bytes_with_overhead;
     else if (num_spills > 0) { counters["ADDITIONAL_SPILLS_BYTES_WRITTEN"] += st.file_out_bytes; counters["OUTPUT_BYTES_WITH_OVERHEAD"] = 0; }
     else counters["OUTPUT_BYTES_WITH_OVERHEAD"] += st.output_bytes_with_overhead;
-    counters["SPILLED_RECORDS"] += st.spilled_records;
+    if (!(last && gc.sorter_impl == TEZGPU_SORTER_UNORDERED)) counters["SPILLED_RECORDS"] += st.spilled_records;
     if (combiner) count_combine(st);
     last_spill_rle = st.rle_used;
     partition_stats.resize((size_t)P, 0);
@@ -330,7 +334,7 @@ struct GpuSorter {
   void flush() {
     collected_bytes += kv.size();
     push_batch();
-    spill();  // "force a spill in flush()" (:679-690)
+    spill(true);  // "force a spill in flush()" (:679-690)
     counters["ADDITIONAL_SPILL_COUNT"] += num_spills - 1;
     if (!final_merge) {
       counters["SHUFFLE_CHUNK_COUNT"] = num_spills;
@@ -358,6 +362,7 @@ struct GpuSorter {
     std::vector<std::vector<uint8_t>> bytes(num_spills);
     std::vector<tezgpu_segment> segs;
     std::vector<int64_t> raws;   // rawLength of every segment (the compressed ones need it)
+    std::vector<int> seg_spill;  // spill of every segment
     for (int s = 0; s < num_spills; s++) {
       bytes[s] = read_file(spill_files[s]);
       counters["ADDITIONAL_SPILLS_BYTES_READ"] += (int64_t)bytes[s].size();
@@ -371,22 +376,40 @@ struct GpuSorter {
           sg.partition = (uint32_t)p;
           segs.push_back(sg);
           raws.push_back(raw);
+          seg_spill.push_back(s);
         }
       }
     }
     tezgpu_conf mc = gc;
     mc.fixed_key_len = mc.fixed_val_len = 0;
     tezgpu_merger *m = nullptr;
-    gpu_check(tezgpu_merge_open_codec(&mc, segs.data(), raws.data(), (uint32_t)segs.size(), codec, &m));
     final_idx.assign((size_t)P * 3, 0);
     tezgpu_stats st;
-    // TezMerger.merge(..., checkForSameKeys = merger.needsRLE()) into Writer(..., rle = merger.needsRLE()), `merger`
-    // being the SpanMerger of the last spill (SORT/PipelinedSorter.java:797-814)
-    int32_t rc = tezgpu_merge_set_check_for_same_keys(m, last_spill_rle);
     const bool combine = combiner && num_spills >= min_spills;
-    if (rc == 0 && combine) rc = tezgpu_merge_set_combiner(m, combiner);
-    if (rc == 0)
-      rc = tezgpu_merge_write_partitions(m, final_out.c_str(), final_index.c_str(), /*rle=*/last_spill_rle, final_idx.data(), &st);
+    int32_t rc;
+    if (gc.sorter_impl == TEZGPU_SORTER_UNORDERED) {
+      // UnorderedPartitionedKVWriter.mergeAll (:1058-1144): per partition the current buffer (the forced last spill),
+      // then the spills in order, concatenated, written without run-length encoding
+      std::vector<int64_t> at((size_t)num_spills * P, -1);   // segment of (spill, partition), if any
+      for (size_t i = 0; i < segs.size(); i++) at[(size_t)seg_spill[i] * P + segs[i].partition] = (int64_t)i;
+      std::vector<tezgpu_segment> cs;
+      std::vector<int64_t> craws;
+      for (int p = 0; p < P; p++)
+        for (int k = 0; k < num_spills; k++) {
+          const int64_t i = at[(size_t)(k == 0 ? num_spills - 1 : k - 1) * P + p];
+          if (i >= 0) { cs.push_back(segs[(size_t)i]); craws.push_back(raws[(size_t)i]); }
+        }
+      gpu_check(tezgpu_concat_open(&mc, cs.data(), craws.data(), (uint32_t)cs.size(), codec, &m));
+      rc = tezgpu_merge_write_partitions(m, final_out.c_str(), final_index.c_str(), /*rle=*/0, final_idx.data(), &st);
+    } else {
+      gpu_check(tezgpu_merge_open_codec(&mc, segs.data(), raws.data(), (uint32_t)segs.size(), codec, &m));
+      // TezMerger.merge(..., checkForSameKeys = merger.needsRLE()) into Writer(..., rle = merger.needsRLE()), `merger`
+      // being the SpanMerger of the last spill (SORT/PipelinedSorter.java:797-814)
+      rc = tezgpu_merge_set_check_for_same_keys(m, last_spill_rle);
+      if (rc == 0 && combine) rc = tezgpu_merge_set_combiner(m, combiner);
+      if (rc == 0)
+        rc = tezgpu_merge_write_partitions(m, final_out.c_str(), final_index.c_str(), /*rle=*/last_spill_rle, final_idx.data(), &st);
+    }
     tezgpu_merge_close(m);
     gpu_check(rc);
     const uint64_t len = (uint64_t)st.file_out_bytes;
@@ -412,6 +435,7 @@ struct Output {
   int64_t task_memory, requested = 0, granted = -1;
   bool initialized = false, started = false, closed = false;
   bool send_empty = true, final_merge = true;
+  bool unordered = false;   // UnorderedPartitionedKVOutput / UnorderedKVOutput: the writer in TEZGPU_SORTER_UNORDERED mode
   std::map<std::string, int64_t> counters;
   GpuSorter *sorter = nullptr;
   std::vector<Event> events;
@@ -421,6 +445,16 @@ struct Output {
   ~Output() { delete sorter; }
 
   void initialize() {
+    if (unordered) {
+      // UnorderedPartitionedKVWriter.getInitialMemoryRequirement (RL/common/writers/UnorderedPartitionedKVWriter.java:705-716)
+      const long mb = conf.getInt(K_UNORDERED_BUFFER_MB, 100);
+      RT_CHECK(mb > 0, TEZGPU_E_INVALID, std::string(K_UNORDERED_BUFFER_MB) + " should be larger than 0");
+      requested = (int64_t)mb << 20;
+      send_empty = true;   // the unordered writer always reports its empty partitions (generateDMEvent)
+      final_merge = conf.getBoolean(K_FINAL_MERGE, true) && !conf.getBoolean(K_PIPELINED_SHUFFLE, false);
+      initialized = true;
+      return;
+    }
     // ExternalSorter.getInitialMemoryRequirement (SORT/ExternalSorter.java:330-347)
     long mb = conf.getInt(K_SORT_MB, 100);
     int64_t req = (int64_t)mb << 20;
@@ -438,7 +472,7 @@ struct Output {
     RT_CHECK(granted >= 0, TEZGPU_E_STATE, "memory update not received (MemoryUpdateCallbackHandler.validateUpdateReceived)");
     std::string sc = conf.get(K_SORTER_CLASS, "PIPELINED");
     std::transform(sc.begin(), sc.end(), sc.begin(), ::toupper);
-    RT_CHECK(sc == "PIPELINED" || sc == "LEGACY", TEZGPU_E_INVALID,
+    RT_CHECK(unordered || sc == "PIPELINED" || sc == "LEGACY", TEZGPU_E_INVALID,
              "Invalid sorter class specified in config, propertyName=" + std::string(K_SORTER_CLASS) + ", value=" + sc + ", validValues=[LEGACY, PIPELINED]");
     const int codec = codec_for(conf);
     tezgpu_conf gc;
@@ -446,15 +480,17 @@ struct Output {
     gc.abi_version = TEZGPU_ABI_VERSION;
     gc.device = device;
     gc.num_partitions = P;
-    gc.comparator = comparator_for(conf);
     std::string pc = conf.get(K_PARTITIONER, "org.apache.tez.runtime.library.partitioner.HashPartitioner");
     gc.partitioner = ends_with(pc, "HashPartitioner") ? TEZGPU_PART_HASH : TEZGPU_PART_GIVEN;
+    // an unordered edge compares no keys: its key class only matters to the HashPartitioner's hashCode
+    gc.comparator = (!unordered || (gc.partitioner == TEZGPU_PART_HASH && P > 1)) ? comparator_for(conf) : TEZGPU_CMP_BYTES;
     gc.rle_policy = TEZGPU_RLE_AUTO;
     gc.send_empty_partition_details = send_empty ? 1 : 0;
-    gc.sorter_impl = sc == "LEGACY" ? 1 : 0;
+    gc.sorter_impl = unordered ? TEZGPU_SORTER_UNORDERED : sc == "LEGACY" ? 1 : 0;
     gc.mem_budget_bytes = (uint64_t)granted;
     sorter = new GpuSorter(gc, granted > 0 ? granted : requested, final_merge, work_dir, uid, counters);
-    if (const int c = combiner_for(conf)) sorter->set_combiner(c, (int)conf.getInt(K_COMBINE_MIN_SPILLS, 3));
+    // UnorderedPartitionedKVWriter runs no combiner (and tezgpu_sorter_set_combiner refuses an unordered handle)
+    if (const int c = unordered ? 0 : combiner_for(conf)) sorter->set_combiner(c, (int)conf.getInt(K_COMBINE_MIN_SPILLS, 3));
     if (codec) sorter->set_codec(codec);
     started = true;
   }
@@ -524,6 +560,7 @@ struct Output {
     }
     pb_int(dm, 5, 0);  // run_duration
     if (!final_merge) { pb_int(dm, 8, last ? 1 : 0); pb_int(dm, 9, spill_id); }
+    if (unordered && P == 1) pb_int(dm, 10, counters["OUTPUT_RECORDS"]);   // num_record (generateDMEvent)
     Event e;
     e.type = TEZRT_EVENT_COMPOSITE_DATA_MOVEMENT;
     e.payload = dm;
@@ -574,11 +611,18 @@ struct Input {
       : conf(c), work_dir(wd ? wd : "."), uid(u ? u : "attempt"), N(n), device(dev), task_memory(mem), delivered(n) {}
   ~Input() { if (merger) tezgpu_merge_close(merger); }
 
+  // UnorderedKVInput (RL/input/UnorderedKVInput.java): every delivered input read in turn, no merge
+  // (UnorderedKVReader :119-230).  Order: delivery order, the spills of one source in spill-id order.
+  bool unordered = false;
+  std::vector<std::pair<int, int>> seg_order;   // (delivery rank of the source, spill id) of every fetched segment
+  std::vector<int> src_rank;
+  int next_rank = 0;
+
   void initialize() {
     // OrderedGroupedKVInput.initialize (:100-125): Shuffle memory = shuffle.fetch.buffer.percent of the task memory
     double pct = conf.getFloat("tez.runtime.shuffle.fetch.buffer.percent", 0.9);
     requested = (int64_t)(pct * (double)task_memory);
-    cmp = comparator_for(conf);
+    cmp = unordered ? TEZGPU_CMP_BYTES : comparator_for(conf);
     codec = codec_for(conf);
     initialized = true;
   }
@@ -608,6 +652,8 @@ struct Input {
       ss.complete = ss.last_id >= 0 && (int)ss.spills.size() == ss.last_id + 1;
     }
     if (ss.complete) num_delivered++;
+    if (src_rank.empty()) src_rank.assign((size_t)N, -1);
+    if (src_rank[src] < 0) src_rank[src] = next_rank++;   // a source's place: its first event, empty or not
     if (empty) { counters["NUM_SKIPPED_INPUTS"]++; return; }
     // TezSpillRecord(indexFile): P x 3 big-endian longs + checksum (SORT/TezSpillRecord.java:76-109)
     std::vector<uint8_t> ib = read_file(index_file);
@@ -624,6 +670,7 @@ struct Input {
     if (!(raw > 6)) { counters["NUM_SKIPPED_INPUTS"]++; return; }  // !hasData
     seg_bytes.push_back(read_file(file_out, (uint64_t)start, part));
     seg_raw.push_back(raw);
+    seg_order.push_back({src_rank[src], spill_id});
     counters["NUM_SHUFFLED_INPUTS"]++;
     counters["SHUFFLE_BYTES"] += part;
     counters["SHUFFLE_BYTES_DECOMPRESSED"] += raw;
@@ -648,11 +695,22 @@ struct Input {
       segs[i].flags = TEZGPU_SEG_HAS_HEADER;
       segs[i].partition = 0;
     }
-    // MergeManager.finalMerge -> TezMerger.merge; compressed segments are inflated with their index rawLength
-    gpu_check(tezgpu_merge_open_codec(&gc, segs.data(), seg_raw.data(), (uint32_t)segs.size(), codec, &merger));
-    counters["MERGED_MAP_OUTPUTS"] += (int64_t)segs.size();
+    if (unordered) {
+      std::vector<size_t> ord(segs.size());
+      for (size_t i = 0; i < ord.size(); i++) ord[i] = i;
+      std::stable_sort(ord.begin(), ord.end(), [&](size_t a, size_t b) { return seg_order[a] < seg_order[b]; });
+      std::vector<tezgpu_segment> os(segs.size());
+      std::vector<int64_t> oraw(segs.size());
+      for (size_t i = 0; i < ord.size(); i++) { os[i] = segs[ord[i]]; oraw[i] = seg_raw[ord[i]]; }
+      gpu_check(tezgpu_concat_open(&gc, os.data(), oraw.data(), (uint32_t)os.size(), codec, &merger));
+    } else {
+      // MergeManager.finalMerge -> TezMerger.merge; compressed segments are inflated with their index rawLength
+      gpu_check(tezgpu_merge_open_codec(&gc, segs.data(), seg_raw.data(), (uint32_t)segs.size(), codec, &merger));
+      counters["MERGED_MAP_OUTPUTS"] += (int64_t)segs.size();
+    }
     seg_bytes.clear();
     seg_raw.clear();
+    seg_order.clear();
     batch.resize(8u << 20);
     idx.resize(1u << 16);
     ready = true;
@@ -680,6 +738,19 @@ struct Input {
     counters["REDUCE_INPUT_GROUPS"]++;
     *key = cur_key.data();
     *klen = (uint32_t)cur_key.size();
+    return true;
+  }
+  // KeyValueReader.next() of UnorderedKVInput: every record in turn; the first call opens the concatenation
+  bool next_kv(const uint8_t **key, uint32_t *klen, const uint8_t **val, uint32_t *vlen) {
+    RT_CHECK(unordered, TEZGPU_E_STATE, "next_kv() is the reader of an unordered input");
+    wait_ready();
+    if (!merger || !fetch()) return false;
+    const tezgpu_kv_index &e = idx[bi];
+    *key = batch.data() + e.key_off;
+    *klen = e.key_len;
+    *val = batch.data() + e.val_off;
+    *vlen = e.val_len;
+    counters["INPUT_RECORDS_PROCESSED"]++;
     return true;
   }
   bool next_value(const uint8_t **val, uint32_t *vlen) {
@@ -721,6 +792,16 @@ int32_t tezrt_output_create(const char *conf, const char *work_dir, const char *
   *out = new tezrt_output(conf, work_dir, unique_id, dest_vertex, host, port, task_memory, P, device);
   RT_END
 }
+int32_t tezrt_output_create_unordered(const char *conf, const char *work_dir, const char *unique_id, const char *dest_vertex,
+                                      const char *host, int32_t port, int64_t task_memory, int32_t P, int32_t partitioned,
+                                      int32_t device, tezrt_output **out) {
+  RT_BEGIN
+  RT_CHECK(out && P >= 1, TEZGPU_E_INVALID, "bad arguments");
+  // UnorderedKVOutput writes one partition whatever the number of physical outputs (RL/output/UnorderedKVOutput.java:107)
+  *out = new tezrt_output(conf, work_dir, unique_id, dest_vertex, host, port, task_memory, partitioned ? P : 1, device);
+  (*out)->o.unordered = true;
+  RT_END
+}
 int32_t tezrt_output_initialize(tezrt_output *o, int64_t *requested) { RT_BEGIN o->o.initialize(); if (requested) *requested = o->o.requested; RT_END }
 int32_t tezrt_output_memory_assigned(tezrt_output *o, int64_t granted) { RT_BEGIN o->o.granted = granted; RT_END }
 int32_t tezrt_output_start(tezrt_output *o) { RT_BEGIN o->o.start(); RT_END }
@@ -751,6 +832,17 @@ int32_t tezrt_input_create(const char *conf, const char *work_dir, const char *u
   RT_CHECK(out && n >= 0, TEZGPU_E_INVALID, "bad arguments");
   *out = new tezrt_input(conf, work_dir, unique_id, task_memory, n, device);
   RT_END
+}
+int32_t tezrt_input_create_unordered(const char *conf, const char *work_dir, const char *unique_id, int64_t task_memory, int32_t n,
+                                     int32_t device, tezrt_input **out) {
+  RT_BEGIN
+  RT_CHECK(out && n >= 0, TEZGPU_E_INVALID, "bad arguments");
+  *out = new tezrt_input(conf, work_dir, unique_id, task_memory, n, device);
+  (*out)->i.unordered = true;
+  RT_END
+}
+int32_t tezrt_input_next_kv(tezrt_input *in, const uint8_t **key, uint32_t *klen, const uint8_t **val, uint32_t *vlen) {
+  try { return in->i.next_kv(key, klen, val, vlen) ? 1 : 0; } catch (const Err &e) { g_err = e.what(); return e.code; }
 }
 int32_t tezrt_input_initialize(tezrt_input *in, int64_t *requested) { RT_BEGIN in->i.initialize(); if (requested) *requested = in->i.requested; RT_END }
 int32_t tezrt_input_start(tezrt_input *in) { RT_BEGIN in->i.start(); RT_END }

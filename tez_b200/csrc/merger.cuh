@@ -18,9 +18,12 @@ struct SegDesc {
   uint64_t len;       // total bytes
   uint64_t body0;     // offset of the first body byte inside the segment (4 with header, 0 in-memory)
   uint64_t body_end;  // offset just past the EOF markers' possible position: len - 4 (checksum / slack excluded)
-  uint32_t has_header;  // bit 0: 'TIF' header present; bit 1: checksum already verified by the transport (skip)
+  uint32_t has_header;  // bit 0: 'TIF' header present; bit 1: checksum already verified by the transport (skip);
+                        // bit 2: decoded image of a compressed segment (its trailer is not the body's checksum)
   uint32_t partition;
 };
+// tezgpu_segment.flags bit the codec path sets on the decoded images it hands to open() (never part of the ABI)
+constexpr uint32_t SEG_DECODED = 1u << 31;
 
 // ------------------------------------------------------------------------------------------------ checksum
 // raw CRC remainder of 64 KiB pieces of the segment bodies, combined per segment by k_crc_combine
@@ -428,7 +431,8 @@ class Merger {
       segs[s].len = sg.len;
       segs[s].body0 = hdr ? 4 : 0;
       segs[s].body_end = sg.len - 4;
-      segs[s].has_header = (hdr ? 1u : 0u) | ((hdr && (sg.flags & TEZGPU_SEG_VERIFIED)) ? 2u : 0u);
+      segs[s].has_header = (hdr ? 1u : 0u) | ((hdr && (sg.flags & TEZGPU_SEG_VERIFIED)) ? 2u : 0u) |
+                           ((hdr && (sg.flags & SEG_DECODED)) ? 4u : 0u);
       segs[s].partition = sg.partition;
       TG_CHECK((int)sg.partition < pipe.conf.num_partitions, TEZGPU_E_INVALID, "segment partition out of range");
       off = align_up(off + sg.len, 16);
@@ -463,12 +467,14 @@ class Merger {
         k_check_headers<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, d_vflags, d_vflags + 1);
         launches++;
       }
-      // ---- checksums of the segments nobody verified yet
+      // ---- checksums of the segments nobody verified yet; a concatenation also needs the body remainder of every
+      //      segment whose trailer is no checksum it can trust (in-memory segments, decoded images)
       std::vector<uint32_t> piece_start(nseg + 1);
       uint32_t np = 0;
       for (uint32_t s = 0; s < nseg; s++) {
         piece_start[s] = np;
-        if (segs[s].has_header == 1u) np += (uint32_t)div_up(segs[s].body_end - segs[s].body0, CRC_PIECE);
+        const uint32_t hh = segs[s].has_header;
+        if (hh == 1u || (concat && (!(hh & 2u) || (hh & 4u)))) np += (uint32_t)div_up(segs[s].body_end - segs[s].body0, CRC_PIECE);
       }
       piece_start[nseg] = np;
       if (np) {
@@ -487,13 +493,20 @@ class Merger {
       }
     }
     auto check_verdicts = [&]() {
-      int f[3] = {0, 0, 0};
-      TG_CUDA(cudaMemcpyAsync(f, d_vflags, 12, cudaMemcpyDeviceToHost, st));
+      int f[4] = {0, 0, 0, 0};
+      TG_CUDA(cudaMemcpyAsync(f, d_vflags, 16, cudaMemcpyDeviceToHost, st));
       TG_CUDA(cudaStreamSynchronize(st));
       TG_CHECK(f[0] == 0, TEZGPU_E_FORMAT, "Not a valid ifile header (segment " + std::to_string(f[0] ? seg_orig[f[0] - 1] : 0) + ")");
       TG_CHECK(f[1] == 0, TEZGPU_E_UNSUPPORTED, "compressed IFile segments are not supported on the device path");
       TG_CHECK(f[2] == 0, TEZGPU_E_FORMAT, "IFile checksum mismatch in segment " + std::to_string(f[2] ? seg_orig[f[2] - 1] : 0));
+      TG_CHECK(f[3] == 0, TEZGPU_E_FORMAT, "IFile segment " + std::to_string(f[3] ? seg_orig[f[3] - 1] : 0) + " does not end in the EOF marker");
     };
+    if (concat) {
+      // tezgpu_concat_open: nothing is parsed or sorted here (concat.cuh)
+      concat_inputs(nseg, d_vflags + 3);
+      check_verdicts();
+      return;
+    }
 
     // ---- records per segment
     h_counts.assign(2 * (size_t)nseg + 2, 0);
@@ -774,7 +787,20 @@ class Merger {
     launches += 2;
   }
 
-  uint64_t raw_output_bound() const { return SortPipeline::output_bound(n, kv_bytes, pipe.conf.num_partitions) + 16; }
+  // ---- concatenation (tezgpu_concat_open, concat.cuh): records leave in (segment, position) order.  The write copies
+  // the record bytes of every input as they are; next_batch parses them on its first call.
+  bool concat = false, concat_parsed = false;
+  uint64_t concat_bytes = 0;              // sum of the input bodies (records + EOF markers)
+  std::vector<uint64_t> cat_rec;          // record bytes of every segment (partition-major, as segs)
+  DeviceBuffer d_cat_tc, d_cat_units, d_cat_parts, d_order;
+  void concat_inputs(uint32_t nseg, int *d_bad_eof);
+  void concat_write(uint8_t *d_out_buf, uint64_t cap, int writer_rle, uint64_t *out_len, int64_t *index, tezgpu_stats *stats);
+  void concat_parse();
+
+  uint64_t raw_output_bound() const {
+    if (concat) return concat_bytes + 10ull * pipe.conf.num_partitions + 64;
+    return SortPipeline::output_bound(n, kv_bytes, pipe.conf.num_partitions) + 16;
+  }
   uint64_t output_bound() const {
     return pipe.codec ? SortPipeline::codec_bound(pipe.codec, raw_output_bound(), pipe.conf.num_partitions) : raw_output_bound();
   }
@@ -797,9 +823,13 @@ class Merger {
     int64_t index[3] = {0, 0, 0};
     uint64_t len = 0;
     tezgpu_stats st;
-    emit(writer_rle, d_out_buf, cap, &len, index, &st);
-    st.output_bytes = (int64_t)kv_bytes;
-    st.kernel_launches += launches - pipe.state.launches;
+    if (concat) {
+      concat_write(d_out_buf, cap, writer_rle, &len, index, &st);
+    } else {
+      emit(writer_rle, d_out_buf, cap, &len, index, &st);
+      st.output_bytes = (int64_t)kv_bytes;
+      st.kernel_launches += launches - pipe.state.launches;
+    }
     if (raw_len) *raw_len = index[1];
     if (part_len) *part_len = index[2];
     if (stats) *stats = st;
@@ -808,9 +838,13 @@ class Merger {
   void write_partitions_device(uint8_t *d_out_buf, uint64_t cap, int writer_rle, uint64_t *out_len, int64_t *index,
                                tezgpu_stats *stats) {
     tezgpu_stats st;
-    emit(writer_rle, d_out_buf, cap, out_len, index, &st);
-    st.output_bytes = (int64_t)kv_bytes;
-    st.kernel_launches += launches - pipe.state.launches;
+    if (concat) {
+      concat_write(d_out_buf, cap, writer_rle, out_len, index, &st);
+    } else {
+      emit(writer_rle, d_out_buf, cap, out_len, index, &st);
+      st.output_bytes = (int64_t)kv_bytes;
+      st.kernel_launches += launches - pipe.state.launches;
+    }
     if (stats) *stats = st;
   }
 
@@ -841,6 +875,7 @@ class Merger {
     cudaStream_t st = pipe.stream;
     *count = 0;
     TG_CHECK(!pipe.combiner, TEZGPU_E_STATE, "a merger with a combiner has no record iterator: use tezgpu_merge_write_*");
+    if (concat) concat_parse();
     if (cursor >= n || idx_cap == 0) return;
     ensure_kvoff();
     uint32_t *d_cnt = pipe.d_large();

@@ -11,6 +11,7 @@
 
 #include "../../include/tezgpu.h"
 #include "codec.cuh"
+#include "concat.cuh"
 #include "merger.cuh"
 #include "sorter.cuh"
 #include "peer_fetch.cuh"
@@ -427,6 +428,31 @@ int32_t tezgpu_debug_zstd_decompress_emulate(const uint8_t *z, uint64_t len, uin
   const int32_t rc = zs_decompress(z, len, out, body_len, &got, *d);
   *out_len = got;
   TG_CHECK(rc == ZS_OK, TEZGPU_E_FORMAT, std::string("compressed segment 0: ") + zs_err_name(rc));
+  TG_API_END
+}
+
+int32_t tezgpu_debug_crc_concat_emulate(const uint8_t *const *bodies, const uint64_t *lens, uint32_t n, uint32_t *crc) {
+  TG_API_BEGIN
+  TG_CHECK(((bodies && lens) || n == 0) && crc, TEZGPU_E_INVALID, "null argument");
+  std::unique_ptr<CrcTables> t(new CrcTables());
+  crc_build_tables(*t, EMIT_CRC_STRIDE_WORDS);
+  // every input's IFile checksum, as its trailer carries it; from here on only the algebra of concat.cuh
+  uint32_t acc = 0;   // raw remainder of the records so far
+  uint64_t rec_total = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    const uint8_t *b = bodies[i];
+    const uint64_t len = lens[i];
+    TG_CHECK(len >= 2 && b && b[len - 2] == 0xFF && b[len - 1] == 0xFF, TEZGPU_E_FORMAT,
+             "body " + std::to_string(i) + " does not end in the EOF marker");
+    uint32_t c = 0xFFFFFFFFu;
+    for (uint64_t k = 0; k < len; k++) c = t->slice[0][(c ^ b[k]) & 0xFF] ^ (c >> 8);
+    const uint32_t stored = ~c;
+    const uint32_t body_raw = stored ^ 0xFFFFFFFFu ^ crc_multmodp(0xFFFFFFFFu, crc_host_xpow8(len));
+    acc = crc_multmodp(acc, crc_host_xpow8(len - 2)) ^ concat_records_raw(body_raw, *t);   // crc(A||B)
+    rec_total += len - 2;
+  }
+  const uint32_t raw = crc_multmodp(acc, crc_host_xpow8(2)) ^ t->eof_raw;
+  *crc = raw ^ crc_multmodp(0xFFFFFFFFu, crc_host_xpow8(rec_total + 2)) ^ 0xFFFFFFFFu;
   TG_API_END
 }
 

@@ -137,14 +137,16 @@ class GpuSorter:
 class GpuMerger:
     def __init__(self, segments, comparator=CMP_BYTES, device=0, has_header=True, device_ptrs=False, fixed=None,
                  partitions=None, num_partitions=1, send_empty=True, verified=None, combiner=COMBINE_NONE,
-                 codec=CODEC_NONE, raw_lens=None):
+                 codec=CODEC_NONE, raw_lens=None, concat=False):
         """segments: list of bytes / uint8 arrays (host) or (ptr, len) tuples when device_ptrs.
         verified: optional per-segment booleans -- the transport already checked that segment's checksum
         (TEZGPU_SEG_VERIFIED: fetch_segments_verified), the merge does not read it again to verify.
         combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG combines the merged stream in write_* (tezgpu_merge_set_combiner).
         codec: CODEC_DEFAULT (zlib), CODEC_LZ4 (Lz4Codec) or CODEC_ZSTD (ZStandardCodec) reads compressed (TIF\\x01) segments of that codec and writes
         compressed output (tezgpu_merge_open_codec); raw_lens: per-segment rawLength, required for the compressed
-        segments."""
+        segments.
+        concat: UnorderedPartitionedKVWriter.mergeAll / UnorderedKVReader (tezgpu_concat_open): records leave in
+        (segment, position) order, the writes copy the record bytes (rle must be False)."""
         self.L = _lib.load()
         self.conf = make_conf(num_partitions, comparator=comparator, partitioner=PART_GIVEN, device=device, fixed=fixed,
                               send_empty=send_empty)
@@ -152,7 +154,10 @@ class GpuMerger:
         self._has_header, self._device_ptrs = has_header, device_ptrs
         arr = self._segments(segments, partitions, verified)
         self.h = C.c_void_p()
-        if codec:
+        if concat:
+            check(self.L.tezgpu_concat_open(C.byref(self.conf), arr, _ptr(self._raw(raw_lens)), len(segments), codec,
+                                            C.byref(self.h)))
+        elif codec:
             check(self.L.tezgpu_merge_open_codec(C.byref(self.conf), arr, _ptr(self._raw(raw_lens)), len(segments), codec,
                                                  C.byref(self.h)))
         else:

@@ -109,11 +109,13 @@ class OrderedPartitionedKVOutput:
         self.context = context
         self.num_physical_outputs = num_physical_outputs
         self._h = C.c_void_p()
-        check_rt(self._L.tezrt_output_create(_conf_text(context.conf), context.work_dir.encode(),
-                                             context.unique_identifier.encode(),
-                                             context.destination_vertex_name.encode(), context.host.encode(),
-                                             context.shuffle_port, context.total_memory_available_to_task,
-                                             num_physical_outputs, context.device, C.byref(self._h)))
+        c = context
+        check_rt(self._create(_conf_text(c.conf), c.work_dir.encode(), c.unique_identifier.encode(),
+                              c.destination_vertex_name.encode(), c.host.encode(), c.shuffle_port,
+                              c.total_memory_available_to_task, num_physical_outputs, c.device, C.byref(self._h)))
+
+    def _create(self, *args):
+        return self._L.tezrt_output_create(*args)
 
     def initialize(self):
         req = C.c_int64()
@@ -163,6 +165,19 @@ class OrderedPartitionedKVOutput:
         if getattr(self, "_h", None):
             self._L.tezrt_output_destroy(self._h)
             self._h = None
+
+
+class UnorderedPartitionedKVOutput(OrderedPartitionedKVOutput):
+    """The same output with the writer of UnorderedPartitionedKVWriter: partitioned, no key order, no combiner."""
+    _partitioned = 1
+
+    def _create(self, *args):
+        return self._L.tezrt_output_create_unordered(*args[:-2], self._partitioned, *args[-2:])
+
+
+class UnorderedKVOutput(UnorderedPartitionedKVOutput):
+    """Broadcast / one-to-one output: one writer partition whatever numPhysicalOutputs is (UnorderedKVOutput.java:107)."""
+    _partitioned = 0
 
 
 @dataclass
@@ -220,9 +235,12 @@ class OrderedGroupedKVInput:
         self._L = _lib.load()
         self.context = context
         self._h = C.c_void_p()
-        check_rt(self._L.tezrt_input_create(_conf_text(context.conf), context.work_dir.encode(),
-                                            context.unique_identifier.encode(), context.total_memory_available_to_task,
-                                            num_physical_inputs, context.device, C.byref(self._h)))
+        check_rt(self._create(_conf_text(context.conf), context.work_dir.encode(), context.unique_identifier.encode(),
+                              context.total_memory_available_to_task, num_physical_inputs, context.device,
+                              C.byref(self._h)))
+
+    def _create(self, *args):
+        return self._L.tezrt_input_create(*args)
 
     def initialize(self):
         req = C.c_int64()
@@ -261,3 +279,38 @@ class OrderedGroupedKVInput:
         if getattr(self, "_h", None):
             self._L.tezrt_input_destroy(self._h)
             self._h = None
+
+
+class KeyValueReader:
+    """UnorderedKVReader: next() / getCurrentKey() / getCurrentValue(), every record in turn."""
+
+    def __init__(self, inp):
+        self._in = inp
+        self._key = self._val = None
+
+    def next(self):
+        k, kl, v, vl = C.c_void_p(), C.c_uint32(), C.c_void_p(), C.c_uint32()
+        rc = self._in._L.tezrt_input_next_kv(self._in._h, C.byref(k), C.byref(kl), C.byref(v), C.byref(vl))
+        if rc < 0:
+            check_rt(rc)
+        if rc == 0:
+            return False
+        self._key = C.string_at(k.value, kl.value) if kl.value else b""
+        self._val = C.string_at(v.value, vl.value) if vl.value else b""
+        return True
+
+    def getCurrentKey(self):
+        return self._key
+
+    def getCurrentValue(self):
+        return self._val
+
+
+class UnorderedKVInput(OrderedGroupedKVInput):
+    """Reads every delivered input in turn, no merge: delivery order, the spills of one source in spill-id order."""
+
+    def _create(self, *args):
+        return self._L.tezrt_input_create_unordered(*args)
+
+    def getReader(self):
+        return KeyValueReader(self)
