@@ -10,6 +10,12 @@
 
 namespace tezgpu {
 
+// the codecs the device writes and reads (TEZGPU_CODEC_*)
+inline void check_codec(int32_t codec) {
+  TG_CHECK(codec == TEZGPU_CODEC_NONE || codec == TEZGPU_CODEC_DEFAULT || codec == TEZGPU_CODEC_LZ4 || codec == TEZGPU_CODEC_ZSTD,
+           TEZGPU_E_UNSUPPORTED, "codec " + std::to_string(codec) + " is not on the device (DefaultCodec, Lz4Codec and ZStandardCodec only)");
+}
+
 // The uncompressed file is in z_img with its index raw_index (start, rawLength, partLength per partition).  Every
 // partition that has a segment gets a compressed one: TIF\x01, the codec stream of the same body (zlib, or LZ4 blocks),
 // CRC-32 of the stream.  index receives (start, the same rawLength, compressed length).  One host round trip (the
@@ -69,13 +75,9 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
       k_zdeflate<<<nchunks, ZLANES, sizeof(ZShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
                                                           z_csize.as<uint32_t>(), z_cadler.as<uint32_t>());
     }
-    const uint32_t nblk = (uint32_t)div_up(nchunks, SCAN_TILE);
-    blk.ensure(((size_t)nblk + 2) * 8);
-    k_sum_u32_blocks<<<nblk, SCAN_THREADS, 0, st>>>(z_csize.as<uint32_t>(), nchunks, blk.as<uint64_t>());
-    k_scan_block_sums<<<1, 1024, 0, st>>>(blk.as<uint64_t>(), nblk);
-    k_scan_u32_apply<<<nblk, SCAN_THREADS, 0, st>>>(z_csize.as<uint32_t>(), nchunks, blk.as<uint64_t>(), z_coff.as<uint64_t>());
+    launches += 1 + scan_u32_exclusive(st, blk, z_csize.as<uint32_t>(), nchunks, z_coff.as<uint64_t>());
     k_zseg_layout<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_coff.as<uint64_t>(), frame);
-    launches += 5;
+    launches++;
     TG_CUDA(cudaGetLastError());
     TG_CUDA(cudaMemcpyAsync(hs, z_segs.p, (size_t)P * sizeof(ZSeg), cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(hs) + (size_t)P * sizeof(ZSeg), z_coff.as<uint64_t>() + nchunks, 8,
@@ -189,33 +191,18 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
     zi[i].dst = z_img.as<uint8_t>() + img_off[i];
     zi[i].body = (uint64_t)raw_len[zs[i]] - 4;
   }
-  // checksums of the compressed bytes: the open() machinery over the staged segments
-  std::vector<uint32_t> piece_start(nz + 1);
-  uint32_t np = 0;
-  for (uint32_t i = 0; i < nz; i++) {
-    piece_start[i] = np;
-    if (sd[i].has_header == 1u) np += (uint32_t)div_up(sd[i].body_end - sd[i].body0, CRC_PIECE);
-  }
-  piece_start[nz] = np;
   z_descs.ensure((size_t)nz * sizeof(SegDesc));
   z_insegs.ensure((size_t)nz * sizeof(ZInSeg));
-  z_pstart.ensure(((size_t)nz + 1) * 4);
   z_status.ensure((size_t)nz * 4 + 16);
   z_flag.ensure(16);
   TG_CUDA(cudaMemcpyAsync(z_descs.p, sd.data(), (size_t)nz * sizeof(SegDesc), cudaMemcpyHostToDevice, st));
   TG_CUDA(cudaMemcpyAsync(z_insegs.p, zi.data(), (size_t)nz * sizeof(ZInSeg), cudaMemcpyHostToDevice, st));
-  TG_CUDA(cudaMemcpyAsync(z_pstart.p, piece_start.data(), ((size_t)nz + 1) * 4, cudaMemcpyHostToDevice, st));
   TG_CUDA(cudaMemsetAsync(z_flag.p, 0, 16, st));
-  const CrcTables *d_crc = DeviceConstants::get(pipe.conf.device).d_crc;
-  if (np) {
-    z_tc.ensure((size_t)np * sizeof(TileCrc));
-    z_crc.ensure((size_t)nz * 4);
-    TG_CUDA(cudaMemsetAsync(z_crc.p, 0, (size_t)nz * 4, st));
-    k_crc_pieces<<<np, CRCV_THREADS, 0, st>>>(z_in.as<uint8_t>(), z_descs.as<SegDesc>(), z_pstart.as<uint32_t>(), nz, d_crc, z_tc.as<TileCrc>());
-    k_crc_combine<<<(uint32_t)div_up(np, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), np, d_crc, z_crc.as<uint32_t>());
-    k_crc_check<<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_in.as<uint8_t>(), z_descs.as<SegDesc>(), nz, z_crc.as<uint32_t>(), d_crc, z_flag.as<int>());
-    launches += 3;
-  }
+  // checksums of the compressed bytes: the open() machinery over the staged segments.  piece_start lives until the
+  // verdict read below; open() reuses the checksum buffers only after it.
+  std::vector<uint32_t> piece_start;
+  launches += check_checksums(z_in.as<uint8_t>(), sd, z_descs.as<SegDesc>(), [](const SegDesc &d) { return d.has_header == 1u; },
+                              piece_start, false, z_flag.as<int>());
   const bool lz4 = pipe.codec == TEZGPU_CODEC_LZ4, zstd = pipe.codec == TEZGPU_CODEC_ZSTD;
   if (zstd) {
     z_nblk.ensure((size_t)nz * 4);

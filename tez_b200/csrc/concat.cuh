@@ -277,36 +277,19 @@ inline void Merger::concat_parse() {
   TG_CUDA(cudaSetDevice(pipe.conf.device));
   cudaStream_t st = pipe.stream;
   const uint32_t nseg = (uint32_t)segs.size();
-  h_counts.assign(2 * (size_t)nseg + 2, 0);
-  h_rec_base.assign(nseg + 1, 0);
-  n = kv_bytes = 0;
-  const uint32_t hl = vint_size_u32(fixed_klen) + vint_size_u32(fixed_vlen), rs = hl + fixed_klen + fixed_vlen;
-  bool fixed_ok = nseg > 0 && fixed_klen + fixed_vlen > 0 && hl <= 8;
-  for (uint32_t s = 0; s < nseg && fixed_ok; s++) {
-    fixed_ok = cat_rec[s] % rs == 0;
-    h_counts[s] = cat_rec[s] / rs;
-  }
+  bool fixed_ok = count_fixed_records(nseg, 8);
   if (fixed_ok) {
-    for (uint32_t s = 0; s < nseg; s++) { h_rec_base[s] = n; n += h_counts[s]; }
-    h_rec_base[nseg] = n;
-    kv_bytes = n * (uint64_t)(fixed_klen + fixed_vlen);
-    TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one merge");
     d_rec_base.ensure((size_t)(nseg + 2) * 8);
     TG_CUDA(cudaMemcpyAsync(d_rec_base.p, h_rec_base.data(), (size_t)(nseg + 1) * 8, cudaMemcpyHostToDevice, st));
-    d_koff.ensure((size_t)(n ? n : 1) * 8); d_voff.ensure((size_t)(n ? n : 1) * 8);
-    d_klen.ensure((size_t)(n ? n : 1) * 4); d_vlen.ensure((size_t)(n ? n : 1) * 4); d_tag.ensure((size_t)(n ? n : 1) * 4); d_part.ensure((size_t)(n ? n : 1) * 4);
-    ParseArrays pa{d_koff.as<uint64_t>(), d_voff.as<uint64_t>(), d_klen.as<uint32_t>(), d_vlen.as<uint32_t>(), d_tag.as<uint32_t>(), d_part.as<int32_t>()};
-    uint64_t hb = 0;
-    int b = 0;
-    for (int i = 0; i < vint_size_u32(fixed_klen); i++) hb |= (uint64_t)vint_byte_u32(fixed_klen, i) << (8 * b++);
-    for (int i = 0; i < vint_size_u32(fixed_vlen); i++) hb |= (uint64_t)vint_byte_u32(fixed_vlen, i) << (8 * b++);
+    const ParseArrays pa = record_arrays(n);
+    const FixedFraming f = fixed_framing(fixed_klen, fixed_vlen);
     int *d_bad = pipe.d_error();
     TG_CUDA(cudaMemsetAsync(d_bad, 0, 4, st));
     int bad = 0;
     if (n) {
       const uint32_t grid = (uint32_t)std::min<uint64_t>(div_up(n, 256), (uint64_t)pipe.num_sms * 16);
-      k_fill_fixed_arrays<<<grid, 256, 0, st>>>(d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), fixed_klen, fixed_vlen, hl, pa);
-      k_concat_check_fixed<<<grid, 256, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), rs, hl, hb, d_bad);
+      k_fill_fixed_arrays<<<grid, 256, 0, st>>>(d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), fixed_klen, fixed_vlen, f.len, pa);
+      k_concat_check_fixed<<<grid, 256, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), f.rec_size, f.len, f.packed(), d_bad);
       launches += 2;
       TG_CUDA(cudaGetLastError());
       TG_CUDA(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
@@ -317,16 +300,8 @@ inline void Merger::concat_parse() {
     parse_rounds = 0;
   }
   if (!fixed_ok) {
-    TG_CUDA(cudaMemsetAsync(pipe.small.p, 0, 16384, st));
-    d_counts.ensure((size_t)(nseg + 1) * 16);
-    d_rec_base.ensure((size_t)(nseg + 2) * 8);
-    n = kv_bytes = 0;
-    if (nseg) {
-      open_general_reparse(nseg, h_counts, h_rec_base);
-    } else {
-      d_koff.ensure(8); d_voff.ensure(8); d_klen.ensure(4); d_vlen.ensure(4); d_tag.ensure(4); d_part.ensure(4);
-      parse_mode = 1;
-    }
+    find_records_general(nseg);
+    if (!nseg) parse_mode = 1;
   }
   arrays_ready = true;
   pipe.state.rec = array_records();

@@ -152,15 +152,6 @@ __device__ __forceinline__ bool read_vlong_dev(const uint8_t *p, uint64_t &pos, 
   return true;
 }
 
-struct ParseArrays {
-  uint64_t *key_off;
-  uint64_t *val_off;
-  uint32_t *key_len;
-  uint32_t *val_len;
-  uint32_t *tag;  // (segment << 1) | read as SAME_KEY (run-length encoded in the input)
-  int32_t *partition;
-};
-
 // Walks the segments with IFile.Reader semantics (positionToNextRecord / readRawKey / nextRawValue,
 // SORT/IFile.java:877-1000).  One WARP per segment: the 32 lanes stage a 4 KiB window of the body in shared memory with
 // coalesced loads, lane 0 decodes the record headers out of it (key / value bytes are skipped, never read), so a walk
@@ -395,13 +386,14 @@ class Merger {
   bool arrays_ready = false;   // the per-record metadata arrays (d_koff ...) are filled (never in run-table mode unless asked)
   std::vector<uint64_t> h_counts, h_rec_base;
 
-  void open(const tezgpu_segment *in, uint32_t nseg) {
+  // ---- intake: builds the segment table (segs, d_segs) and launches the header and checksum checks, whose verdicts
+  //      check_verdicts() reads.  Segments already on this device are used in place (no copy; kernels handle any byte
+  //      alignment); host segments are staged contiguously with 16-byte aligned starts.
+  void intake(const tezgpu_segment *in, uint32_t nseg) {
     cudaStream_t st = pipe.stream;
     TG_CUDA(cudaSetDevice(pipe.conf.device));
     parsed_fixed = false;
     arrays_ready = false;
-    // ---- segments already on this device are used in place (no copy; kernels handle any byte alignment);
-    //      host segments are staged contiguously with 16-byte aligned starts
     segs.resize(nseg);
     bool all_device = nseg > 0;
     for (uint32_t s = 0; s < nseg; s++) all_device &= (in[s].flags & TEZGPU_SEG_DEVICE) != 0;
@@ -461,7 +453,6 @@ class Merger {
     d_flags.ensure(64);
     TG_CUDA(cudaMemsetAsync(d_flags.p, 0, 64, st));
     int *d_vflags = d_flags.as<int>();
-    const CrcTables *d_crc = DeviceConstants::get(pipe.conf.device).d_crc;
     if (nseg) {
       if (any_header) {
         k_check_headers<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, d_vflags, d_vflags + 1);
@@ -469,68 +460,37 @@ class Merger {
       }
       // ---- checksums of the segments nobody verified yet; a concatenation also needs the body remainder of every
       //      segment whose trailer is no checksum it can trust (in-memory segments, decoded images)
-      std::vector<uint32_t> piece_start(nseg + 1);
-      uint32_t np = 0;
-      for (uint32_t s = 0; s < nseg; s++) {
-        piece_start[s] = np;
-        const uint32_t hh = segs[s].has_header;
-        if (hh == 1u || (concat && (!(hh & 2u) || (hh & 4u)))) np += (uint32_t)div_up(segs[s].body_end - segs[s].body0, CRC_PIECE);
-      }
-      piece_start[nseg] = np;
-      if (np) {
-        d_piece_start.ensure((size_t)(nseg + 1) * 4);
-        TG_CUDA(cudaMemcpyAsync(d_piece_start.p, piece_start.data(), (size_t)(nseg + 1) * 4, cudaMemcpyHostToDevice, st));
-        TG_CUDA(cudaStreamSynchronize(st));  // piece_start is a stack-lifetime vector
-        d_piece_crc.ensure((size_t)np * sizeof(TileCrc));
-        d_seg_crc.ensure((size_t)nseg * 4);
-        TG_CUDA(cudaMemsetAsync(d_seg_crc.p, 0, (size_t)nseg * 4, st));
-        k_crc_pieces<<<np, CRCV_THREADS, 0, st>>>(data, d_segs.as<SegDesc>(), d_piece_start.as<uint32_t>(), nseg, d_crc,
-                                                  d_piece_crc.as<TileCrc>());
-        k_crc_combine<<<(uint32_t)div_up(np, 256), 256, 0, st>>>(d_piece_crc.as<TileCrc>(), np, d_crc, d_seg_crc.as<uint32_t>());
-        k_crc_check<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, d_seg_crc.as<uint32_t>(), d_crc, d_vflags + 2);
-        launches += 3;
-        TG_CUDA(cudaGetLastError());
-      }
+      std::vector<uint32_t> piece_start;
+      launches += check_checksums(data, segs, d_segs.as<SegDesc>(), [&](const SegDesc &sd) {
+        return sd.has_header == 1u || (concat && (!(sd.has_header & 2u) || (sd.has_header & 4u)));
+      }, piece_start, true, d_vflags + 2);
     }
-    auto check_verdicts = [&]() {
-      int f[4] = {0, 0, 0, 0};
-      TG_CUDA(cudaMemcpyAsync(f, d_vflags, 16, cudaMemcpyDeviceToHost, st));
-      TG_CUDA(cudaStreamSynchronize(st));
-      TG_CHECK(f[0] == 0, TEZGPU_E_FORMAT, "Not a valid ifile header (segment " + std::to_string(f[0] ? seg_orig[f[0] - 1] : 0) + ")");
-      TG_CHECK(f[1] == 0, TEZGPU_E_UNSUPPORTED, "compressed IFile segments are not supported on the device path");
-      TG_CHECK(f[2] == 0, TEZGPU_E_FORMAT, "IFile checksum mismatch in segment " + std::to_string(f[2] ? seg_orig[f[2] - 1] : 0));
-      TG_CHECK(f[3] == 0, TEZGPU_E_FORMAT, "IFile segment " + std::to_string(f[3] ? seg_orig[f[3] - 1] : 0) + " does not end in the EOF marker");
-    };
+  }
+
+  // waits for the verdict words and throws the first one set
+  void check_verdicts() {
+    cudaStream_t st = pipe.stream;
+    int f[4] = {0, 0, 0, 0};
+    TG_CUDA(cudaMemcpyAsync(f, d_flags.p, 16, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaStreamSynchronize(st));
+    TG_CHECK(f[0] == 0, TEZGPU_E_FORMAT, "Not a valid ifile header (segment " + std::to_string(f[0] ? seg_orig[f[0] - 1] : 0) + ")");
+    TG_CHECK(f[1] == 0, TEZGPU_E_UNSUPPORTED, "compressed IFile segments are not supported on the device path");
+    TG_CHECK(f[2] == 0, TEZGPU_E_FORMAT, "IFile checksum mismatch in segment " + std::to_string(f[2] ? seg_orig[f[2] - 1] : 0));
+    TG_CHECK(f[3] == 0, TEZGPU_E_FORMAT, "IFile segment " + std::to_string(f[3] ? seg_orig[f[3] - 1] : 0) + " does not end in the EOF marker");
+  }
+
+  void open(const tezgpu_segment *in, uint32_t nseg) {
+    intake(in, nseg);
     if (concat) {
       // tezgpu_concat_open: nothing is parsed or sorted here (concat.cuh)
-      concat_inputs(nseg, d_vflags + 3);
+      concat_inputs(nseg, d_flags.as<int>() + 3);
       check_verdicts();
       return;
     }
-
-    // ---- records per segment
-    h_counts.assign(2 * (size_t)nseg + 2, 0);
-    h_rec_base.assign(nseg + 1, 0);
-    bool fixed_ok = false;
-    const uint32_t rs = vint_size_u32(fixed_klen) + vint_size_u32(fixed_vlen) + fixed_klen + fixed_vlen;
-    if (nseg && fixed_klen + fixed_vlen > 0) {
-      // candidate: every body is exactly k records of the fixed framing + EOF markers
-      fixed_ok = true;
-      for (uint32_t s = 0; s < nseg && fixed_ok; s++) {
-        uint64_t body = segs[s].body_end - segs[s].body0;
-        fixed_ok = body >= 2 && (body - 2) % rs == 0;
-        h_counts[s] = fixed_ok ? (body - 2) / rs : 0;
-        h_counts[nseg + s] = h_counts[s] * (fixed_klen + fixed_vlen);
-      }
-    }
-    if (fixed_ok) {
+    if (count_fixed_records(nseg, FRAMING_MAX_LEN)) {
       // ---- run-table mode: offsets are arithmetic, the stage kernel checks the framing bytes it passes over anyway.
       //      No per-record arrays, no host round trip before the sort's own.
-      n = 0;
-      kv_bytes = 0;
-      for (uint32_t s = 0; s < nseg; s++) { h_rec_base[s] = n; n += h_counts[s]; kv_bytes += h_counts[nseg + s]; }
-      h_rec_base[nseg] = n;
-      TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one merge");
+      cudaStream_t st = pipe.stream;
       std::vector<uint64_t> roff(nseg);
       std::vector<uint32_t> rbase(nseg + 1), rpart(nseg);
       for (uint32_t s = 0; s < nseg; s++) { roff[s] = segs[s].off + segs[s].body0; rbase[s] = (uint32_t)h_rec_base[s]; rpart[s] = segs[s].partition; }
@@ -546,6 +506,7 @@ class Merger {
       TG_CUDA(cudaMemcpyAsync(d_run_base.p, rbase.data(), (size_t)(nseg + 1) * 4, cudaMemcpyHostToDevice, st));
       TG_CUDA(cudaMemcpyAsync(d_run_part.p, rpart.data(), (size_t)nseg * 4, cudaMemcpyHostToDevice, st));
       TG_CUDA(cudaStreamSynchronize(st));  // stack-lifetime staging vectors (and: the caller's host segments may go away)
+      const FixedFraming f = fixed_framing(fixed_klen, fixed_vlen);
       Records r;
       memset(&r, 0, sizeof(r));
       r.kv = data;
@@ -560,13 +521,9 @@ class Merger {
       r.runs.seg_part = d_run_part.as<uint32_t>();
       r.runs.part_seg0 = d_run_pseg.as<uint32_t>();
       r.runs.nseg = nseg;
-      r.runs.rec_size = rs;
-      r.runs.hdr_len = vint_size_u32(fixed_klen) + vint_size_u32(fixed_vlen);
-      uint64_t hb = 0;
-      int b = 0;
-      for (int i = 0; i < vint_size_u32(fixed_klen); i++) hb |= (uint64_t)vint_byte_u32(fixed_klen, i) << (8 * b++);
-      for (int i = 0; i < vint_size_u32(fixed_vlen); i++) hb |= (uint64_t)vint_byte_u32(fixed_vlen, i) << (8 * b++);
-      r.runs.hdr_bytes = hb;
+      r.runs.rec_size = f.rec_size;
+      r.runs.hdr_len = f.len;
+      r.runs.hdr_bytes = f.packed();
       bool mismatch = false;
       pipe.merge_inputs_plain = true;
       try {
@@ -587,29 +544,87 @@ class Merger {
     } else {
       check_verdicts();  // also: the caller's host buffers may go away after open()
     }
+    find_records_general(nseg);
 
-    // ---- general path: walk the segments (IFile.Reader semantics), materialise the per-record metadata
-    int *d_bad = pipe.d_error();
-    TG_CUDA(cudaMemsetAsync(pipe.small.p, 0, 16384, st));
+    // ---- merge = stable sort of the union of the runs by the RawComparator
+    pipe.merge_inputs_plain = false;
+    pipe.sort_phase(array_records());
+    launches += pipe.state.launches;
+    cursor = 0;
+    have_kvoff = false;
+  }
+
+  // Checksums of the segments `need` selects (open() and open_codec()): raw CRC remainders of 64 KiB pieces of each
+  // body, folded per segment into d_seg_crc and compared with the trailer; a mismatch writes segment + 1 to *d_bad.
+  // piece_start receives the host piece table, which must live until the stream has copied it: sync_copy waits for
+  // the copy here, otherwise the caller keeps the table until its next synchronise.  Returns the launches.
+  template <typename Need>
+  int check_checksums(const uint8_t *bytes, const std::vector<SegDesc> &sd, const SegDesc *d_sd, Need need,
+                      std::vector<uint32_t> &piece_start, bool sync_copy, int *d_bad) {
+    cudaStream_t st = pipe.stream;
+    const uint32_t nseg = (uint32_t)sd.size();
+    piece_start.resize(nseg + 1);
+    uint32_t np = 0;
+    for (uint32_t s = 0; s < nseg; s++) {
+      piece_start[s] = np;
+      if (need(sd[s])) np += (uint32_t)div_up(sd[s].body_end - sd[s].body0, CRC_PIECE);
+    }
+    piece_start[nseg] = np;
+    if (!np) return 0;
+    const CrcTables *d_crc = DeviceConstants::get(pipe.conf.device).d_crc;
+    d_piece_start.ensure((size_t)(nseg + 1) * 4);
+    TG_CUDA(cudaMemcpyAsync(d_piece_start.p, piece_start.data(), (size_t)(nseg + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (sync_copy) TG_CUDA(cudaStreamSynchronize(st));
+    d_piece_crc.ensure((size_t)np * sizeof(TileCrc));
+    d_seg_crc.ensure((size_t)nseg * 4);
+    TG_CUDA(cudaMemsetAsync(d_seg_crc.p, 0, (size_t)nseg * 4, st));
+    k_crc_pieces<<<np, CRCV_THREADS, 0, st>>>(bytes, d_sd, d_piece_start.as<uint32_t>(), nseg, d_crc, d_piece_crc.as<TileCrc>());
+    k_crc_combine<<<(uint32_t)div_up(np, 256), 256, 0, st>>>(d_piece_crc.as<TileCrc>(), np, d_crc, d_seg_crc.as<uint32_t>());
+    k_crc_check<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(bytes, d_sd, nseg, d_seg_crc.as<uint32_t>(), d_crc, d_bad);
+    TG_CUDA(cudaGetLastError());
+    return 3;
+  }
+
+  // ---- record finding, shared by open() and concat_parse().  Run-table candidate: every body is exactly k records of
+  //      the fixed framing (at most max_len bytes) + EOF markers.  Fills h_counts / h_rec_base, n and kv_bytes when it
+  //      holds and returns whether it does.
+  bool count_fixed_records(uint32_t nseg, uint32_t max_len) {
+    h_counts.assign(2 * (size_t)nseg + 2, 0);
+    h_rec_base.assign(nseg + 1, 0);
+    n = kv_bytes = 0;
+    const FixedFraming f = fixed_framing(fixed_klen, fixed_vlen);
+    if (!nseg || fixed_klen + fixed_vlen == 0 || f.len > max_len) return false;
+    for (uint32_t s = 0; s < nseg; s++) {
+      const uint64_t body = segs[s].body_end - segs[s].body0;
+      if (body < 2 || (body - 2) % f.rec_size) return false;
+      h_counts[s] = (body - 2) / f.rec_size;
+    }
+    for (uint32_t s = 0; s < nseg; s++) { h_rec_base[s] = n; n += h_counts[s]; }
+    h_rec_base[nseg] = n;
+    kv_bytes = n * (uint64_t)(fixed_klen + fixed_vlen);
+    TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one merge");
+    return true;
+  }
+
+  // general path: walk the segments (IFile.Reader semantics), materialise the per-record metadata
+  void find_records_general(uint32_t nseg) {
+    TG_CUDA(cudaMemsetAsync(pipe.small.p, 0, 16384, pipe.stream));
     d_counts.ensure((size_t)(nseg + 1) * 16);
     d_rec_base.ensure((size_t)(nseg + 2) * 8);
     n = 0;
     kv_bytes = 0;
     if (nseg) open_general_reparse(nseg, h_counts, h_rec_base);
-    else {
-      d_koff.ensure(8); d_voff.ensure(8); d_klen.ensure(4); d_vlen.ensure(4); d_tag.ensure(4); d_part.ensure(4);
-    }
-    (void)d_bad;
+    else record_arrays(0);
     TG_CUDA(cudaGetLastError());
     arrays_ready = true;
+  }
 
-    // ---- merge = stable sort of the union of the runs by the RawComparator
-    Records r = array_records();
-    pipe.merge_inputs_plain = false;
-    pipe.sort_phase(r);
-    launches += pipe.state.launches;
-    cursor = 0;
-    have_kvoff = false;
+  // the per-record metadata arrays, sized for nrec records
+  ParseArrays record_arrays(uint64_t nrec) {
+    const size_t m = (size_t)(nrec ? nrec : 1);
+    d_koff.ensure(m * 8); d_voff.ensure(m * 8);
+    d_klen.ensure(m * 4); d_vlen.ensure(m * 4); d_tag.ensure(m * 4); d_part.ensure(m * 4);
+    return {d_koff.as<uint64_t>(), d_voff.as<uint64_t>(), d_klen.as<uint32_t>(), d_vlen.as<uint32_t>(), d_tag.as<uint32_t>(), d_part.as<int32_t>()};
   }
 
   // Records over the materialised per-record arrays
@@ -637,13 +652,10 @@ class Merger {
     const uint32_t nseg = (uint32_t)segs.size();
     d_rec_base.ensure((size_t)(nseg + 2) * 8);
     TG_CUDA(cudaMemcpyAsync(d_rec_base.p, h_rec_base.data(), (size_t)(nseg + 1) * 8, cudaMemcpyHostToDevice, st));
-    d_koff.ensure((size_t)(n ? n : 1) * 8); d_voff.ensure((size_t)(n ? n : 1) * 8);
-    d_klen.ensure((size_t)(n ? n : 1) * 4); d_vlen.ensure((size_t)(n ? n : 1) * 4); d_tag.ensure((size_t)(n ? n : 1) * 4); d_part.ensure((size_t)(n ? n : 1) * 4);
-    ParseArrays pa{d_koff.as<uint64_t>(), d_voff.as<uint64_t>(), d_klen.as<uint32_t>(), d_vlen.as<uint32_t>(), d_tag.as<uint32_t>(), d_part.as<int32_t>()};
+    const ParseArrays pa = record_arrays(n);
     if (n) {
-      const uint32_t hl = vint_size_u32(fixed_klen) + vint_size_u32(fixed_vlen);
       k_fill_fixed_arrays<<<(uint32_t)std::min<uint64_t>(div_up(n, 256), (uint64_t)pipe.num_sms * 16), 256, 0, st>>>(
-          d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), fixed_klen, fixed_vlen, hl, pa);
+          d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), fixed_klen, fixed_vlen, fixed_framing(fixed_klen, fixed_vlen).len, pa);
       launches++;
       TG_CUDA(cudaGetLastError());
     }
@@ -689,17 +701,14 @@ class Merger {
     d_pwflags.ensure(64);
     TG_CUDA(cudaMemcpyAsync(d_pwseg.p, ps.data(), (size_t)nseg * sizeof(PwSeg), cudaMemcpyHostToDevice, st));
     const uint32_t grid = (uint32_t)div_up(nwin, PW_THREADS);
-    PwArrays none{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    ParseArrays none{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     // guess -> evaluate from the guessed entries -> chase the true chain (parse_windows.cuh); one host round trip
     TG_CUDA(cudaMemsetAsync(d_pwflags.p, 0, 64, st));
     PwFixedHint hint{0, 0, 0, 0};
-    if (fixed_klen + fixed_vlen > 0 && vint_size_u32(fixed_klen) + vint_size_u32(fixed_vlen) <= 7) {
-      int b = 0;
-      for (int i = 0; i < vint_size_u32(fixed_klen); i++) hint.full |= (uint64_t)vint_byte_u32(fixed_klen, i) << (8 * b++);
-      for (int i = 0; i < vint_size_u32(fixed_vlen); i++) hint.full |= (uint64_t)vint_byte_u32(fixed_vlen, i) << (8 * b++);
-      hint.full_len = (uint32_t)b;
-      for (int i = 0; i < vint_size_u32(fixed_vlen); i++) hint.rep |= (uint64_t)vint_byte_u32(fixed_vlen, i) << (8 * i);
-      hint.rep_len = (uint32_t)vint_size_u32(fixed_vlen);
+    const FixedFraming f = fixed_framing(fixed_klen, fixed_vlen);
+    if (fixed_klen + fixed_vlen > 0 && f.len <= 7) {
+      const uint32_t vl = (uint32_t)vint_size_u32(fixed_vlen);   // the framing ends in vint(vlen)
+      hint = PwFixedHint{f.packed(), f.packed() >> (8 * (f.len - vl)), f.len, vl};
     }
     k_parse_guess<<<(uint32_t)div_up((uint64_t)nwin * 32, PW_GUESS_THREADS), PW_GUESS_THREADS, 0, st>>>(data, d_pwseg.as<PwSeg>(), nseg, nwin,
                                                                                                         d_entry[0].as<uint64_t>(), hint);
@@ -719,14 +728,10 @@ class Merger {
     if (flags[1]) return false;
     const int cur = 0;         // d_entry[0] now holds the true entries
     // ---- record offsets of every window, totals
-    const uint32_t nblk = (uint32_t)div_up(nwin, SCAN_TILE);
-    pipe.blk.ensure(((size_t)nblk + 2) * 8);
-    k_sum_u32_blocks<<<nblk, SCAN_THREADS, 0, st>>>(d_wcount.as<uint32_t>(), nwin, pipe.blk.as<uint64_t>());
-    k_scan_block_sums<<<1, 1024, 0, st>>>(pipe.blk.as<uint64_t>(), nblk);
-    k_scan_u32_apply<<<nblk, SCAN_THREADS, 0, st>>>(d_wcount.as<uint32_t>(), nwin, pipe.blk.as<uint64_t>(), d_wbase.as<uint64_t>());
+    launches += scan_u32_exclusive(st, pipe.blk, d_wcount.as<uint32_t>(), nwin, d_wbase.as<uint64_t>());
     d_counts.ensure((size_t)(nseg + 1) * 16);
     k_parse_seg_counts<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(d_pwseg.as<PwSeg>(), nseg, d_wbase.as<uint64_t>(), d_counts.as<uint64_t>());
-    launches += 4;
+    launches++;
     uint64_t total = 0;
     TG_CUDA(cudaMemcpyAsync(&total, d_wbase.as<uint64_t>() + nwin, 8, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaMemcpyAsync(h_counts.data(), d_counts.p, (size_t)nseg * 8, cudaMemcpyDeviceToHost, st));
@@ -736,9 +741,7 @@ class Merger {
     uint64_t acc = 0;
     for (uint32_t s = 0; s < nseg; s++) { h_rec_base[s] = acc; acc += h_counts[s]; }
     h_rec_base[nseg] = acc;
-    d_koff.ensure((size_t)(n ? n : 1) * 8); d_voff.ensure((size_t)(n ? n : 1) * 8);
-    d_klen.ensure((size_t)(n ? n : 1) * 4); d_vlen.ensure((size_t)(n ? n : 1) * 4); d_tag.ensure((size_t)(n ? n : 1) * 4); d_part.ensure((size_t)(n ? n : 1) * 4);
-    PwArrays pa{d_koff.as<uint64_t>(), d_voff.as<uint64_t>(), d_klen.as<uint32_t>(), d_vlen.as<uint32_t>(), d_tag.as<uint32_t>(), d_part.as<int32_t>()};
+    const ParseArrays pa = record_arrays(n);
     d_carry.ensure((size_t)nwin * 16);
     k_parse_carry<<<grid, PW_THREADS, 0, st>>>(d_pwseg.as<PwSeg>(), nseg, nwin, d_entry[cur].as<uint64_t>(), d_wlast.as<uint64_t>(), d_carry.as<uint64_t>());
     const uint64_t *carry = d_carry.as<uint64_t>();
@@ -779,9 +782,7 @@ class Merger {
     rec_base[nseg] = n;
     TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one merge");
     TG_CUDA(cudaMemcpyAsync(d_rec_base.p, rec_base.data(), (size_t)(nseg + 1) * 8, cudaMemcpyHostToDevice, st));
-    d_koff.ensure((size_t)(n ? n : 1) * 8); d_voff.ensure((size_t)(n ? n : 1) * 8);
-    d_klen.ensure((size_t)(n ? n : 1) * 4); d_vlen.ensure((size_t)(n ? n : 1) * 4); d_tag.ensure((size_t)(n ? n : 1) * 4); d_part.ensure((size_t)(n ? n : 1) * 4);
-    pa = ParseArrays{d_koff.as<uint64_t>(), d_voff.as<uint64_t>(), d_klen.as<uint32_t>(), d_vlen.as<uint32_t>(), d_tag.as<uint32_t>(), d_part.as<int32_t>()};
+    pa = record_arrays(n);
     if (n) k_parse_segments<true><<<(uint32_t)div_up(nseg, PARSE_WARPS), PARSE_WARPS * 32, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, nullptr, nullptr,
                                                                             d_rec_base.as<uint64_t>(), pa, d_bad);
     launches += 2;
@@ -806,7 +807,7 @@ class Merger {
   }
 
   // ---- codec (codec.cuh): compressed segments are checked, decompressed into z_img and merged as ordinary segments
-  DeviceBuffer z_in, z_img, z_insegs, z_status, z_descs, z_pstart, z_tc, z_crc, z_flag;
+  DeviceBuffer z_in, z_img, z_insegs, z_status, z_descs, z_flag;
   DeviceBuffer z_nblk, z_base, z_blks, z_slow;   // LZ4 / zstd: blocks (frames) per segment, their first index, the units, serial-path flags
   void open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg);
 
@@ -856,12 +857,8 @@ class Merger {
     d_sizes.ensure((size_t)(nn ? nn : 1) * 4);
     d_kvoff.ensure(((size_t)nn + 2) * 8);
     if (nn) {
-      const uint32_t nblk = (uint32_t)div_up(nn, SCAN_TILE);
-      pipe.blk.ensure(((size_t)nblk + 2) * 8);
       k_kv_sizes<<<(uint32_t)div_up(nn, 256), 256, 0, st>>>(pipe.state.rec, pipe.state.order, d_sizes.as<uint32_t>());
-      k_sum_u32_blocks<<<nblk, SCAN_THREADS, 0, st>>>(d_sizes.as<uint32_t>(), nn, pipe.blk.as<uint64_t>());
-      k_scan_block_sums<<<1, 1024, 0, st>>>(pipe.blk.as<uint64_t>(), nblk);
-      k_scan_u32_apply<<<nblk, SCAN_THREADS, 0, st>>>(d_sizes.as<uint32_t>(), nn, pipe.blk.as<uint64_t>(), d_kvoff.as<uint64_t>());
+      scan_u32_exclusive(st, pipe.blk, d_sizes.as<uint32_t>(), nn, d_kvoff.as<uint64_t>());
       TG_CUDA(cudaGetLastError());
     } else {
       TG_CUDA(cudaMemsetAsync(d_kvoff.p, 0, 16, st));

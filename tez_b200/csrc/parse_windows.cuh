@@ -116,7 +116,7 @@ __device__ __forceinline__ bool pw_vlong(const uint8_t *__restrict__ seg, uint64
   return true;
 }
 
-struct PwArrays {
+struct ParseArrays {
   uint64_t *key_off;
   uint64_t *val_off;
   uint32_t *key_len;
@@ -143,7 +143,7 @@ struct PwWalk {
 // (29 MB).
 template <bool EMIT>
 __device__ __forceinline__ PwWalk pw_walk(const uint8_t *__restrict__ seg, const PwSeg &sd, uint32_t s, uint64_t wend, bool last_win,
-                                          uint64_t e, uint64_t base, uint64_t carry_off, uint64_t carry_len, const PwArrays &out,
+                                          uint64_t e, uint64_t base, uint64_t carry_off, uint64_t carry_len, const ParseArrays &out,
                                           uint32_t lane = 0) {  // lane: position inside the emit group
   PwWalk r;
   r.exit_v = e;
@@ -259,7 +259,7 @@ __global__ void __launch_bounds__(PW_GUESS_THREADS)
   const uint64_t ws = sd.body0 + (uint64_t)k * PW_WINDOW;
   const uint64_t wend = min(sd.body_end, ws + PW_WINDOW);
   const bool last_win = (k + 1 == sd.nwin);
-  PwArrays none{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  ParseArrays none{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   if (k == 0 && lane == 0) entry_out[w] = sd.body0 << 1;
   if (last_win) return;                       // nobody to hand an exit to
   if (k == 0) {                               // the first window's entry is known: its exit is exact
@@ -352,7 +352,7 @@ __global__ void __launch_bounds__(PW_THREADS)
                     uint32_t nwin_total, const uint64_t *__restrict__ entry_in, uint64_t *__restrict__ entry_out,
                     uint32_t *__restrict__ wcount, uint64_t *__restrict__ wlastkey /*[2*nwin]: off, len*/,
                     unsigned long long *__restrict__ kv_total, int *__restrict__ flags /*[0] changed, [1] bad*/,
-                    const uint64_t *__restrict__ rec_base, const uint64_t *__restrict__ carry /*[2*nwin]*/, PwArrays out) {
+                    const uint64_t *__restrict__ rec_base, const uint64_t *__restrict__ carry /*[2*nwin]*/, ParseArrays out) {
   constexpr bool EMIT = MODE == 2;
   const uint32_t gt = blockIdx.x * blockDim.x + threadIdx.x;
   const uint32_t w = EMIT ? gt / PW_EMIT_GROUP : gt, lane = threadIdx.x & (PW_EMIT_GROUP - 1u);
@@ -401,7 +401,7 @@ __global__ void __launch_bounds__(32 * PW_CHASE_WARPS)
   if (s >= nseg) return;
   const PwSeg sd = segs[s];
   const uint8_t *__restrict__ seg = data + sd.off;
-  PwArrays none{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  ParseArrays none{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   uint64_t e = sd.body0 << 1;   // true entry of window k
   uint32_t k = 0, by_hand = 0;
   bool bad = false;

@@ -1,6 +1,6 @@
 // scan.cuh -- small device-wide scan / compaction building blocks (reduce-then-scan, 2048 elements per block).
 #pragma once
-#include "common.cuh"
+#include "device_util.h"
 
 namespace tezgpu {
 
@@ -101,6 +101,17 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_u32_apply(const uint32_t 
     ex += v[k];
   }
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == SCAN_THREADS - 1) out[n] = blk[gridDim.x];
+}
+
+// u32 sizes -> u64 exclusive offsets: out[i] = in[0] + ... + in[i-1] for i < n, out[n] = the total (n > 0).  blk holds the
+// block sums.  Returns the launches.
+inline int scan_u32_exclusive(cudaStream_t st, DeviceBuffer &blk, const uint32_t *in, uint32_t n, uint64_t *out) {
+  const uint32_t nblk = (uint32_t)div_up(n, SCAN_TILE);
+  blk.ensure(((size_t)nblk + 2) * 8);
+  k_sum_u32_blocks<<<nblk, SCAN_THREADS, 0, st>>>(in, n, blk.as<uint64_t>());
+  k_scan_block_sums<<<1, 1024, 0, st>>>(blk.as<uint64_t>(), nblk);
+  k_scan_u32_apply<<<nblk, SCAN_THREADS, 0, st>>>(in, n, blk.as<uint64_t>(), out);
+  return 3;
 }
 
 }  // namespace tezgpu

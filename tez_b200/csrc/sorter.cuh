@@ -58,6 +58,27 @@ struct DeviceConstants {
   }
 };
 
+// The framing vint(klen) vint(vlen) in front of every fixed-width record written without repeats
+constexpr uint32_t FRAMING_MAX_LEN = 10;   // two vints of at most 5 bytes
+struct FixedFraming {
+  uint8_t bytes[FRAMING_MAX_LEN];
+  uint32_t len;        // framing bytes
+  uint32_t rec_size;   // len + klen + vlen
+  // the first 8 framing bytes, little-endian packed
+  uint64_t packed() const {
+    uint64_t x = 0;
+    for (uint32_t b = 0; b < len && b < 8; b++) x |= (uint64_t)bytes[b] << (8 * b);
+    return x;
+  }
+};
+static inline FixedFraming fixed_framing(uint32_t klen, uint32_t vlen) {
+  FixedFraming f{};
+  for (int b = 0; b < vint_size_u32(klen); b++) f.bytes[f.len++] = vint_byte_u32(klen, b);
+  for (int b = 0; b < vint_size_u32(vlen); b++) f.bytes[f.len++] = vint_byte_u32(vlen, b);
+  f.rec_size = f.len + klen + vlen;
+  return f;
+}
+
 // thrown by sort_phase in run-table mode (Records::use_runs): the merger then re-parses the segments with the walker
 struct FramingMismatch {};
 
@@ -214,11 +235,10 @@ class SortPipeline {
   }
   // fixed framing (vint klen, vint vlen) and the tile size of the emit kernel the plan picks, which it returns
   FixedEmitKernel set_fixed_layout(EmitParams &e, const Records &rec) {
-    int h = 0;
-    for (int b = 0; b < vint_size_u32(rec.klen); b++) e.fixed_hdr[h++] = vint_byte_u32(rec.klen, b);
-    for (int b = 0; b < vint_size_u32(rec.vlen); b++) e.fixed_hdr[h++] = vint_byte_u32(rec.vlen, b);
-    e.fixed_hdr_len = h;
-    e.rec_size = h + rec.klen + rec.vlen;
+    const FixedFraming f = fixed_framing(rec.klen, rec.vlen);
+    memcpy(e.fixed_hdr, f.bytes, f.len);
+    e.fixed_hdr_len = f.len;
+    e.rec_size = f.rec_size;
     const FixedEmitPlan plan = plan_fixed_emit(rec, e.rec_size);
     e.recs_per_tile = plan.recs_per_tile;
     e.rec_off = nullptr;
@@ -517,7 +537,6 @@ class SortPipeline {
     int launches = state.launches;
     const CrcTables *d_crc = DeviceConstants::get(conf.device).d_crc;
     const size_t n4 = (size_t)(n ? n : 1) * 4;
-    const uint32_t nblk = (uint32_t)div_up(n ? n : 1, SCAN_TILE);
     TG_CUDA(cudaMemsetAsync(seg_crc.p, 0, (size_t)P * 4, stream));
     if (timer.n > (n ? 4 : 2)) timer.n = n ? 4 : 2;  // re-emit: drop the marks of a previous emit
 
@@ -550,10 +569,7 @@ class SortPipeline {
           launches++;
           e.rep = rep_flags.as<uint8_t>();
           k_emit_sizes<<<(uint32_t)div_up(n, 256), 256, 0, stream>>>(e, K, sizes.as<uint32_t>());
-          k_sum_u32_blocks<<<nblk, SCAN_THREADS, 0, stream>>>(sizes.as<uint32_t>(), n, blk.as<uint64_t>());
-          k_scan_block_sums<<<1, 1024, 0, stream>>>(blk.as<uint64_t>(), nblk);
-          k_scan_u32_apply<<<nblk, SCAN_THREADS, 0, stream>>>(sizes.as<uint32_t>(), n, blk.as<uint64_t>(), rec_off.as<uint64_t>());
-          launches += 4;
+          launches += 1 + scan_u32_exclusive(stream, blk, sizes.as<uint32_t>(), n, rec_off.as<uint64_t>());
           TG_CUDA(cudaGetLastError());
         } else {
           TG_CUDA(cudaMemsetAsync(rec_off.p, 0, 16, stream));
@@ -710,15 +726,10 @@ class SortPipeline {
       return false;
     }
     // ---- group ids: exclusive scan of the heads
-    const uint32_t nblk = (uint32_t)div_up(n, SCAN_TILE);
     c_head.ensure((size_t)n * 4);
     c_gid.ensure(((size_t)n + 1) * 8);
-    blk.ensure(((size_t)nblk + 2) * 8);
     k_combine_heads<<<(uint32_t)div_up(n, 256), 256, 0, stream>>>(same.as<uint8_t>(), n, c_head.as<uint32_t>());
-    k_sum_u32_blocks<<<nblk, SCAN_THREADS, 0, stream>>>(c_head.as<uint32_t>(), n, blk.as<uint64_t>());
-    k_scan_block_sums<<<1, 1024, 0, stream>>>(blk.as<uint64_t>(), nblk);
-    k_scan_u32_apply<<<nblk, SCAN_THREADS, 0, stream>>>(c_head.as<uint32_t>(), n, blk.as<uint64_t>(), c_gid.as<uint64_t>());
-    launches += 4;
+    launches += 1 + scan_u32_exclusive(stream, blk, c_head.as<uint32_t>(), n, c_gid.as<uint64_t>());
     // ---- segmented sums (groups <= n: sized by n, no round trip first)
     c_sums.ensure((size_t)n * 8);
     c_hpos.ensure((size_t)n * 4);
@@ -761,12 +772,8 @@ class SortPipeline {
       out.vlen = W;
     } else {
       // key offsets: scan of (key length + width) over the groups; c_head / c_gid are free again
-      const uint32_t mblk = (uint32_t)div_up(m, SCAN_TILE);
       k_combine_sizes<<<(uint32_t)div_up(m, 256), 256, 0, stream>>>(rec, state.order, c_hpos.as<uint32_t>(), m, W, c_head.as<uint32_t>());
-      k_sum_u32_blocks<<<mblk, SCAN_THREADS, 0, stream>>>(c_head.as<uint32_t>(), m, blk.as<uint64_t>());
-      k_scan_block_sums<<<1, 1024, 0, stream>>>(blk.as<uint64_t>(), mblk);
-      k_scan_u32_apply<<<mblk, SCAN_THREADS, 0, stream>>>(c_head.as<uint32_t>(), m, blk.as<uint64_t>(), c_gid.as<uint64_t>());
-      launches += 4;
+      launches += 1 + scan_u32_exclusive(stream, blk, c_head.as<uint32_t>(), m, c_gid.as<uint64_t>());
       TG_CUDA(cudaGetLastError());
       TG_CUDA(cudaMemcpyAsync(h + 4, c_gid.as<uint64_t>() + m, 8, cudaMemcpyDeviceToHost, stream));
       TG_CUDA(cudaStreamSynchronize(stream));

@@ -355,8 +355,7 @@ int32_t tezgpu_sorter_set_combiner(tezgpu_sorter *h, int32_t combiner) {
 int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec) {
   TG_API_BEGIN
   TG_CHECK(h, TEZGPU_E_INVALID, "null handle");
-  TG_CHECK(codec == TEZGPU_CODEC_NONE || codec == TEZGPU_CODEC_DEFAULT || codec == TEZGPU_CODEC_LZ4 || codec == TEZGPU_CODEC_ZSTD,
-           TEZGPU_E_UNSUPPORTED, "codec " + std::to_string(codec) + " is not on the device (DefaultCodec, Lz4Codec and ZStandardCodec only)");
+  check_codec(codec);
   TG_CHECK(h->n == 0 && !h->flushed, TEZGPU_E_STATE, "set the codec before the first collect (or after a reset)");
   h->pipe.codec = codec;
   TG_API_END
