@@ -57,20 +57,16 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     z_slots.ensure((size_t)nchunks * slot);
     z_csize.ensure((size_t)nchunks * 4);
     z_coff.ensure(((size_t)nchunks + 2) * 8);
-    static bool attr[4][64] = {};   // the attribute is per device
-    if (!attr[codec & 3][conf.device & 63]) {
-      if (lz4) TG_CUDA(cudaFuncSetAttribute(k_l4compress, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(L4Shared)));
-      else if (zstd) TG_CUDA(cudaFuncSetAttribute(k_zscompress, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZsShared)));
-      else TG_CUDA(cudaFuncSetAttribute(k_zdeflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ZShared)));
-      attr[codec & 3][conf.device & 63] = true;
-    }
     if (zstd) {
+      set_smem_limit<k_zscompress>(conf.device, sizeof(ZsShared));
       k_zscompress<<<nchunks, ZS_LANES, sizeof(ZsShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
                                                                z_csize.as<uint32_t>());
     } else if (lz4) {
+      set_smem_limit<k_l4compress>(conf.device, sizeof(L4Shared));
       k_l4compress<<<nchunks, L4_LANES, sizeof(L4Shared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
                                                                z_csize.as<uint32_t>());
     } else {
+      set_smem_limit<k_zdeflate>(conf.device, sizeof(ZShared));
       z_cadler.ensure((size_t)nchunks * 4);
       k_zdeflate<<<nchunks, ZLANES, sizeof(ZShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
                                                           z_csize.as<uint32_t>(), z_cadler.as<uint32_t>());

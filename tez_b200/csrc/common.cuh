@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <atomic>
 #include <stdexcept>
 #include <string>
 
@@ -31,6 +32,16 @@ struct Error : public std::runtime_error {
 
 static inline uint64_t div_up(uint64_t a, uint64_t b) { return (a + b - 1) / b; }
 static inline uint64_t align_up(uint64_t a, uint64_t b) { return div_up(a, b) * b; }
+
+// Lets kernel Kern take `bytes` of dynamic shared memory on `device`, the current device.  The limit is an attribute
+// per device: it is set once per kernel and device (racing first calls set the same value); later calls load one flag.
+template <auto Kern>
+inline void set_smem_limit(int device, size_t bytes) {
+  static std::atomic<bool> done[64];
+  if ((unsigned)device < 64 && done[device].load(std::memory_order_acquire)) return;
+  TG_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  if ((unsigned)device < 64) done[device].store(true, std::memory_order_release);
+}
 
 // comparator ids (include/tezgpu.h)
 enum { CMP_BYTES = 0, CMP_TEXT = 1, CMP_BYTESWRITABLE = 2, CMP_INT = 3, CMP_LONG = 4 };

@@ -283,7 +283,7 @@ inline void Merger::concat_parse() {
     TG_CUDA(cudaMemcpyAsync(d_rec_base.p, h_rec_base.data(), (size_t)(nseg + 1) * 8, cudaMemcpyHostToDevice, st));
     const ParseArrays pa = record_arrays(n);
     const FixedFraming f = fixed_framing(fixed_klen, fixed_vlen);
-    int *d_bad = pipe.d_error();
+    int *d_bad = &pipe.d_scratch()->verdict.error;
     TG_CUDA(cudaMemsetAsync(d_bad, 0, 4, st));
     int bad = 0;
     if (n) {

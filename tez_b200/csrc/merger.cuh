@@ -608,7 +608,7 @@ class Merger {
 
   // general path: walk the segments (IFile.Reader semantics), materialise the per-record metadata
   void find_records_general(uint32_t nseg) {
-    TG_CUDA(cudaMemsetAsync(pipe.small.p, 0, 16384, pipe.stream));
+    TG_CUDA(cudaMemsetAsync(pipe.small.p, 0, SORT_SCRATCH_BYTES, pipe.stream));
     d_counts.ensure((size_t)(nseg + 1) * 16);
     d_rec_base.ensure((size_t)(nseg + 2) * 8);
     n = 0;
@@ -767,7 +767,7 @@ class Merger {
     parse_mode = 1;
     if (!serial_only && parse_parallel(nseg)) return;
     parse_mode = 2;
-    int *d_bad = pipe.d_error();
+    int *d_bad = &pipe.d_scratch()->verdict.error;
     ParseArrays pa{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     k_parse_segments<false><<<(uint32_t)div_up(nseg, PARSE_WARPS), PARSE_WARPS * 32, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, d_counts.as<uint64_t>(),
                                                                      d_counts.as<uint64_t>() + nseg, nullptr, pa, d_bad);
@@ -875,7 +875,7 @@ class Merger {
     if (concat) concat_parse();
     if (cursor >= n || idx_cap == 0) return;
     ensure_kvoff();
-    uint32_t *d_cnt = pipe.d_large();
+    uint32_t *d_cnt = &pipe.d_scratch()->verdict.batch_count;
     k_find_batch<<<1, 1, 0, st>>>(d_kvoff.as<uint64_t>(), (uint32_t)n, (uint32_t)cursor, idx_cap, cap, d_cnt);
     uint32_t cnt = 0;
     TG_CUDA(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, st));

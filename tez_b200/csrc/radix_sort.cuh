@@ -326,6 +326,7 @@ struct RadixWorkspace {
   uint32_t *tile_state = nullptr;  // [npass][ntiles][RADIX]
   uint32_t *tile_counter = nullptr;  // [8]
   size_t tile_state_words = 0;
+  int device = 0;                  // the current device
 };
 
 // MINB: CTAs per SM that __launch_bounds__ asks for, which caps the registers at 64K / (MINB * THREADS).
@@ -346,19 +347,16 @@ static inline size_t radix_tile_state_words(uint32_t n, int npass) {
   return (size_t)radix_num_tiles<KeyT>(n) * RADIX * (size_t)npass;
 }
 
+// launches pass p of a sort that starts at begin_bit; its digit offsets, look-back state and tile counter come from ws
 template <typename KeyT, int IN, int OUT>
-static void radix_launch_pass(cudaStream_t st, uint32_t ntiles, const KeyT *kin, KeyT *kout, const uint32_t *vin,
-                              uint32_t *vout, uint32_t n, int shift, const uint32_t *hist, uint32_t *state,
-                              uint32_t *counter) {
+static void radix_launch_pass(cudaStream_t st, const RadixWorkspace &ws, uint32_t ntiles, int begin_bit, int p, const KeyT *kin,
+                              KeyT *kout, const uint32_t *vin, uint32_t *vout, uint32_t n) {
   using T = RadixTuning<KeyT>;
   using Cfg = OnesweepCfg<KeyT, T::THREADS, T::IPT>;
-  auto kern = k_onesweep_pass<KeyT, T::THREADS, T::IPT, T::MINB, IN, OUT>;
-  static bool attr_set = false;  // one flag per instantiation
-  if (!attr_set) {
-    TG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
-    attr_set = true;
-  }
-  kern<<<ntiles, T::THREADS, Cfg::SMEM, st>>>(kin, kout, vin, vout, n, shift, hist, state, counter);
+  constexpr auto kern = k_onesweep_pass<KeyT, T::THREADS, T::IPT, T::MINB, IN, OUT>;
+  set_smem_limit<kern>(ws.device, Cfg::SMEM);
+  kern<<<ntiles, T::THREADS, Cfg::SMEM, st>>>(kin, kout, vin, vout, n, begin_bit + p * RADIX_BITS, ws.hist + p * RADIX,
+                                               ws.tile_state + (size_t)p * ntiles * RADIX, ws.tile_counter + p);
   TG_CUDA(cudaGetLastError());
 }
 
@@ -390,17 +388,14 @@ static int radix_sort_pairs(cudaStream_t st, const RadixWorkspace &ws, uint32_t 
     if (!((pass_mask >> p) & 1u)) continue;
     uint32_t *in = (done & 1) ? blk_b : blk_a, *out = (done & 1) ? blk_a : blk_b;
     const bool first = done == 0, last = done + 1 == total;
-    const int shift = begin_bit + p * RADIX_BITS;
-    const uint32_t *hist = ws.hist + p * RADIX;
-    uint32_t *state = ws.tile_state + (size_t)p * ntiles * RADIX, *counter = ws.tile_counter + p;
     if (first && last)
-      radix_launch_pass<uint32_t, IO_SEP_IOTA, IO_SEP>(st, ntiles, in, out, nullptr, out + n, n, shift, hist, state, counter);
+      radix_launch_pass<uint32_t, IO_SEP_IOTA, IO_SEP>(st, ws, ntiles, begin_bit, p, in, out, nullptr, out + n, n);
     else if (first)
-      radix_launch_pass<uint32_t, IO_SEP_IOTA, IO_PAIR>(st, ntiles, in, out, nullptr, nullptr, n, shift, hist, state, counter);
+      radix_launch_pass<uint32_t, IO_SEP_IOTA, IO_PAIR>(st, ws, ntiles, begin_bit, p, in, out, nullptr, nullptr, n);
     else if (last)
-      radix_launch_pass<uint32_t, IO_PAIR, IO_SEP>(st, ntiles, in, out, nullptr, out + n, n, shift, hist, state, counter);
+      radix_launch_pass<uint32_t, IO_PAIR, IO_SEP>(st, ws, ntiles, begin_bit, p, in, out, nullptr, out + n, n);
     else
-      radix_launch_pass<uint32_t, IO_PAIR, IO_PAIR>(st, ntiles, in, out, nullptr, nullptr, n, shift, hist, state, counter);
+      radix_launch_pass<uint32_t, IO_PAIR, IO_PAIR>(st, ws, ntiles, begin_bit, p, in, out, nullptr, nullptr, n);
     if (launches) (*launches)++;
     done++;
   }
@@ -419,9 +414,7 @@ static int radix_sort_passes(cudaStream_t st, const RadixWorkspace &ws, KeyT *ke
     if (!((pass_mask >> p) & 1u)) continue;
     KeyT *kin = (done & 1) ? keys_b : keys_a, *kout = (done & 1) ? keys_a : keys_b;
     uint32_t *vin = (done & 1) ? vals_b : vals_a, *vout = (done & 1) ? vals_a : vals_b;
-    radix_launch_pass<KeyT, IO_SEP, IO_SEP>(st, ntiles, kin, kout, vin, vout, n, begin_bit + p * RADIX_BITS,
-                                            ws.hist + p * RADIX, ws.tile_state + (size_t)p * ntiles * RADIX,
-                                            ws.tile_counter + p);
+    radix_launch_pass<KeyT, IO_SEP, IO_SEP>(st, ws, ntiles, begin_bit, p, kin, kout, vin, vout, n);
     if (launches) (*launches)++;
     done++;
   }

@@ -1,6 +1,7 @@
 // sorter.cuh -- host orchestration of the device sort pipeline (one "spill" covering everything collected:
 // HBM is the sort buffer, so this is always the numSpills==1 branch of PipelinedSorter.flush, :730-756).
 #pragma once
+#include <stddef.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -81,6 +82,35 @@ static inline FixedFraming fixed_framing(uint32_t klen, uint32_t vlen) {
 
 // thrown by sort_phase in run-table mode (Records::use_runs): the merger then re-parses the segments with the walker
 struct FramingMismatch {};
+
+// The sort's device scratch (SortPipeline::small), cleared before every sort
+struct SortVerdict {          // what the sort's one host round trip reads, in one piece
+  int error;                  // STAGE_ERR_* bits; the handle's other steps borrow it as their error word
+  union { uint32_t large_groups; uint32_t batch_count; };  // tie groups > TIE_SMALL_MAX (k_tie_fix); the merger's batch size
+  unsigned long long dups;    // adjacent equal keys
+  uint64_t totals[2];         // k_layout: file bytes, tiles
+};
+struct SortScratch {
+  uint32_t hist[8 * RADIX];   // digit offsets of up to eight radix passes
+  uint32_t trivial[8];        // per pass: one digit holds every key
+  uint32_t tile_counter[8];
+  SortVerdict verdict;
+  uint32_t unused[2];
+  unsigned long long ties;    // tied records (k_tie_fix)
+};
+constexpr size_t SORT_SCRATCH_BYTES = 16 * 1024;
+struct SortHostScratch {           // its pinned mirror (SortPipeline::h_small): what the host reads, then the spill index
+  SortVerdict verdict;             // sort_phase's round trip; emit_phase's totals when it lays the records out itself
+  uint32_t ties;                   // the low word of SortScratch::ties
+  uint64_t total;                  // refine_large_groups: a scan total, then the duplicate count
+  uint32_t trivial[8];             // SortScratch::trivial of a refinement round
+  static constexpr size_t INDEX_OFFSET = 4096;  // P (start, rawLength, partLength) triples
+  int64_t *index() { return reinterpret_cast<int64_t *>(reinterpret_cast<uint8_t *>(this) + INDEX_OFFSET); }
+};
+static_assert(offsetof(SortScratch, trivial) == 2048 * 4 && offsetof(SortScratch, tile_counter) == 2056 * 4 &&
+                  offsetof(SortScratch, verdict) == 2064 * 4 && sizeof(SortVerdict) == 32 && offsetof(SortScratch, ties) == 2074 * 4 &&
+                  sizeof(SortScratch) <= SORT_SCRATCH_BYTES && offsetof(SortHostScratch, ties) == 32 &&
+                  sizeof(SortHostScratch) <= SortHostScratch::INDEX_OFFSET, "sort scratch layout");
 
 // The emit kernels for fixed-width records written without repeats (records with repeats take k_emit<false>).
 enum class FixedEmitKernel {
@@ -168,8 +198,8 @@ class SortPipeline {
     }
     pbits = partition_bits(c.num_partitions);
     TG_CHECK(pbits <= 31, TEZGPU_E_INVALID, "too many partitions");
-    h_small.ensure(4096);
-    small.ensure(16384);
+    h_small.ensure(SortHostScratch::INDEX_OFFSET);
+    small.ensure(SORT_SCRATCH_BYTES);
     DeviceConstants::get(c.device);
   }
   ~SortPipeline() {
@@ -178,18 +208,8 @@ class SortPipeline {
 
   static uint64_t output_bound(uint64_t n, uint64_t kv_bytes, int P) { return kv_bytes + 12 * n + 10ull * P + 64; }
 
-  // `small` device scratch layout (u32 words): [0..2047] radix hist (8*256), [2048..2055] trivial flags,
-  // [2056..2063] tile counters, [2064] error flag, [2066..2067] dup count (u64), [2068..2071] totals (2 x u64)
-  uint32_t *d_hist() { return small.as<uint32_t>(); }
-  uint32_t *d_trivial() { return small.as<uint32_t>() + 2048; }
-  uint32_t *d_tile_counter() { return small.as<uint32_t>() + 2056; }
-  int *d_error() { return reinterpret_cast<int *>(small.as<uint32_t>() + 2064); }
-  uint32_t *d_large() { return small.as<uint32_t>() + 2065; }
-  uint32_t *d_m() { return small.as<uint32_t>() + 2072; }
-  unsigned long long *d_ties() { return reinterpret_cast<unsigned long long *>(small.as<uint32_t>() + 2074); }
-  uint32_t *d_ticket() { return small.as<uint32_t>() + 2073; }
-  unsigned long long *d_dups() { return reinterpret_cast<unsigned long long *>(small.as<uint32_t>() + 2066); }
-  uint64_t *d_totals() { return reinterpret_cast<uint64_t *>(small.as<uint32_t>() + 2068); }
+  SortScratch *d_scratch() const { return small.as<SortScratch>(); }
+  SortHostScratch *h_scratch() const { return h_small.as<SortHostScratch>(); }
 
   // state left behind by sort_phase for emit_phase / the merger's record iterator
   struct SortState {
@@ -198,8 +218,7 @@ class SortPipeline {
     uint32_t *order = nullptr;  // sorted position -> record index
     uint64_t dup_count = 0, tie_records = 0;
     int launches = 0;
-    bool have_bounds = false, spec_layout = false;  // partition bounds / fixed-width layout already on the device
-    uint64_t spec_file_bytes = 0, spec_tiles = 0;
+    bool have_bounds = false, spec_layout = false;  // partition bounds / fixed-width layout (totals, index: h_scratch()) on the device
     const uint8_t *same = nullptr;  // the combined records' same[] (all zero); nullptr = the sort's own `same`
   } state;
   // merge mode only (the Merger sets them): MergeQueue.checkForSameKeys, and "no input record was run-length encoded"
@@ -296,10 +315,8 @@ class SortPipeline {
     rec.hash_partition = conf.partitioner == TEZGPU_PART_HASH;
     rec.num_partitions = P;
     rec.pbits = pbits;
-    const bool unordered = conf.sorter_impl == TEZGPU_SORTER_UNORDERED;
-    rec.unordered = unordered ? 1 : 0;
+    rec.unordered = conf.sorter_impl == TEZGPU_SORTER_UNORDERED ? 1 : 0;
     TG_CHECK(rec.hash_partition || rec.partition || rec.use_runs || n == 0 || P == 1, TEZGPU_E_INVALID, "partition ids required (partitioner=GIVEN)");
-    int launches = 0;
     state.have_bounds = state.spec_layout = false;
     state.same = nullptr;
     timer.reset();
@@ -308,219 +325,211 @@ class SortPipeline {
     const size_t n4 = (size_t)(n ? n : 1) * 4;
     sortA.ensure(2 * n4); sortB.ensure(2 * n4);
     same.ensure(n ? n : 1);
-    const uint32_t nblk = (uint32_t)div_up(n ? n : 1, SCAN_TILE);
-    blk.ensure(((size_t)nblk + 2) * 8);
+    blk.ensure((div_up(n ? n : 1, SCAN_TILE) + 2) * 8);
     part_start.ensure(((size_t)P + 1) * 4);
     seg_start.ensure(((size_t)P + 1) * 8);
     tile_start.ensure(((size_t)P + 1) * 4);
     d_index.ensure((size_t)P * 24);
     seg_crc.ensure((size_t)P * 4);
-    h_small.ensure(4096 + (size_t)P * 24);
+    h_small.ensure(SortHostScratch::INDEX_OFFSET + (size_t)P * 24);
 
-    TG_CUDA(cudaMemsetAsync(small.p, 0, 16384, stream));
+    TG_CUDA(cudaMemsetAsync(small.p, 0, SORT_SCRATCH_BYTES, stream));
     TG_CUDA(cudaMemsetAsync(seg_crc.p, 0, (size_t)P * 4, stream));
 
-    uint64_t dup_count = 0;
-    uint64_t tie_records = 0;
-    uint32_t *K = sortA.as<uint32_t>();
-    uint32_t *order = sortA.as<uint32_t>() + n;
-
-    uint32_t sym_npos = 0;
-    if (n && !rec.fixed && !unordered && !(getenv("TEZGPU_NO_SYM") && atoi(getenv("TEZGPU_NO_SYM")))) {
-      // ---------------- alphabet-compressed sort word (SymTable, sorter_kernels.cuh): which byte values occur at the
-      // first content positions -> per-position ranks, packed while they fit the (32 - pbits)-bit key field
-      sym_sets.ensure(SYM_MAX_POS * 8 * 4);
-      sym_tab.ensure(sizeof(SymTable));
-      TG_CUDA(cudaMemsetAsync(sym_sets.p, 0, SYM_MAX_POS * 8 * 4, stream));
-      k_symbols<<<(int)std::min<uint64_t>(div_up(n, 256), (uint64_t)num_sms * 8), 256, 0, stream>>>(rec, sym_sets.as<uint32_t>());
-      launches++;
-      uint32_t hs[SYM_MAX_POS * 8];
-      TG_CUDA(cudaMemcpyAsync(hs, sym_sets.p, sizeof(hs), cudaMemcpyDeviceToHost, stream));
-      TG_CUDA(cudaStreamSynchronize(stream));
-      SymTable *t = new SymTable();
-      const uint32_t np = sym_table_build(hs, pbits, t);
-      if (sym_table_pays(np, pbits)) {             // packs more positions than the raw bytes would
-        TG_CUDA(cudaMemcpyAsync(sym_tab.p, t, sizeof(SymTable), cudaMemcpyHostToDevice, stream));
-        TG_CUDA(cudaStreamSynchronize(stream));
-        rec.sym = sym_tab.as<SymTable>();
-        sym_npos = np;
-      }
-      delete t;
-    }
+    state.K = sortA.as<uint32_t>();
+    state.order = sortA.as<uint32_t>() + n;
+    state.dup_count = state.tie_records = 0;
+    int launches = 0;
     if (n) {
-      // ---------------- stage
-      TG_CUDA(cudaMemsetAsync(same.p, 0, n, stream));
-      const bool fast16 = rec.fixed && !rec.key_off && !rec.use_runs && rec.klen == 16 && ((rec.klen + rec.vlen) % 16 == 0) && rec.cmp == CMP_BYTES &&
-                          (((uintptr_t)rec.kv & 15u) == 0);
-      int sgrid = (int)std::min<uint64_t>(div_up(n, 256), (uint64_t)num_sms * 16);
-      if (fast16) k_stage<true><<<sgrid, 256, 0, stream>>>(rec, K, d_hist(), d_error());
-      else k_stage<false><<<sgrid, 256, 0, stream>>>(rec, K, d_hist(), d_error());
-      TG_CUDA(cudaGetLastError());
-      k_radix_scan_hist<<<1, RADIX, 0, stream>>>(d_hist(), 4, n, d_trivial());
-      TG_CUDA(cudaGetLastError());
-      launches += 2;
-      timer.mark(stream);
-
-      // ---------------- radix sort of (sort word, record index)
-      RadixWorkspace ws;
-      ws.hist = d_hist();
-      ws.trivial = d_trivial();
-      ws.tile_counter = d_tile_counter();
-      ws.tile_state_words = radix_tile_state_words<uint32_t>(n, 4);
-      tile_state.ensure(ws.tile_state_words * 4);
-      ws.tile_state = tile_state.as<uint32_t>();
-      // unordered: only the passes that cover the partition bits (the top pbits of the word); none when P == 1 -- the
-      // first pass is still needed then, to produce the identity index array
-      uint32_t pass_mask = 0xF;
-      if (unordered) {
-        pass_mask = 0;
-        for (int q = 0; q < 4; q++) if (8 * q + 8 > 32 - pbits) pass_mask |= 1u << q;
-        if (!pass_mask) pass_mask = 1;
-      }
-      int done = radix_sort_pairs(stream, ws, sortA.as<uint32_t>(), sortB.as<uint32_t>(), n, 0, 4, pass_mask, &launches);
-      if (done & 1) { K = sortB.as<uint32_t>(); order = sortB.as<uint32_t>() + n; }
-      if (unordered) {
-        k_flip_order<<<(uint32_t)div_up(n, 256), 256, 0, stream>>>(order, n);
-        launches++;
-      }
-      timer.mark(stream);
-
-      // ---------------- ties: records whose sort words collide are ordered by the rest of the key.
-      // One streaming kernel finds the groups and orders the (common) small ones in place; the partition bounds and
-      // -- for fixed-width records -- the segment layout are computed speculatively so that the whole common path needs a
-      // single host round trip (tie count, large groups, duplicates, error flag, layout totals).
-      // normalised content bytes the sort word fully covers (equal words <=> equal on these bytes)
-      const uint32_t depth0 = rec.sym ? sym_npos : (uint32_t)((32 - pbits) / 8);
-      int per_sm_tf = 0;
-      TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_tf, k_tie_fix, TIEFIX_THREADS, 0));
-      if (!unordered)   // no comparator on an unordered edge: records of a partition keep their (reversed arrival) order
-        k_tie_fix<<<(uint32_t)std::min<uint64_t>(div_up(n, TIEFIX_TILE), (uint64_t)num_sms * std::max(per_sm_tf, 1)), TIEFIX_THREADS, 0, stream>>>(
-            rec, K, order, n, depth0, same.as<uint8_t>(), d_dups(), d_large(), d_ties());
-      const uint32_t *d_m_ptr = reinterpret_cast<const uint32_t *>(d_ties());
-      k_part_bounds<<<(uint32_t)div_up((uint64_t)P + 1, 256), 256, 0, stream>>>(K, n, P, pbits, part_start.as<uint32_t>());
-      launches += 2;
-      state.have_bounds = true;
-      state.spec_layout = false;
-      if (rec.fixed) {
-        EmitParams e = make_emit_params(rec, order, 0, false, nullptr);
-        set_fixed_layout(e, rec);
-        k_layout<<<1, 1024, 0, stream>>>(e, seg_start.as<uint64_t>(), tile_start.as<uint32_t>(), d_index.as<int64_t>(), d_totals());
-        launches++;
-        state.spec_layout = true;
-      }
-      TG_CUDA(cudaGetLastError());
-      uint32_t *hw = h_small.as<uint32_t>();
-      store_to_host(stream, hw, small.as<uint32_t>() + 2064, 32, hw + 8, d_m_ptr, 4, h_small.as<uint8_t>() + 4096, d_index.p,
-                    state.spec_layout ? (size_t)P * 24 : 0);
-      TG_CUDA(cudaGetLastError());
-      TG_CUDA(cudaStreamSynchronize(stream));
-      // words: [0] error, [1] large groups, [2..3] duplicates, [4..7] layout totals, [8] tied records
-      TG_CHECK(!(hw[0] & 1u), TEZGPU_E_INVALID, "Illegal partition (outside [0, numPartitions))");
-      if (hw[0] & 2u) throw FramingMismatch();  // run-table mode: some record position lacks the fixed framing bytes
-      uint32_t m = hw[8];
-      tie_records = m;
-      memcpy(&dup_count, hw + 2, 8);
-      memcpy(&state.spec_file_bytes, hw + 4, 8);
-      memcpy(&state.spec_tiles, hw + 6, 8);
-      uint64_t *hs = h_small.as<uint64_t>() + 16;
-      if (hw[1]) {
-        // some group is larger than TIE_SMALL_MAX: radix refinement rounds over all tied records
-        k_tie_count<<<nblk, SCAN_THREADS, 0, stream>>>(K, n, blk.as<uint64_t>());
-        k_scan_block_sums<<<1, 1024, 0, stream>>>(blk.as<uint64_t>(), nblk);
-        TG_CUDA(cudaMemcpyAsync(&hs[0], blk.as<uint64_t>() + nblk, 8, cudaMemcpyDeviceToHost, stream));
-        TG_CUDA(cudaStreamSynchronize(stream));
-        m = (uint32_t)hs[0];
-        tie_records = m;
-        for (int s2 = 0; s2 < 2; s2++) { t_pos[s2].ensure((size_t)m * 4); t_gid[s2].ensure((size_t)m * 4); t_lidx[s2].ensure((size_t)m * 4); }
-        k_tie_compact<<<nblk, SCAN_THREADS, 0, stream>>>(K, order, n, blk.as<uint64_t>(), t_pos[0].as<uint32_t>(),
-                                                         t_gid[0].as<uint32_t>(), t_lidx[0].as<uint32_t>());
-        launches += 3;
-        // ---- groups larger than TIE_SMALL_MAX whose members all carry the same key need no ordering (the radix sort
-        // is stable): settle them here; only groups with really different keys go through the refinement rounds.
-        // Small groups keep the order, flags and duplicate count k_tie_fix gave them.
-        const uint32_t ngroups = (uint32_t)(hs[0] >> 32);
-        int cur = 0;
-        {
-          t_ghead.ensure(((size_t)ngroups + 2) * 4);
-          t_gneq.ensure((size_t)ngroups + 1);
-          TG_CUDA(cudaMemsetAsync(t_gneq.p, 0, (size_t)ngroups + 1, stream));
-          const uint32_t mgrid = (uint32_t)div_up(m, 256), mblk0 = (uint32_t)div_up(m, SCAN_TILE);
-          k_group_heads<<<mgrid, 256, 0, stream>>>(t_gid[0].as<uint32_t>(), m, t_ghead.as<uint32_t>());
-          k_group_equal<<<mgrid, 256, 0, stream>>>(rec, t_gid[0].as<uint32_t>(), t_lidx[0].as<uint32_t>(), t_ghead.as<uint32_t>(), m, depth0,
-                                                 TIE_SMALL_MAX, t_gneq.as<uint8_t>());
-          blk.ensure(((size_t)std::max(mblk0, nblk) + 2) * 8);
-          k_group_mark<<<mblk0, SCAN_THREADS, 0, stream>>>(t_pos[0].as<uint32_t>(), t_gid[0].as<uint32_t>(), t_ghead.as<uint32_t>(),
-                                                          t_gneq.as<uint8_t>(), m, TIE_SMALL_MAX, same.as<uint8_t>(), d_dups(), blk.as<uint64_t>());
-          k_scan_block_sums<<<1, 1024, 0, stream>>>(blk.as<uint64_t>(), mblk0);
-          launches += 4;
-          TG_CUDA(cudaGetLastError());
-          TG_CUDA(cudaMemcpyAsync(&hs[0], blk.as<uint64_t>() + mblk0, 8, cudaMemcpyDeviceToHost, stream));
-          TG_CUDA(cudaStreamSynchronize(stream));
-          const uint32_t m2 = (uint32_t)hs[0];
-          if (m2) {
-            k_group_compact<<<mblk0, SCAN_THREADS, 0, stream>>>(t_pos[0].as<uint32_t>(), t_gid[0].as<uint32_t>(), t_lidx[0].as<uint32_t>(),
-                                                               t_ghead.as<uint32_t>(), t_gneq.as<uint8_t>(), m, TIE_SMALL_MAX, blk.as<uint64_t>(),
-                                                               t_pos[1].as<uint32_t>(), t_gid[1].as<uint32_t>(), t_lidx[1].as<uint32_t>());
-            launches++;
-            TG_CUDA(cudaGetLastError());
-            cur = 1;
-          }
-          m = m2;
-        }
-        uint32_t depth = depth0;
-        while (m) {
-          t_key64[0].ensure((size_t)m * 8); t_key64[1].ensure((size_t)m * 8); t_val[0].ensure((size_t)m * 4);
-          const uint32_t mblk = (uint32_t)div_up(m, SCAN_TILE);
-          k_ref_build_keys<<<(uint32_t)div_up(m, 256), 256, 0, stream>>>(rec, t_gid[cur].as<uint32_t>(), t_lidx[cur].as<uint32_t>(), m,
-                                                                    depth, t_key64[0].as<uint64_t>());
-          TG_CUDA(cudaMemsetAsync(d_hist(), 0, 8 * RADIX * 4, stream));
-          k_radix_hist<uint64_t, 8><<<(int)std::min<uint64_t>(div_up(m, 512 * 8), (uint64_t)num_sms * 4), 512, 0, stream>>>(t_key64[0].as<uint64_t>(), m, 0, d_hist());
-          k_radix_scan_hist<<<1, RADIX, 0, stream>>>(d_hist(), 8, m, d_trivial());
-          launches += 3;
-          TG_CUDA(cudaGetLastError());
-          uint32_t *ht = h_small.as<uint32_t>() + 64;
-          TG_CUDA(cudaMemcpyAsync(ht, d_trivial(), 8 * 4, cudaMemcpyDeviceToHost, stream));
-          TG_CUDA(cudaStreamSynchronize(stream));
-          uint32_t mask = 0;
-          for (int q = 0; q < 8; q++) if (!ht[q]) mask |= 1u << q;
-          RadixWorkspace w2 = ws;
-          w2.tile_state_words = radix_tile_state_words<uint64_t>(m, 8);
-          t_state.ensure(w2.tile_state_words * 4);
-          w2.tile_state = t_state.as<uint32_t>();
-          int d2 = radix_sort_passes<uint64_t>(stream, w2, t_key64[0].as<uint64_t>(), t_key64[1].as<uint64_t>(), t_lidx[cur].as<uint32_t>(),
-                                               t_val[0].as<uint32_t>(), m, 0, 8, mask, &launches);
-          const uint64_t *Ks = (d2 & 1) ? t_key64[1].as<uint64_t>() : t_key64[0].as<uint64_t>();
-          const uint32_t *Ls = (d2 & 1) ? t_val[0].as<uint32_t>() : t_lidx[cur].as<uint32_t>();
-          k_ref_apply_count<<<mblk, SCAN_THREADS, 0, stream>>>(Ks, Ls, t_pos[cur].as<uint32_t>(), m, order, same.as<uint8_t>(), d_dups(),
-                                                              blk.as<uint64_t>());
-          k_scan_block_sums<<<1, 1024, 0, stream>>>(blk.as<uint64_t>(), mblk);
-          launches += 2;
-          TG_CUDA(cudaMemcpyAsync(&hs[0], blk.as<uint64_t>() + mblk, 8, cudaMemcpyDeviceToHost, stream));
-          TG_CUDA(cudaStreamSynchronize(stream));
-          uint32_t m2 = (uint32_t)hs[0];
-          if (m2) {
-            k_ref_compact<<<mblk, SCAN_THREADS, 0, stream>>>(Ks, Ls, t_pos[cur].as<uint32_t>(), m, blk.as<uint64_t>(),
-                                                            t_pos[cur ^ 1].as<uint32_t>(), t_gid[cur ^ 1].as<uint32_t>(),
-                                                            t_lidx[cur ^ 1].as<uint32_t>());
-            launches++;
-            TG_CUDA(cudaGetLastError());
-          }
-          cur ^= 1;
-          m = m2;
-          depth += 3;
-        }
-        TG_CUDA(cudaMemcpyAsync(&hs[0], d_dups(), 8, cudaMemcpyDeviceToHost, stream));
-        TG_CUDA(cudaStreamSynchronize(stream));
-        dup_count = hs[0];
-      }
+      uint32_t depth0;
+      launches += alphabet_table(rec, &depth0);
+      launches += stage_and_sort(rec);
+      launches += fix_ties(rec, depth0);
+      if (h_scratch()->verdict.large_groups) launches += refine_large_groups(rec, depth0);
     }
     timer.mark(stream);
     state.rec = rec;
-    state.K = K;
-    state.order = order;
-    state.dup_count = dup_count;
-    state.tie_records = tie_records;
     state.launches = launches;
+  }
+
+  // The alphabet-compressed sort word (SymTable, sorter_kernels.cuh): the byte values at the first content positions ->
+  // ranks, packed while they fit the key field.  *depth = normalised content bytes the sort word fully covers.
+  int alphabet_table(Records &rec, uint32_t *depth) {
+    *depth = (uint32_t)((32 - pbits) / 8);
+    if (rec.fixed || rec.unordered || (getenv("TEZGPU_NO_SYM") && atoi(getenv("TEZGPU_NO_SYM")))) return 0;
+    sym_sets.ensure(SYM_MAX_POS * 8 * 4);
+    sym_tab.ensure(sizeof(SymTable));
+    TG_CUDA(cudaMemsetAsync(sym_sets.p, 0, SYM_MAX_POS * 8 * 4, stream));
+    k_symbols<<<(int)std::min<uint64_t>(div_up(rec.n, 256), (uint64_t)num_sms * 8), 256, 0, stream>>>(rec, sym_sets.as<uint32_t>());
+    uint32_t hs[SYM_MAX_POS * 8];
+    TG_CUDA(cudaMemcpyAsync(hs, sym_sets.p, sizeof(hs), cudaMemcpyDeviceToHost, stream));
+    TG_CUDA(cudaStreamSynchronize(stream));
+    SymTable *t = new SymTable();
+    const uint32_t np = sym_table_build(hs, pbits, t);
+    if (sym_table_pays(np, pbits)) {
+      TG_CUDA(cudaMemcpyAsync(sym_tab.p, t, sizeof(SymTable), cudaMemcpyHostToDevice, stream));
+      TG_CUDA(cudaStreamSynchronize(stream));
+      rec.sym = sym_tab.as<SymTable>();
+      *depth = np;
+    }
+    delete t;
+    return 1;
+  }
+
+  // The stage (sort words, and the digit histograms of every pass) and the radix sort of (sort word, record index)
+  int stage_and_sort(const Records &rec) {
+    const uint32_t n = rec.n;
+    SortScratch *d = d_scratch();
+    TG_CUDA(cudaMemsetAsync(same.p, 0, n, stream));
+    const bool fast16 = rec.fixed && !rec.key_off && !rec.use_runs && rec.klen == 16 && ((rec.klen + rec.vlen) % 16 == 0) && rec.cmp == CMP_BYTES &&
+                        (((uintptr_t)rec.kv & 15u) == 0);
+    int sgrid = (int)std::min<uint64_t>(div_up(n, 256), (uint64_t)num_sms * 16);
+    if (fast16) k_stage<true><<<sgrid, 256, 0, stream>>>(rec, state.K, d->hist, &d->verdict.error);
+    else k_stage<false><<<sgrid, 256, 0, stream>>>(rec, state.K, d->hist, &d->verdict.error);
+    TG_CUDA(cudaGetLastError());
+    k_radix_scan_hist<<<1, RADIX, 0, stream>>>(d->hist, 4, n, d->trivial);
+    TG_CUDA(cudaGetLastError());
+    int launches = 2;
+    timer.mark(stream);
+
+    const size_t words = radix_tile_state_words<uint32_t>(n, 4);
+    tile_state.ensure(words * 4);
+    const RadixWorkspace ws{d->hist, d->trivial, tile_state.as<uint32_t>(), d->tile_counter, words, conf.device};
+    // unordered: only the passes that cover the partition bits (the top pbits of the word); none when P == 1 -- the
+    // first pass is still needed then, to produce the identity index array
+    uint32_t pass_mask = 0xF;
+    if (rec.unordered) {
+      pass_mask = 0;
+      for (int q = 0; q < 4; q++) if (8 * q + 8 > 32 - pbits) pass_mask |= 1u << q;
+      if (!pass_mask) pass_mask = 1;
+    }
+    const int done = radix_sort_pairs(stream, ws, sortA.as<uint32_t>(), sortB.as<uint32_t>(), n, 0, 4, pass_mask, &launches);
+    if (done & 1) { state.K = sortB.as<uint32_t>(); state.order = sortB.as<uint32_t>() + n; }
+    if (rec.unordered) {
+      k_flip_order<<<(uint32_t)div_up(n, 256), 256, 0, stream>>>(state.order, n);
+      launches++;
+    }
+    timer.mark(stream);
+    return launches;
+  }
+
+  // Ties: records whose sort words collide are ordered by the rest of the key.  One streaming kernel finds the groups
+  // and orders the (common) small ones in place; the partition bounds and -- for fixed-width records -- the segment
+  // layout are computed speculatively, so that the whole common path needs this one host round trip (its verdict).
+  int fix_ties(const Records &rec, uint32_t depth0) {
+    const uint32_t n = rec.n;
+    const int P = conf.num_partitions;
+    SortScratch *d = d_scratch();
+    SortHostScratch *h = h_scratch();
+    int per_sm_tf = 0;
+    TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_tf, k_tie_fix, TIEFIX_THREADS, 0));
+    if (!rec.unordered)   // no comparator on an unordered edge: records of a partition keep their (reversed arrival) order
+      k_tie_fix<<<(uint32_t)std::min<uint64_t>(div_up(n, TIEFIX_TILE), (uint64_t)num_sms * std::max(per_sm_tf, 1)), TIEFIX_THREADS, 0, stream>>>(
+          rec, state.K, state.order, n, depth0, same.as<uint8_t>(), &d->verdict.dups, &d->verdict.large_groups, &d->ties);
+    k_part_bounds<<<(uint32_t)div_up((uint64_t)P + 1, 256), 256, 0, stream>>>(state.K, n, P, pbits, part_start.as<uint32_t>());
+    int launches = 2;   // k_tie_fix is counted on unordered edges too
+    state.have_bounds = true;
+    if (rec.fixed) {
+      EmitParams e = make_emit_params(rec, state.order, 0, false, nullptr);
+      set_fixed_layout(e, rec);
+      k_layout<<<1, 1024, 0, stream>>>(e, seg_start.as<uint64_t>(), tile_start.as<uint32_t>(), d_index.as<int64_t>(), d->verdict.totals);
+      launches++;
+      state.spec_layout = true;
+    }
+    TG_CUDA(cudaGetLastError());
+    store_to_host(stream, &h->verdict, &d->verdict, sizeof(SortVerdict), &h->ties, &d->ties, 4, h->index(), d_index.p,
+                  state.spec_layout ? (size_t)P * 24 : 0);
+    TG_CUDA(cudaGetLastError());
+    TG_CUDA(cudaStreamSynchronize(stream));
+    TG_CHECK(!(h->verdict.error & STAGE_ERR_PARTITION), TEZGPU_E_INVALID, "Illegal partition (outside [0, numPartitions))");
+    if (h->verdict.error & STAGE_ERR_FRAMING) throw FramingMismatch();
+    state.tie_records = h->ties;
+    state.dup_count = h->verdict.dups;
+    return launches;
+  }
+
+  // Some tie group is larger than TIE_SMALL_MAX: radix refinement rounds over all tied records.  Groups whose members
+  // all carry the same key need no ordering (the radix sort is stable) and are settled first; only groups with really
+  // different keys go through the rounds.  Small groups keep the order, flags and duplicate count k_tie_fix gave them.
+  int refine_large_groups(const Records &rec, uint32_t depth0) {
+    const uint32_t n = rec.n, nblk = (uint32_t)div_up(n, SCAN_TILE);
+    SortScratch *d = d_scratch();
+    SortHostScratch *h = h_scratch();
+    int launches = 0;
+    auto scan_total = [&](uint32_t nb) {
+      k_scan_block_sums<<<1, 1024, 0, stream>>>(blk.as<uint64_t>(), nb);
+      launches++;
+      TG_CUDA(cudaGetLastError());
+      TG_CUDA(cudaMemcpyAsync(&h->total, blk.as<uint64_t>() + nb, 8, cudaMemcpyDeviceToHost, stream));
+      TG_CUDA(cudaStreamSynchronize(stream));
+      return h->total;
+    };
+    k_tie_count<<<nblk, SCAN_THREADS, 0, stream>>>(state.K, n, blk.as<uint64_t>());
+    const uint64_t tied = scan_total(nblk);
+    uint32_t m = (uint32_t)tied;
+    const uint32_t ngroups = (uint32_t)(tied >> 32);
+    state.tie_records = m;
+    for (int s2 = 0; s2 < 2; s2++) { t_pos[s2].ensure((size_t)m * 4); t_gid[s2].ensure((size_t)m * 4); t_lidx[s2].ensure((size_t)m * 4); }
+    k_tie_compact<<<nblk, SCAN_THREADS, 0, stream>>>(state.K, state.order, n, blk.as<uint64_t>(), t_pos[0].as<uint32_t>(),
+                                                     t_gid[0].as<uint32_t>(), t_lidx[0].as<uint32_t>());
+    launches += 2;
+    t_ghead.ensure(((size_t)ngroups + 2) * 4);
+    t_gneq.ensure((size_t)ngroups + 1);
+    TG_CUDA(cudaMemsetAsync(t_gneq.p, 0, (size_t)ngroups + 1, stream));
+    const uint32_t mgrid = (uint32_t)div_up(m, 256), mblk0 = (uint32_t)div_up(m, SCAN_TILE);
+    k_group_heads<<<mgrid, 256, 0, stream>>>(t_gid[0].as<uint32_t>(), m, t_ghead.as<uint32_t>());
+    k_group_equal<<<mgrid, 256, 0, stream>>>(rec, t_gid[0].as<uint32_t>(), t_lidx[0].as<uint32_t>(), t_ghead.as<uint32_t>(), m, depth0,
+                                           TIE_SMALL_MAX, t_gneq.as<uint8_t>());
+    blk.ensure(((size_t)std::max(mblk0, nblk) + 2) * 8);
+    k_group_mark<<<mblk0, SCAN_THREADS, 0, stream>>>(t_pos[0].as<uint32_t>(), t_gid[0].as<uint32_t>(), t_ghead.as<uint32_t>(),
+                                                    t_gneq.as<uint8_t>(), m, TIE_SMALL_MAX, same.as<uint8_t>(), &d->verdict.dups, blk.as<uint64_t>());
+    launches += 3;
+    uint32_t left = (uint32_t)scan_total(mblk0);   // records of the groups whose keys differ
+    if (left) {
+      k_group_compact<<<mblk0, SCAN_THREADS, 0, stream>>>(t_pos[0].as<uint32_t>(), t_gid[0].as<uint32_t>(), t_lidx[0].as<uint32_t>(),
+                                                         t_ghead.as<uint32_t>(), t_gneq.as<uint8_t>(), m, TIE_SMALL_MAX, blk.as<uint64_t>(),
+                                                         t_pos[1].as<uint32_t>(), t_gid[1].as<uint32_t>(), t_lidx[1].as<uint32_t>());
+      launches++;
+      TG_CUDA(cudaGetLastError());
+    }
+    for (uint32_t depth = depth0, cur = 1; left; depth += 3, cur ^= 1) {
+      m = left;
+      t_key64[0].ensure((size_t)m * 8); t_key64[1].ensure((size_t)m * 8); t_val[0].ensure((size_t)m * 4);
+      const uint32_t mblk = (uint32_t)div_up(m, SCAN_TILE);
+      k_ref_build_keys<<<(uint32_t)div_up(m, 256), 256, 0, stream>>>(rec, t_gid[cur].as<uint32_t>(), t_lidx[cur].as<uint32_t>(), m,
+                                                                depth, t_key64[0].as<uint64_t>());
+      TG_CUDA(cudaMemsetAsync(d->hist, 0, sizeof(d->hist), stream));
+      k_radix_hist<uint64_t, 8><<<(int)std::min<uint64_t>(div_up(m, 512 * 8), (uint64_t)num_sms * 4), 512, 0, stream>>>(t_key64[0].as<uint64_t>(), m, 0, d->hist);
+      k_radix_scan_hist<<<1, RADIX, 0, stream>>>(d->hist, 8, m, d->trivial);
+      launches += 3;
+      TG_CUDA(cudaGetLastError());
+      TG_CUDA(cudaMemcpyAsync(h->trivial, d->trivial, sizeof(h->trivial), cudaMemcpyDeviceToHost, stream));
+      TG_CUDA(cudaStreamSynchronize(stream));
+      uint32_t mask = 0;
+      for (int q = 0; q < 8; q++) if (!h->trivial[q]) mask |= 1u << q;
+      const size_t words = radix_tile_state_words<uint64_t>(m, 8);
+      t_state.ensure(words * 4);
+      const RadixWorkspace ws{d->hist, d->trivial, t_state.as<uint32_t>(), d->tile_counter, words, conf.device};
+      const int passes = radix_sort_passes<uint64_t>(stream, ws, t_key64[0].as<uint64_t>(), t_key64[1].as<uint64_t>(), t_lidx[cur].as<uint32_t>(),
+                                                     t_val[0].as<uint32_t>(), m, 0, 8, mask, &launches);
+      const uint64_t *Ks = (passes & 1) ? t_key64[1].as<uint64_t>() : t_key64[0].as<uint64_t>();
+      const uint32_t *Ls = (passes & 1) ? t_val[0].as<uint32_t>() : t_lidx[cur].as<uint32_t>();
+      k_ref_apply_count<<<mblk, SCAN_THREADS, 0, stream>>>(Ks, Ls, t_pos[cur].as<uint32_t>(), m, state.order, same.as<uint8_t>(), &d->verdict.dups,
+                                                          blk.as<uint64_t>());
+      launches++;
+      left = (uint32_t)scan_total(mblk);
+      if (left) {
+        k_ref_compact<<<mblk, SCAN_THREADS, 0, stream>>>(Ks, Ls, t_pos[cur].as<uint32_t>(), m, blk.as<uint64_t>(),
+                                                        t_pos[cur ^ 1].as<uint32_t>(), t_gid[cur ^ 1].as<uint32_t>(),
+                                                        t_lidx[cur ^ 1].as<uint32_t>());
+        launches++;
+        TG_CUDA(cudaGetLastError());
+      }
+    }
+    TG_CUDA(cudaMemcpyAsync(&h->total, &d->verdict.dups, 8, cudaMemcpyDeviceToHost, stream));
+    TG_CUDA(cudaStreamSynchronize(stream));
+    state.dup_count = h->total;
+    return launches;
   }
 
   // layout + emit of the sorted records as IFile segments.  merge_mode: REPEAT_KEY semantics of TezMerger.writeFile
@@ -551,13 +560,9 @@ class SortPipeline {
     const bool no_repeats = !rle && (!merge_mode || (!merge_check_same && merge_inputs_plain));
     const bool fixed_emit = rec.fixed && (dup_count == 0 || no_repeats);
     uint64_t bound = output_bound(n, rec.fixed ? (uint64_t)n * (rec.klen + rec.vlen) : rec.kv_bytes, P);
-    uint64_t *hs = h_small.as<uint64_t>();
     const FixedEmitKernel kernel = fixed_emit ? set_fixed_layout(e, rec) : FixedEmitKernel::General;
-    if (fixed_emit && state.spec_layout) {
-      // layout, totals and index triples were produced during the sort phase (same plan): no round trip here
-      hs[0] = state.spec_file_bytes;
-      hs[1] = state.spec_tiles;
-    } else {
+    // layout, totals and index triples produced during the sort phase (same plan) need no round trip here
+    if (!fixed_emit || !state.spec_layout) {
       if (!fixed_emit) {
         uint64_t avg = n ? (rec.fixed ? (uint64_t)(rec.klen + rec.vlen) : rec.kv_bytes / n) + 4 : 16;
         e.recs_per_tile = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(EMIT_MAX_RECS, (EMIT_IMG_BYTES - 32) / avg));
@@ -576,16 +581,16 @@ class SortPipeline {
         }
         e.rec_off = rec_off.as<uint64_t>();
       }
-      k_layout<<<1, 1024, 0, stream>>>(e, seg_start.as<uint64_t>(), tile_start.as<uint32_t>(), d_index.as<int64_t>(), d_totals());
+      k_layout<<<1, 1024, 0, stream>>>(e, seg_start.as<uint64_t>(), tile_start.as<uint32_t>(), d_index.as<int64_t>(), d_scratch()->verdict.totals);
       launches++;
       TG_CUDA(cudaGetLastError());
-      store_to_host(stream, &hs[0], d_totals(), 16, h_small.as<uint8_t>() + 4096, d_index.p, (size_t)P * 24);
+      store_to_host(stream, h_scratch()->verdict.totals, d_scratch()->verdict.totals, 16, h_scratch()->index(), d_index.p, (size_t)P * 24);
       TG_CUDA(cudaGetLastError());
       TG_CUDA(cudaStreamSynchronize(stream));
       state.spec_layout = false;  // the device layout now belongs to this emit
     }
-    const uint64_t file_bytes = hs[0];
-    const uint64_t tiles = hs[1];
+    const uint64_t file_bytes = h_scratch()->verdict.totals[0];
+    const uint64_t tiles = h_scratch()->verdict.totals[1];
     TG_CHECK(file_bytes <= bound, TEZGPU_E_INVALID, "internal: output exceeds bound");
     TG_CHECK(file_bytes <= out_cap, TEZGPU_E_NOMEM, "output buffer too small for file.out");
     // the source-oriented kernels (emit_fast.cuh, emit_pipe*.cuh) gather 16-byte pieces of the records tile by tile
@@ -623,11 +628,7 @@ class SortPipeline {
             // next to their images, indices and parked partials (54 KB): 125 KB keeps the CTA in the 132 KB
             // shared-memory carveout, which leaves the random gather enough L1 for its loads in flight (larger
             // footprints measured slower, DESIGN.md §7).
-            static bool attr = false;
-            if (!attr) {
-              TG_CUDA(cudaFuncSetAttribute(k_emit_fast4<FE4_UNROLL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Emit4Smem::TOTAL));
-              attr = true;
-            }
+            set_smem_limit<k_emit_fast4<FE4_UNROLL>>(conf.device, Emit4Smem::TOTAL);
             const uint32_t grid = (uint32_t)std::min<uint64_t>(div_up(tiles, FE4_GROUPS), (uint64_t)num_sms);
             k_emit_fast4<FE4_UNROLL><<<grid, FE_THREADS * FE4_GROUPS, Emit4Smem::TOTAL, stream>>>(fp);
             break;
@@ -635,16 +636,11 @@ class SortPipeline {
           case FixedEmitKernel::Fast:
             k_emit_fast<5, true><<<persistent_grid(k_emit_fast<5, true>, FE_THREADS, 0), FE_THREADS, 0, stream>>>(fp);
             break;
-          case FixedEmitKernel::PipeUnaligned: {
-            static bool attr = false;
-            if (!attr) {
-              TG_CUDA(cudaFuncSetAttribute(k_emit_fast4u<FE4U_UNROLL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Emit4uSmem::TOTAL));
-              attr = true;
-            }
-            const uint32_t grid = persistent_grid(k_emit_fast4u<FE4U_UNROLL>, FE_THREADS, Emit4uSmem::TOTAL);
-            k_emit_fast4u<FE4U_UNROLL><<<grid, FE_THREADS, Emit4uSmem::TOTAL, stream>>>(fp);
+          case FixedEmitKernel::PipeUnaligned:
+            set_smem_limit<k_emit_fast4u<FE4U_UNROLL>>(conf.device, Emit4uSmem::TOTAL);
+            k_emit_fast4u<FE4U_UNROLL><<<persistent_grid(k_emit_fast4u<FE4U_UNROLL>, FE_THREADS, Emit4uSmem::TOTAL), FE_THREADS,
+                                         Emit4uSmem::TOTAL, stream>>>(fp);
             break;
-          }
           case FixedEmitKernel::FastUnaligned:
             k_emit_fast<5, false><<<persistent_grid(k_emit_fast<5, false>, FE_THREADS, 0), FE_THREADS, 0, stream>>>(fp);
             break;
@@ -668,7 +664,7 @@ class SortPipeline {
     TG_CUDA(cudaStreamSynchronize(stream));
 
     if (out_len) *out_len = file_bytes;
-    const int64_t *hidx = reinterpret_cast<const int64_t *>(h_small.as<uint8_t>() + 4096);
+    const int64_t *hidx = h_scratch()->index();
     if (index) memcpy(index, hidx, (size_t)P * 24);
     if (stats) {
       memset(stats, 0, sizeof(*stats));

@@ -174,6 +174,9 @@ __host__ __device__ __forceinline__ uint32_t stage_sort_word(const Records &r, c
   return compose_sort_word(r, p, prefix, bad);
 }
 
+constexpr int STAGE_ERR_PARTITION = 1;  // k_stage's error bits: "Illegal partition" (PipelinedSorter.java:410-413),
+constexpr int STAGE_ERR_FRAMING = 2;    // and in run-table mode, a record position that lacks the fixed framing bytes
+
 // One thread per record: its sort word (stage_sort_word, or inline for 16-byte fixed keys) and the digit histograms of
 // all four radix passes (so the sort never re-reads the keys for counting).
 template <bool FAST16>
@@ -221,14 +224,14 @@ __global__ void __launch_bounds__(256) k_stage(Records r, uint32_t *__restrict__
         // framing bytes (same sector as the key: free); a mismatch sends the merge to the general parser
         bool ok = true;
         for (uint32_t b = 0; b < r.runs.hdr_len; b++) ok &= r.kv[roff + b] == (uint8_t)(r.runs.hdr_bytes >> (8 * b));
-        if (!ok) atomicOr(error_flag, 2);
+        if (!ok) atomicOr(error_flag, STAGE_ERR_FRAMING);
       } else {
         record_lookup(r, i, koff, klen, vlen);
       }
       const int32_t given = r.hash_partition ? 0 : ((r.fixed && r.use_runs) ? run_part : (r.partition ? r.partition[i] : 0));
       K = stage_sort_word(r, r.kv + koff, klen, given, bad);
     }
-    if (bad) atomicOr(error_flag, 1);  // "Illegal partition" (PipelinedSorter.java:410-413)
+    if (bad) atomicOr(error_flag, STAGE_ERR_PARTITION);
     keys_out[r.unordered ? r.n - 1u - i : i] = K;
 #pragma unroll
     for (int q = 0; q < 4; q++) atomicAdd(&s_hist[q * RADIX + ((K >> (8 * q)) & 0xFF)], 1u);

@@ -194,13 +194,13 @@ int32_t tezgpu_sorter_collect_batch(tezgpu_sorter *h, const uint8_t *kv, uint64_
   TG_CUDA(cudaMemcpyAsync(t + 2 * (size_t)n, val_len, (size_t)n * 4, cudaMemcpyHostToDevice, st));
   if (partition)
     TG_CUDA(cudaMemcpyAsync(h->d_part.as<int32_t>() + h->n, partition, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  TG_CUDA(cudaMemsetAsync(h->pipe.d_error(), 0, 4, st));
+  TG_CUDA(cudaMemsetAsync(&h->pipe.d_scratch()->verdict.error, 0, 4, st));
   k_rebase_offsets<<<(uint32_t)div_up(n, 256), 256, 0, st>>>(t, t + n, t + 2 * (size_t)n, n, base, kv_bytes,
                                                            h->d_koff.as<uint64_t>() + h->n, h->d_klen.as<uint32_t>() + h->n,
-                                                           h->d_vlen.as<uint32_t>() + h->n, h->pipe.d_error());
+                                                           h->d_vlen.as<uint32_t>() + h->n, &h->pipe.d_scratch()->verdict.error);
   TG_CUDA(cudaGetLastError());
   int err = 0;
-  TG_CUDA(cudaMemcpyAsync(&err, h->pipe.d_error(), 4, cudaMemcpyDeviceToHost, st));
+  TG_CUDA(cudaMemcpyAsync(&err, &h->pipe.d_scratch()->verdict.error, 4, cudaMemcpyDeviceToHost, st));
   TG_CUDA(cudaStreamSynchronize(st));  // caller may reuse its buffers once we return
   TG_CHECK(err == 0, TEZGPU_E_INVALID, "record offsets outside the batch buffer");
   for (uint32_t i = 0; i < n; i++) h->payload_bytes += (uint64_t)(val_off[i] - key_off[i]) + val_len[i];
