@@ -1,8 +1,10 @@
 // codec.cuh -- DefaultCodec, Lz4Codec and ZStandardCodec on both sides of the shuffle: the compress phase behind every
-// emit (SortPipeline) and the decompress step in front of every merge open (Merger).  Formats and kernels: deflate.cuh,
-// inflate.cuh (DefaultCodec), lz4.cuh (Lz4Codec), zstd.cuh (ZStandardCodec).  The codecs share the chunk layout, the
-// size scan, the pack and the checksum kernels; only the chunk kernels and the segment finish differ.
+// emit (SortPipeline) and the decompress step in front of every merge open (Merger).  Formats, chunk kernels and
+// decoders: deflate.cuh, inflate.cuh (DefaultCodec), lz4.cuh (Lz4Codec), zstd.cuh (ZStandardCodec).  What the codecs
+// share is here: the segment layout and its kernels, the finish of LZ4 and zstd segments, the reader's staging and
+// checksum check, its block-parallel sequence for LZ4 and zstd, and the writers' host runs.
 #pragma once
+#include <memory>
 #include "inflate.cuh"
 #include "lz4.cuh"
 #include "zstd.cuh"
@@ -16,6 +18,89 @@ inline void check_codec(int32_t codec) {
            TEZGPU_E_UNSUPPORTED, "codec " + std::to_string(codec) + " is not on the device (DefaultCodec, Lz4Codec and ZStandardCodec only)");
 }
 
+// How a codec's compressed segment is laid out around its chunks.  zlib: 32 KiB chunks, framed by
+// TIF\x01 78 01 | chunks | Adler-32 CRC; LZ4: blocks of one chunk each (their 8 header bytes in the slot), framed by
+// TIF\x01 | blocks | CRC; zstd: one frame per chunk, framed by TIF\x01 | frames | CRC.
+struct CodecLayout {
+  uint64_t chunk;   // body bytes per chunk
+  uint32_t slot;    // device bytes reserved per compressed chunk
+  uint32_t frame;   // segment bytes outside the chunks
+  uint32_t head;    // segment bytes before the first chunk
+  uint32_t tail;    // checksummed bytes after the last chunk
+};
+inline CodecLayout codec_layout(int32_t codec) {
+  switch (codec) {
+    case TEZGPU_CODEC_LZ4: return {L4_BLOCK, L4_SLOT, 8, 4, 0};
+    case TEZGPU_CODEC_ZSTD: return {ZS_BLOCK, ZS_SLOT, 8, 4, 0};
+    default: return {ZCHUNK, ZSLOT, 14, 6, 4};
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ writer kernels
+// chunk descriptors for k_crc_pieces (one piece per chunk: a chunk is < CRC_PIECE bytes); slot: bytes per chunk slot
+__global__ void k_zchunk_descs(const uint32_t *__restrict__ csize, uint32_t nchunks, uint32_t slot, SegDesc *__restrict__ descs,
+                               uint32_t *__restrict__ piece_start) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c > nchunks) return;
+  piece_start[c] = c;
+  if (c == nchunks) return;
+  SegDesc d;
+  d.off = (uint64_t)c * slot;
+  d.len = csize[c] + 4;
+  d.body0 = 0;
+  d.body_end = csize[c];
+  d.has_header = 1;
+  d.partition = 0;
+  descs[c] = d;
+}
+
+// per partition: file offset and length of its compressed segment; frame: bytes of a segment outside its chunks
+__global__ void k_zseg_layout(ZSeg *__restrict__ segs, uint32_t P, const uint64_t *__restrict__ coff, uint32_t frame) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  ZSeg &s = segs[p];
+  s.zstart = coff[s.chunk0] + frame * s.rank;
+  s.zlen = s.nchunks ? coff[s.chunk0 + s.nchunks] - coff[s.chunk0] + frame : 0;
+}
+
+// chunk checksums -> positions in their segment's checksummed bytes (zlib: header, chunks, Adler-32; LZ4 and zstd: the
+// chunks); tail: checksummed bytes after the last chunk
+__global__ void k_zcrc_place(TileCrc *__restrict__ tc, uint32_t nchunks, const ZSeg *__restrict__ segs, uint32_t P,
+                             const uint64_t *__restrict__ coff, uint32_t tail) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= nchunks) return;
+  const uint32_t p = z_chunk_part(segs, P, c);
+  const ZSeg s = segs[p];
+  tc[c].p = p;
+  tc[c].after = coff[s.chunk0 + s.nchunks] - coff[c + 1] + tail;
+}
+
+// one CTA per chunk: the chunk's bytes into the file (slot: bytes per chunk slot; head: segment bytes before the chunks)
+__global__ void k_zpack(const uint8_t *__restrict__ slots, const uint32_t *__restrict__ csize, const uint64_t *__restrict__ coff,
+                        const ZSeg *__restrict__ segs, uint32_t P, uint32_t slot, uint32_t head, uint8_t *__restrict__ out) {
+  const uint32_t c = blockIdx.x;
+  const ZSeg s = segs[z_chunk_part(segs, P, c)];
+  uint8_t *dst = out + s.zstart + head + (coff[c] - coff[s.chunk0]);
+  const uint8_t *src = slots + (uint64_t)c * slot;
+  const uint32_t n = csize[c];
+  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
+}
+
+// per block-framed (LZ4, zstd) segment: TIF\x01 and the CRC-32 of the stream (the chunks' raw remainders are in seg_crc)
+__global__ void k_zfinish_blocks(const ZSeg *__restrict__ segs, uint32_t P, const uint32_t *__restrict__ seg_crc,
+                                 const CrcTables *__restrict__ t, uint8_t *__restrict__ out) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  const ZSeg s = segs[p];
+  if (!s.nchunks) return;
+  uint8_t *o = out + s.zstart;
+  o[0] = 'T'; o[1] = 'I'; o[2] = 'F'; o[3] = 1;
+  const uint64_t region = s.zlen - 8;
+  const uint32_t crc = seg_crc[p] ^ crc_shift_bytes(t, 0xFFFFFFFFu, region) ^ 0xFFFFFFFFu;
+  uint8_t *tr = o + s.zlen - 4;
+  tr[0] = (uint8_t)(crc >> 24); tr[1] = (uint8_t)(crc >> 16); tr[2] = (uint8_t)(crc >> 8); tr[3] = (uint8_t)crc;
+}
+
 // The uncompressed file is in z_img with its index raw_index (start, rawLength, partLength per partition).  Every
 // partition that has a segment gets a compressed one: TIF\x01, the codec stream of the same body (zlib, or LZ4 blocks),
 // CRC-32 of the stream.  index receives (start, the same rawLength, compressed length).  One host round trip (the
@@ -24,11 +109,7 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
                                          int64_t *index, tezgpu_stats *stats) {
   const int P = conf.num_partitions;
   cudaStream_t st = stream;
-  // zlib: 32 KiB chunks, framed by TIF\x01 78 01 | chunks | Adler-32 CRC; LZ4: blocks of one chunk each (their 8 header
-  // bytes in the slot), framed by TIF\x01 | blocks | CRC; zstd: one frame per chunk, framed by TIF\x01 | frames | CRC
-  const bool lz4 = codec == TEZGPU_CODEC_LZ4, zstd = codec == TEZGPU_CODEC_ZSTD, blocks = lz4 || zstd;
-  const uint64_t chunk = lz4 ? L4_BLOCK : zstd ? ZS_BLOCK : ZCHUNK;
-  const uint32_t slot = lz4 ? L4_SLOT : zstd ? ZS_SLOT : ZSLOT, frame = blocks ? 8 : 14, head = blocks ? 4 : 6, tail = blocks ? 0 : 4;
+  const CodecLayout L = codec_layout(codec);
   z_timer.reset();
   z_timer.mark(st);
   z_host.ensure((size_t)P * sizeof(ZSeg) + 64);
@@ -44,7 +125,7 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     if (part > 0) {
       s.body_off = (uint64_t)start + 4;
       s.body_len = (uint64_t)part - 8;
-      s.nchunks = (uint32_t)std::max<uint64_t>(1, div_up(s.body_len, chunk));
+      s.nchunks = (uint32_t)std::max<uint64_t>(1, div_up(s.body_len, L.chunk));
       nchunks += s.nchunks;
       nsegs++;
     }
@@ -54,25 +135,28 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
   if (nchunks) {
     z_segs.ensure((size_t)P * sizeof(ZSeg));
     TG_CUDA(cudaMemcpyAsync(z_segs.p, hs, (size_t)P * sizeof(ZSeg), cudaMemcpyHostToDevice, st));
-    z_slots.ensure((size_t)nchunks * slot);
+    z_slots.ensure((size_t)nchunks * L.slot);
     z_csize.ensure((size_t)nchunks * 4);
     z_coff.ensure(((size_t)nchunks + 2) * 8);
-    if (zstd) {
-      set_smem_limit<k_zscompress>(conf.device, sizeof(ZsShared));
-      k_zscompress<<<nchunks, ZS_LANES, sizeof(ZsShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
-                                                               z_csize.as<uint32_t>());
-    } else if (lz4) {
-      set_smem_limit<k_l4compress>(conf.device, sizeof(L4Shared));
-      k_l4compress<<<nchunks, L4_LANES, sizeof(L4Shared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
-                                                               z_csize.as<uint32_t>());
-    } else {
-      set_smem_limit<k_zdeflate>(conf.device, sizeof(ZShared));
-      z_cadler.ensure((size_t)nchunks * 4);
-      k_zdeflate<<<nchunks, ZLANES, sizeof(ZShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
-                                                          z_csize.as<uint32_t>(), z_cadler.as<uint32_t>());
+    switch (codec) {
+      case TEZGPU_CODEC_LZ4:
+        set_smem_limit<k_l4compress>(conf.device, sizeof(L4Shared));
+        k_l4compress<<<nchunks, L4_LANES, sizeof(L4Shared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
+                                                                 z_csize.as<uint32_t>());
+        break;
+      case TEZGPU_CODEC_ZSTD:
+        set_smem_limit<k_zscompress>(conf.device, sizeof(ZsShared));
+        k_zscompress<<<nchunks, ZS_LANES, sizeof(ZsShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
+                                                                 z_csize.as<uint32_t>());
+        break;
+      default:
+        set_smem_limit<k_zdeflate>(conf.device, sizeof(ZShared));
+        z_cadler.ensure((size_t)nchunks * 4);
+        k_zdeflate<<<nchunks, ZLANES, sizeof(ZShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
+                                                            z_csize.as<uint32_t>(), z_cadler.as<uint32_t>());
     }
     launches += 1 + scan_u32_exclusive(st, blk, z_csize.as<uint32_t>(), nchunks, z_coff.as<uint64_t>());
-    k_zseg_layout<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_coff.as<uint64_t>(), frame);
+    k_zseg_layout<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_coff.as<uint64_t>(), L.frame);
     launches++;
     TG_CUDA(cudaGetLastError());
     TG_CUDA(cudaMemcpyAsync(hs, z_segs.p, (size_t)P * sizeof(ZSeg), cudaMemcpyDeviceToHost, st));
@@ -81,7 +165,7 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     TG_CUDA(cudaStreamSynchronize(st));
     uint64_t cbytes;
     memcpy(&cbytes, reinterpret_cast<uint8_t *>(hs) + (size_t)P * sizeof(ZSeg), 8);
-    total = cbytes + frame * nsegs;
+    total = cbytes + L.frame * nsegs;
     TG_CHECK(total <= out_cap, TEZGPU_E_NOMEM, "output buffer too small for the compressed file.out");
     // checksums of the chunks (k_crc_pieces, one piece per chunk), placed in their segments and folded per segment
     const CrcTables *d_crc = DeviceConstants::get(conf.device).d_crc;
@@ -90,20 +174,24 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     z_tc.ensure((size_t)nchunks * sizeof(TileCrc));
     z_crc.ensure((size_t)P * 4);
     TG_CUDA(cudaMemsetAsync(z_crc.p, 0, (size_t)P * 4, st));
-    k_zchunk_descs<SegDesc><<<(uint32_t)div_up((uint64_t)nchunks + 1, 256), 256, 0, st>>>(z_csize.as<uint32_t>(), nchunks, slot,
-                                                                                       z_descs.as<SegDesc>(), z_pstart.as<uint32_t>());
+    k_zchunk_descs<<<(uint32_t)div_up((uint64_t)nchunks + 1, 256), 256, 0, st>>>(z_csize.as<uint32_t>(), nchunks, L.slot,
+                                                                              z_descs.as<SegDesc>(), z_pstart.as<uint32_t>());
     k_crc_pieces<<<nchunks, CRCV_THREADS, 0, st>>>(z_slots.as<uint8_t>(), z_descs.as<SegDesc>(), z_pstart.as<uint32_t>(), nchunks, d_crc,
                                                    z_tc.as<TileCrc>());
-    k_zcrc_place<TileCrc><<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, z_segs.as<ZSeg>(), (uint32_t)P,
-                                                                         z_coff.as<uint64_t>(), tail);
+    k_zcrc_place<<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, z_segs.as<ZSeg>(), (uint32_t)P,
+                                                                z_coff.as<uint64_t>(), L.tail);
     k_crc_combine<<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, d_crc, z_crc.as<uint32_t>());
     k_zpack<<<nchunks, 256, 0, st>>>(z_slots.as<uint8_t>(), z_csize.as<uint32_t>(), z_coff.as<uint64_t>(), z_segs.as<ZSeg>(), (uint32_t)P,
-                                     slot, head, d_out);
-    if (blocks)   // TIF\x01 and the CRC: LZ4 and zstd segments frame their stream alike
-      k_l4finish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_crc.as<uint32_t>(), d_crc, d_out);
-    else
-      k_zfinish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_cadler.as<uint32_t>(), z_csize.as<uint32_t>(),
-                                                         z_crc.as<uint32_t>(), d_crc, d_out);
+                                     L.slot, L.head, d_out);
+    switch (codec) {
+      case TEZGPU_CODEC_LZ4:
+      case TEZGPU_CODEC_ZSTD:
+        k_zfinish_blocks<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_crc.as<uint32_t>(), d_crc, d_out);
+        break;
+      default:
+        k_zfinish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_cadler.as<uint32_t>(), z_csize.as<uint32_t>(),
+                                                           z_crc.as<uint32_t>(), d_crc, d_out);
+    }
     launches += 6;
     TG_CUDA(cudaGetLastError());
   }
@@ -124,6 +212,15 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     stats->file_out_bytes = (int64_t)total;
     stats->ms_total += z_timer.ms(0, 1);
     stats->kernel_launches += launches;
+  }
+}
+
+// the name of status rc of a codec's reader (0: "ok")
+static inline const char *codec_err_name(int32_t codec, int32_t rc) {
+  switch (codec) {
+    case TEZGPU_CODEC_LZ4: return l4_err_name(rc);
+    case TEZGPU_CODEC_ZSTD: return zs_err_name(rc);
+    default: return z_err_name(rc);
   }
 }
 
@@ -199,57 +296,44 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
   std::vector<uint32_t> piece_start;
   launches += check_checksums(z_in.as<uint8_t>(), sd, z_descs.as<SegDesc>(), [](const SegDesc &d) { return d.has_header == 1u; },
                               piece_start, false, z_flag.as<int>());
-  const bool lz4 = pipe.codec == TEZGPU_CODEC_LZ4, zstd = pipe.codec == TEZGPU_CODEC_ZSTD;
-  if (zstd) {
+  // LZ4 and zstd: the count walk, one host round trip for the unit counts, the base table, the fill walk, one warp per
+  // unit (`warps` per CTA), and the serial kernel, which decodes the segments the units did not take
+  using Walk = void (*)(const ZInSeg *, uint32_t, uint32_t *, const uint32_t *, ZUnit *);
+  using Units = void (*)(const ZUnit *, uint32_t, int32_t *);
+  using Serial = void (*)(const ZInSeg *, uint32_t, const uint32_t *, const int32_t *, int32_t *);
+  auto decode_units = [&](Walk count, Walk fill, Units units, Serial serial, uint32_t warps, const char *too_many) {
     z_nblk.ensure((size_t)nz * 4);
     z_slow.ensure((size_t)nz * 4);
     TG_CUDA(cudaMemsetAsync(z_slow.p, 0, (size_t)nz * 4, st));
-    k_zswalk<0><<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), nullptr, nullptr);
+    count<<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), nullptr, nullptr);
     launches++;
     TG_CUDA(cudaGetLastError());
-    std::vector<uint32_t> nfr(nz), base(nz);
-    TG_CUDA(cudaMemcpyAsync(nfr.data(), z_nblk.p, (size_t)nz * 4, cudaMemcpyDeviceToHost, st));
+    std::vector<uint32_t> nunit(nz), base(nz);
+    TG_CUDA(cudaMemcpyAsync(nunit.data(), z_nblk.p, (size_t)nz * 4, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaStreamSynchronize(st));
-    uint64_t nf = 0;
-    for (uint32_t i = 0; i < nz; i++) { base[i] = (uint32_t)nf; nf += nfr[i]; }
-    TG_CHECK(nf < (1ull << 32), TEZGPU_E_INVALID, "too many zstd frames in one merge");
-    if (nf) {
+    uint64_t nu = 0;
+    for (uint32_t i = 0; i < nz; i++) { base[i] = (uint32_t)nu; nu += nunit[i]; }
+    TG_CHECK(nu < (1ull << 32), TEZGPU_E_INVALID, too_many);
+    if (nu) {
       z_base.ensure((size_t)nz * 4);
-      z_blks.ensure((size_t)nf * sizeof(ZsFrm));
+      z_blks.ensure((size_t)nu * sizeof(ZUnit));
       TG_CUDA(cudaMemcpyAsync(z_base.p, base.data(), (size_t)nz * 4, cudaMemcpyHostToDevice, st));
-      k_zswalk<1><<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), z_base.as<uint32_t>(),
-                                                            z_blks.as<ZsFrm>());
-      k_zsframes<<<(uint32_t)div_up(nf, ZSD_WARPS), ZSD_WARPS * 32, 0, st>>>(z_blks.as<ZsFrm>(), (uint32_t)nf, z_slow.as<int32_t>());
+      fill<<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), z_base.as<uint32_t>(), z_blks.as<ZUnit>());
+      units<<<(uint32_t)div_up(nu, warps), warps * 32, 0, st>>>(z_blks.as<ZUnit>(), (uint32_t)nu, z_slow.as<int32_t>());
       launches += 2;
     }
-    k_zsserial<<<(uint32_t)div_up(nz, ZSD_WARPS), ZSD_WARPS * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(),
-                                                                          z_slow.as<int32_t>(), z_status.as<int32_t>());
-  } else if (lz4) {
-    z_nblk.ensure((size_t)nz * 4);
-    z_slow.ensure((size_t)nz * 4);
-    TG_CUDA(cudaMemsetAsync(z_slow.p, 0, (size_t)nz * 4, st));
-    k_l4walk<0><<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), nullptr, nullptr);
-    launches++;
-    TG_CUDA(cudaGetLastError());
-    std::vector<uint32_t> nblk(nz), base(nz);
-    TG_CUDA(cudaMemcpyAsync(nblk.data(), z_nblk.p, (size_t)nz * 4, cudaMemcpyDeviceToHost, st));
-    TG_CUDA(cudaStreamSynchronize(st));
-    uint64_t nb = 0;
-    for (uint32_t i = 0; i < nz; i++) { base[i] = (uint32_t)nb; nb += nblk[i]; }
-    TG_CHECK(nb < (1ull << 32), TEZGPU_E_INVALID, "too many LZ4 blocks in one merge");
-    if (nb) {
-      z_base.ensure((size_t)nz * 4);
-      z_blks.ensure((size_t)nb * sizeof(L4Blk));
-      TG_CUDA(cudaMemcpyAsync(z_base.p, base.data(), (size_t)nz * 4, cudaMemcpyHostToDevice, st));
-      k_l4walk<1><<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), z_base.as<uint32_t>(),
-                                                            z_blks.as<L4Blk>());
-      k_l4blocks<<<(uint32_t)div_up(nb, L4DEC_WARPS), L4DEC_WARPS * 32, 0, st>>>(z_blks.as<L4Blk>(), (uint32_t)nb, z_slow.as<int32_t>());
-      launches += 2;
-    }
-    k_l4serial<<<(uint32_t)div_up(nz, L4DEC_WARPS), L4DEC_WARPS * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(),
-                                                                              z_slow.as<int32_t>(), z_status.as<int32_t>());
-  } else {
-    k_zinflate<<<(uint32_t)div_up(nz, ZINF_WARPS), ZINF_WARPS * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_status.as<int32_t>());
+    serial<<<(uint32_t)div_up(nz, warps), warps * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), z_slow.as<int32_t>(),
+                                                               z_status.as<int32_t>());
+  };
+  switch (pipe.codec) {
+    case TEZGPU_CODEC_LZ4:
+      decode_units(k_l4walk<0>, k_l4walk<1>, k_l4blocks, k_l4serial, L4DEC_WARPS, "too many LZ4 blocks in one merge");
+      break;
+    case TEZGPU_CODEC_ZSTD:
+      decode_units(k_zswalk<0>, k_zswalk<1>, k_zsframes, k_zsserial, ZSD_WARPS, "too many zstd frames in one merge");
+      break;
+    default:
+      k_zinflate<<<(uint32_t)div_up(nz, ZINF_WARPS), ZINF_WARPS * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_status.as<int32_t>());
   }
   launches++;
   TG_CUDA(cudaGetLastError());
@@ -261,8 +345,7 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
   TG_CHECK(bad_crc == 0, TEZGPU_E_FORMAT, "IFile checksum mismatch in segment " + std::to_string(bad_crc ? zs[bad_crc - 1] : 0));
   for (uint32_t i = 0; i < nz; i++)
     TG_CHECK(status[i] == Z_OK, TEZGPU_E_FORMAT,
-             std::string("compressed segment ") + std::to_string(zs[i]) + ": " +
-                 (zstd ? zs_err_name(status[i]) : lz4 ? l4_err_name(status[i]) : z_err_name(status[i])));
+             std::string("compressed segment ") + std::to_string(zs[i]) + ": " + codec_err_name(pipe.codec, status[i]));
   std::vector<tezgpu_segment> segs2(in, in + nseg);
   for (uint32_t i = 0; i < nz; i++) {
     tezgpu_segment &sg = segs2[zs[i]];
@@ -289,6 +372,30 @@ static inline std::vector<uint8_t> z_deflate_host(const uint8_t *body, uint64_t 
   delete sh;
   for (int b = 3; b >= 0; b--) out.push_back((uint8_t)(adler >> (8 * b)));
   return out;
+}
+
+// host run of a block-framed device writer over one body: run(sh, piece, clen, slot) compresses each `block`-byte piece
+// into a slot of slot_bytes, which then holds head + sh.bytes bytes of the stream
+template <typename Shared>
+static inline std::vector<uint8_t> blocks_compress_host(const uint8_t *body, uint64_t len, uint32_t block, uint32_t slot_bytes,
+                                                       uint32_t head, void (*run)(Shared &, const uint8_t *, uint32_t, uint8_t *)) {
+  std::vector<uint8_t> out, slot(slot_bytes);
+  std::unique_ptr<Shared> sh(new Shared());
+  const uint64_t nb = div_up(len, block);
+  for (uint64_t k = 0; k < nb; k++) {
+    const uint32_t clen = (uint32_t)std::min<uint64_t>(block, len - k * block);
+    run(*sh, body + k * block, clen, slot.data());
+    out.insert(out.end(), slot.begin(), slot.begin() + head + sh->bytes);
+  }
+  return out;
+}
+// LZ4: the blocks, each its 8 header bytes and one chunk (tezgpu_debug_lz4_compress_emulate)
+static inline std::vector<uint8_t> l4_compress_host(const uint8_t *body, uint64_t len) {
+  return blocks_compress_host<L4Shared>(body, len, L4_BLOCK, L4_SLOT, 8, l4_compress_block_host);
+}
+// zstd: the frames (tezgpu_debug_zstd_compress_emulate)
+static inline std::vector<uint8_t> zs_compress_host(const uint8_t *body, uint64_t len) {
+  return blocks_compress_host<ZsShared>(body, len, ZS_BLOCK, ZS_SLOT, 0, zs_compress_block_host);
 }
 
 // worst case of the compressed file given the uncompressed file's bound.  zlib: every chunk stored.  LZ4: every block

@@ -137,4 +137,26 @@ __device__ __forceinline__ void st_volatile_u64(uint64_t *p, uint64_t v) {
   asm volatile("st.volatile.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
+// -------------------------------------------------------------------------------------------- compressed segments
+// The codec writers' segment table (codec.cuh): per output partition, where its uncompressed segment lies in the
+// emit's image and where its chunks are.  Every codec's chunk kernel finds its chunk's segment through it.
+struct ZSeg {
+  uint64_t body_off;   // image offset of the first body byte (after TIF\x00)
+  uint64_t body_len;   // body bytes (records + EOF marker)
+  uint32_t chunk0, nchunks;
+  uint64_t rank;       // segments before this partition
+  uint64_t zstart;     // out: file offset of the compressed segment
+  uint64_t zlen;       // out: its length (0: no segment)
+};
+
+// chunk c -> its partition: the last p with chunk0 <= c (partitions without a segment own no chunk)
+__device__ __forceinline__ uint32_t z_chunk_part(const ZSeg *__restrict__ segs, uint32_t P, uint32_t c) {
+  uint32_t lo = 0, hi = P;
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (segs[mid].chunk0 <= c) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 }  // namespace tezgpu

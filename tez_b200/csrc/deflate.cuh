@@ -460,26 +460,7 @@ static inline void z_deflate_chunk_host(ZShared &sh, const uint8_t *chunk, uint3
 }
 
 // ------------------------------------------------------------------------------------------------ device writer
-// per output partition: where its uncompressed segment lies in the emit's image and where its chunks are
-struct ZSeg {
-  uint64_t body_off;   // image offset of the first body byte (after TIF\x00)
-  uint64_t body_len;   // body bytes (records + EOF marker)
-  uint32_t chunk0, nchunks;
-  uint64_t rank;       // segments before this partition
-  uint64_t zstart;     // out: file offset of the compressed segment
-  uint64_t zlen;       // out: its length (0: no segment)
-};
-
-// chunk c -> its partition: the last p with chunk0 <= c (partitions without a segment own no chunk)
-__device__ __forceinline__ uint32_t z_chunk_part(const ZSeg *__restrict__ segs, uint32_t P, uint32_t c) {
-  uint32_t lo = 0, hi = P;
-  while (hi - lo > 1) {
-    const uint32_t mid = (lo + hi) >> 1;
-    if (segs[mid].chunk0 <= c) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
+// one CTA per chunk; segs / chunk numbering: ZSeg, z_chunk_part (common.cuh)
 __global__ void __launch_bounds__(ZLANES)
     k_zdeflate(const uint8_t *__restrict__ img, const ZSeg *__restrict__ segs, uint32_t P, uint8_t *__restrict__ slots,
                uint32_t *__restrict__ csize, uint32_t *__restrict__ cadler) {
@@ -516,57 +497,6 @@ __global__ void __launch_bounds__(ZLANES)
     z_lane<2>(sh, tid, w);
   }
   if (tid == 0) { csize[c] = sh.bytes; cadler[c] = sh.adler; }
-}
-
-// chunk descriptors for k_crc_pieces (one piece per chunk: a chunk is < CRC_PIECE bytes); slot: bytes per chunk slot
-template <typename SegDescT>
-__global__ void k_zchunk_descs(const uint32_t *__restrict__ csize, uint32_t nchunks, uint32_t slot, SegDescT *__restrict__ descs,
-                               uint32_t *__restrict__ piece_start) {
-  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c > nchunks) return;
-  piece_start[c] = c;
-  if (c == nchunks) return;
-  SegDescT d;
-  d.off = (uint64_t)c * slot;
-  d.len = csize[c] + 4;
-  d.body0 = 0;
-  d.body_end = csize[c];
-  d.has_header = 1;
-  d.partition = 0;
-  descs[c] = d;
-}
-
-// per partition: file offset and length of its compressed segment; frame: bytes of a segment outside its chunks
-__global__ void k_zseg_layout(ZSeg *__restrict__ segs, uint32_t P, const uint64_t *__restrict__ coff, uint32_t frame) {
-  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= P) return;
-  ZSeg &s = segs[p];
-  s.zstart = coff[s.chunk0] + frame * s.rank;
-  s.zlen = s.nchunks ? coff[s.chunk0 + s.nchunks] - coff[s.chunk0] + frame : 0;
-}
-
-// chunk checksums -> positions in their segment's checksummed bytes (zlib: header, chunks, Adler-32; LZ4: the chunks);
-// tail: checksummed bytes after the last chunk
-template <typename TileCrcT>
-__global__ void k_zcrc_place(TileCrcT *__restrict__ tc, uint32_t nchunks, const ZSeg *__restrict__ segs, uint32_t P,
-                             const uint64_t *__restrict__ coff, uint32_t tail) {
-  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= nchunks) return;
-  const uint32_t p = z_chunk_part(segs, P, c);
-  const ZSeg s = segs[p];
-  tc[c].p = p;
-  tc[c].after = coff[s.chunk0 + s.nchunks] - coff[c + 1] + tail;
-}
-
-// one CTA per chunk: the chunk's bytes into the file (slot: bytes per chunk slot; head: segment bytes before the chunks)
-__global__ void k_zpack(const uint8_t *__restrict__ slots, const uint32_t *__restrict__ csize, const uint64_t *__restrict__ coff,
-                        const ZSeg *__restrict__ segs, uint32_t P, uint32_t slot, uint32_t head, uint8_t *__restrict__ out) {
-  const uint32_t c = blockIdx.x;
-  const ZSeg s = segs[z_chunk_part(segs, P, c)];
-  uint8_t *dst = out + s.zstart + head + (coff[c] - coff[s.chunk0]);
-  const uint8_t *src = slots + (uint64_t)c * slot;
-  const uint32_t n = csize[c];
-  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
 }
 
 // per segment: TIF\x01, zlib header, Adler-32 (combined over the chunks), CRC-32 of the compressed bytes

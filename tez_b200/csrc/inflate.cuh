@@ -360,6 +360,26 @@ struct ZInSeg {
   uint64_t body;       // expected body bytes: rawLength - 4
 };
 
+// lane 0 of the warp that decoded segment z: the image frame around the body (TIF\x00, 4 zero bytes after it) and the
+// decode status
+__device__ __forceinline__ void z_image_frame(const ZInSeg &z, uint32_t lane, int32_t rc, int32_t *status) {
+  if (lane == 0) {
+    z.dst[0] = 'T'; z.dst[1] = 'I'; z.dst[2] = 'F'; z.dst[3] = 0;
+    for (int b = 0; b < 4; b++) z.dst[4 + z.body + b] = 0;
+    *status = rc;
+  }
+}
+
+// the unit of the LZ4 and zstd block-parallel readers (one LZ4 block assumed to be one chunk, or one zstd frame with
+// Frame_Content_Size): src[0..clen) decodes to exactly raw bytes at dst, or segment seg goes to the serial path
+struct ZUnit {
+  const uint8_t *src;
+  uint8_t *dst;
+  uint64_t clen, raw;
+  uint32_t seg;         // index into the ZInSeg array
+  uint32_t pad;
+};
+
 // one warp per segment (a Java-written segment is one serial zlib stream: parallelism comes from the segments); the
 // decode tables of the warp's segment are in shared memory
 constexpr int ZINF_WARPS = 4;
@@ -371,11 +391,7 @@ __global__ void __launch_bounds__(ZINF_WARPS * 32) k_zinflate(const ZInSeg *__re
   const ZInSeg z = segs[s];
   uint64_t got = 0;
   const int32_t rc = z_inflate(z.src + 4, z.len - 8, z.dst + 4, z.body, &got, s_work[wid], lane, 32);
-  if (lane == 0) {
-    z.dst[0] = 'T'; z.dst[1] = 'I'; z.dst[2] = 'F'; z.dst[3] = 0;
-    for (int b = 0; b < 4; b++) z.dst[4 + z.body + b] = 0;
-    status[s] = rc;
-  }
+  z_image_frame(z, lane, rc, status + s);
 }
 
 }  // namespace tezgpu

@@ -20,7 +20,6 @@
 // chunk follows LZ4_decompress_safe(src, dst, n, 262144) of liblz4, including its end-of-chunk conditions, except
 // that a match offset of 0 is refused (liblz4 1.9 accepts it on one code path, with undefined output bytes).
 #pragma once
-#include <vector>
 #include "inflate.cuh"
 
 namespace tezgpu {
@@ -225,7 +224,7 @@ static inline void l4_compress_block_host(L4Shared &sh, const uint8_t *block, ui
   l4_copy_runs(sh, slot + 8, 0, 1);
 }
 
-// one CTA per block; segs / chunk numbering as k_zdeflate (ZSeg, z_chunk_part), with L4_BLOCK-byte chunks
+// one CTA per block; segs / chunk numbering: ZSeg, z_chunk_part (common.cuh), with L4_BLOCK-byte chunks
 __global__ void __launch_bounds__(L4_LANES)
     k_l4compress(const uint8_t *__restrict__ img, const ZSeg *__restrict__ segs, uint32_t P, uint8_t *__restrict__ slots,
                  uint32_t *__restrict__ csize) {
@@ -249,20 +248,6 @@ __global__ void __launch_bounds__(L4_LANES)
   __syncthreads();
   l4_copy_runs(sh, slot + 8, tid, L4_LANES);
   if (tid == 0) csize[c] = 8 + sh.bytes;
-}
-
-// per segment: TIF\x01 and the CRC-32 of the stream (the blocks' raw remainders are in seg_crc)
-__global__ void k_l4finish(const ZSeg *__restrict__ segs, uint32_t P, const uint32_t *__restrict__ seg_crc,
-                           const CrcTables *__restrict__ t, uint8_t *__restrict__ out) {
-  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= P) return;
-  const ZSeg s = segs[p];
-  if (!s.nchunks) return;
-  uint8_t *o = out + s.zstart;
-  o[0] = 'T'; o[1] = 'I'; o[2] = 'F'; o[3] = 1;
-  const uint64_t region = s.zlen - 8;
-  const uint32_t crc = seg_crc[p] ^ crc_shift_bytes(t, 0xFFFFFFFFu, region) ^ 0xFFFFFFFFu;
-  l4_put_be32(o + s.zlen - 4, crc);
 }
 
 // ------------------------------------------------------------------------------------------------ reader
@@ -360,21 +345,12 @@ Z_HD int32_t l4_decompress(const uint8_t *in, uint64_t n, uint8_t *out, uint64_t
   return rc;
 }
 
-// the fast path's unit: one block assumed to be one chunk
-struct L4Blk {
-  const uint8_t *src;   // the chunk
-  uint8_t *dst;         // where its raw bytes go
-  uint32_t clen, raw;
-  uint32_t seg;         // index into the ZInSeg array
-  uint32_t pad;
-};
-
 // One thread per segment walks the block headers on the assumption of one chunk per block.  FILL 0: counts the
 // blocks into nblk[s] (0 = the assumption or the framing fails: the serial path decodes the segment); FILL 1: writes
-// the blocks from blk_base[s] on.
+// the blocks (ZUnit: the chunk and where its raw bytes go) from blk_base[s] on.
 template <int FILL>
 __global__ void k_l4walk(const ZInSeg *__restrict__ segs, uint32_t nseg, uint32_t *__restrict__ nblk, const uint32_t *__restrict__ blk_base,
-                         L4Blk *__restrict__ blks) {
+                         ZUnit *__restrict__ blks) {
   const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= nseg) return;
   const ZInSeg z = segs[s];
@@ -390,7 +366,7 @@ __global__ void k_l4walk(const ZInSeg *__restrict__ segs, uint32_t nseg, uint32_
     ip += 8;
     if (raw == 0 || raw > L4_CHUNK_CAP || raw > z.body - op || c > L4_CHUNK_CAP || c > n - ip) { ok = false; break; }
     if (FILL) {
-      L4Blk b;
+      ZUnit b;
       b.src = in + ip; b.dst = z.dst + 4 + op; b.clen = c; b.raw = raw; b.seg = s; b.pad = 0;
       blks[blk_base[s] + k] = b;
     }
@@ -404,13 +380,13 @@ __global__ void k_l4walk(const ZInSeg *__restrict__ segs, uint32_t nseg, uint32_
 // one warp per block: a block that does not decode to exactly its raw length from exactly its chunk sends its segment
 // to the serial path (slow[seg] = 1)
 constexpr int L4DEC_WARPS = 4;
-__global__ void __launch_bounds__(L4DEC_WARPS * 32) k_l4blocks(const L4Blk *__restrict__ blks, uint32_t n, int32_t *__restrict__ slow) {
+__global__ void __launch_bounds__(L4DEC_WARPS * 32) k_l4blocks(const ZUnit *__restrict__ blks, uint32_t n, int32_t *__restrict__ slow) {
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t b = blockIdx.x * L4DEC_WARPS + (threadIdx.x >> 5);
   if (b >= n) return;
-  const L4Blk k = blks[b];
-  uint32_t got = 0;
-  const int32_t rc = l4_decode_chunk(k.src, k.clen, k.dst, k.raw, &got, lane, 32);
+  const ZUnit k = blks[b];
+  uint32_t got = 0;   // the walk put clen and raw within L4_CHUNK_CAP
+  const int32_t rc = l4_decode_chunk(k.src, (uint32_t)k.clen, k.dst, (uint32_t)k.raw, &got, lane, 32);
   if (lane == 0 && (rc != L4_OK || got != k.raw)) slow[k.seg] = 1;
 }
 
@@ -427,26 +403,7 @@ __global__ void __launch_bounds__(L4DEC_WARPS * 32) k_l4serial(const ZInSeg *__r
     uint64_t got = 0;
     rc = l4_decompress(z.src + 4, z.len - 8, z.dst + 4, z.body, &got, lane, 32);
   }
-  if (lane == 0) {
-    z.dst[0] = 'T'; z.dst[1] = 'I'; z.dst[2] = 'F'; z.dst[3] = 0;
-    for (int b = 0; b < 4; b++) z.dst[4 + z.body + b] = 0;
-    status[s] = rc;
-  }
-}
-
-// host run of the device writer over one body: the blocks (tezgpu_debug_lz4_compress_emulate)
-static inline std::vector<uint8_t> l4_compress_host(const uint8_t *body, uint64_t len) {
-  std::vector<uint8_t> out;
-  L4Shared *sh = new L4Shared();
-  std::vector<uint8_t> slot(L4_SLOT);
-  const uint64_t nb = div_up(len, L4_BLOCK);
-  for (uint64_t k = 0; k < nb; k++) {
-    const uint32_t clen = (uint32_t)std::min<uint64_t>(L4_BLOCK, len - k * L4_BLOCK);
-    l4_compress_block_host(*sh, body + k * L4_BLOCK, clen, slot.data());
-    out.insert(out.end(), slot.begin(), slot.begin() + 8 + sh->bytes);
-  }
-  delete sh;
-  return out;
+  z_image_frame(z, lane, rc, status + s);
 }
 
 }  // namespace tezgpu

@@ -10,7 +10,6 @@
 #include "../../include/tezgpu.h"
 #include "device_util.h"
 #include "combine.cuh"
-#include "deflate.cuh"
 #include "emit_pipe_u.cuh"
 #include "sorter_kernels.cuh"
 

@@ -116,6 +116,33 @@ __global__ void k_rebase_offsets(const uint32_t *__restrict__ key_off, const uin
   vlen[i] = vl;
 }
 
+// the body of the tezgpu_debug_*_compress_emulate entry points: host_run is the codec's host run of the device writer
+static int32_t compress_emulate(std::vector<uint8_t> (*host_run)(const uint8_t *, uint64_t), const uint8_t *body, uint64_t len,
+                                uint8_t *out, uint64_t cap, uint64_t *out_len) {
+  TG_API_BEGIN
+  TG_CHECK((body || len == 0) && out && out_len, TEZGPU_E_INVALID, "null argument");
+  const std::vector<uint8_t> z = host_run(body, len);
+  *out_len = z.size();
+  TG_CHECK(z.size() <= cap, TEZGPU_E_NOMEM, "output buffer too small");
+  memcpy(out, z.data(), z.size());
+  TG_API_END
+}
+
+// the body of the tezgpu_debug_*_decompress_emulate entry points: decode(&got) runs the codec's host decoder and returns
+// its status
+template <typename Decode>
+static int32_t decompress_emulate(int32_t codec, const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
+                                  uint64_t *out_len, Decode decode) {
+  TG_API_BEGIN
+  TG_CHECK((z || len == 0) && (out || body_len == 0) && out_len, TEZGPU_E_INVALID, "null argument");
+  TG_CHECK(body_len <= cap, TEZGPU_E_INVALID, "output buffer smaller than body_len");
+  uint64_t got = 0;
+  const int32_t rc = decode(&got);
+  *out_len = got;
+  TG_CHECK(rc == 0, TEZGPU_E_FORMAT, std::string("compressed segment 0: ") + codec_err_name(codec, rc));
+  TG_API_END
+}
+
 extern "C" {
 
 const char *tezgpu_last_error(void) { return g_last_error.c_str(); }
@@ -362,72 +389,37 @@ int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec) {
 }
 
 int32_t tezgpu_debug_deflate_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len) {
-  TG_API_BEGIN
-  TG_CHECK((body || len == 0) && out && out_len, TEZGPU_E_INVALID, "null argument");
-  const std::vector<uint8_t> z = z_deflate_host(body, len);
-  *out_len = z.size();
-  TG_CHECK(z.size() <= cap, TEZGPU_E_NOMEM, "output buffer too small");
-  memcpy(out, z.data(), z.size());
-  TG_API_END
+  return compress_emulate(z_deflate_host, body, len, out, cap, out_len);
 }
 
 int32_t tezgpu_debug_inflate_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
                                      uint64_t *out_len) {
-  TG_API_BEGIN
-  TG_CHECK((z || len == 0) && (out || body_len == 0) && out_len, TEZGPU_E_INVALID, "null argument");
-  TG_CHECK(body_len <= cap, TEZGPU_E_INVALID, "output buffer smaller than body_len");
-  ZInflateWork *w = new ZInflateWork();
-  uint64_t got = 0;
-  const int32_t rc = z_inflate(z, len, out, body_len, &got, *w);
-  delete w;
-  *out_len = got;
-  TG_CHECK(rc == Z_OK, TEZGPU_E_FORMAT, std::string("compressed segment 0: ") + z_err_name(rc));
-  TG_API_END
+  return decompress_emulate(TEZGPU_CODEC_DEFAULT, z, len, body_len, out, cap, out_len, [&](uint64_t *got) {
+    std::unique_ptr<ZInflateWork> w(new ZInflateWork());
+    return z_inflate(z, len, out, body_len, got, *w);
+  });
 }
 
 int32_t tezgpu_debug_lz4_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len) {
-  TG_API_BEGIN
-  TG_CHECK((body || len == 0) && out && out_len, TEZGPU_E_INVALID, "null argument");
-  const std::vector<uint8_t> z = l4_compress_host(body, len);
-  *out_len = z.size();
-  TG_CHECK(z.size() <= cap, TEZGPU_E_NOMEM, "output buffer too small");
-  memcpy(out, z.data(), z.size());
-  TG_API_END
+  return compress_emulate(l4_compress_host, body, len, out, cap, out_len);
 }
 
 int32_t tezgpu_debug_lz4_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
                                             uint64_t *out_len) {
-  TG_API_BEGIN
-  TG_CHECK((z || len == 0) && (out || body_len == 0) && out_len, TEZGPU_E_INVALID, "null argument");
-  TG_CHECK(body_len <= cap, TEZGPU_E_INVALID, "output buffer smaller than body_len");
-  uint64_t got = 0;
-  const int32_t rc = l4_decompress(z, len, out, body_len, &got);
-  *out_len = got;
-  TG_CHECK(rc == L4_OK, TEZGPU_E_FORMAT, std::string("compressed segment 0: ") + l4_err_name(rc));
-  TG_API_END
+  return decompress_emulate(TEZGPU_CODEC_LZ4, z, len, body_len, out, cap, out_len,
+                            [&](uint64_t *got) { return l4_decompress(z, len, out, body_len, got); });
 }
 
 int32_t tezgpu_debug_zstd_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len) {
-  TG_API_BEGIN
-  TG_CHECK((body || len == 0) && out && out_len, TEZGPU_E_INVALID, "null argument");
-  const std::vector<uint8_t> z = zs_compress_host(body, len);
-  *out_len = z.size();
-  TG_CHECK(z.size() <= cap, TEZGPU_E_NOMEM, "output buffer too small");
-  memcpy(out, z.data(), z.size());
-  TG_API_END
+  return compress_emulate(zs_compress_host, body, len, out, cap, out_len);
 }
 
 int32_t tezgpu_debug_zstd_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
                                              uint64_t *out_len) {
-  TG_API_BEGIN
-  TG_CHECK((z || len == 0) && (out || body_len == 0) && out_len, TEZGPU_E_INVALID, "null argument");
-  TG_CHECK(body_len <= cap, TEZGPU_E_INVALID, "output buffer smaller than body_len");
-  uint64_t got = 0;
-  std::unique_ptr<ZsDec> d(new ZsDec());
-  const int32_t rc = zs_decompress(z, len, out, body_len, &got, *d);
-  *out_len = got;
-  TG_CHECK(rc == ZS_OK, TEZGPU_E_FORMAT, std::string("compressed segment 0: ") + zs_err_name(rc));
-  TG_API_END
+  return decompress_emulate(TEZGPU_CODEC_ZSTD, z, len, body_len, out, cap, out_len, [&](uint64_t *got) {
+    std::unique_ptr<ZsDec> d(new ZsDec());
+    return zs_decompress(z, len, out, body_len, got, *d);
+  });
 }
 
 int32_t tezgpu_debug_crc_concat_emulate(const uint8_t *const *bodies, const uint64_t *lens, uint32_t n, uint32_t *crc) {

@@ -21,7 +21,6 @@
 // are placed at the end of the block's output range and consumed from there (a literal is never needed after the
 // output reaches its position), so no scratch buffer is needed; matches read earlier output of the frame in place.
 #pragma once
-#include <vector>
 #include "lz4.cuh"
 
 namespace tezgpu {
@@ -714,21 +713,13 @@ Z_HD int32_t zs_decompress(const uint8_t *in, uint64_t n, uint8_t *out, uint64_t
   return rc;
 }
 
-// the frame-parallel path's unit: one frame with Frame_Content_Size
-struct ZsFrm {
-  const uint8_t *src;   // the frame
-  uint8_t *dst;         // where its content goes
-  uint64_t clen, fcs;
-  uint32_t seg;         // index into the ZInSeg array
-  uint32_t pad;
-};
-
 // One thread per segment walks the frame and block headers.  FILL 0: counts the frames into nfr[s] (0 = a frame
-// without Frame_Content_Size, or a framing error: the serial path decodes the segment); FILL 1: writes the frames from
-// fr_base[s] on.  Skippable frames are passed over.
+// without Frame_Content_Size, or a framing error: the serial path decodes the segment); FILL 1: writes the frames
+// (ZUnit: the frame, where its content goes, its Frame_Content_Size as raw) from fr_base[s] on.  Skippable frames are
+// passed over.
 template <int FILL>
 __global__ void k_zswalk(const ZInSeg *__restrict__ segs, uint32_t nseg, uint32_t *__restrict__ nfr, const uint32_t *__restrict__ fr_base,
-                         ZsFrm *__restrict__ frs) {
+                         ZUnit *__restrict__ frs) {
   const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= nseg) return;
   const ZInSeg z = segs[s];
@@ -756,8 +747,8 @@ __global__ void k_zswalk(const ZInSeg *__restrict__ segs, uint32_t nseg, uint32_
     q += h.cksum ? 4 : 0;
     if (q > n) { ok = false; break; }
     if (FILL) {
-      ZsFrm f;
-      f.src = in + ip; f.dst = z.dst + 4 + op; f.clen = q - ip; f.fcs = h.fcs; f.seg = s; f.pad = 0;
+      ZUnit f;
+      f.src = in + ip; f.dst = z.dst + 4 + op; f.clen = q - ip; f.raw = h.fcs; f.seg = s; f.pad = 0;
       frs[fr_base[s] + k] = f;
     }
     k++;
@@ -770,15 +761,15 @@ __global__ void k_zswalk(const ZInSeg *__restrict__ segs, uint32_t nseg, uint32_
 // one warp per frame: a frame that does not decode to exactly its content size from exactly its bytes sends its
 // segment to the serial path (slow[seg] = 1)
 constexpr int ZSD_WARPS = 2;
-__global__ void __launch_bounds__(ZSD_WARPS * 32) k_zsframes(const ZsFrm *__restrict__ frs, uint32_t n, int32_t *__restrict__ slow) {
+__global__ void __launch_bounds__(ZSD_WARPS * 32) k_zsframes(const ZUnit *__restrict__ frs, uint32_t n, int32_t *__restrict__ slow) {
   __shared__ ZsDec s_dec[ZSD_WARPS];
   const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const uint32_t f = blockIdx.x * ZSD_WARPS + wid;
   if (f >= n) return;
-  const ZsFrm fr = frs[f];
+  const ZUnit fr = frs[f];
   uint64_t used = 0, got = 0;
-  const int32_t rc = zs_frame(fr.src, fr.clen, &used, fr.dst, 0, fr.fcs, &got, s_dec[wid], lane, 32);
-  if (lane == 0 && (rc != ZS_OK || used != fr.clen || got != fr.fcs)) slow[fr.seg] = 1;
+  const int32_t rc = zs_frame(fr.src, fr.clen, &used, fr.dst, 0, fr.raw, &got, s_dec[wid], lane, 32);
+  if (lane == 0 && (rc != ZS_OK || used != fr.clen || got != fr.raw)) slow[fr.seg] = 1;
 }
 
 // one warp per segment: the image frame (TIF\x00, 4 zero bytes after the body); segments marked slow (or never walked)
@@ -795,11 +786,7 @@ __global__ void __launch_bounds__(ZSD_WARPS * 32) k_zsserial(const ZInSeg *__res
     uint64_t got = 0;
     rc = zs_decompress(z.src + 4, z.len - 8, z.dst + 4, z.body, &got, s_dec[wid], lane, 32);
   }
-  if (lane == 0) {
-    z.dst[0] = 'T'; z.dst[1] = 'I'; z.dst[2] = 'F'; z.dst[3] = 0;
-    for (int b = 0; b < 4; b++) z.dst[4 + z.body + b] = 0;
-    status[s] = rc;
-  }
+  z_image_frame(z, lane, rc, status + s);
 }
 
 // ------------------------------------------------------------------------------------------------ writer
@@ -1198,7 +1185,7 @@ static inline void zs_compress_block_host(ZsShared &sh, const uint8_t *block, ui
   if (!sh.huf) memcpy(slot + zs_fh_bytes(clen) + 3, block, clen);
 }
 
-// one CTA per piece; segs / chunk numbering as k_zdeflate (ZSeg, z_chunk_part), with ZS_BLOCK-byte chunks
+// one CTA per piece; segs / chunk numbering: ZSeg, z_chunk_part (common.cuh), with ZS_BLOCK-byte chunks
 __global__ void __launch_bounds__(ZS_LANES)
     k_zscompress(const uint8_t *__restrict__ img, const ZSeg *__restrict__ segs, uint32_t P, uint8_t *__restrict__ slots,
                  uint32_t *__restrict__ csize) {
@@ -1234,21 +1221,6 @@ __global__ void __launch_bounds__(ZS_LANES)
   if (!sh.huf)
     for (uint32_t i = tid; i < clen; i += ZS_LANES) out[i] = src[i];
   if (tid == 0) csize[c] = sh.bytes;
-}
-
-// host run of the device writer over one body: its frames (tezgpu_debug_zstd_compress_emulate)
-static inline std::vector<uint8_t> zs_compress_host(const uint8_t *body, uint64_t len) {
-  std::vector<uint8_t> out;
-  ZsShared *sh = new ZsShared();
-  std::vector<uint8_t> slot(ZS_SLOT);
-  const uint64_t nb = div_up(len, ZS_BLOCK);
-  for (uint64_t k = 0; k < nb; k++) {
-    const uint32_t clen = (uint32_t)std::min<uint64_t>(ZS_BLOCK, len - k * ZS_BLOCK);
-    zs_compress_block_host(*sh, body + k * ZS_BLOCK, clen, slot.data());
-    out.insert(out.end(), slot.begin(), slot.begin() + sh->bytes);
-  }
-  delete sh;
-  return out;
 }
 
 }  // namespace tezgpu
