@@ -177,6 +177,8 @@ int32_t tezgpu_sorter_reset(tezgpu_sorter *h);
 /* Device-resident variant (records already in HBM; used by the multi-GPU shuffle and by bench.py's kernel-only
  * measurement).  d_kv: n packed fixed-width records on conf.device; d_partition may be 0.  d_out receives file.out
  * bytes (capacity out_cap); index (host, 3*P int64) and stats are filled after an internal stream sync.
+ * Without a codec d_out must be 16-byte aligned (the emit stores 16-byte words); a misaligned d_out returns
+ * TEZGPU_E_INVALID and writes nothing.
  * Runs on the handle's stream (tezgpu_sorter_stream). */
 int32_t tezgpu_sorter_sort_device_fixed(tezgpu_sorter *h, const void *d_kv, const void *d_partition, uint64_t n,
                                         void *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index,
@@ -284,11 +286,14 @@ int32_t tezgpu_merge_next_batch(tezgpu_merger *m, uint8_t *out_kv, uint64_t cap,
 int32_t tezgpu_merge_write_ifile(tezgpu_merger *m, const char *path, uint8_t *out, uint64_t out_cap, int32_t rle,
                                  int64_t *raw_len, int64_t *part_len, tezgpu_stats *stats);
 uint64_t tezgpu_merge_output_bound(const tezgpu_merger *m);
-/* device-resident output of the merged IFile segment (multi-GPU reduce side, bench) */
+/* device-resident output of the merged IFile segment (multi-GPU reduce side, bench).  Unless the merger was opened
+ * with a codec or as a concatenation, d_out must be 16-byte aligned (the emit stores 16-byte words); a misaligned
+ * d_out returns TEZGPU_E_INVALID before anything is launched or written, and the handle can write again. */
 int32_t tezgpu_merge_write_ifile_device(tezgpu_merger *m, void *d_out, uint64_t out_cap, int32_t rle, int64_t *raw_len,
                                         int64_t *part_len, tezgpu_stats *stats);
 /* Batched reduce side (multi-GPU shuffle): the merger was opened with conf.num_partitions = P and every segment
- * names its partition; writes the P merged segments back to back like a file.out and fills index[3*P]. */
+ * names its partition; writes the P merged segments back to back like a file.out and fills index[3*P].  d_out: as
+ * for tezgpu_merge_write_ifile_device, 16-byte aligned unless the merger has a codec or is a concatenation. */
 int32_t tezgpu_merge_write_partitions_device(tezgpu_merger *m, void *d_out, uint64_t out_cap, int32_t rle,
                                              uint64_t *out_len, int64_t *index, tezgpu_stats *stats);
 /* same, written to file.out + file.out.index (mode 0640): the final merge of PipelinedSorter.flush over several spills

@@ -810,6 +810,8 @@ class SortPipeline {
   // the uncombined stream, ms_emit the emit alone) except output_records = records that entered the combine and
   // spilled_records = records written.  The sort's state is restored afterwards, so a merger can write again.
   void emit_combined(int rle, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index, tezgpu_stats *stats) {
+    // emit_phase's precondition, checked before the combine launches anything
+    TG_CHECK(((uintptr_t)d_out & 15u) == 0, TEZGPU_E_INVALID, "output buffer must be 16-byte aligned");
     const SortState saved = state;
     c_timer.reset();
     c_timer.mark(stream);
