@@ -45,6 +45,8 @@ extern "C" {
 /* partitioner (RL/partitioner/HashPartitioner.java:33-35) */
 #define TEZGPU_PART_GIVEN 0         /* caller computed Partitioner.getPartition in Java and passes the ids */
 #define TEZGPU_PART_HASH 1          /* device computes (key.hashCode() & MAX_VALUE) % P for the comparator's key class */
+#define TEZGPU_PART_TOTAL_ORDER 2   /* Hadoop TotalOrderPartitioner: the device computes the number of split points <= key
+                                       (tezgpu_sorter_set_split_points) */
 
 /* RLE policy of IFile.Writer (SORT/IFile.java:541-544; decision SORT/PipelinedSorter.java:1436-1438) */
 #define TEZGPU_RLE_AUTO (-1)        /* on iff (#adjacent equal keys in sorted order) > 0.1 * records -- see DESIGN.md "RLE decision" */
@@ -198,6 +200,21 @@ int32_t tezgpu_sorter_set_combiner(tezgpu_sorter *h, int32_t combiner);
  * output_bytes_with_overhead is still the sum of rawLength, and ms_total includes the compression (ms_emit does not).
  * TEZGPU_E_UNSUPPORTED for any other codec. */
 int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec);
+
+/* TotalOrderPartitioner (org.apache.hadoop.mapreduce.lib.partition / org.apache.hadoop.mapred.lib): the split points of a
+ * TEZGPU_PART_TOTAL_ORDER handle.  Split i is keys[key_off[i] .. + key_len[i]), serialized like the handle's record keys
+ * (Text: vint length + bytes; BytesWritable: 4-byte length + bytes; Int / Long: 4 / 8 bytes big-endian).  The partition
+ * of a key is the number of split points <= key in the search order `order` (a TEZGPU_CMP_*): TEXT or BYTESWRITABLE for
+ * mapreduce.totalorderpartitioner.naturalorder = true on Text / BytesWritable keys (unsigned bytes of the content, even
+ * when the sort comparator is BYTES), else the handle's comparator; any other pairing fails with TEZGPU_E_INVALID.  So a
+ * key equal to split i goes to partition i + 1.  Fails with TEZGPU_E_INVALID unless n == num_partitions - 1 ("Wrong number of partitions in keyset") and the splits are
+ * strictly increasing under the handle's comparator ("Split points are out of order"), or on a handle that is not
+ * TOTAL_ORDER; with TEZGPU_E_STATE unless called before the first collect (or right after a reset).  Survives reset.
+ * On a TOTAL_ORDER handle with num_partitions > 1, collecting or flushing before the split points are set fails with
+ * TEZGPU_E_STATE; a partition array passed to collect_batch, collect_fixed or sort_device_fixed fails with
+ * TEZGPU_E_INVALID.  With num_partitions = 1 no split points are needed. */
+int32_t tezgpu_sorter_set_split_points(tezgpu_sorter *h, const uint8_t *keys, const uint64_t *key_off, const uint32_t *key_len,
+                                       uint32_t n, int32_t order);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Merger: replaces TezMerger.merge(...) -> TezRawKeyValueIterator (SORT/TezMerger.java:717-912,
@@ -411,6 +428,13 @@ int32_t tezgpu_debug_zstd_decompress_emulate(const uint8_t *z, uint64_t len, uin
 int32_t tezgpu_debug_sort_words_emulate(const uint8_t *kv, const uint64_t *key_off, const uint32_t *key_len, uint32_t n,
                                         int32_t comparator, int32_t num_partitions, const int32_t *partition,
                                         int32_t use_sym, uint32_t *words, uint32_t *npos, int32_t *sym_used);
+
+/* diagnostics: tezgpu_sorter_set_split_points' checks and the device's split search, on the host with the same code.
+ * Key i = kv[key_off[i] .. + key_len[i]), split j = splits[split_off[j] .. + split_len[j]]; comparator is the sort
+ * comparator the checks use, order the search order.  partition[i] receives key i's partition (P = nsplits + 1). */
+int32_t tezgpu_debug_total_order_emulate(const uint8_t *kv, const uint64_t *key_off, const uint32_t *key_len, uint32_t n,
+                                         const uint8_t *splits, const uint64_t *split_off, const uint32_t *split_len,
+                                         uint32_t nsplits, int32_t comparator, int32_t order, int32_t *partition);
 
 #ifdef __cplusplus
 }

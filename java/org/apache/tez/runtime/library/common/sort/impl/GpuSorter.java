@@ -16,16 +16,24 @@ import java.nio.ByteOrder;
 import java.nio.IntBuffer;
 
 import org.apache.hadoop.conf.Configuration;
+import org.apache.hadoop.fs.Path;
 import org.apache.hadoop.io.BytesWritable;
 import org.apache.hadoop.io.IntWritable;
 import org.apache.hadoop.io.LongWritable;
 import org.apache.hadoop.io.RawComparator;
+import org.apache.hadoop.io.SequenceFile;
 import org.apache.hadoop.io.Text;
 import org.apache.hadoop.io.compress.CompressionCodec;
 import org.apache.hadoop.io.compress.DefaultCodec;
 import org.apache.hadoop.io.compress.Lz4Codec;
 import org.apache.hadoop.io.compress.ZStandardCodec;
+import org.apache.hadoop.io.serializer.SerializationFactory;
+import org.apache.hadoop.io.serializer.Serializer;
+import org.apache.hadoop.mapreduce.lib.partition.TotalOrderPartitioner;
+import org.apache.hadoop.util.ReflectionUtils;
 import org.apache.tez.runtime.api.OutputContext;
+import org.apache.tez.runtime.library.api.TezRuntimeConfiguration;
+import org.apache.tez.runtime.library.common.ConfigUtils;
 import org.apache.tez.runtime.library.common.comparator.TezBytesComparator;
 import org.apache.tez.runtime.library.partitioner.HashPartitioner;
 
@@ -37,7 +45,10 @@ public class GpuSorter extends ExternalSorter {
 
   // ids of include/tezgpu.h
   static final int CMP_BYTES = 0, CMP_TEXT = 1, CMP_BYTESWRITABLE = 2, CMP_INT = 3, CMP_LONG = 4;
-  static final int PART_GIVEN = 0, PART_HASH = 1;
+  static final int PART_GIVEN = 0, PART_HASH = 1, PART_TOTAL_ORDER = 2;
+  static final String TOTAL_ORDER_NEW = "org.apache.hadoop.mapreduce.lib.partition.TotalOrderPartitioner";
+  static final String TOTAL_ORDER_OLD = "org.apache.hadoop.mapred.lib.TotalOrderPartitioner";
+  static final String MR_PARTITIONER = "org.apache.tez.mapreduce.partition.MRPartitioner";
   static final int COMBINE_NONE = 0, COMBINE_SUM_INT = 1, COMBINE_SUM_LONG = 2;
   static final int CODEC_NONE = 0, CODEC_DEFAULT = 1, CODEC_LZ4 = 2, CODEC_ZSTD = 3;
   static final int SORTER_UNORDERED = 2;
@@ -48,7 +59,7 @@ public class GpuSorter extends ExternalSorter {
   private final ByteBuffer kv = ByteBuffer.allocateDirect(BATCH_BYTES).order(ByteOrder.nativeOrder());
   private final IntBuffer keyOff = direct(BATCH_RECORDS), valOff = direct(BATCH_RECORDS), valLen = direct(BATCH_RECORDS),
       part = direct(BATCH_RECORDS);
-  private final boolean deviceHash;
+  private final boolean devicePartitioner; // HashPartitioner or TotalOrderPartitioner: write() passes no partition
   private final ByteBufferOutputStream sink = new ByteBufferOutputStream(kv);
   private int n;
   private long collectedBytes;
@@ -72,10 +83,15 @@ public class GpuSorter extends ExternalSorter {
       boolean unordered) throws IOException {
     super(outputContext, conf, numOutputs, initialMemoryAvailable);
     this.unordered = unordered;
-    deviceHash = partitioner instanceof HashPartitioner;
-    handle = nativeCreate(numOutputs, unordered ? CMP_BYTES : comparatorId(comparator, conf), deviceHash ? PART_HASH : PART_GIVEN,
+    final boolean deviceHash = partitioner instanceof HashPartitioner;
+    final boolean totalOrder = totalOrderPartitioner(conf, numOutputs, unordered);
+    devicePartitioner = deviceHash || totalOrder;
+    // an unordered edge compares no keys; with TotalOrderPartitioner the split points are still checked in key order
+    final int cmp = unordered && !totalOrder ? CMP_BYTES : comparatorId(comparator, conf);
+    handle = nativeCreate(numOutputs, cmp, totalOrder ? PART_TOTAL_ORDER : deviceHash ? PART_HASH : PART_GIVEN,
         sendEmptyPartitionDetails, initialMemoryAvailable, /* CUDA ordinal, from the container's environment */
         Integer.parseInt(System.getenv().getOrDefault("TEZGPU_DEVICE", "0")), unordered ? SORTER_UNORDERED : 0);
+    if (totalOrder) setSplitPoints(conf, cmp);
     keySerializer.open(sink);
     valSerializer.open(sink);
     // ExternalSorter.codec = CodecUtils.getCodec(conf): every spill and the final merge write through it
@@ -109,6 +125,65 @@ public class GpuSorter extends ExternalSorter {
     nativeSetCombiner(handle, combiner);
   }
 
+  /**
+   * TotalOrderPartitioner (new or old API) is the output's partitioner: named as tez.runtime.partitioner.class, or
+   * wrapped by MRPartitioner with more than one partition as mapreduce.job.partitioner.class (new API) /
+   * mapred.partitioner.class (old API), as MRPartitioner picks it.  An unordered writer with one partition
+   * (UnorderedKVOutput) runs no partitioner.  The plugin mirror decides the same way (tez_runtime_library.cc
+   * total_order_partitioner).
+   */
+  static boolean totalOrderPartitioner(Configuration conf, int partitions, boolean unordered) {
+    final String pc = conf.get(TezRuntimeConfiguration.TEZ_RUNTIME_PARTITIONER_CLASS, "");
+    if (TOTAL_ORDER_NEW.equals(pc) || TOTAL_ORDER_OLD.equals(pc)) return !(unordered && partitions == 1);
+    if (!MR_PARTITIONER.equals(pc) || partitions <= 1) return false;
+    final String wrapped = conf.getBoolean("mapred.mapper.new-api", false) ? conf.get("mapreduce.job.partitioner.class", "")
+        : conf.get("mapred.partitioner.class", "");
+    return TOTAL_ORDER_NEW.equals(wrapped) || TOTAL_ORDER_OLD.equals(wrapped);
+  }
+
+  /**
+   * TotalOrderPartitioner.setConf on the device: the split keys of TotalOrderPartitioner.getPartitionFile(conf)
+   * (mapreduce.totalorderpartitioner.path, default _partition.lst; both APIs read the same key), read with
+   * SequenceFile.Reader, serialized with the job's key serialization (what keySerializer writes for record keys) into
+   * one direct buffer, and handed to tezgpu_sorter_set_split_points, which checks their count and order with Hadoop's
+   * messages.  Search order: the content order of Text / BytesWritable keys with
+   * mapreduce.totalorderpartitioner.naturalorder (default true), else the comparator's.
+   */
+  private void setSplitPoints(Configuration conf, int cmp) throws IOException {
+    final Class<?> keyClass = ConfigUtils.getIntermediateOutputKeyClass(conf);
+    final Path file = new Path(TotalOrderPartitioner.getPartitionFile(conf));
+    final java.io.ByteArrayOutputStream bytes = new java.io.ByteArrayOutputStream();
+    final java.util.ArrayList<Integer> lens = new java.util.ArrayList<>();
+    @SuppressWarnings("unchecked")
+    final Serializer<Object> ser = (Serializer<Object>) new SerializationFactory(conf).getSerializer(keyClass);
+    ser.open(bytes);
+    try (SequenceFile.Reader reader = new SequenceFile.Reader(conf, SequenceFile.Reader.file(file))) {
+      Object key = ReflectionUtils.newInstance(keyClass, conf);
+      while ((key = reader.next(key)) != null) {   // "wrong key class" comes from the reader, as in Hadoop
+        final int before = bytes.size();
+        ser.serialize(key);
+        lens.add(bytes.size() - before);
+      }
+    } finally {
+      ser.close();
+    }
+    final int n = lens.size();
+    final ByteBuffer keys = ByteBuffer.allocateDirect(Math.max(1, bytes.size()));
+    keys.put(bytes.toByteArray());
+    final long[] off = new long[n];
+    final int[] len = new int[n];
+    for (int i = 0, at = 0; i < n; i++) {
+      off[i] = at;
+      len[i] = lens.get(i);
+      at += len[i];
+    }
+    final boolean natural = conf.getBoolean(TotalOrderPartitioner.NATURAL_ORDER, true);
+    final int order = natural && keyClass == Text.class ? CMP_TEXT
+        : natural && keyClass == BytesWritable.class ? CMP_BYTESWRITABLE : cmp;
+    // mapreduce.totalorderpartitioner.trie.maxdepth only shapes Java's index over the split points: nothing to pass
+    nativeSetSplitPoints(handle, keys, off, len, n, order);
+  }
+
   /** The device path supports a closed set of RawComparators; anything else keeps tez.runtime.sorter.class=PIPELINED. */
   static int comparatorId(RawComparator<?> c, Configuration conf) throws IOException {
     if (c instanceof TezBytesComparator) return CMP_BYTES;
@@ -122,8 +197,8 @@ public class GpuSorter extends ExternalSorter {
 
   @Override
   public void write(Object key, Object value) throws IOException {
-    final int p = deviceHash ? -1 : partitioner.getPartition(key, value, partitions);
-    if (!deviceHash && (p < 0 || p >= partitions)) {
+    final int p = devicePartitioner ? -1 : partitioner.getPartition(key, value, partitions);
+    if (!devicePartitioner && (p < 0 || p >= partitions)) {
       throw new IOException("Illegal partition for " + key + " (" + p + ")"); // PipelinedSorter.java:410-413
     }
     final int ks = kv.position();
@@ -133,7 +208,7 @@ public class GpuSorter extends ExternalSorter {
     keyOff.put(n, ks);
     valOff.put(n, vs);
     valLen.put(n, kv.position() - vs);
-    if (!deviceHash) part.put(n, p);
+    if (!devicePartitioner) part.put(n, p);
     mapOutputRecordCounter.increment(1);
     mapOutputByteCounter.increment(kv.position() - ks);
     if (++n == BATCH_RECORDS || kv.remaining() < (BATCH_BYTES >> 3)) pushBatch();
@@ -146,7 +221,7 @@ public class GpuSorter extends ExternalSorter {
 
   private void pushBatch() throws IOException {
     if (n == 0) return;
-    nativeCollect(handle, kv, kv.position(), keyOff, valOff, valLen, deviceHash ? null : part, n); // tezgpu_sorter_collect_batch
+    nativeCollect(handle, kv, kv.position(), keyOff, valOff, valLen, devicePartitioner ? null : part, n); // tezgpu_sorter_collect_batch
     collectedBytes += kv.position();
     kv.clear();
     n = 0;
@@ -260,6 +335,9 @@ public class GpuSorter extends ExternalSorter {
   private static native void nativeReset(long h) throws IOException;
   private static native void nativeSetCombiner(long h, int combiner) throws IOException;
   private static native void nativeSetCodec(long h, int codec) throws IOException;
+  /** tezgpu_sorter_set_split_points: split i = keys[off[i] .. off[i] + len[i]) */
+  private static native void nativeSetSplitPoints(long h, ByteBuffer keys, long[] off, int[] len, int n, int order)
+      throws IOException;
   private static native void nativeDestroy(long h);
 
   /** DataOutputStream target that appends to the direct batch buffer. */

@@ -96,6 +96,20 @@ JNIEXPORT void JNICALL SORTER(nativeSetCodec)(JNIEnv *env, jclass cls, jlong h, 
   failed(env, tezgpu_sorter_set_codec((tezgpu_sorter *)(intptr_t)h, codec));
 }
 
+/* TotalOrderPartitioner's split keys, serialized like the record keys, and the search order (TEZGPU_CMP_*) */
+JNIEXPORT void JNICALL SORTER(nativeSetSplitPoints)(JNIEnv *env, jclass cls, jlong h, jobject keys, jlongArray off,
+                                                    jintArray len, jint n, jint order) {
+  (void)cls;
+  jlong *o = (*env)->GetLongArrayElements(env, off, NULL);
+  jint *l = (*env)->GetIntArrayElements(env, len, NULL);
+  /* jlong / jint are 64 / 32-bit: the arrays are the uint64_t offsets and uint32_t lengths of the C ABI */
+  int32_t rc = tezgpu_sorter_set_split_points((tezgpu_sorter *)(intptr_t)h, (const uint8_t *)addr(env, keys),
+                                              (const uint64_t *)o, (const uint32_t *)l, (uint32_t)n, order);
+  (*env)->ReleaseLongArrayElements(env, off, o, JNI_ABORT);
+  (*env)->ReleaseIntArrayElements(env, len, l, JNI_ABORT);
+  failed(env, rc);
+}
+
 JNIEXPORT void JNICALL SORTER(nativeDestroy)(JNIEnv *env, jclass cls, jlong h) {
   (void)env; (void)cls;
   tezgpu_sorter_destroy((tezgpu_sorter *)(intptr_t)h);

@@ -5,6 +5,6 @@ This package is the host-side mirror used where no JVM exists; it never falls ba
 """
 from . import _lib  # noqa: F401
 from .constants import *  # noqa: F401,F403
-from .native import GpuSorter, GpuMerger, PeerBuffer, PeerMapping, fetch_ranges, fetch_segments_verified  # noqa: F401
+from .native import GpuSorter, GpuMerger, PeerBuffer, PeerMapping, debug_total_order, fetch_ranges, fetch_segments_verified  # noqa: F401
 
-__all__ = ["GpuSorter", "GpuMerger", "PeerBuffer", "PeerMapping", "fetch_ranges", "fetch_segments_verified"]
+__all__ = ["GpuSorter", "GpuMerger", "PeerBuffer", "PeerMapping", "debug_total_order", "fetch_ranges", "fetch_segments_verified"]

@@ -64,6 +64,7 @@ SYMBOLS = [
     ("tezgpu_sorter_stream", _V, [_V]),
     ("tezgpu_sorter_set_combiner", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_sorter_set_codec", C.c_int32, [_V, C.c_int32]),
+    ("tezgpu_sorter_set_split_points", C.c_int32, [_V, _V, _V, _V, C.c_uint32, C.c_int32]),
     ("tezgpu_shuffle_header_size", C.c_uint64, [C.c_char_p, C.c_int64, C.c_int64, C.c_int32]),
     ("tezgpu_shuffle_header_write", C.c_int32, [C.c_char_p, C.c_int64, C.c_int64, C.c_int32, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_shuffle_header_read", C.c_int32, [_V, C.c_uint64, _V, C.c_uint64, _P(C.c_int64), _P(C.c_int64), _P(C.c_int32), _P(C.c_uint64)]),
@@ -81,6 +82,7 @@ SYMBOLS = [
     ("tezgpu_debug_zstd_decompress_emulate", C.c_int32, [_V, C.c_uint64, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_debug_sort_words_emulate", C.c_int32, [_V, _V, _V, C.c_uint32, C.c_int32, C.c_int32, _V, C.c_int32, _V,
                                                      _P(C.c_uint32), _P(C.c_int32)]),
+    ("tezgpu_debug_total_order_emulate", C.c_int32, [_V, _V, _V, C.c_uint32, _V, _V, _V, C.c_uint32, C.c_int32, C.c_int32, _V]),
     ("tezgpu_merge_open", C.c_int32, [_P(Conf), _P(Segment), C.c_uint32, _P(_V)]),
     ("tezgpu_merge_reopen", C.c_int32, [_V, _P(Segment), C.c_uint32]),
     ("tezgpu_merge_open_codec", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, _P(_V)]),

@@ -113,6 +113,111 @@ static int combiner_for(const Configuration &c) {
   return TEZGPU_COMBINE_NONE;
 }
 
+// ---------------------------------------------------------------- TotalOrderPartitioner
+static const char *TOTAL_ORDER_NEW = "org.apache.hadoop.mapreduce.lib.partition.TotalOrderPartitioner";
+static const char *TOTAL_ORDER_OLD = "org.apache.hadoop.mapred.lib.TotalOrderPartitioner";
+static const char *K_PARTITION_PATH = "mapreduce.totalorderpartitioner.path";           // default _partition.lst
+static const char *K_NATURAL_ORDER = "mapreduce.totalorderpartitioner.naturalorder";    // default true
+// (mapreduce.totalorderpartitioner.trie.maxdepth only shapes Java's index over the split points: nothing to do here)
+
+// The output's partitioner is TotalOrderPartitioner: named directly, or wrapped by MRPartitioner (with more than one
+// partition, where MRPartitioner instantiates it) as mapreduce.job.partitioner.class under the new API and
+// mapred.partitioner.class under the old one (tez-mapreduce partition/MRPartitioner.java).
+static bool total_order_partitioner(const Configuration &c, int P) {
+  auto is_total = [](const std::string &cls) { return cls == TOTAL_ORDER_NEW || cls == TOTAL_ORDER_OLD; };
+  const std::string pc = c.get(K_PARTITIONER, "");
+  if (is_total(pc)) return true;
+  if (pc != "org.apache.tez.mapreduce.partition.MRPartitioner" || P <= 1) return false;
+  const bool new_api = c.getBoolean("mapred.mapper.new-api", false);
+  return is_total(c.get(new_api ? "mapreduce.job.partitioner.class" : "mapred.partitioner.class", ""));
+}
+
+// The split keys of a partition file (what TotalOrderPartitioner.readPartitions reads with SequenceFile.Reader):
+// SequenceFile version 6, uncompressed or record-compressed (only values are compressed there, and they are skipped).
+// Keys come back serialized, exactly as stored.  Refusals name the file: TEZGPU_E_INVALID for an unreadable file, a
+// key class other than `key_class`, or a malformed header or record; TEZGPU_E_UNSUPPORTED for block compression.
+struct PartitionFile {
+  std::vector<uint8_t> keys;
+  std::vector<uint64_t> off;
+  std::vector<uint32_t> len;
+};
+static PartitionFile read_partition_file(const std::string &path, const std::string &key_class) {
+  std::vector<uint8_t> b;
+  {
+    int fd = ::open(path.c_str(), O_RDONLY);
+    RT_CHECK(fd >= 0, TEZGPU_E_INVALID, "Can't read partitions file " + path + ": " + strerror(errno));
+    uint8_t buf[1 << 16];
+    ssize_t r;
+    while ((r = ::read(fd, buf, sizeof(buf))) > 0) b.insert(b.end(), buf, buf + r);
+    const int e = errno;
+    ::close(fd);
+    RT_CHECK(r == 0, TEZGPU_E_INVALID, "Can't read partitions file " + path + ": " + strerror(e));
+  }
+  size_t pos = 0;
+  auto bad = [&](const std::string &why) { return Err(TEZGPU_E_INVALID, "partitions file " + path + ": " + why); };
+  auto need = [&](size_t n, const char *what) { if (b.size() - pos < n) throw bad(std::string("truncated ") + what); };
+  auto i32 = [&](const char *what) {
+    need(4, what);
+    const uint32_t v = ((uint32_t)b[pos] << 24) | ((uint32_t)b[pos + 1] << 16) | ((uint32_t)b[pos + 2] << 8) | b[pos + 3];
+    pos += 4;
+    return (int32_t)v;
+  };
+  auto vint = [&](const char *what) {   // WritableUtils.readVInt
+    need(1, what);
+    const int8_t first = (int8_t)b[pos++];
+    if (first >= -112) return (int64_t)first;
+    const bool neg = first < -120;
+    const int n = neg ? -(first + 120) : -(first + 112);
+    need((size_t)n, what);
+    int64_t v = 0;
+    for (int i = 0; i < n; i++) v = (v << 8) | b[pos++];
+    return neg ? ~v : v;
+  };
+  auto text = [&](const char *what) {   // Text.readString
+    const int64_t n = vint(what);
+    if (n < 0) throw bad(std::string("negative length in ") + what);
+    need((size_t)n, what);
+    std::string t(b.begin() + pos, b.begin() + pos + n);
+    pos += (size_t)n;
+    return t;
+  };
+  need(4, "header");
+  if (memcmp(b.data(), "SEQ", 3) != 0 || b[3] != 6) throw bad("not a SequenceFile of version 6");
+  pos = 4;
+  const std::string kc = text("key class");
+  if (kc != key_class) throw bad("wrong key class: " + key_class + " is not " + kc);   // SequenceFile.Reader.next's order
+  text("value class");
+  need(2, "header");
+  const bool compressed = b[pos++] != 0, block = b[pos++] != 0;
+  if (block) throw Err(TEZGPU_E_UNSUPPORTED, "partitions file " + path + ": block-compressed SequenceFiles are not read");
+  if (compressed) text("codec class");
+  const int32_t meta = i32("metadata");
+  if (meta < 0) throw bad("negative metadata count");
+  for (int32_t i = 0; i < 2 * meta; i++) text("metadata");
+  need(16, "sync marker");
+  const size_t sync = pos;
+  pos += 16;
+  PartitionFile f;
+  while (pos < b.size()) {
+    const int32_t rec = i32("record");
+    if (rec == -1) {
+      need(16, "sync marker");
+      if (memcmp(b.data() + pos, b.data() + sync, 16) != 0) throw bad("sync marker mismatch");
+      pos += 16;
+      continue;
+    }
+    const int32_t kl = i32("record");
+    if (rec < 0 || kl < 0 || kl > rec) throw bad("malformed record");
+    need((size_t)rec, "record");
+    f.off.push_back(f.keys.size());
+    f.len.push_back((uint32_t)kl);
+    f.keys.insert(f.keys.end(), b.begin() + pos, b.begin() + pos + kl);
+    pos += (size_t)rec;
+  }
+  f.keys.reserve(f.keys.size() + 1);   // a valid pointer even when every split key is empty
+  return f;
+}
+
 // ---------------------------------------------------------------- small utilities
 static void mkdirs(const std::string &path) {
   for (size_t i = 1; i <= path.size(); i++)
@@ -436,12 +541,13 @@ struct Output {
   bool initialized = false, started = false, closed = false;
   bool send_empty = true, final_merge = true;
   bool unordered = false;   // UnorderedPartitionedKVOutput / UnorderedKVOutput: the writer in TEZGPU_SORTER_UNORDERED mode
+  bool total_order;         // TotalOrderPartitioner: the device partitions by the split points of the partition file
   std::map<std::string, int64_t> counters;
   GpuSorter *sorter = nullptr;
   std::vector<Event> events;
   Output(const char *c, const char *wd, const char *u, const char *dv, const char *h, int pt, int64_t mem, int p, int dev)
       : conf(c), work_dir(wd ? wd : "."), uid(u ? u : "attempt"), dest_vertex(dv ? dv : ""), host(h ? h : "localhost"),
-        port(pt), P(p), device(dev), task_memory(mem) {}
+        port(pt), P(p), device(dev), task_memory(mem), total_order(total_order_partitioner(conf, p)) {}
   ~Output() { delete sorter; }
 
   void initialize() {
@@ -481,9 +587,27 @@ struct Output {
     gc.device = device;
     gc.num_partitions = P;
     std::string pc = conf.get(K_PARTITIONER, "org.apache.tez.runtime.library.partitioner.HashPartitioner");
-    gc.partitioner = ends_with(pc, "HashPartitioner") ? TEZGPU_PART_HASH : TEZGPU_PART_GIVEN;
-    // an unordered edge compares no keys: its key class only matters to the HashPartitioner's hashCode
-    gc.comparator = (!unordered || (gc.partitioner == TEZGPU_PART_HASH && P > 1)) ? comparator_for(conf) : TEZGPU_CMP_BYTES;
+    gc.partitioner = total_order ? TEZGPU_PART_TOTAL_ORDER : ends_with(pc, "HashPartitioner") ? TEZGPU_PART_HASH : TEZGPU_PART_GIVEN;
+    // an unordered edge compares no keys: its key class only matters to the HashPartitioner's hashCode and to the
+    // split points' order check
+    gc.comparator = (!unordered || total_order || (gc.partitioner == TEZGPU_PART_HASH && P > 1)) ? comparator_for(conf) : TEZGPU_CMP_BYTES;
+    // TotalOrderPartitioner.setConf: the partition file is read and checked here, before any device call
+    PartitionFile splits;
+    int32_t split_order = gc.comparator;
+    if (total_order) {
+      std::string path = conf.get(K_PARTITION_PATH, "_partition.lst");
+      if (path.empty() || path[0] != '/') path = work_dir + "/" + path;
+      const std::string kc = conf.get(K_KEY_CLASS, "");
+      splits = read_partition_file(path, kc);
+      if (conf.getBoolean(K_NATURAL_ORDER, true)) {
+        if (ends_with(kc, "io.Text")) split_order = TEZGPU_CMP_TEXT;
+        else if (ends_with(kc, "io.BytesWritable")) split_order = TEZGPU_CMP_BYTESWRITABLE;
+      }
+      // the count and order checks of tezgpu_sorter_set_split_points, on the host
+      RT_CHECK((int64_t)splits.len.size() == (int64_t)P - 1, TEZGPU_E_INVALID, "Wrong number of partitions in keyset");
+      gpu_check(tezgpu_debug_total_order_emulate(nullptr, nullptr, nullptr, 0, splits.keys.data(), splits.off.data(), splits.len.data(),
+                                                 (uint32_t)splits.len.size(), gc.comparator, split_order, nullptr));
+    }
     gc.rle_policy = TEZGPU_RLE_AUTO;
     gc.send_empty_partition_details = send_empty ? 1 : 0;
     gc.sorter_impl = unordered ? TEZGPU_SORTER_UNORDERED : sc == "LEGACY" ? 1 : 0;
@@ -492,11 +616,16 @@ struct Output {
     // UnorderedPartitionedKVWriter runs no combiner (and tezgpu_sorter_set_combiner refuses an unordered handle)
     if (const int c = unordered ? 0 : combiner_for(conf)) sorter->set_combiner(c, (int)conf.getInt(K_COMBINE_MIN_SPILLS, 3));
     if (codec) sorter->set_codec(codec);
+    if (total_order)
+      gpu_check(tezgpu_sorter_set_split_points(sorter->h, splits.keys.data(), splits.off.data(), splits.len.data(),
+                                               (uint32_t)splits.len.size(), split_order));
     started = true;
   }
   void write(const uint8_t *k, uint32_t kl, const uint8_t *v, uint32_t vl, int32_t partition) {
+    RT_CHECK(!(total_order && partition >= 0), TEZGPU_E_INVALID,
+             "TotalOrderPartitioner output: the device computes the partition, write() takes none");
     RT_CHECK(started && !closed, TEZGPU_E_STATE, "write() outside start()..close()");
-    RT_CHECK(partition >= 0 || sorter->gc.partitioner == TEZGPU_PART_HASH, TEZGPU_E_UNSUPPORTED,
+    RT_CHECK(partition >= 0 || sorter->gc.partitioner != TEZGPU_PART_GIVEN, TEZGPU_E_UNSUPPORTED,
              "custom partitioner: the caller must pass Partitioner.getPartition(key, value, numPartitions)");
     sorter->write(k, kl, v, vl, partition);
   }
@@ -800,6 +929,7 @@ int32_t tezrt_output_create_unordered(const char *conf, const char *work_dir, co
   // UnorderedKVOutput writes one partition whatever the number of physical outputs (RL/output/UnorderedKVOutput.java:107)
   *out = new tezrt_output(conf, work_dir, unique_id, dest_vertex, host, port, task_memory, partitioned ? P : 1, device);
   (*out)->o.unordered = true;
+  if (!partitioned) (*out)->o.total_order = false;   // UnorderedKVOutput has no partitioner
   RT_END
 }
 int32_t tezrt_output_initialize(tezrt_output *o, int64_t *requested) { RT_BEGIN o->o.initialize(); if (requested) *requested = o->o.requested; RT_END }

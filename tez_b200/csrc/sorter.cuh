@@ -175,8 +175,8 @@ class SortPipeline {
     TG_CHECK(c.num_partitions >= 1, TEZGPU_E_INVALID, "num_partitions must be >= 1");
     TG_CHECK(c.comparator >= TEZGPU_CMP_BYTES && c.comparator <= TEZGPU_CMP_LONG, TEZGPU_E_UNSUPPORTED,
              "comparator outside the device-supported set (BYTES, TEXT, BYTESWRITABLE, INT, LONG)");
-    TG_CHECK(c.partitioner == TEZGPU_PART_GIVEN || c.partitioner == TEZGPU_PART_HASH, TEZGPU_E_UNSUPPORTED,
-             "partitioner outside the device-supported set (GIVEN, HASH)");
+    TG_CHECK(c.partitioner == TEZGPU_PART_GIVEN || c.partitioner == TEZGPU_PART_HASH || c.partitioner == TEZGPU_PART_TOTAL_ORDER,
+             TEZGPU_E_UNSUPPORTED, "partitioner outside the device-supported set (GIVEN, HASH, TOTAL_ORDER)");
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev == 0) {
@@ -225,6 +225,30 @@ class SortPipeline {
   int merge_check_same = 1;
   bool merge_inputs_plain = false;
   int combiner = TEZGPU_COMBINE_NONE;  // TEZGPU_COMBINE_*: combine_phase runs between the sort and the emit
+  // TOTAL_ORDER: the split table (total_order.cuh) in device memory, grow-only; splits.n = 0 until set_split_points
+  DeviceBuffer sp_prefix, sp_len, sp_off, sp_blob;
+  SplitTable splits{};
+  bool have_splits = false;
+  // uploads a table build_split_table made; the stream is idle between flushes, so the old table is no longer read
+  void set_split_points(const HostSplitTable &t) {
+    TG_CUDA(cudaSetDevice(conf.device));
+    const size_t n = t.prefix.size();
+    sp_prefix.ensure(std::max<size_t>(n, 1) * 8);
+    sp_len.ensure(std::max<size_t>(n, 1) * 4);
+    sp_off.ensure(std::max<size_t>(n, 1) * 8);
+    sp_blob.ensure(std::max<size_t>(t.blob.size(), 16));
+    if (n) {
+      TG_CUDA(cudaMemcpyAsync(sp_prefix.p, t.prefix.data(), n * 8, cudaMemcpyHostToDevice, stream));
+      TG_CUDA(cudaMemcpyAsync(sp_len.p, t.len.data(), n * 4, cudaMemcpyHostToDevice, stream));
+      TG_CUDA(cudaMemcpyAsync(sp_off.p, t.off.data(), n * 8, cudaMemcpyHostToDevice, stream));
+    }
+    if (!t.blob.empty()) TG_CUDA(cudaMemcpyAsync(sp_blob.p, t.blob.data(), t.blob.size(), cudaMemcpyHostToDevice, stream));
+    TG_CUDA(cudaStreamSynchronize(stream));
+    splits = SplitTable{sp_prefix.as<uint64_t>(), sp_len.as<uint32_t>(), sp_off.as<uint64_t>(), sp_blob.as<uint8_t>(), (uint32_t)n, t.order};
+    have_splits = true;
+  }
+  // the split points k_stage searches: none unless the handle is TOTAL_ORDER (the merger's pipeline never is)
+  SplitTable stage_splits() const { return conf.partitioner == TEZGPU_PART_TOTAL_ORDER ? splits : SplitTable{}; }
   // combine workspace (grow-only): head flags / group ids, sums, head positions, and the combined records' sort words,
   // order, same[], bytes and (variable width) metadata
   DeviceBuffer c_head, c_gid, c_sums, c_hpos, c_K, c_order, c_same, c_kv, c_koff, c_klen, c_vlen, c_bad;
@@ -315,7 +339,8 @@ class SortPipeline {
     rec.num_partitions = P;
     rec.pbits = pbits;
     rec.unordered = conf.sorter_impl == TEZGPU_SORTER_UNORDERED ? 1 : 0;
-    TG_CHECK(rec.hash_partition || rec.partition || rec.use_runs || n == 0 || P == 1, TEZGPU_E_INVALID, "partition ids required (partitioner=GIVEN)");
+    TG_CHECK(rec.hash_partition || rec.partition || rec.use_runs || stage_splits().n || n == 0 || P == 1, TEZGPU_E_INVALID,
+             "partition ids required (partitioner=GIVEN)");
     state.have_bounds = state.spec_layout = false;
     state.same = nullptr;
     timer.reset();
@@ -383,8 +408,16 @@ class SortPipeline {
     const bool fast16 = rec.fixed && !rec.key_off && !rec.use_runs && rec.klen == 16 && ((rec.klen + rec.vlen) % 16 == 0) && rec.cmp == CMP_BYTES &&
                         (((uintptr_t)rec.kv & 15u) == 0);
     int sgrid = (int)std::min<uint64_t>(div_up(n, 256), (uint64_t)num_sms * 16);
-    if (fast16) k_stage<true><<<sgrid, 256, 0, stream>>>(rec, state.K, d->hist, &d->verdict.error);
-    else k_stage<false><<<sgrid, 256, 0, stream>>>(rec, state.K, d->hist, &d->verdict.error);
+    const SplitTable sp = stage_splits();
+    if (sp.n) {
+      const size_t smem = sp.n <= SPLIT_SMEM_MAX ? (size_t)sp.n * 8 : 0;
+      if (fast16) k_stage<true, true><<<sgrid, 256, smem, stream>>>(rec, state.K, d->hist, &d->verdict.error, sp);
+      else k_stage<false, true><<<sgrid, 256, smem, stream>>>(rec, state.K, d->hist, &d->verdict.error, sp);
+    } else if (fast16) {
+      k_stage<true><<<sgrid, 256, 0, stream>>>(rec, state.K, d->hist, &d->verdict.error, sp);
+    } else {
+      k_stage<false><<<sgrid, 256, 0, stream>>>(rec, state.K, d->hist, &d->verdict.error, sp);
+    }
     TG_CUDA(cudaGetLastError());
     k_radix_scan_hist<<<1, RADIX, 0, stream>>>(d->hist, 4, n, d->trivial);
     TG_CUDA(cudaGetLastError());

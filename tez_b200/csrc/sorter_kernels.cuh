@@ -8,6 +8,7 @@
 #include "crc32.cuh"
 #include "radix_sort.cuh"
 #include "scan.cuh"
+#include "total_order.cuh"
 
 namespace tezgpu {
 
@@ -151,10 +152,13 @@ __host__ __device__ __forceinline__ uint32_t compose_sort_word(const Records &r,
 }
 
 // Sort word of one record with its key at `key` (every path of k_stage but the 16-byte fast one; the host emulation
-// tezgpu_debug_sort_words_emulate runs the same code): partition id (HashPartitioner, else `given`) and prefix = the
-// first normalised content bytes or the packed SymTable ranks.
+// tezgpu_debug_sort_words_emulate runs the same code): partition id (TOTAL_ORDER: the search among the split points of
+// `sp`, whose prefix words are read from `split_pw`; else HashPartitioner, else `given`) and prefix = the first
+// normalised content bytes or the packed SymTable ranks.
+template <bool TOTAL_ORDER = false>
 __host__ __device__ __forceinline__ uint32_t stage_sort_word(const Records &r, const uint8_t *key, uint32_t klen,
-                                                             int32_t given, bool &bad) {
+                                                             int32_t given, bool &bad, const SplitTable *sp = nullptr,
+                                                             const uint64_t *split_pw = nullptr) {
   const uint32_t skip = key_content_skip(r.cmp, key, klen);
   const uint8_t *content = key + skip;
   const uint32_t clen = klen - skip;
@@ -168,9 +172,10 @@ __host__ __device__ __forceinline__ uint32_t stage_sort_word(const Records &r, c
 #pragma unroll
     for (uint32_t b = 0; b < 4; b++) prefix = (prefix << 8) | (b < clen ? norm_byte(r.cmp, content, b) : 0u);
   }
-  const int32_t p = r.hash_partition
-                        ? (int32_t)((uint32_t)(key_hash_dev(r.cmp, key, klen) & 0x7fffffff) % (uint32_t)r.num_partitions)
-                        : given;
+  int32_t p;
+  if constexpr (TOTAL_ORDER) p = split_partition(*sp, split_pw, key, klen);
+  else p = r.hash_partition ? (int32_t)((uint32_t)(key_hash_dev(r.cmp, key, klen) & 0x7fffffff) % (uint32_t)r.num_partitions)
+                            : given;
   return compose_sort_word(r, p, prefix, bad);
 }
 
@@ -178,11 +183,23 @@ constexpr int STAGE_ERR_PARTITION = 1;  // k_stage's error bits: "Illegal partit
 constexpr int STAGE_ERR_FRAMING = 2;    // and in run-table mode, a record position that lacks the fixed framing bytes
 
 // One thread per record: its sort word (stage_sort_word, or inline for 16-byte fixed keys) and the digit histograms of
-// all four radix passes (so the sort never re-reads the keys for counting).
-template <bool FAST16>
+// all four radix passes (so the sort never re-reads the keys for counting).  TOTAL_ORDER: the partition is the search
+// among the split points `sp` (TotalOrderPartitioner; unused otherwise -- it is the last parameter, so the other
+// instantiations keep their parameter layout); the launch passes sp.n * 8 bytes of dynamic shared memory when
+// sp.n <= SPLIT_SMEM_MAX (the prefix words are staged there), else 0 and the search reads the table in global memory.
+template <bool FAST16, bool TOTAL_ORDER = false>
 __global__ void __launch_bounds__(256) k_stage(Records r, uint32_t *__restrict__ keys_out, uint32_t *__restrict__ hist,
-                                               int *__restrict__ error_flag) {
+                                               int *__restrict__ error_flag, SplitTable sp) {
   __shared__ uint32_t s_hist[4 * RADIX];
+  const uint64_t *split_pw = nullptr;
+  if constexpr (TOTAL_ORDER) {
+    extern __shared__ uint64_t s_split_pw[];
+    split_pw = sp.prefix;
+    if (sp.n <= SPLIT_SMEM_MAX) {
+      for (uint32_t i = threadIdx.x; i < sp.n; i += blockDim.x) s_split_pw[i] = sp.prefix[i];
+      split_pw = s_split_pw;
+    }
+  }
   for (int i = threadIdx.x; i < 4 * RADIX; i += blockDim.x) s_hist[i] = 0;
   __syncthreads();
   const uint32_t stride = gridDim.x * blockDim.x;
@@ -194,7 +211,12 @@ __global__ void __launch_bounds__(256) k_stage(Records r, uint32_t *__restrict__
       const uint4 kq = *reinterpret_cast<const uint4 *>(r.kv + (uint64_t)i * (r.klen + r.vlen));
       const uint32_t prefix = __byte_perm(kq.x, 0, 0x0123);
       int32_t p;
-      if (r.hash_partition) {
+      if constexpr (TOTAL_ORDER) {
+        const uint8_t *key = r.kv + (uint64_t)i * (r.klen + r.vlen);
+        p = sp.order == CMP_BYTES
+                ? (int32_t)split_upper_bound(sp, split_pw, ((uint64_t)prefix << 32) | __byte_perm(kq.y, 0, 0x0123), key, 16)
+                : split_partition(sp, split_pw, key, 16);
+      } else if (r.hash_partition) {
         uint32_t h = 1;
         const uint32_t w[4] = {kq.x, kq.y, kq.z, kq.w};
 #pragma unroll
@@ -229,7 +251,7 @@ __global__ void __launch_bounds__(256) k_stage(Records r, uint32_t *__restrict__
         record_lookup(r, i, koff, klen, vlen);
       }
       const int32_t given = r.hash_partition ? 0 : ((r.fixed && r.use_runs) ? run_part : (r.partition ? r.partition[i] : 0));
-      K = stage_sort_word(r, r.kv + koff, klen, given, bad);
+      K = stage_sort_word<TOTAL_ORDER>(r, r.kv + koff, klen, given, bad, &sp, split_pw);
     }
     if (bad) atomicOr(error_flag, STAGE_ERR_PARTITION);
     keys_out[r.unordered ? r.n - 1u - i : i] = K;

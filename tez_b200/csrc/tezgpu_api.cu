@@ -103,6 +103,18 @@ struct tezgpu_sorter {
   }
 };
 
+// the partition source of a collect or flush: a TOTAL_ORDER handle takes no partition ids and needs its split points
+static void check_partition_source(const tezgpu_sorter *h, bool given) {
+  const tezgpu_conf &c = h->pipe.conf;
+  if (c.partitioner == TEZGPU_PART_TOTAL_ORDER) {
+    TG_CHECK(!given, TEZGPU_E_INVALID, "partition ids given to a TotalOrderPartitioner handle (the device computes them)");
+    TG_CHECK(h->pipe.have_splits || c.num_partitions == 1, TEZGPU_E_STATE,
+             "TotalOrderPartitioner: set the split points (tezgpu_sorter_set_split_points) first");
+    return;
+  }
+  TG_CHECK(given || c.partitioner == TEZGPU_PART_HASH, TEZGPU_E_INVALID, "partition ids required (partitioner=GIVEN)");
+}
+
 __global__ void k_rebase_offsets(const uint32_t *__restrict__ key_off, const uint32_t *__restrict__ val_off,
                                  const uint32_t *__restrict__ val_len, uint32_t n, uint64_t base, uint64_t kv_bytes,
                                  uint64_t *__restrict__ koff64, uint32_t *__restrict__ klen, uint32_t *__restrict__ vlen,
@@ -192,8 +204,7 @@ int32_t tezgpu_sorter_collect_batch(tezgpu_sorter *h, const uint8_t *kv, uint64_
   TG_CHECK(h->n + n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records collected");
   TG_CHECK((h->n == 0) || (h->has_partition == (partition != nullptr)), TEZGPU_E_INVALID,
            "partition ids must be given for all batches or none");
-  TG_CHECK(partition || h->pipe.conf.partitioner == TEZGPU_PART_HASH, TEZGPU_E_INVALID,
-           "partition ids required (partitioner=GIVEN)");
+  check_partition_source(h, partition != nullptr);
   {
     // the sort memory granted to this output (ExternalSorter.getInitialMemoryRequirement, SORT/ExternalSorter.java:330-347;
     // PipelinedSorter spills when its kvbuffer is full, :415-444): past it the caller must spill -- flush + reset --
@@ -247,8 +258,7 @@ int32_t tezgpu_sorter_collect_fixed(tezgpu_sorter *h, const uint8_t *kv, const i
   TG_CHECK(h->n + n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records collected");
   TG_CHECK((h->n == 0) || (h->has_partition == (partition != nullptr)), TEZGPU_E_INVALID,
            "partition ids must be given for all batches or none");
-  TG_CHECK(partition || h->pipe.conf.partitioner == TEZGPU_PART_HASH, TEZGPU_E_INVALID,
-           "partition ids required (partitioner=GIVEN)");
+  check_partition_source(h, partition != nullptr);
   const uint64_t stride = (uint64_t)h->klen + h->vlen;
   {
     const uint64_t budget = h->pipe.conf.mem_budget_bytes;
@@ -287,6 +297,7 @@ uint64_t tezgpu_sorter_output_bound(const tezgpu_sorter *h) {
 static void sorter_run(tezgpu_sorter *h, uint8_t *host_out, uint64_t out_cap, uint64_t *out_len, int64_t *index,
                        tezgpu_stats *stats, std::vector<int64_t> &idx_store) {
   TG_CHECK(!h->flushed, TEZGPU_E_STATE, "flush called twice");
+  if (h->pipe.conf.partitioner == TEZGPU_PART_TOTAL_ORDER) check_partition_source(h, false);
   const int P = h->pipe.conf.num_partitions;
   idx_store.assign((size_t)P * 3, 0);
   uint64_t bound = tezgpu_sorter_output_bound(h);
@@ -345,8 +356,7 @@ int32_t tezgpu_sorter_sort_device_fixed(tezgpu_sorter *h, const void *d_kv, cons
   TG_CHECK(h && (d_kv || n == 0) && d_out, TEZGPU_E_INVALID, "null argument");
   TG_CHECK(h->fixed, TEZGPU_E_STATE, "handle is not in fixed-width mode");
   TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one sort");
-  TG_CHECK(d_partition || h->pipe.conf.partitioner == TEZGPU_PART_HASH, TEZGPU_E_INVALID,
-           "partition ids required (partitioner=GIVEN)");
+  check_partition_source(h, d_partition != nullptr);
   Records r;
   memset(&r, 0, sizeof(r));
   r.kv = (const uint8_t *)d_kv;
@@ -385,6 +395,33 @@ int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec) {
   check_codec(codec);
   TG_CHECK(h->n == 0 && !h->flushed, TEZGPU_E_STATE, "set the codec before the first collect (or after a reset)");
   h->pipe.codec = codec;
+  TG_API_END
+}
+
+int32_t tezgpu_sorter_set_split_points(tezgpu_sorter *h, const uint8_t *keys, const uint64_t *key_off, const uint32_t *key_len,
+                                       uint32_t n, int32_t order) {
+  TG_API_BEGIN
+  TG_CHECK(h, TEZGPU_E_INVALID, "null handle");
+  const tezgpu_conf &c = h->pipe.conf;
+  TG_CHECK(c.partitioner == TEZGPU_PART_TOTAL_ORDER, TEZGPU_E_INVALID, "split points on a handle whose partitioner is not TOTAL_ORDER");
+  TG_CHECK(h->n == 0 && !h->flushed, TEZGPU_E_STATE, "set the split points before the first collect (or after a reset)");
+  HostSplitTable t;
+  build_split_table(c.comparator, order, c.num_partitions, keys, key_off, key_len, n, t);
+  h->pipe.set_split_points(t);
+  TG_API_END
+}
+
+int32_t tezgpu_debug_total_order_emulate(const uint8_t *kv, const uint64_t *key_off, const uint32_t *key_len, uint32_t n,
+                                         const uint8_t *splits, const uint64_t *split_off, const uint32_t *split_len,
+                                         uint32_t nsplits, int32_t comparator, int32_t order, int32_t *partition) {
+  TG_API_BEGIN
+  TG_CHECK(((kv && key_off && key_len && partition) || n == 0), TEZGPU_E_INVALID, "null argument");
+  TG_CHECK(comparator >= TEZGPU_CMP_BYTES && comparator <= TEZGPU_CMP_LONG, TEZGPU_E_UNSUPPORTED, "unknown comparator");
+  TG_CHECK(nsplits < (1u << 31) - 1, TEZGPU_E_INVALID, "too many split points");
+  HostSplitTable t;
+  build_split_table(comparator, order, (int)nsplits + 1, splits, split_off, split_len, nsplits, t);
+  const SplitTable v = t.view();
+  for (uint32_t i = 0; i < n; i++) partition[i] = split_partition(v, v.prefix, kv + key_off[i], key_len[i]);
   TG_API_END
 }
 

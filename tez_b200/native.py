@@ -32,12 +32,36 @@ def make_conf(num_partitions, comparator=CMP_BYTES, partitioner=PART_HASH, rle_p
     return c
 
 
+def _pack_keys(keys):
+    """Serialized keys -> (bytes uint8, offsets uint64, lengths uint32), back to back."""
+    kl = np.array([len(k) for k in keys], dtype=np.uint32)
+    ko = np.zeros(len(keys), dtype=np.uint64)
+    if len(keys):
+        ko[1:] = np.cumsum(kl[:-1], dtype=np.uint64)
+    return np.frombuffer(b"".join(keys) + b"\0", dtype=np.uint8).copy(), ko, kl
+
+
+def debug_total_order(keys, split_points, comparator, order=None):
+    """Partitions TotalOrderPartitioner gives the serialized keys with these split points, computed on the host with the
+    device's checks and search (tezgpu_debug_total_order_emulate).  order: search order (default: the comparator)."""
+    L = _lib.load()
+    kv, ko, kl = _pack_keys(keys)
+    sv, so, sl = _pack_keys(split_points)
+    part = np.zeros(max(1, len(keys)), dtype=np.int32)
+    check(L.tezgpu_debug_total_order_emulate(_ptr(kv), _ptr(ko), _ptr(kl), len(keys), _ptr(sv), _ptr(so), _ptr(sl),
+                                             len(split_points), comparator, comparator if order is None else order,
+                                             _ptr(part)))
+    return part[:len(keys)]
+
+
 class GpuSorter:
-    def __init__(self, num_partitions, combiner=COMBINE_NONE, codec=CODEC_NONE, **kw):
+    def __init__(self, num_partitions, combiner=COMBINE_NONE, codec=CODEC_NONE, split_points=None, split_order=None, **kw):
         """combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG runs MRCombiner with IntSumReducer / LongSumReducer on every
         flush (tezgpu_sorter_set_combiner).  codec: CODEC_DEFAULT writes zlib-compressed segments, CODEC_LZ4 Lz4Codec
         segments (blocks of LZ4_BLOCK_BYTES raw bytes, one chunk each), CODEC_ZSTD ZStandardCodec segments (one frame per
-        ZSTD_BLOCK_BYTES raw bytes) (tezgpu_sorter_set_codec)."""
+        ZSTD_BLOCK_BYTES raw bytes) (tezgpu_sorter_set_codec).  split_points: the serialized split keys of a
+        partitioner=PART_TOTAL_ORDER handle, searched in split_order (a CMP_*; None = the handle's comparator)
+        (tezgpu_sorter_set_split_points)."""
         self.L = _lib.load()
         self.conf = make_conf(num_partitions, **kw)
         self.P = num_partitions
@@ -48,6 +72,8 @@ class GpuSorter:
                 self.set_combiner(combiner)
             if codec:
                 self.set_codec(codec)
+            if split_points is not None:
+                self.set_split_points(split_points, split_order)
         except Exception:
             self.close()
             raise
@@ -59,6 +85,12 @@ class GpuSorter:
     def set_codec(self, codec):
         """CODEC_NONE / CODEC_DEFAULT / CODEC_LZ4 / CODEC_ZSTD; before the first collect (or after reset); survives reset."""
         check(self.L.tezgpu_sorter_set_codec(self.h, codec))
+
+    def set_split_points(self, split_points, order=None):
+        """TotalOrderPartitioner split keys; before the first collect (or after reset); survives reset."""
+        kv, ko, kl = _pack_keys(split_points)
+        check(self.L.tezgpu_sorter_set_split_points(self.h, _ptr(kv), _ptr(ko), _ptr(kl), len(split_points),
+                                                    self.conf.comparator if order is None else order))
 
     def close(self):
         if self.h:
