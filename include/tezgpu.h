@@ -317,6 +317,29 @@ int32_t tezgpu_merge_write_partitions_device(tezgpu_merger *m, void *d_out, uint
  * (SORT/PipelinedSorter.java:774-836) */
 int32_t tezgpu_merge_write_partitions(tezgpu_merger *m, const char *out_path, const char *index_path, int32_t rle,
                                       int64_t *index, tezgpu_stats *stats);
+/* Bounded-memory merge (TezMerger merges any number of segments through one small buffer per segment,
+ * SORT/TezMerger.java:717-912): the k-way merge of tezgpu_merge_open_codec over HOST segments, holding at most
+ * budget_bytes of device memory.  budget_bytes = 0: the device's free memory at open; a budget below
+ * TEZGPU_MERGE_BUDGET_MIN fails with TEZGPU_E_INVALID, a device segment (TEZGPU_SEG_DEVICE) too.  codec must be
+ * TEZGPU_CODEC_NONE (else TEZGPU_E_UNSUPPORTED); raw_len is not read.
+ *   When the inputs fit the budget with one record per input byte (the worst case of the workspace bound in DESIGN
+ *   section 3, "Bounded-memory merge"), the handle takes one step: exactly tezgpu_merge_open.  Otherwise it merges in
+ *   key-range steps over windows of the segments; when the first step's windows hold every segment whole and the
+ *   bound on their scanned records fits, that step is the whole merge and the handle behaves as a one-step one.  With
+ *   several steps the segments must stay valid and unchanged until close.  The stream, the written bytes and
+ *   the counts are those of the one-step merge; a checksum mismatch fails with TEZGPU_E_FORMAT naming the segment
+ *   before the stream ends or a write succeeds; a key group larger than the budget allows fails with TEZGPU_E_NOMEM.
+ *   The handle takes set_check_for_same_keys, set_combiner, next_batch, write_ifile, write_partitions, parse_info
+ *   (of the last step), counts and close.  With several steps: counts fails with TEZGPU_E_STATE until the stream has
+ *   been read to its end or written, output_bound returns 0 until then, every write runs the steps again (a
+ *   next_batch after it starts from the first record), and write_*_device and reopen* fail with TEZGPU_E_STATE. */
+#define TEZGPU_MERGE_BUDGET_MIN (16ull << 20)
+int32_t tezgpu_merge_open_bounded(const tezgpu_conf *conf, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg,
+                                  int32_t codec, uint64_t budget_bytes, tezgpu_merger **out);
+/* steps the last pass over the inputs took (1 for a one-step handle), the most device memory the handle's buffers
+ * held at once, and the bytes uploaded from the host segments by all passes.  TEZGPU_E_STATE on a handle that was
+ * not opened bounded. */
+int32_t tezgpu_merge_bounded_info(tezgpu_merger *m, int32_t *steps, uint64_t *peak_device_bytes, uint64_t *h2d_bytes);
 void *tezgpu_merge_stream(tezgpu_merger *m);
 int32_t tezgpu_merge_close(tezgpu_merger *m);
 

@@ -88,6 +88,8 @@ SYMBOLS = [
     ("tezgpu_merge_open_codec", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, _P(_V)]),
     ("tezgpu_merge_reopen_codec", C.c_int32, [_V, _P(Segment), _V, C.c_uint32]),
     ("tezgpu_concat_open", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, _P(_V)]),
+    ("tezgpu_merge_open_bounded", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, C.c_uint64, _P(_V)]),
+    ("tezgpu_merge_bounded_info", C.c_int32, [_V, _P(C.c_int32), _P(C.c_uint64), _P(C.c_uint64)]),
     ("tezgpu_debug_crc_concat_emulate", C.c_int32, [_V, _V, C.c_uint32, _P(C.c_uint32)]),
     ("tezgpu_merge_set_check_for_same_keys", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_merge_set_combiner", C.c_int32, [_V, C.c_int32]),

@@ -4,17 +4,32 @@
 
 namespace tezgpu {
 
+// Device bytes a group of DeviceBuffers holds, and the most it held at once.  A buffer allocated while a thread has
+// g_device_tally set counts against that tally until it is freed (merge_steps.cuh reports a bounded merge's peak).
+struct DeviceTally {
+  uint64_t live = 0, peak = 0;
+  void add(size_t b) { live += b; if (live > peak) peak = live; }
+};
+inline thread_local DeviceTally *g_device_tally = nullptr;
+
 struct DeviceBuffer {
   void *p = nullptr;
   size_t cap = 0;
+  DeviceTally *tally = nullptr;
   ~DeviceBuffer() { release(); }
   DeviceBuffer() = default;
   DeviceBuffer(const DeviceBuffer &) = delete;
   DeviceBuffer &operator=(const DeviceBuffer &) = delete;
   void release() {
     if (p) cudaFree(p);
+    if (tally) tally->live -= cap;
     p = nullptr;
     cap = 0;
+    tally = nullptr;
+  }
+  void counted(size_t bytes) {
+    tally = g_device_tally;
+    if (tally) tally->add(bytes);
   }
   // grow-only; contents are NOT preserved
   void ensure(size_t bytes) {
@@ -23,6 +38,7 @@ struct DeviceBuffer {
     release();
     TG_CUDA(cudaMalloc(&p, bytes));
     cap = bytes;
+    counted(bytes);
   }
   // grow preserving the first `keep` bytes
   void grow_preserve(size_t bytes, size_t keep, cudaStream_t st) {
@@ -42,9 +58,12 @@ struct DeviceBuffer {
       TG_CUDA(cudaMemcpyAsync(np, p, keep, cudaMemcpyDeviceToDevice, st));
       TG_CUDA(cudaStreamSynchronize(st));
     }
-    if (p) cudaFree(p);
+    DeviceTally *t = g_device_tally;
+    if (t) t->add(ncap);  // old and new are both held until the copy is done
+    release();
     p = np;
     cap = ncap;
+    tally = t;
   }
   template <typename T>
   T *as() const { return reinterpret_cast<T *>(p); }

@@ -13,6 +13,7 @@
 #include "codec.cuh"
 #include "concat.cuh"
 #include "merger.cuh"
+#include "merge_steps.cuh"
 #include "sorter.cuh"
 #include "peer_fetch.cuh"
 

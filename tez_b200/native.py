@@ -4,6 +4,8 @@ GpuSorter  ~ ExternalSorter seam (SORT/ExternalSorter.java:74-92): write/collect
 GpuMerger  ~ TezMerger.merge(...) -> TezRawKeyValueIterator (SORT/TezMerger.java:717-912).
 """
 import ctypes as C
+import os
+import tempfile
 
 import numpy as np
 
@@ -169,7 +171,7 @@ class GpuSorter:
 class GpuMerger:
     def __init__(self, segments, comparator=CMP_BYTES, device=0, has_header=True, device_ptrs=False, fixed=None,
                  partitions=None, num_partitions=1, send_empty=True, verified=None, combiner=COMBINE_NONE,
-                 codec=CODEC_NONE, raw_lens=None, concat=False):
+                 codec=CODEC_NONE, raw_lens=None, concat=False, device_budget=None):
         """segments: list of bytes / uint8 arrays (host) or (ptr, len) tuples when device_ptrs.
         verified: optional per-segment booleans -- the transport already checked that segment's checksum
         (TEZGPU_SEG_VERIFIED: fetch_segments_verified), the merge does not read it again to verify.
@@ -178,7 +180,9 @@ class GpuMerger:
         compressed output (tezgpu_merge_open_codec); raw_lens: per-segment rawLength, required for the compressed
         segments.
         concat: UnorderedPartitionedKVWriter.mergeAll / UnorderedKVReader (tezgpu_concat_open): records leave in
-        (segment, position) order, the writes copy the record bytes (rle must be False)."""
+        (segment, position) order, the writes copy the record bytes (rle must be False).
+        device_budget: bytes of device memory the merge may hold (tezgpu_merge_open_bounded; 0 = the free memory):
+        host segments larger than that merge in key-range steps, with the same stream and output."""
         self.L = _lib.load()
         self.conf = make_conf(num_partitions, comparator=comparator, partitioner=PART_GIVEN, device=device, fixed=fixed,
                               send_empty=send_empty)
@@ -186,7 +190,11 @@ class GpuMerger:
         self._has_header, self._device_ptrs = has_header, device_ptrs
         arr = self._segments(segments, partitions, verified)
         self.h = C.c_void_p()
-        if concat:
+        self.bounded = device_budget is not None
+        if self.bounded:
+            check(self.L.tezgpu_merge_open_bounded(C.byref(self.conf), arr, _ptr(self._raw(raw_lens)), len(segments), codec,
+                                                   int(device_budget), C.byref(self.h)))
+        elif concat:
             check(self.L.tezgpu_concat_open(C.byref(self.conf), arr, _ptr(self._raw(raw_lens)), len(segments), codec,
                                             C.byref(self.h)))
         elif codec:
@@ -268,6 +276,12 @@ class GpuMerger:
         check(self.L.tezgpu_merge_parse_info(self.h, C.byref(m), C.byref(r)))
         return m.value, r.value
 
+    def bounded_info(self):
+        """(steps, peak device bytes, bytes uploaded from the host) of a merger opened with device_budget."""
+        steps, peak, h2d = C.c_int32(), C.c_uint64(), C.c_uint64()
+        check(self.L.tezgpu_merge_bounded_info(self.h, C.byref(steps), C.byref(peak), C.byref(h2d)))
+        return steps.value, peak.value, h2d.value
+
     def counts(self):
         r, b = C.c_uint64(), C.c_uint64()
         check(self.L.tezgpu_merge_counts(self.h, C.byref(r), C.byref(b)))
@@ -298,7 +312,15 @@ class GpuMerger:
             check(self.L.tezgpu_merge_write_ifile(self.h, path.encode(), None, 0, 1 if rle else 0, C.byref(raw),
                                                   C.byref(part), C.byref(st)))
             return None, raw.value, part.value, st.as_dict()
-        out = np.empty(self.output_bound(), dtype=np.uint8)
+        bound = self.output_bound()
+        if bound == 0 and self.bounded:
+            # a merge in several steps knows its output size only once it has run: write through a file
+            with tempfile.TemporaryDirectory() as d:
+                f = os.path.join(d, "merged")
+                _, raw_len, part_len, stats = self.write_ifile(rle, f)
+                with open(f, "rb") as fh:
+                    return fh.read(), raw_len, part_len, stats
+        out = np.empty(bound, dtype=np.uint8)
         check(self.L.tezgpu_merge_write_ifile(self.h, None, _ptr(out), out.size, 1 if rle else 0, C.byref(raw),
                                               C.byref(part), C.byref(st)))
         return out[:part.value].tobytes(), raw.value, part.value, st.as_dict()
@@ -309,6 +331,14 @@ class GpuMerger:
         check(self.L.tezgpu_merge_write_ifile_device(self.h, d_out, out_cap, 1 if rle else 0, C.byref(raw),
                                                      C.byref(part), C.byref(st)))
         return raw.value, part.value, st.as_dict()
+
+    def write_partitions(self, out_path, index_path, rle=False):
+        """file.out + file.out.index of the merged partitions. Returns (index[P,3], stats)."""
+        index = np.zeros((self.P, 3), dtype=np.int64)
+        st = Stats()
+        check(self.L.tezgpu_merge_write_partitions(self.h, out_path.encode(), index_path.encode(), 1 if rle else 0,
+                                                   _ptr(index), C.byref(st)))
+        return index, st.as_dict()
 
     def write_partitions_device(self, d_out, out_cap, rle=False):
         """Batched reduce side: P merged segments back to back. Returns (out_len, index[P,3], stats)."""
