@@ -295,7 +295,10 @@ int32_t tezgpu_merge_set_combiner(tezgpu_merger *m, int32_t combiner);
 int32_t tezgpu_merge_parse_info(tezgpu_merger *m, int32_t *mode, int32_t *by_hand);
 int32_t tezgpu_merge_counts(tezgpu_merger *m, uint64_t *records, uint64_t *kv_bytes);
 /* replaces the next()/getKey()/getValue()/isSameKey() loop: fills up to idx_cap records (key||value bytes appended to
- * out_kv, at most cap bytes); *n = 0 at end of stream */
+ * out_kv, at most cap bytes; a cap above 2^32 - 1 counts as 2^32 - 1, the reach of the 32-bit offsets in idx); *n = 0
+ * at end of stream.  When the next record alone needs more than cap bytes the call returns TEZGPU_E_NOMEM with *n = 0,
+ * idx[0].key_len and idx[0].val_len set to that record's lengths and the stream where it was: a caller grows its buffer
+ * to at least key_len + val_len bytes and calls again. */
 int32_t tezgpu_merge_next_batch(tezgpu_merger *m, uint8_t *out_kv, uint64_t cap, tezgpu_kv_index *idx,
                                 uint32_t idx_cap, uint32_t *n);
 /* replaces TezMerger.writeFile(iter, new IFile.Writer(..., rle)) (SORT/TezMerger.java:215-245): one IFile segment.
@@ -420,6 +423,13 @@ uint32_t tezgpu_debug_chunk_fold_emulate(const uint8_t *data, uint32_t nchunks, 
 
 /* diagnostics: host-side run of the per-thread-run CRC fold of the packed fixed-width emit kernel (nchunks <= 1280) */
 uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks);
+
+/* diagnostics: the emit kernel and tile size the device picks for fixed-width records of klen + vlen bytes written
+ * without repeats.  layout: 0 packed, 16-byte aligned records (the map side); 1 records at explicit offsets; 2 a run
+ * table of fixed-framing segments (the reduce side).  *kernel: 0 k_emit_fast4 (20480-byte tile image), 1
+ * k_emit_fast<5, true>, 2 k_emit_fast4u, 3 k_emit_fast<5, false> (22016-byte images), 4 k_emit<true> (tiles written
+ * in pieces, any record size). */
+int32_t tezgpu_debug_fixed_emit_plan(uint32_t klen, uint32_t vlen, int32_t layout, int32_t *kernel, uint32_t *recs_per_tile);
 
 /* diagnostics: the checksum algebra of tezgpu_concat_open on the host: bodies[i] (lens[i] bytes, ending in FF FF) are
  * the input bodies; each one's CRC-32 becomes the remainder of its record bytes, those are folded with crc(A||B), and

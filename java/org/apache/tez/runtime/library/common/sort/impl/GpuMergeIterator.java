@@ -24,9 +24,10 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
   private static final int BATCH_BYTES = 8 << 20, BATCH_RECORDS = 1 << 16;
 
   private long handle; // tezgpu_merger*
-  private final ByteBuffer batch = ByteBuffer.allocateDirect(BATCH_BYTES).order(ByteOrder.nativeOrder());
+  // both grow to fit a record larger than BATCH_BYTES
+  private ByteBuffer batch = ByteBuffer.allocateDirect(BATCH_BYTES).order(ByteOrder.nativeOrder());
   private final IntBuffer idx = ByteBuffer.allocateDirect(5 * 4 * BATCH_RECORDS).order(ByteOrder.nativeOrder()).asIntBuffer();
-  private final byte[] heap = new byte[BATCH_BYTES];   // DataInputBuffer wants a byte[]
+  private byte[] heap = new byte[BATCH_BYTES];   // DataInputBuffer wants a byte[]
   private final DataInputBuffer key = new DataInputBuffer(), value = new DataInputBuffer();
   private final Progress progress = new Progress();
   private int n, i = -1;
@@ -89,7 +90,13 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
   @Override
   public boolean next() throws IOException {
     if (++i >= n) {
-      n = nativeNextBatch(handle, batch, BATCH_BYTES, idx, BATCH_RECORDS); // tezgpu_merge_next_batch
+      n = nativeNextBatch(handle, batch, batch.capacity(), idx, BATCH_RECORDS); // tezgpu_merge_next_batch
+      if (n < 0) {
+        // the next record alone needs -n bytes: grow both buffers and ask again (the stream has not moved)
+        batch = ByteBuffer.allocateDirect(-n).order(ByteOrder.nativeOrder());
+        heap = new byte[-n];
+        n = nativeNextBatch(handle, batch, batch.capacity(), idx, BATCH_RECORDS);
+      }
       i = 0;
       if (n > 0) {
         batch.position(0);

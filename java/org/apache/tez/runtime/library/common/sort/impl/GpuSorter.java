@@ -56,12 +56,14 @@ public class GpuSorter extends ExternalSorter {
   private static final int BATCH_RECORDS = 1 << 20;
 
   private long handle; // tezgpu_sorter*
-  private final ByteBuffer kv = ByteBuffer.allocateDirect(BATCH_BYTES).order(ByteOrder.nativeOrder());
+  // the batch being serialised; a record larger than BATCH_BYTES is staged alone in a buffer sized for it
+  private ByteBuffer kv = ByteBuffer.allocateDirect(BATCH_BYTES).order(ByteOrder.nativeOrder());
   private final IntBuffer keyOff = direct(BATCH_RECORDS), valOff = direct(BATCH_RECORDS), valLen = direct(BATCH_RECORDS),
       part = direct(BATCH_RECORDS);
   private final boolean devicePartitioner; // HashPartitioner or TotalOrderPartitioner: write() passes no partition
-  private final ByteBufferOutputStream sink = new ByteBufferOutputStream(kv);
+  private final BatchOutputStream sink = new BatchOutputStream();
   private int n;
+  private int recStart; // offset in kv of the record being serialised
   private long collectedBytes;
   private boolean lastSpillRle;
   private final boolean unordered;
@@ -201,22 +203,48 @@ public class GpuSorter extends ExternalSorter {
     if (!devicePartitioner && (p < 0 || p >= partitions)) {
       throw new IOException("Illegal partition for " + key + " (" + p + ")"); // PipelinedSorter.java:410-413
     }
-    final int ks = kv.position();
+    recStart = kv.position();
     keySerializer.serialize(key); // the same serializers PipelinedSorter.collect drives
-    final int vs = kv.position();
+    final int keyLen = kv.position() - recStart;
     valSerializer.serialize(value);
-    keyOff.put(n, ks);
-    valOff.put(n, vs);
-    valLen.put(n, kv.position() - vs);
+    // read after both serialisations: overflow() may have moved the record to the front of a new buffer
+    keyOff.put(n, recStart);
+    valOff.put(n, recStart + keyLen);
+    valLen.put(n, kv.position() - recStart - keyLen);
     if (!devicePartitioner) part.put(n, p);
     mapOutputRecordCounter.increment(1);
-    mapOutputByteCounter.increment(kv.position() - ks);
+    mapOutputByteCounter.increment(kv.position() - recStart);
     if (++n == BATCH_RECORDS || kv.remaining() < (BATCH_BYTES >> 3)) pushBatch();
+    if (kv.capacity() > BATCH_BYTES) {
+      pushBatch(); // the oversized record goes alone; the next batch takes a buffer of the usual size
+      kv = ByteBuffer.allocateDirect(BATCH_BYTES).order(ByteOrder.nativeOrder());
+    }
     // the granted sort memory bounds what one spill holds (ExternalSorter.getInitialMemoryRequirement, :330-347)
     if (collectedBytes + kv.position() > availableMemoryMb * 1024L * 1024L) {
       pushBatch();
       spill(false);
     }
+  }
+
+  /**
+   * The record being serialised needs `more` bytes beyond the end of kv: push the records before it, then carry its
+   * bytes so far to the front of kv, or of a new buffer sized for it when kv cannot hold it.
+   */
+  private void overflow(int more) throws IOException {
+    final byte[] head = new byte[kv.position() - recStart];
+    kv.position(recStart);
+    kv.get(head);
+    kv.position(recStart);
+    pushBatch();
+    kv.clear();
+    final long need = (long) head.length + more;
+    if (need > kv.capacity()) {
+      if (need > Integer.MAX_VALUE - 8) throw new IOException("GpuSorter: record of " + need + " bytes or more");
+      kv = ByteBuffer.allocateDirect((int) Math.min(Integer.MAX_VALUE - 8, Math.max(need, 2L * kv.capacity())))
+          .order(ByteOrder.nativeOrder());
+    }
+    kv.put(head);
+    recStart = 0;
   }
 
   private void pushBatch() throws IOException {
@@ -340,11 +368,15 @@ public class GpuSorter extends ExternalSorter {
       throws IOException;
   private static native void nativeDestroy(long h);
 
-  /** DataOutputStream target that appends to the direct batch buffer. */
-  private static final class ByteBufferOutputStream extends java.io.OutputStream {
-    private final ByteBuffer b;
-    ByteBufferOutputStream(ByteBuffer b) { this.b = b; }
-    @Override public void write(int v) { b.put((byte) v); }
-    @Override public void write(byte[] a, int off, int len) { b.put(a, off, len); }
+  /** DataOutputStream target that appends to the direct batch buffer, making room through overflow(). */
+  private final class BatchOutputStream extends java.io.OutputStream {
+    @Override public void write(int v) throws IOException {
+      if (!kv.hasRemaining()) overflow(1);
+      kv.put((byte) v);
+    }
+    @Override public void write(byte[] a, int off, int len) throws IOException {
+      if (kv.remaining() < len) overflow(len);
+      kv.put(a, off, len);
+    }
   }
 }

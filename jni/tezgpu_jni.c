@@ -196,12 +196,18 @@ JNIEXPORT void JNICALL MERGER(nativeSetCombiner)(JNIEnv *env, jclass cls, jlong 
   failed(env, tezgpu_merge_set_combiner((tezgpu_merger *)(intptr_t)h, combiner));
 }
 
+/* records in the batch; -(bytes) when the next record alone needs more than cap bytes (the stream has not moved) */
 JNIEXPORT jint JNICALL MERGER(nativeNextBatch)(JNIEnv *env, jclass cls, jlong h, jobject out, jint cap, jobject idx, jint idx_cap) {
   (void)cls;
   uint32_t n = 0;
-  if (failed(env, tezgpu_merge_next_batch((tezgpu_merger *)(intptr_t)h, (uint8_t *)addr(env, out), (uint64_t)cap,
-                                          (tezgpu_kv_index *)addr(env, idx), (uint32_t)idx_cap, &n)))
-    return 0;
+  tezgpu_kv_index *ix = (tezgpu_kv_index *)addr(env, idx);
+  int32_t rc = tezgpu_merge_next_batch((tezgpu_merger *)(intptr_t)h, (uint8_t *)addr(env, out), (uint64_t)cap, ix,
+                                       (uint32_t)idx_cap, &n);
+  if (rc == TEZGPU_E_NOMEM && n == 0 && ix) {
+    const uint64_t need = (uint64_t)ix[0].key_len + ix[0].val_len;
+    if (need > (uint64_t)cap && need <= 0x7FFFFFFFu) return -(jint)need;
+  }
+  if (failed(env, rc)) return 0;
   return (jint)n;
 }
 

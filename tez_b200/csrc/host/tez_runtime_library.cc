@@ -848,7 +848,13 @@ struct Input {
     if (eos) return false;
     if (bi + 1 < bn) { bi++; return true; }
     uint32_t n = 0;
-    gpu_check(tezgpu_merge_next_batch(merger, batch.data(), batch.size(), idx.data(), (uint32_t)idx.size(), &n));
+    int32_t rc = tezgpu_merge_next_batch(merger, batch.data(), batch.size(), idx.data(), (uint32_t)idx.size(), &n);
+    if (rc == TEZGPU_E_NOMEM && n == 0 && (uint64_t)idx[0].key_len + idx[0].val_len > batch.size()) {
+      // a record larger than the batch buffer: the stream has not moved, grow to fit it and ask again
+      batch.resize((size_t)idx[0].key_len + idx[0].val_len);
+      rc = tezgpu_merge_next_batch(merger, batch.data(), batch.size(), idx.data(), (uint32_t)idx.size(), &n);
+    }
+    gpu_check(rc);
     if (n == 0) { eos = true; return false; }
     bn = n;
     bi = 0;

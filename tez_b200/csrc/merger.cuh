@@ -523,7 +523,8 @@ class Merger {
       r.runs.nseg = nseg;
       r.runs.rec_size = f.rec_size;
       r.runs.hdr_len = f.len;
-      r.runs.hdr_bytes = f.packed();
+      r.runs.hdr_bytes[0] = f.packed(0);
+      r.runs.hdr_bytes[1] = f.packed(1);
       bool mismatch = false;
       pipe.merge_inputs_plain = true;
       try {
@@ -875,12 +876,26 @@ class Merger {
     if (concat) concat_parse();
     if (cursor >= n || idx_cap == 0) return;
     ensure_kvoff();
+    cap = std::min<uint64_t>(cap, 0xFFFFFFFFull);   // tezgpu_kv_index offsets are 32-bit
     uint32_t *d_cnt = &pipe.d_scratch()->verdict.batch_count;
     k_find_batch<<<1, 1, 0, st>>>(d_kvoff.as<uint64_t>(), (uint32_t)n, (uint32_t)cursor, idx_cap, cap, d_cnt);
     uint32_t cnt = 0;
     TG_CUDA(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaStreamSynchronize(st));
-    TG_CHECK(cnt > 0, TEZGPU_E_NOMEM, "batch buffer smaller than one record");
+    if (cnt == 0) {
+      // the next record alone exceeds cap: report its lengths in idx[0] so that the caller can grow its buffer and
+      // call again; the cursor stays where it is
+      const Records &rec = pipe.state.rec;
+      uint32_t i = 0, kl = 0, vl = 0;
+      TG_CUDA(cudaMemcpyAsync(&i, pipe.state.order + cursor, 4, cudaMemcpyDeviceToHost, st));
+      TG_CUDA(cudaStreamSynchronize(st));
+      TG_CUDA(cudaMemcpyAsync(&kl, rec.key_len + i, 4, cudaMemcpyDeviceToHost, st));
+      TG_CUDA(cudaMemcpyAsync(&vl, rec.val_len + i, 4, cudaMemcpyDeviceToHost, st));
+      TG_CUDA(cudaStreamSynchronize(st));
+      idx[0] = tezgpu_kv_index{0, kl, kl, vl, 0};
+      throw Error(TEZGPU_E_NOMEM, "batch buffer smaller than one record: the next record needs " +
+                                      std::to_string((uint64_t)kl + vl) + " bytes");
+    }
     uint64_t ends[2];
     TG_CUDA(cudaMemcpyAsync(&ends[0], d_kvoff.as<uint64_t>() + cursor, 8, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaMemcpyAsync(&ends[1], d_kvoff.as<uint64_t>() + cursor + cnt, 8, cudaMemcpyDeviceToHost, st));

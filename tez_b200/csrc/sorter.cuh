@@ -64,10 +64,10 @@ struct FixedFraming {
   uint8_t bytes[FRAMING_MAX_LEN];
   uint32_t len;        // framing bytes
   uint32_t rec_size;   // len + klen + vlen
-  // the first 8 framing bytes, little-endian packed
-  uint64_t packed() const {
+  // framing bytes [8 * word, 8 * word + 8), little-endian packed
+  uint64_t packed(uint32_t word = 0) const {
     uint64_t x = 0;
-    for (uint32_t b = 0; b < len && b < 8; b++) x |= (uint64_t)bytes[b] << (8 * b);
+    for (uint32_t b = 8 * word; b < len && b < 8 * word + 8; b++) x |= (uint64_t)bytes[b] << (8 * (b - 8 * word));
     return x;
   }
 };
@@ -130,7 +130,10 @@ static inline FixedEmitPlan plan_fixed_emit(const Records &rec, uint32_t rec_siz
   const uint32_t stride = rec.klen + rec.vlen, cpr = stride / 16;
   // the tile image must fit the image buffer of the source-oriented emit kernels (FE_IMG_BYTES)
   const uint32_t cap = std::max<uint32_t>(1, std::min<uint32_t>(EMIT_MAX_RECS, (FE_IMG_BYTES - 32) / rec_size));
-  if (stride < 16 || stride % 16) return {FixedEmitKernel::General, cap};
+  // Those kernels build a whole tile in that buffer without cutting it: a record that does not fit it with the worst-case
+  // lead, the segment header and the EOF marker takes k_emit<true>, which writes a tile in pieces of any size.
+  // (k_emit_fast4's smaller image is bounded by emit4_max_recs below.)
+  if (stride < 16 || stride % 16 || (uint64_t)rec_size + 15 + 4 + 2 > FE_IMG_BYTES) return {FixedEmitKernel::General, cap};
   if (!rec.key_off && !rec.use_runs && ((uintptr_t)rec.kv & 15u) == 0) {
     // k_emit_fast4's image holds exactly FE4_RUN checksum rounds, so a tile takes as many records as fit it in the
     // worst case (249 of 82 bytes: 1278 chunks, 1280 slots)

@@ -23,7 +23,7 @@ struct RunTable {
   uint32_t nseg;
   uint32_t rec_size;          // framing + key + value bytes
   uint32_t hdr_len;           // framing bytes: vint(klen) vint(vlen)
-  uint64_t hdr_bytes;         // the framing bytes, little-endian packed (checked by k_stage)
+  uint64_t hdr_bytes[2];      // the framing bytes (up to 10), little-endian packed: bytes 0-7, 8-9 (checked by k_stage)
 };
 
 // last segment s with rec_base[s] <= i (rec_base is small and hot in L1)
@@ -245,7 +245,7 @@ __global__ void __launch_bounds__(256) k_stage(Records r, uint32_t *__restrict__
         // the sequential IFile.Reader walk visits exactly these positions iff every one of them carries the fixed
         // framing bytes (same sector as the key: free); a mismatch sends the merge to the general parser
         bool ok = true;
-        for (uint32_t b = 0; b < r.runs.hdr_len; b++) ok &= r.kv[roff + b] == (uint8_t)(r.runs.hdr_bytes >> (8 * b));
+        for (uint32_t b = 0; b < r.runs.hdr_len; b++) ok &= r.kv[roff + b] == (uint8_t)(r.runs.hdr_bytes[b >> 3] >> (8 * (b & 7)));
         if (!ok) atomicOr(error_flag, STAGE_ERR_FRAMING);
       } else {
         record_lookup(r, i, koff, klen, vlen);

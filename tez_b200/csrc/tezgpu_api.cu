@@ -849,6 +849,27 @@ uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks) {
   return total;
 }
 
+int32_t tezgpu_debug_fixed_emit_plan(uint32_t klen, uint32_t vlen, int32_t layout, int32_t *kernel, uint32_t *recs_per_tile) {
+  TG_API_BEGIN
+  TG_CHECK(kernel && recs_per_tile, TEZGPU_E_INVALID, "null argument");
+  TG_CHECK(layout >= 0 && layout <= 2, TEZGPU_E_INVALID, "layout must be 0 (packed, aligned), 1 (explicit offsets) or 2 (run table)");
+  TG_CHECK((uint64_t)klen + vlen > 0 && (uint64_t)klen + vlen + 10 < (1ull << 32), TEZGPU_E_INVALID, "record size out of range");
+  // only the view's shape is read: which layout, and the alignment of kv
+  static const uint64_t some_offsets[1] = {0};
+  Records r;
+  memset(&r, 0, sizeof(r));
+  r.kv = reinterpret_cast<const uint8_t *>(uintptr_t(1) << 12);
+  r.fixed = 1;
+  r.klen = klen;
+  r.vlen = vlen;
+  if (layout == 1) r.key_off = some_offsets;
+  if (layout == 2) r.use_runs = 1;
+  const FixedEmitPlan plan = plan_fixed_emit(r, fixed_framing(klen, vlen).rec_size);
+  *kernel = (int32_t)plan.kernel;
+  *recs_per_tile = plan.recs_per_tile;
+  TG_API_END
+}
+
 }  // extern "C"
 
 #include "merger_api.inl"

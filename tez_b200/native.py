@@ -288,12 +288,17 @@ class GpuMerger:
         return r.value, b.value
 
     def records(self, batch_records=1 << 16, batch_bytes=1 << 24):
-        """Iterates (key, value, is_same_key) like TezRawKeyValueIterator.next/getKey/getValue/isSameKey."""
+        """Iterates (key, value, is_same_key) like TezRawKeyValueIterator.next/getKey/getValue/isSameKey.  The batch
+        buffer grows to fit a record larger than batch_bytes."""
         buf = np.empty(batch_bytes, dtype=np.uint8)
         idx = (KvIndex * batch_records)()
         n = C.c_uint32()
         while True:
-            check(self.L.tezgpu_merge_next_batch(self.h, _ptr(buf), buf.size, idx, batch_records, C.byref(n)))
+            rc = self.L.tezgpu_merge_next_batch(self.h, _ptr(buf), buf.size, idx, batch_records, C.byref(n))
+            if rc == E_NOMEM and n.value == 0 and idx[0].key_len + idx[0].val_len > buf.size:
+                buf = np.empty(idx[0].key_len + idx[0].val_len, dtype=np.uint8)
+                continue
+            check(rc)
             if n.value == 0:
                 return
             raw = buf.tobytes()
