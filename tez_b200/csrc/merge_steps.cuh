@@ -78,25 +78,21 @@ __device__ __forceinline__ int step_compare(int cmp, uint32_t pa, const uint8_t 
   return la < lb ? -1 : (la == lb ? 0 : 1);
 }
 
-// Walks every window with IFile.Reader semantics, one warp per window staging PARSE_WIN bytes in shared memory (as
-// k_parse_segments), lane 0 decoding.  A window ends wherever the bytes end, usually inside a record: the walk stops
-// there.  CUT=false fills scan[] (complete records, the last complete key, EOF, malformed); CUT=true counts the
-// records with (partition, key) < S, S being the last complete key of window *split (none when *split < 0), and
-// fills cut[].
+// Walks every window with IFile.Reader semantics, one warp per window (warp_window_walk).  A window ends wherever the
+// bytes end, usually inside a record: the walk stops there (status REC_PAST_END).  CUT=false fills scan[] (complete
+// records, the last complete key, EOF, malformed); CUT=true counts the records with (partition, key) < S, S being the
+// last complete key of window *split (none when *split < 0), and fills cut[].
+constexpr int STEP_AT_SPLIT = 4;   // k_step_walk<true> stopped at a record with key >= S
 template <bool CUT>
 __global__ void __launch_bounds__(PARSE_WARPS * 32)
     k_step_walk(const uint8_t *__restrict__ win, const StepWin *__restrict__ wins, uint32_t nw, int cmp,
                 StepScan *__restrict__ scan, const int32_t *__restrict__ split, StepCut *__restrict__ cut) {
   __shared__ __align__(16) uint8_t s_win[PARSE_WARPS][PARSE_WIN];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int warp = threadIdx.x >> 5;
   const uint32_t s = blockIdx.x * PARSE_WARPS + warp;
   if (s >= nw) return;
   const StepWin sw = wins[s];
-  ParseWin w;
-  w.seg = win + sw.off;
-  w.win = s_win[warp];
-  w.end = sw.len;
-  w.wbase = 0;
+  const uint8_t *src = win + sw.off;
   const uint8_t *skey = nullptr;
   uint32_t sklen = 0, spart = 0;
   bool bounded = false;
@@ -107,85 +103,42 @@ __global__ void __launch_bounds__(PARSE_WARPS * 32)
     spart = wins[*split].partition;
     bounded = true;
   }
-  uint64_t pos = 0, orig_koff = 0, n = 0, kv = 0, last_koff = 0, stop = 0;
-  int64_t cur_klen = 0, cur_vlen = 0, orig_klen = 0;
-  int status = 0;  // 0 running, 1 EOF markers, 2 malformed, 3 window ends inside a record, 4 record >= S
-  while (true) {
-    for (uint32_t o = lane * 4; o < PARSE_WIN; o += 128) {
-      const uint64_t p = w.wbase + o;
-      uint32_t v = 0;
-      if (p + 4 <= sw.len && (((uintptr_t)(w.seg + p)) & 3u) == 0) v = *reinterpret_cast<const uint32_t *>(w.seg + p);
-      else for (int b = 0; b < 4; b++) if (p + b < sw.len) v |= (uint32_t)w.seg[p + b] << (8 * b);
-      *reinterpret_cast<uint32_t *>(w.win + o) = v;
+  uint64_t orig_koff = 0, orig_klen = 0, n = 0, kv = 0;
+  const WalkEnd e = warp_window_walk(src, sw.len, 0, sw.len, s_win[warp], [&](const RecHdr &h) {
+    uint64_t q = h.pos, ko = orig_koff, kfull = orig_klen;
+    if (h.kl != -2) {
+      if (q + (uint64_t)h.kl > sw.len) return REC_PAST_END;
+      ko = q;
+      kfull = (uint64_t)h.kl;
+      q += (uint64_t)h.kl;
+    } else if (n == 0) {
+      return REC_BAD;   // a window starts at a full record: a repeat needs a previous key
     }
-    __syncwarp();
-    if (lane == 0) {
-      while (status == 0) {
-        uint64_t p2 = pos;
-        int64_t kl = cur_klen, vl = cur_vlen;
-        bool marker = false;
-        int rc;
-        if (cur_klen == -2) {
-          rc = pw_vlong(w, p2, vl);
-          if (rc == 0 && vl == -3) { marker = true; rc = pw_vlong(w, p2, kl); if (rc == 0) rc = pw_vlong(w, p2, vl); }
-        } else {
-          rc = pw_vlong(w, p2, kl);
-          if (rc == 0) rc = pw_vlong(w, p2, vl);
-        }
-        if (rc == 1) { w.wbase = pos & ~(uint64_t)15; break; }
-        const uint64_t rstart = pos + (marker ? 1 : 0);   // a record's own bytes start after a V_END_MARKER
-        if (rc == 2) { status = 3; stop = rstart; break; }
-        if (kl == -1 && vl == -1) { status = 1; stop = rstart; break; }
-        if ((kl != -2 && kl < 0) || vl < 0 || kl > 0x7fffffffll || vl > 0x7fffffffll) { status = 2; break; }
-        uint64_t q = p2, ko = orig_koff;
-        int64_t kfull = orig_klen;
-        if (kl != -2) {
-          if (q + (uint64_t)kl > w.end) { status = 3; stop = rstart; break; }
-          ko = q;
-          kfull = kl;
-          q += (uint64_t)kl;
-        } else if (n == 0) {
-          status = 2;   // a window starts at a full record: a repeat needs a previous key
-          break;
-        }
-        if (q + (uint64_t)vl > w.end) { status = 3; stop = rstart; break; }
-        if (CUT && bounded && kl != -2 &&
-            step_compare(cmp, sw.partition, w.seg + ko, (uint32_t)kfull, spart, skey, sklen) >= 0) {
-          status = 4;
-          stop = rstart;
-          break;
-        }
-        pos = q + (uint64_t)vl;
-        cur_klen = kl;
-        cur_vlen = vl;
-        orig_koff = ko;
-        orig_klen = kfull;
-        n++;
-        kv += (uint64_t)kfull + (uint64_t)vl;
-        last_koff = ko;
-      }
-    }
-    status = __shfl_sync(0xffffffffu, status, 0);
-    w.wbase = __shfl_sync(0xffffffffu, w.wbase, 0);
-    if (status != 0) break;
-    __syncwarp();
-  }
-  if (lane != 0) return;
+    if (q + (uint64_t)h.vl > sw.len) return REC_PAST_END;
+    if (CUT && bounded && h.kl != -2 && step_compare(cmp, sw.partition, src + ko, (uint32_t)kfull, spart, skey, sklen) >= 0)
+      return STEP_AT_SPLIT;
+    orig_koff = ko;
+    orig_klen = kfull;
+    n++;
+    kv += kfull + (uint64_t)h.vl;
+    return REC_OK;
+  });
+  if ((threadIdx.x & 31) != 0) return;
   if (CUT) {
     StepCut c;
-    c.bytes = status == 2 ? 0 : stop;
+    c.bytes = e.status == REC_BAD ? 0 : e.stop;
     c.kv = kv;
     c.nrec = (uint32_t)n;
     c.pad = 0;
     cut[s] = c;
   } else {
     StepScan q;
-    q.last_koff = last_koff;
+    q.last_koff = orig_koff;
     q.kv = kv;
     q.last_klen = (uint32_t)orig_klen;
     q.nrec = (uint32_t)n;
-    q.eof = status == 1;
-    q.bad = status == 2 || (status == 3 && sw.at_end);
+    q.eof = e.status == REC_EOF;
+    q.bad = e.status == REC_BAD || (e.status == REC_PAST_END && sw.at_end);
     scan[s] = q;
   }
 }
@@ -294,7 +247,7 @@ class BoundedMerge {
   int iter = 0;                            // record iterator: 0 not started, 1 streaming, 2 ended
   bool in_step = false, have_counts = false;
   uint64_t pass_n = 0, pass_kv = 0, total_n = 0, total_kv = 0;
-  DeviceBuffer d_win, d_wins, d_scan, d_cut, d_split, d_on_split, d_acc, d_step_raw, d_crcseg, d_crcsd, d_bad;
+  DeviceBuffer d_win, d_wins, d_scan, d_cut, d_split, d_on_split, d_acc, d_crcseg, d_crcsd, d_bad;
   DeviceBuffer d_pieces, d_piece_tc, d_part_raw, d_part_body, d_part_crc;
   std::vector<StepWin> wins;
   std::vector<uint32_t> win_seg;           // window -> caller's segment
@@ -545,22 +498,12 @@ class BoundedMerge {
       const uint32_t nc = (uint32_t)cd.size();
       d_crcsd.ensure(nc * sizeof(SegDesc));
       d_crcseg.ensure(nc * sizeof(StepCrcSeg));
-      d_step_raw.ensure(nc * 4);
       TG_CUDA(cudaMemcpyAsync(d_crcsd.p, cd.data(), nc * sizeof(SegDesc), cudaMemcpyHostToDevice, st));
       TG_CUDA(cudaMemcpyAsync(d_crcseg.p, cs.data(), nc * sizeof(StepCrcSeg), cudaMemcpyHostToDevice, st));
       std::vector<uint32_t> piece_start;
-      uint32_t np = 0;
-      piece_start.resize(nc + 1);
-      for (uint32_t i = 0; i < nc; i++) { piece_start[i] = np; np += (uint32_t)div_up(cd[i].body_end, CRC_PIECE); }
-      piece_start[nc] = np;
-      m.d_piece_start.ensure((size_t)(nc + 1) * 4);
-      m.d_piece_crc.ensure((size_t)np * sizeof(TileCrc));
-      TG_CUDA(cudaMemcpyAsync(m.d_piece_start.p, piece_start.data(), (size_t)(nc + 1) * 4, cudaMemcpyHostToDevice, st));
-      TG_CUDA(cudaMemsetAsync(d_step_raw.p, 0, nc * 4, st));
-      k_crc_pieces<<<np, CRCV_THREADS, 0, st>>>(d_win.as<uint8_t>(), d_crcsd.as<SegDesc>(), m.d_piece_start.as<uint32_t>(), nc,
-                                                d_crc, m.d_piece_crc.as<TileCrc>());
-      k_crc_combine<<<(uint32_t)div_up(np, 256), 256, 0, st>>>(m.d_piece_crc.as<TileCrc>(), np, d_crc, d_step_raw.as<uint32_t>());
-      k_step_crc_fold<<<(uint32_t)div_up(nc, 128), 128, 0, st>>>(d_step_raw.as<uint32_t>(), d_crcseg.as<StepCrcSeg>(), nc, d_crc,
+      m.segment_remainders(d_win.as<uint8_t>(), cd, d_crcsd.as<SegDesc>(), [](const SegDesc &) { return true; }, piece_start, false);
+      // (the m.open() below checks no checksum of its header-less segments, so d_seg_crc is not touched before the fold)
+      k_step_crc_fold<<<(uint32_t)div_up(nc, 128), 128, 0, st>>>(m.d_seg_crc.as<uint32_t>(), d_crcseg.as<StepCrcSeg>(), nc, d_crc,
                                                                 d_acc.as<uint32_t>(), d_bad.as<int>());
       TG_CUDA(cudaGetLastError());
       TG_CUDA(cudaStreamSynchronize(st));   // the host tables above live on this stack

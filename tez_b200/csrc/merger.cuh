@@ -137,145 +137,44 @@ __global__ void k_crc_check(const uint8_t *__restrict__ data, const SegDesc *__r
 }
 
 // ------------------------------------------------------------------------------------------------ parse
-// hadoop WritableUtils.readVLong with bounds; returns false when the buffer ends inside the vint
-__device__ __forceinline__ bool read_vlong_dev(const uint8_t *p, uint64_t &pos, uint64_t end, int64_t &out) {
-  if (pos >= end) return false;
-  int8_t first = (int8_t)p[pos];
-  int len = vint_decode_size((uint8_t)first);
-  if (pos + (uint64_t)len > end) return false;
-  if (len == 1) { out = first; pos += 1; return true; }
-  uint64_t v = 0;
-  for (int i = 1; i < len; i++) v = (v << 8) | p[pos + i];
-  bool neg = first < -120 || (first >= -112 && first < 0);
-  out = neg ? (int64_t)~v : (int64_t)v;
-  pos += len;
-  return true;
-}
-
-// Walks the segments with IFile.Reader semantics (positionToNextRecord / readRawKey / nextRawValue,
-// SORT/IFile.java:877-1000).  One WARP per segment: the 32 lanes stage a 4 KiB window of the body in shared memory with
-// coalesced loads, lane 0 decodes the record headers out of it (key / value bytes are skipped, never read), so a walk
-// step costs tens of cycles instead of a DRAM round trip.  EMIT=false counts records, EMIT=true writes their metadata
-// at rec_base[s]...
-constexpr int PARSE_WARPS = 8;
-constexpr uint32_t PARSE_WIN = 4096;
-
-struct ParseWin {
-  const uint8_t *seg;   // segment base in global memory
-  uint8_t *win;         // this warp's shared window
-  uint64_t wbase;       // segment offset of win[0]
-  uint64_t end;         // body end
-};
-// byte of the segment at offset pos; returns false when pos is outside the staged window (caller reloads)
-__device__ __forceinline__ bool pw_byte(const ParseWin &w, uint64_t pos, uint8_t &out) {
-  if (pos < w.wbase || pos >= w.wbase + PARSE_WIN) return false;
-  out = w.win[pos - w.wbase];
-  return true;
-}
-// readVLong from the window: 0 = ok, 1 = need reload at pos, 2 = runs past the body end
-__device__ __forceinline__ int pw_vlong(const ParseWin &w, uint64_t &pos, int64_t &out) {
-  if (pos >= w.end) return 2;
-  uint8_t first;
-  if (!pw_byte(w, pos, first)) return 1;
-  const int len = vint_decode_size(first);
-  if (pos + (uint64_t)len > w.end) return 2;
-  if (pos + (uint64_t)len > w.wbase + PARSE_WIN) return 1;
-  if (len == 1) { out = (int8_t)first; pos += 1; return 0; }
-  uint64_t v = 0;
-  for (int i = 1; i < len; i++) v = (v << 8) | w.win[pos + i - w.wbase];
-  const int8_t f = (int8_t)first;
-  const bool neg = f < -120 || (f >= -112 && f < 0);
-  out = neg ? (int64_t)~v : (int64_t)v;
-  pos += len;
-  return 0;
-}
-
+// Walks the segments with IFile.Reader semantics, one warp per segment (warp_window_walk).  EMIT=false counts records,
+// EMIT=true writes their metadata at rec_base[s]...
 template <bool EMIT>
 __global__ void __launch_bounds__(PARSE_WARPS * 32)
     k_parse_segments(const uint8_t *__restrict__ data, const SegDesc *__restrict__ segs, uint32_t nseg,
                      uint64_t *__restrict__ counts /*[nseg] records*/, uint64_t *__restrict__ kvbytes /*[nseg]*/,
                      const uint64_t *__restrict__ rec_base, ParseArrays out, int *__restrict__ bad) {
   __shared__ __align__(16) uint8_t s_win[PARSE_WARPS][PARSE_WIN];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int warp = threadIdx.x >> 5;
   const uint32_t s = blockIdx.x * PARSE_WARPS + warp;
   if (s >= nseg) return;
   const SegDesc sd = segs[s];
-  ParseWin w;
-  w.seg = data + sd.off;
-  w.win = s_win[warp];
-  w.end = sd.body_end;
-  w.wbase = sd.body0;
-  // walker state (lane 0)
-  uint64_t pos = sd.body0;
-  int64_t cur_klen = 0, cur_vlen = 0;
-  uint64_t orig_koff = 0;
-  int64_t orig_klen = 0;
-  uint64_t n = 0, bytes = 0;
+  uint64_t orig_koff = 0, orig_klen = 0, n = 0, bytes = 0;
   const uint64_t base = EMIT ? rec_base[s] : 0;
-  int status = 0;  // 0 running, 1 done ok, 2 malformed
-  int phase = 0;   // resume point inside a record: 0 = lengths not read yet
-  while (true) {
-    // ---- stage the window [wbase, wbase + WIN) (clamped to the segment) with coalesced loads
-    {
-      const uint64_t seg_len = sd.len;
-      for (uint32_t o = lane * 4; o < PARSE_WIN; o += 128) {
-        const uint64_t p = w.wbase + o;
-        uint32_t v = 0;
-        if (p + 4 <= seg_len && (((uintptr_t)(w.seg + p)) & 3u) == 0) v = *reinterpret_cast<const uint32_t *>(w.seg + p);
-        else for (int b = 0; b < 4; b++) if (p + b < seg_len) v |= (uint32_t)w.seg[p + b] << (8 * b);
-        *reinterpret_cast<uint32_t *>(w.win + o) = v;
-      }
+  const WalkEnd e = warp_window_walk(data + sd.off, sd.len, sd.body0, sd.body_end, s_win[warp], [&](const RecHdr &h) {
+    uint64_t q = h.pos;
+    if (h.kl != -2) {
+      if (q + (uint64_t)h.kl > sd.body_end) return REC_BAD;
+      orig_koff = q;
+      orig_klen = (uint64_t)h.kl;
+      q += (uint64_t)h.kl;
+    } else if (n == 0) return REC_BAD;  // a repeat needs a previous key
+    if (q + (uint64_t)h.vl > sd.body_end) return REC_BAD;
+    if (EMIT) {
+      // a repeated key points at the bytes of the last full key; its value bytes are not adjacent to it
+      out.key_off[base + n] = sd.off + orig_koff;
+      out.val_off[base + n] = sd.off + q;
+      out.key_len[base + n] = (uint32_t)orig_klen;
+      out.val_len[base + n] = (uint32_t)h.vl;
+      out.tag[base + n] = (s << 1) | (h.kl == -2 ? 1u : 0u);
+      out.partition[base + n] = (int32_t)sd.partition;
     }
-    __syncwarp();
-    if (lane == 0) {
-      while (status == 0) {
-        // record lengths (restartable: nothing is committed until all vints of the record header are decoded)
-        uint64_t p2 = pos;
-        int64_t kl = cur_klen, vl = cur_vlen;
-        int rc;
-        if (cur_klen == -2) {  // previous record was a repeat: a value length (or V_END_MARKER + both lengths) follows
-          rc = pw_vlong(w, p2, vl);
-          if (rc == 0 && vl == -3) { rc = pw_vlong(w, p2, kl); if (rc == 0) rc = pw_vlong(w, p2, vl); }
-        } else {
-          rc = pw_vlong(w, p2, kl);
-          if (rc == 0) rc = pw_vlong(w, p2, vl);
-        }
-        if (rc == 1) { w.wbase = pos & ~(uint64_t)15; break; }  // reload the window at the record start
-        if (rc == 2) { status = 2; break; }
-        if (kl == -1 && vl == -1) { status = 1; break; }           // EOF markers
-        if ((kl != -2 && kl < 0) || vl < 0 || kl > 0x7fffffffll || vl > 0x7fffffffll) { status = 2; break; }
-        pos = p2;
-        cur_klen = kl;
-        cur_vlen = vl;
-        if (kl != -2) {
-          if (pos + (uint64_t)kl > w.end) { status = 2; break; }
-          orig_koff = pos;
-          orig_klen = kl;
-          pos += (uint64_t)kl;
-        } else if (n == 0) { status = 2; break; }  // a repeat needs a previous key
-        if (pos + (uint64_t)vl > w.end) { status = 2; break; }
-        if (EMIT) {
-          // a repeated key points at the bytes of the last full key; its value bytes are not adjacent to it
-          out.key_off[base + n] = sd.off + orig_koff;
-          out.val_off[base + n] = sd.off + pos;
-          out.key_len[base + n] = (uint32_t)orig_klen;
-          out.val_len[base + n] = (uint32_t)vl;
-          out.tag[base + n] = (s << 1) | (kl == -2 ? 1u : 0u);
-          out.partition[base + n] = (int32_t)sd.partition;
-        }
-        n++;
-        bytes += (uint64_t)orig_klen + (uint64_t)vl;
-        pos += (uint64_t)vl;
-      }
-    }
-    (void)phase;
-    status = __shfl_sync(0xffffffffu, status, 0);
-    w.wbase = __shfl_sync(0xffffffffu, w.wbase, 0);
-    if (status != 0) break;
-    __syncwarp();
-  }
-  if (lane == 0) {
-    if (status == 2) atomicExch(bad, (int)s + 1);
+    n++;
+    bytes += orig_klen + (uint64_t)h.vl;
+    return REC_OK;
+  });
+  if ((threadIdx.x & 31) == 0) {
+    if (e.status != REC_EOF) atomicExch(bad, (int)s + 1);
     if (!EMIT) { counts[s] = n; kvbytes[s] = bytes; }
   }
 }
@@ -555,13 +454,27 @@ class Merger {
     have_kvoff = false;
   }
 
-  // Checksums of the segments `need` selects (open() and open_codec()): raw CRC remainders of 64 KiB pieces of each
-  // body, folded per segment into d_seg_crc and compared with the trailer; a mismatch writes segment + 1 to *d_bad.
-  // piece_start receives the host piece table, which must live until the stream has copied it: sync_copy waits for
-  // the copy here, otherwise the caller keeps the table until its next synchronise.  Returns the launches.
+  // Checksums of the segments `need` selects (open() and open_codec()): segment_remainders, then the trailers are
+  // compared; a mismatch writes segment + 1 to *d_bad.  Returns the launches.
   template <typename Need>
   int check_checksums(const uint8_t *bytes, const std::vector<SegDesc> &sd, const SegDesc *d_sd, Need need,
                       std::vector<uint32_t> &piece_start, bool sync_copy, int *d_bad) {
+    const int launches = segment_remainders(bytes, sd, d_sd, need, piece_start, sync_copy);
+    if (!launches) return 0;
+    const uint32_t nseg = (uint32_t)sd.size();
+    k_crc_check<<<(uint32_t)div_up(nseg, 128), 128, 0, pipe.stream>>>(bytes, d_sd, nseg, d_seg_crc.as<uint32_t>(),
+                                                                      DeviceConstants::get(pipe.conf.device).d_crc, d_bad);
+    TG_CUDA(cudaGetLastError());
+    return launches + 1;
+  }
+
+  // Raw CRC remainders of the bodies of the segments `need` selects, from 64 KiB pieces, folded per segment into
+  // d_seg_crc (0 for the others).  piece_start receives the host piece table, which must live until the stream has
+  // copied it: sync_copy waits for the copy here, otherwise the caller keeps the table until its next synchronise.
+  // Returns the launches (none when no segment is selected: d_seg_crc is then left alone).
+  template <typename Need>
+  int segment_remainders(const uint8_t *bytes, const std::vector<SegDesc> &sd, const SegDesc *d_sd, Need need,
+                         std::vector<uint32_t> &piece_start, bool sync_copy) {
     cudaStream_t st = pipe.stream;
     const uint32_t nseg = (uint32_t)sd.size();
     piece_start.resize(nseg + 1);
@@ -581,9 +494,8 @@ class Merger {
     TG_CUDA(cudaMemsetAsync(d_seg_crc.p, 0, (size_t)nseg * 4, st));
     k_crc_pieces<<<np, CRCV_THREADS, 0, st>>>(bytes, d_sd, d_piece_start.as<uint32_t>(), nseg, d_crc, d_piece_crc.as<TileCrc>());
     k_crc_combine<<<(uint32_t)div_up(np, 256), 256, 0, st>>>(d_piece_crc.as<TileCrc>(), np, d_crc, d_seg_crc.as<uint32_t>());
-    k_crc_check<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(bytes, d_sd, nseg, d_seg_crc.as<uint32_t>(), d_crc, d_bad);
     TG_CUDA(cudaGetLastError());
-    return 3;
+    return 2;
   }
 
   // ---- record finding, shared by open() and concat_parse().  Run-table candidate: every body is exactly k records of

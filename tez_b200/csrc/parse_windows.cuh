@@ -29,7 +29,7 @@
 // Cost: guess = one or two rounds of 32 concurrent candidate walks per window (a warp; most die at once, the survivors
 // share their loads), evaluate 1 walk, emit 1 walk; chase ~(#windows / 32) steps per segment + the hand-walked windows.
 #pragma once
-#include "common.cuh"
+#include "ifile_walk.cuh"
 
 namespace tezgpu {
 
@@ -77,45 +77,6 @@ __global__ void k_parse_seg_counts(const PwSeg *__restrict__ segs, uint32_t nseg
   if (s < nseg) counts[s] = wbase[segs[s].win0 + segs[s].nwin] - wbase[segs[s].win0];
 }
 
-// 8 bytes of the segment at offset pos (little endian); bytes past the segment read as zero.  fast: two aligned loads
-__device__ __forceinline__ uint64_t pw_load8(const uint8_t *__restrict__ seg, uint64_t pos, uint64_t seg_len) {
-  if (pos + 16 <= seg_len) {
-    const uintptr_t a = (uintptr_t)(seg + pos);
-    const uint32_t sh = (uint32_t)(a & 7u);
-    const uint64_t *q = reinterpret_cast<const uint64_t *>(a - sh);
-    const uint64_t x = __ldg(q);
-    if (sh == 0) return x;
-    const uint64_t y = __ldg(q + 1);
-    return (x >> (8u * sh)) | (y << (64u - 8u * sh));
-  }
-  uint64_t v = 0;
-  for (uint32_t b = 0; b < 8; b++)
-    if (pos + b < seg_len) v |= (uint64_t)seg[pos + b] << (8u * b);
-  return v;
-}
-
-// hadoop WritableUtils.readVLong at pos (bounded by end); false = runs past `end`
-__device__ __forceinline__ bool pw_vlong(const uint8_t *__restrict__ seg, uint64_t seg_len, uint64_t &pos, uint64_t end,
-                                         int64_t &out) {
-  if (pos >= end) return false;
-  const uint64_t x = pw_load8(seg, pos, seg_len);
-  const int8_t first = (int8_t)(x & 0xFF);
-  if (first >= -112) { out = first; pos += 1; return true; }
-  const int len = vint_decode_size((uint8_t)first);
-  if (pos + (uint64_t)len > end) return false;
-  uint64_t v = 0;
-  if (len <= 8) {
-    for (int i = 1; i < len; i++) v = (v << 8) | ((x >> (8 * i)) & 0xFF);
-  } else {  // 9-byte vlong: the last byte lies outside the 8-byte window
-    for (int i = 1; i < 8; i++) v = (v << 8) | ((x >> (8 * i)) & 0xFF);
-    v = (v << 8) | seg[pos + 8];
-  }
-  const bool neg = first < -120;   // (first >= -112 handled above)
-  out = neg ? (int64_t)~v : (int64_t)v;
-  pos += (uint64_t)len;
-  return true;
-}
-
 struct ParseArrays {
   uint64_t *key_off;
   uint64_t *val_off;
@@ -154,7 +115,7 @@ __device__ __forceinline__ PwWalk pw_walk(const uint8_t *__restrict__ seg, const
   r.early_eof = false;
   if (e == PW_EOF || e == PW_BAD) return r;
   uint64_t pos = e >> 1;
-  int state = (int)(e & 1u);        // 1: the previous record was a repeat (cur_klen == -2 in the walker of merger.cuh)
+  int state = (int)(e & 1u);        // 1: the previous record was a repeat
   // the key a repeat at the start of this window refers to: the last full key before the window (a window may begin
   // inside a run-length encoded run, or with the run's RLE marker right after the key)
   uint64_t orig_koff = carry_off, orig_klen = carry_len;
@@ -162,21 +123,12 @@ __device__ __forceinline__ PwWalk pw_walk(const uint8_t *__restrict__ seg, const
   int status = 0;                   // 0 running, 1 EOF, 2 malformed
   // records that START inside this window belong to it; the last window also owns whatever lies up to the body end
   while (pos < wend || last_win) {
-    uint64_t p2 = pos;
-    int64_t kl = 0, vl = 0;
-    bool ok;
-    if (state == 1) {  // a value length, or V_END_MARKER followed by both lengths
-      ok = pw_vlong(seg, sd.len, p2, sd.body_end, vl);
-      kl = -2;
-      if (ok && vl == -3) { ok = pw_vlong(seg, sd.len, p2, sd.body_end, kl); if (ok) ok = pw_vlong(seg, sd.len, p2, sd.body_end, vl); }
-    } else {
-      ok = pw_vlong(seg, sd.len, p2, sd.body_end, kl);
-      if (ok) ok = pw_vlong(seg, sd.len, p2, sd.body_end, vl);
-    }
-    if (!ok) { status = 2; break; }
-    if (kl == -1 && vl == -1) { status = 1; r.early_eof = p2 != sd.body_end; break; }   // EOF markers
-    if ((kl != -2 && kl < 0) || vl < 0 || kl > 0x7fffffffll || vl > 0x7fffffffll) { status = 2; break; }
-    uint64_t q = p2;
+    RecHdr h;
+    const int d = decode_header(GlobalVlong{seg, sd.len, sd.body_end}, state == 1, pos, h);
+    if (d == REC_EOF) { status = 1; r.early_eof = h.pos != sd.body_end; break; }
+    if (d != REC_OK) { status = 2; break; }
+    const int64_t kl = h.kl, vl = h.vl;
+    uint64_t q = h.pos;
     if (kl != -2) {
       if (q + (uint64_t)kl > sd.body_end) { status = 2; break; }
       orig_koff = q;
