@@ -68,9 +68,9 @@ def sort_combine(P, cmp_kind, combiner, kv, key_off, key_len, val_len, partition
     return dict(file_out=f, index=idx, index_out=ib, combine_input=n_in, combine_output=n_out)
 
 
-def merge_combine(segments, cmp_kind, combiner):
+def merge_combine(segments, cmp_kind, combiner, has_header=True):
     """TezMerger.merge over IFile segments into a combining writer -> (segment bytes, rawLen, partLen)."""
-    res = O.merge(segments, cmp_kind)
+    res = O.merge(segments, cmp_kind, has_header=has_header)
     comb = combine_records([(k, v) for k, v, _ in res["records"]], cmp_kind, combiner)
     return O.write_ifile(comb)
 

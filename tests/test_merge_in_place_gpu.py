@@ -36,105 +36,14 @@ from tez_b200._lib import TezGpuError  # noqa: E402
 import codec_model as CM  # noqa: E402
 import combine_model as CBM  # noqa: E402
 import lz4_model as L4  # noqa: E402
-import sort_order_model as SOM  # noqa: E402
 import unordered_model as UM  # noqa: E402
 import zstd_model as ZS  # noqa: E402
+from merge_model import GUARD, LAYOUTS, POISONS, check_oracle, partition_segments, place, run  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-GUARD = 4096       # controlled bytes before the first and after the last segment of every buffer
 WINDOW = 32768     # the window parser's window (parse_windows.cuh)
 PARSE_WIN = 4096   # the sequential walker's staging window (merger.cuh)
-
-
-# ------------------------------------------------------------------------------------------------ placement
-# A layout maps n segments to (address order, per-segment slot).  A slot is (buffer, residue, gap): the segment starts
-# `gap` bytes after the previous segment of its buffer, then rounded up to 16 plus `residue`; residue None starts it
-# exactly `gap` bytes after the previous one (back to back when 0).
-def _layout_aligned(n):
-    """every start 16-aligned, addresses descending against the caller's order"""
-    return list(range(n))[::-1], [(0, 0, 16 * (1 + i % 4)) for i in range(n)]
-
-
-def _layout_residues(n):
-    """residues 1..15, one per segment, in two allocations, addresses in a shuffled order"""
-    order = list(range(n))
-    random.Random(n).shuffle(order)
-    return order, [(i % 2, 1 + i % 15, 16 + (7 * i) % 48) for i in range(n)]
-
-
-def _layout_packed(n):
-    """back to back from an odd offset, in the caller's order (each start inherits the previous lengths)"""
-    return list(range(n)), [(0, 3 if i == 0 else None, 0) for i in range(n)]
-
-
-LAYOUTS = {"aligned": _layout_aligned, "residues": _layout_residues, "packed": _layout_packed}
-POISONS = ["ff", "body", "random"]
-
-
-def _body(seg):
-    return bytes(seg[4:]) if bytes(seg[:3]) == b"TIF" else bytes(seg)
-
-
-def place(segs, layout, poison, seed=0):
-    """Copies segs into cuda:0 buffers laid out by `layout`, every other byte of the buffers set by `poison`.  Returns
-    ([(ptr, len)] in the caller's order, the buffers to keep alive)."""
-    n = len(segs)
-    order, slots = LAYOUTS[layout](n)
-    starts, ends = [0] * n, {}
-    for i in order:
-        b, res, gap = slots[i]
-        end = ends.get(b)
-        if end is None:
-            start = GUARD + (res or 0)
-        elif res is None:
-            start = end + gap
-        else:
-            start = (end + gap + 15) // 16 * 16 + res
-        starts[i] = start
-        ends[b] = start + len(segs[i])
-    bufs = {}
-    for b, end in ends.items():
-        size = end + GUARD
-        rng = np.random.default_rng(seed * 31 + b)
-        mine = [i for i in order if slots[i][0] == b]
-        if poison == "ff":
-            img = np.full(size, 0xFF, dtype=np.uint8)
-        elif poison == "random":
-            img = rng.integers(0, 256, size, dtype=np.uint8)
-        else:
-            donor = np.frombuffer(_body(segs[(mine[0] + 1) % n]), dtype=np.uint8)
-            img = np.resize(donor, size).copy()
-            for i in mine:   # right behind every segment: the start of another segment's records
-                d = np.frombuffer(_body(segs[(i + 1) % n]), dtype=np.uint8)
-                e = starts[i] + len(segs[i])
-                img[e:e + min(len(d), size - e)] = d[:size - e]
-        for i in mine:
-            img[starts[i]:starts[i] + len(segs[i])] = np.frombuffer(bytes(segs[i]), dtype=np.uint8)
-        bufs[b] = torch.from_numpy(img).to("cuda:0")
-    return [(bufs[slots[i][0]].data_ptr() + starts[i], len(segs[i])) for i in range(n)], bufs
-
-
-# ------------------------------------------------------------------------------------------------ merge and compare
-def run(segs, device_ptrs=False, P=1, parts=None, check=True, writer_rle=False, combiner=T.COMBINE_NONE, **kw):
-    """Everything a merge hands out: mode, the merged IFile (P = 1), write_partitions_device's bytes and index, counts
-    and records (without a combiner)."""
-    out = {}
-    with T.GpuMerger(segs, device_ptrs=device_ptrs, partitions=parts, num_partitions=P, combiner=combiner, **kw) as m:
-        if not check:
-            m.set_check_for_same_keys(False)
-        out["mode"] = m.parse_info()[0]
-        if P == 1:
-            out["ifile"] = m.write_ifile(rle=writer_rle)[0]
-        cap = m.output_bound()
-        d = torch.full((cap + 32,), 0xA5, dtype=torch.uint8, device="cuda:0")
-        n, index, _ = m.write_partitions_device(d.data_ptr(), cap, rle=writer_rle)
-        out["file"] = d[:n].cpu().numpy().tobytes()
-        out["index"] = index.tolist()
-        if not combiner:
-            out["counts"] = m.counts()
-            out["records"] = list(m.records(batch_records=1 << 14, batch_bytes=1 << 22))
-    return out
 
 
 def check_in_place(segs, mode, layouts=tuple(LAYOUTS), poisons=tuple(POISONS), **kw):
@@ -149,55 +58,6 @@ def check_in_place(segs, mode, layouts=tuple(LAYOUTS), poisons=tuple(POISONS), *
             for key in host:
                 assert dev[key] == host[key], "%s differs from the host merge (layout %s, poison %s)" % (key, layout, poison)
     return host
-
-
-def partition_segments(out):
-    """[IFile segment bytes or b""] per partition of a write_partitions_device result"""
-    return [out["file"][s:s + n] for s, _, n in out["index"]]
-
-
-def stable_model(segs, parts, P, cmp, has_header=True):
-    """The device's merge contract: per partition, the stable sort of its segments' records (caller order) by key."""
-    res = []
-    for p in range(P):
-        recs = [(k, v) for s, q in zip(segs, parts or [0] * len(segs)) if q == p
-                for _, k, v in O.read_ifile(bytes(s), has_header=has_header)]
-        res.append(sorted(recs, key=lambda r: SOM.content(cmp, r[0])))
-    return res
-
-
-def _canon(records):
-    """IFile records grouped by key: (key, key states, values sorted).  The oracle's order inside a group of equal keys
-    from different segments is its heap's (parity unpinned, DESIGN.md section 6); keys, states and values are pinned."""
-    out = []
-    for ks, k, v in records:
-        if out and out[-1][0] == k:
-            out[-1][1].append(ks)
-            out[-1][2].append(v)
-        else:
-            out.append((k, [ks], [v]))
-    return [(k, s, sorted(v)) for k, s, v in out]
-
-
-def check_oracle(host, segs, parts, P, cmp, check=True, writer_rle=False, has_header=True):
-    """host merge vs the oracle's TezMerger (factor 100) per partition, and -- every value is its record's global
-    index -- record for record against the stable merge model"""
-    got = partition_segments(host)
-    model = stable_model(segs, parts, P, cmp, has_header)
-    for p in range(P):
-        mine = [bytes(s) for s, q in zip(segs, parts or [0] * len(segs)) if q == p]
-        exp = O.merge(mine, cmp, factor=100, check_for_same_keys=check, writer_rle=writer_rle, has_header=has_header)
-        assert len(got[p]) == len(exp["ifile"]), "partition %d: %d bytes, oracle %d" % (p, len(got[p]), len(exp["ifile"]))
-        mine_recs = O.read_ifile(got[p])
-        assert _canon(mine_recs) == _canon(O.read_ifile(exp["ifile"])), "partition %d differs from the oracle" % p
-        assert [(k, v) for _, k, v in mine_recs] == model[p], "partition %d: not the stable merge" % p
-    if P == 1:
-        assert host["ifile"] == host["file"]
-        exp = O.merge([bytes(s) for s in segs], cmp, factor=100, check_for_same_keys=check, writer_rle=writer_rle,
-                      has_header=has_header)
-        assert [(k, s) for k, _, s in host["records"]] == [(k, s) for k, _, s in exp["records"]]
-        assert [(k, v) for k, v, _ in host["records"]] == model[0]
-    assert host["counts"][0] == len(host["records"]) == sum(len(m) for m in model)
 
 
 # ------------------------------------------------------------------------------------------------ inputs

@@ -9,9 +9,10 @@ import numpy as np
 import pytest
 
 from oracle import tez_oracle as O
+import merge_scenarios as MS
 import tez_b200 as T
-from tez_b200.runtime_library import (BYTES_WRITABLE, INT_WRITABLE, TEXT, TEZ_BYTES_COMPARATOR, InputContext, LocalOutput,
-                                      OrderedGroupedKVInput, OrderedPartitionedKVOutput, OutputContext,
+from tez_b200.runtime_library import (BYTES_WRITABLE, INT_WRITABLE, LONG_WRITABLE, TEXT, TEZ_BYTES_COMPARATOR, InputContext,
+                                      LocalOutput, OrderedGroupedKVInput, OrderedPartitionedKVOutput, OutputContext,
                                       empty_partitions_from_payload, parse_proto)
 
 pytestmark = pytest.mark.gpu
@@ -96,6 +97,39 @@ def test_multiple_spills_and_final_merge_match_single_sort(tmp_path):
     assert out.counter("ADDITIONAL_SPILLS_BYTES_READ") > 0 and out.counter("ADDITIONAL_SPILLS_BYTES_WRITTEN") > 0
     assert out.counter("OUTPUT_BYTES_PHYSICAL") == len(exp["file_out"])
     assert not os.path.exists(str(tmp_path / "output" / (out.context.unique_identifier + "_0")))   # spill dirs removed
+
+
+@pytest.mark.parametrize("key_class,comparator_class,cmp", [
+    (TEXT, None, O.CMP_TEXT), (INT_WRITABLE, None, O.CMP_INT), (LONG_WRITABLE, None, O.CMP_LONG),
+    (BYTES_WRITABLE, TEZ_BYTES_COMPARATOR, O.CMP_BYTES), (BYTES_WRITABLE, None, O.CMP_BYTESWRITABLE)],
+    ids=["text", "int", "long", "byteswritable-tezbytes", "byteswritable"])
+def test_final_merge_of_every_key_class_matches_single_sort(tmp_path, key_class, comparator_class, cmp):
+    """The final merge of 4+ spills with the device comparator of every key class: the palette keys of
+    tests/merge_scenarios.py (raw byte order and comparator order disagree) and random keys, each once, value = f(key),
+    so file.out and file.out.index equal the oracle's single sort with that comparator"""
+    rng = random.Random(cmp)
+    keys = list(MS.PALETTES[cmp])
+    seen = set(keys)
+    while len(keys) < 70000:
+        k = MS._random_key(rng, cmp, False)
+        if k not in seen:
+            seen.add(k)
+            keys.append(k)
+    rng.shuffle(keys)
+    recs = [(k, zlib.crc32(k).to_bytes(4, "big") * 15) for k in keys]
+    P = 8
+    conf = {"tez.runtime.key.class": key_class, "tez.runtime.io.sort.mb": 1}
+    if comparator_class:
+        conf["tez.runtime.key.comparator.class"] = comparator_class
+    out, events = _run_output(tmp_path, conf, recs, P)
+    assert out.num_spills >= 4
+    kv = b"".join(k + v for k, v in recs)
+    ko = np.cumsum([0] + [len(k) + len(v) for k, v in recs[:-1]])
+    exp = O.pipelined_sort(O.sorter_conf(P, cmp_kind=cmp), kv, ko, [len(k) for k, _ in recs], [len(v) for _, v in recs])
+    assert not exp["rle_used"]
+    assert open(out.final_output_file, "rb").read() == exp["file_out"]
+    assert open(out.final_index_file, "rb").read() == exp["index_out"]
+    assert out.counter("OUTPUT_RECORDS") == len(recs) and out.counter("SPILLED_RECORDS") == 2 * len(recs)
 
 
 @pytest.mark.parametrize("dup_pct", [1, 5, 9, 30])
