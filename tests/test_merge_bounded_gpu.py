@@ -187,6 +187,26 @@ def test_device_output_and_counts_before_the_stream_on_several_steps():
         assert sum(1 for _ in m.records()) == n          # the iterator starts again after a write
 
 
+def test_several_steps_written_into_the_callers_buffer():
+    """tezgpu_merge_write_ifile into a buffer of the caller (the wrapper writes a merge of several steps through a file):
+    a buffer that fits receives the file's bytes, one a byte short fails with TEZGPU_E_NOMEM"""
+    import ctypes as C
+    segs, _ = O.gen_c3_segments(8, 256 << 10, seed=2, threads=8, id_bits=12)
+    segs = [s.tobytes() for s in segs]
+    with T.GpuMerger(segs, comparator=T.CMP_TEXT, device_budget=FLOOR) as m:
+        exp, raw_exp, part_exp, _ = m.write_ifile()
+        assert m.bounded_info()[0] > 1
+
+        def write(cap):
+            buf, raw, part = (C.c_uint8 * cap)(), C.c_int64(), C.c_int64()
+            rc = m.L.tezgpu_merge_write_ifile(m.h, None, C.addressof(buf), cap, 0, C.byref(raw), C.byref(part), None)
+            return rc, bytes(buf), raw.value, part.value
+
+        assert write(len(exp)) == (0, exp, raw_exp, part_exp)
+        assert write(len(exp) - 1)[0] == T.E_NOMEM
+        assert m.L.tezgpu_last_error().decode() == "output buffer too small for the merged segment"
+
+
 def test_scale_digest_equals_the_unbounded_merge():
     """about 1 GiB of config-3 segments at a 256 MiB budget"""
     import torch

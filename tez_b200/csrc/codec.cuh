@@ -95,10 +95,8 @@ __global__ void k_zfinish_blocks(const ZSeg *__restrict__ segs, uint32_t P, cons
   if (!s.nchunks) return;
   uint8_t *o = out + s.zstart;
   o[0] = 'T'; o[1] = 'I'; o[2] = 'F'; o[3] = 1;
-  const uint64_t region = s.zlen - 8;
-  const uint32_t crc = seg_crc[p] ^ crc_shift_bytes(t, 0xFFFFFFFFu, region) ^ 0xFFFFFFFFu;
-  uint8_t *tr = o + s.zlen - 4;
-  tr[0] = (uint8_t)(crc >> 24); tr[1] = (uint8_t)(crc >> 16); tr[2] = (uint8_t)(crc >> 8); tr[3] = (uint8_t)crc;
+  const uint32_t crc = crc_from_raw(t, seg_crc[p], s.zlen - 8);
+  store_be32(o + s.zlen - 4, crc);
 }
 
 // The uncompressed file is in z_img with its index raw_index (start, rawLength, partLength per partition).  Every

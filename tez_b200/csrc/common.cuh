@@ -33,6 +33,14 @@ struct Error : public std::runtime_error {
 static inline uint64_t div_up(uint64_t a, uint64_t b) { return (a + b - 1) / b; }
 static inline uint64_t align_up(uint64_t a, uint64_t b) { return div_up(a, b) * b; }
 
+// 4-byte big-endian words at any alignment (IFile checksum trailers, LZ4 block headers)
+__host__ __device__ __forceinline__ uint32_t load_be32(const uint8_t *p) {
+  return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3];
+}
+__host__ __device__ __forceinline__ void store_be32(uint8_t *p, uint32_t v) {
+  p[0] = (uint8_t)(v >> 24); p[1] = (uint8_t)(v >> 16); p[2] = (uint8_t)(v >> 8); p[3] = (uint8_t)v;
+}
+
 // Lets kernel Kern take `bytes` of dynamic shared memory on `device`, the current device.  The limit is an attribute
 // per device: it is set once per kernel and device (racing first calls set the same value); later calls load one flag.
 template <auto Kern>

@@ -32,14 +32,8 @@ __global__ void k_concat_inputs(const uint8_t *__restrict__ data, const SegDesc 
   const uint64_t body = sd.body_end - sd.body0;   // >= 2: open() refuses shorter segments
   const uint8_t *b = data + sd.off + sd.body0;
   if (b[body - 2] != 0xFF || b[body - 1] != 0xFF) atomicExch(bad_eof, (int)s + 1);
-  uint32_t body_raw;
-  if ((sd.has_header & 2u) && !(sd.has_header & 4u)) {
-    const uint8_t *tr = data + sd.off + sd.body_end;
-    const uint32_t stored = ((uint32_t)tr[0] << 24) | ((uint32_t)tr[1] << 16) | ((uint32_t)tr[2] << 8) | tr[3];
-    body_raw = stored ^ 0xFFFFFFFFu ^ crc_shift_bytes(t, 0xFFFFFFFFu, body);
-  } else {
-    body_raw = seg_crc[s];
-  }
+  const bool trusted = (sd.has_header & 2u) && !(sd.has_header & 4u);
+  const uint32_t body_raw = trusted ? crc_to_raw(t, load_be32(data + sd.off + sd.body_end), body) : seg_crc[s];
   TileCrc c;
   c.raw = concat_records_raw(body_raw, *t);
   c.p = sd.partition;
@@ -123,9 +117,8 @@ __global__ void k_concat_finish(const CatPart *__restrict__ parts, uint32_t P, c
   o[4 + c.rec] = 0xFF;
   o[5 + c.rec] = 0xFF;
   const uint64_t body = c.rec + 2;
-  const uint32_t crc = (seg_crc[p] ^ t->eof_raw) ^ crc_shift_bytes(t, 0xFFFFFFFFu, body) ^ 0xFFFFFFFFu;
-  uint8_t *tr = o + 4 + body;
-  tr[0] = (uint8_t)(crc >> 24); tr[1] = (uint8_t)(crc >> 16); tr[2] = (uint8_t)(crc >> 8); tr[3] = (uint8_t)crc;
+  const uint32_t crc = crc_from_raw(t, seg_crc[p] ^ t->eof_raw, body);
+  store_be32(o + 4 + body, crc);
 }
 
 // ------------------------------------------------------------------------------------------------ record iterator
@@ -279,18 +272,15 @@ inline void Merger::concat_parse() {
   const uint32_t nseg = (uint32_t)segs.size();
   bool fixed_ok = count_fixed_records(nseg, 8);
   if (fixed_ok) {
-    d_rec_base.ensure((size_t)(nseg + 2) * 8);
-    TG_CUDA(cudaMemcpyAsync(d_rec_base.p, h_rec_base.data(), (size_t)(nseg + 1) * 8, cudaMemcpyHostToDevice, st));
-    const ParseArrays pa = record_arrays(n);
     const FixedFraming f = fixed_framing(fixed_klen, fixed_vlen);
     int *d_bad = &pipe.d_scratch()->verdict.error;
     TG_CUDA(cudaMemsetAsync(d_bad, 0, 4, st));
     int bad = 0;
+    launches += fill_fixed_arrays();
     if (n) {
-      const uint32_t grid = (uint32_t)std::min<uint64_t>(div_up(n, 256), (uint64_t)pipe.num_sms * 16);
-      k_fill_fixed_arrays<<<grid, 256, 0, st>>>(d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), fixed_klen, fixed_vlen, f.len, pa);
-      k_concat_check_fixed<<<grid, 256, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), f.rec_size, f.len, f.packed(), d_bad);
-      launches += 2;
+      k_concat_check_fixed<<<record_grid(), 256, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), f.rec_size,
+                                                          f.len, f.packed(), d_bad);
+      launches++;
       TG_CUDA(cudaGetLastError());
       TG_CUDA(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
     }
@@ -309,7 +299,7 @@ inline void Merger::concat_parse() {
   pipe.same.ensure(n ? n : 1);
   TG_CUDA(cudaMemsetAsync(pipe.same.p, 0, n ? n : 1, st));
   if (n) {
-    k_iota<<<(uint32_t)std::min<uint64_t>(div_up(n, 256), (uint64_t)pipe.num_sms * 16), 256, 0, st>>>(d_order.as<uint32_t>(), (uint32_t)n);
+    k_iota<<<record_grid(), 256, 0, st>>>(d_order.as<uint32_t>(), (uint32_t)n);
     launches++;
   }
   TG_CUDA(cudaGetLastError());

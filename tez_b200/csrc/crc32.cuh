@@ -188,4 +188,14 @@ __device__ __forceinline__ uint32_t crc_shift_bytes(const CrcTables *__restrict_
   return crc;
 }
 
+// The IFile checksum trailer is the standard CRC-32 of the `len` body bytes (stored big-endian after them).  From the
+// body's raw remainder (zero initial value, no final xor): crc = raw xor (0xFFFFFFFF * x^(8*len)) xor 0xFFFFFFFF.
+__device__ __forceinline__ uint32_t crc_from_raw(const CrcTables *__restrict__ t, uint32_t raw, uint64_t len) {
+  return raw ^ crc_shift_bytes(t, 0xFFFFFFFFu, len) ^ 0xFFFFFFFFu;
+}
+// the inverse: the raw remainder of a body from its stored checksum
+__device__ __forceinline__ uint32_t crc_to_raw(const CrcTables *__restrict__ t, uint32_t crc, uint64_t len) {
+  return crc ^ 0xFFFFFFFFu ^ crc_shift_bytes(t, 0xFFFFFFFFu, len);
+}
+
 }  // namespace tezgpu

@@ -515,7 +515,7 @@ __global__ void k_zfinish(const ZSeg *__restrict__ segs, uint32_t P, const uint3
     adler = z_adler_combine(adler, cadler[s.chunk0 + k], z_min64(ZCHUNK, s.body_len - a));
   }
   uint8_t *tr = o + s.zlen - 8;
-  tr[0] = (uint8_t)(adler >> 24); tr[1] = (uint8_t)(adler >> 16); tr[2] = (uint8_t)(adler >> 8); tr[3] = (uint8_t)adler;
+  store_be32(tr, adler);
   // checksummed bytes = 78 01 | chunks | adler: the chunks' raw remainders are in seg_crc (shifted past the adler)
   const uint64_t region = s.zlen - 8;
   uint32_t hraw = 0;
@@ -524,8 +524,7 @@ __global__ void k_zfinish(const ZSeg *__restrict__ segs, uint32_t P, const uint3
   uint32_t araw = 0;
   for (int b = 0; b < 4; b++) araw = t->slice[0][(araw ^ tr[b]) & 0xFF] ^ (araw >> 8);
   uint32_t raw = seg_crc[p] ^ crc_shift_bytes(t, hraw, region - 2) ^ araw;
-  const uint32_t crc = raw ^ crc_shift_bytes(t, 0xFFFFFFFFu, region) ^ 0xFFFFFFFFu;
-  tr[4] = (uint8_t)(crc >> 24); tr[5] = (uint8_t)(crc >> 16); tr[6] = (uint8_t)(crc >> 8); tr[7] = (uint8_t)crc;
+  store_be32(tr + 4, crc_from_raw(t, raw, region));
 }
 
 }  // namespace tezgpu

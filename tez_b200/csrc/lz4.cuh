@@ -69,8 +69,6 @@ static inline const char *l4_err_name(int32_t e) {
   }
 }
 
-Z_HD uint32_t l4_be32(const uint8_t *p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
-Z_HD void l4_put_be32(uint8_t *p, uint32_t v) { p[0] = (uint8_t)(v >> 24); p[1] = (uint8_t)(v >> 16); p[2] = (uint8_t)(v >> 8); p[3] = (uint8_t)v; }
 Z_HD uint32_t l4_min(uint32_t a, uint32_t b) { return a < b ? a : b; }
 // bytes after the token that a literal / match length n (its nibble part included) takes: 0 below 15
 Z_HD uint32_t l4_ext_bytes(uint32_t n) { return n >= 15 ? (n - 15) / 255 + 1 : 0; }
@@ -198,8 +196,8 @@ Z_HD void l4_plan(L4Shared &sh) {
 
 // Thread 0, after the plan: the last sequence's token and literal length, the block and chunk lengths before the chunk
 Z_HD void l4_write_frame(const L4Shared &sh, uint8_t *slot) {
-  l4_put_be32(slot, sh.clen);
-  l4_put_be32(slot + 4, sh.bytes);
+  store_be32(slot, sh.clen);
+  store_be32(slot + 4, sh.bytes);
   uint8_t *out = slot + 8;
   out[sh.fin_out] = (uint8_t)(l4_min(sh.fin_len, 15) << 4);
   l4_put_ext(out + sh.fin_out + 1, sh.fin_len);
@@ -321,13 +319,13 @@ Z_HD int32_t l4_decompress(const uint8_t *in, uint64_t n, uint8_t *out, uint64_t
   int32_t rc = L4_OK;
   while (op < expect) {
     if (ip + 4 > n) { rc = ip == n ? L4_ERR_LENGTH : L4_ERR_HEADER; break; }
-    const uint32_t raw = l4_be32(in + ip);
+    const uint32_t raw = load_be32(in + ip);
     ip += 4;
     if (raw == 0 || raw > 0x7FFFFFFFu || raw > expect - op) { rc = L4_ERR_BLOCK; break; }
     uint32_t got = 0;
     while (got < raw) {
       if (ip + 4 > n) { rc = L4_ERR_HEADER; break; }
-      const uint32_t c = l4_be32(in + ip);
+      const uint32_t c = load_be32(in + ip);
       ip += 4;
       if (c > L4_CHUNK_CAP || c > n - ip) { rc = L4_ERR_CHUNK; break; }
       uint32_t r = 0;
@@ -362,7 +360,7 @@ __global__ void k_l4walk(const ZInSeg *__restrict__ segs, uint32_t nseg, uint32_
   bool ok = true;
   while (ip < n) {
     if (ip + 8 > n) { ok = false; break; }
-    const uint32_t raw = l4_be32(in + ip), c = l4_be32(in + ip + 4);
+    const uint32_t raw = load_be32(in + ip), c = load_be32(in + ip + 4);
     ip += 8;
     if (raw == 0 || raw > L4_CHUNK_CAP || raw > z.body - op || c > L4_CHUNK_CAP || c > n - ip) { ok = false; break; }
     if (FILL) {

@@ -190,7 +190,7 @@ __global__ void k_step_crc_fold(const uint32_t *__restrict__ raw, const StepCrcS
   const StepCrcSeg c = cs[w];
   const uint32_t a = crc_shift_bytes(t, acc[c.seg], c.len) ^ raw[w];
   acc[c.seg] = a;
-  if (c.last && (a ^ crc_shift_bytes(t, 0xFFFFFFFFu, c.total) ^ 0xFFFFFFFFu) != c.stored) atomicExch(bad, (int)c.seg + 1);
+  if (c.last && crc_from_raw(t, a, c.total) != c.stored) atomicExch(bad, (int)c.seg + 1);
 }
 
 // One piece = the records R one step wrote for one partition, between its TIF\0 header and its FF FF EOF markers.  Its
@@ -208,7 +208,7 @@ __global__ void k_stitch_raw(const StitchPiece *__restrict__ pc, uint32_t n, con
   if (i >= n) return;
   const StitchPiece c = pc[i];
   TileCrc tc;
-  tc.raw = c.trailer ^ 0xFFFFFFFFu ^ crc_shift_bytes(t, 0xFFFFFFFFu, c.body + 2) ^ t->eof_raw;
+  tc.raw = crc_to_raw(t, c.trailer, c.body + 2) ^ t->eof_raw;
   tc.p = c.partition;
   tc.after = c.after;
   out[i] = tc;
@@ -218,7 +218,7 @@ __global__ void k_stitch_finish(const uint32_t *__restrict__ part_raw, const uin
                                 const CrcTables *__restrict__ t, uint32_t *__restrict__ crc) {
   const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= P) return;
-  crc[p] = (part_raw[p] ^ t->eof_raw) ^ crc_shift_bytes(t, 0xFFFFFFFFu, part_body[p] + 2) ^ 0xFFFFFFFFu;
+  crc[p] = crc_from_raw(t, part_raw[p] ^ t->eof_raw, part_body[p] + 2);
 }
 
 // ------------------------------------------------------------------------------------------------ host loop
@@ -273,10 +273,8 @@ class BoundedMerge {
     for (uint32_t s = 0; s < nseg; s++) {
       const tezgpu_segment &sg = segs[s];
       TG_CHECK(!(sg.flags & TEZGPU_SEG_DEVICE), TEZGPU_E_INVALID, "tezgpu_merge_open_bounded takes host segments only");
-      TG_CHECK(sg.data || sg.len == 0, TEZGPU_E_INVALID, "null segment");
+      m.check_segment(sg);
       const bool hdr = sg.flags & TEZGPU_SEG_HAS_HEADER;
-      TG_CHECK(sg.len >= (hdr ? 10u : 6u), TEZGPU_E_FORMAT, "IFile segment shorter than an empty segment");
-      TG_CHECK((int)sg.partition < std::max(1, m.pipe.conf.num_partitions), TEZGPU_E_INVALID, "segment partition out of range");
       const uint8_t *d = static_cast<const uint8_t *>(sg.data);
       if (hdr) {
         TG_CHECK(d[0] == 'T' && d[1] == 'I' && d[2] == 'F', TEZGPU_E_FORMAT, "Not a valid ifile header (segment " + std::to_string(s) + ")");
@@ -284,8 +282,7 @@ class BoundedMerge {
       }
       body0[s] = hdr ? 4 : 0;
       body_end[s] = sg.len - 4;
-      const uint8_t *tr = d + body_end[s];
-      stored[s] = ((uint32_t)tr[0] << 24) | ((uint32_t)tr[1] << 16) | ((uint32_t)tr[2] << 8) | tr[3];
+      stored[s] = load_be32(d + body_end[s]);
       check_crc[s] = hdr && !(sg.flags & TEZGPU_SEG_VERIFIED);
       total += align_up(sg.len, 16);
     }
@@ -605,14 +602,9 @@ class BoundedMerge {
     std::vector<int64_t> idx((size_t)P * 3);
     while ((in_step = next_step())) {
       if (!m.n) continue;
-      m.d_out.ensure(m.output_bound());
       uint64_t len = 0;
       tezgpu_stats s;
-      m.write_partitions_device(m.d_out.as<uint8_t>(), m.d_out.cap, rle, &len, idx.data(), &s);
-      m.h_out.ensure(len + 16);
-      TG_CUDA(cudaMemcpyAsync(m.h_out.p, m.d_out.p, len, cudaMemcpyDeviceToHost, st));
-      TG_CUDA(cudaStreamSynchronize(st));
-      const uint8_t *img = m.h_out.as<uint8_t>();
+      const uint8_t *img = m.write_host(rle, nullptr, 0, &len, idx.data(), &s);
       for (int p = 0; p < P; p++) {
         const int64_t seglen = idx[3 * p + 2];
         if (seglen <= 10) continue;   // no records of p in this step
@@ -626,11 +618,10 @@ class BoundedMerge {
         }
         const uint64_t body = (uint64_t)seglen - 10;
         out.insert(out.end(), seg + 4, seg + 4 + body);
-        const uint8_t *tr = seg + seglen - 4;
         StitchPiece pc;
         pc.body = body;
         pc.after = 0;
-        pc.trailer = ((uint32_t)tr[0] << 24) | ((uint32_t)tr[1] << 16) | ((uint32_t)tr[2] << 8) | tr[3];
+        pc.trailer = load_be32(seg + seglen - 4);
         pc.partition = (uint32_t)p;
         pieces.push_back(pc);
         part_body[p] += body;
@@ -672,11 +663,8 @@ class BoundedMerge {
     std::vector<uint32_t> crc((size_t)P);
     TG_CUDA(cudaMemcpyAsync(crc.data(), d_part_crc.p, (size_t)P * 4, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaStreamSynchronize(st));
-    for (int p = 0; p < P; p++) {
-      if (!index[3 * p + 2]) continue;
-      uint8_t *tr = out.data() + index[3 * p] + index[3 * p + 2] - 4;
-      tr[0] = (uint8_t)(crc[p] >> 24); tr[1] = (uint8_t)(crc[p] >> 16); tr[2] = (uint8_t)(crc[p] >> 8); tr[3] = (uint8_t)crc[p];
-    }
+    for (int p = 0; p < P; p++)
+      if (index[3 * p + 2]) store_be32(out.data() + index[3 * p] + index[3 * p + 2] - 4, crc[p]);
     for (int p = 0; p < P; p++) sum.output_bytes_with_overhead += index[3 * p + 1];
     sum.output_bytes_physical = sum.file_out_bytes = (int64_t)out.size();
     sum.num_spills = 1;

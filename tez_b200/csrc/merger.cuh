@@ -6,6 +6,7 @@
 // (TezMerger.writeFile, :215-245) with REPEAT_KEY run-length encoding of equal adjacent keys.
 #pragma once
 #include <algorithm>
+#include <tuple>
 #include <vector>
 
 #include "sorter.cuh"
@@ -129,11 +130,7 @@ __global__ void k_crc_check(const uint8_t *__restrict__ data, const SegDesc *__r
   // in-memory segments carry no checksum stream (OG/InMemoryReader.java:142-254); segments the transport verified
   // while copying them (IFile.Reader.readToMemory, SORT/IFile.java:764-809) are not verified twice
   if (sd.has_header != 1u) return;
-  const uint64_t body = sd.body_end - sd.body0;
-  uint32_t crc = seg_crc[s] ^ crc_shift_bytes(t, 0xFFFFFFFFu, body) ^ 0xFFFFFFFFu;
-  const uint8_t *tr = data + sd.off + sd.body_end;
-  uint32_t stored = ((uint32_t)tr[0] << 24) | ((uint32_t)tr[1] << 16) | ((uint32_t)tr[2] << 8) | tr[3];
-  if (crc != stored) atomicExch(bad, (int)s + 1);
+  if (crc_from_raw(t, seg_crc[s], sd.body_end - sd.body0) != load_be32(data + sd.off + sd.body_end)) atomicExch(bad, (int)s + 1);
 }
 
 // ------------------------------------------------------------------------------------------------ parse
@@ -275,7 +272,6 @@ class Merger {
     return c;
   }
   uint32_t fixed_klen = 0, fixed_vlen = 0;
-  bool parsed_fixed = false;
   uint32_t data_slack = 32;
 
   explicit Merger(const tezgpu_conf &c) : pipe(pipe_conf(c)), fixed_klen(c.fixed_key_len), fixed_vlen(c.fixed_val_len) {}
@@ -285,13 +281,19 @@ class Merger {
   bool arrays_ready = false;   // the per-record metadata arrays (d_koff ...) are filled (never in run-table mode unless asked)
   std::vector<uint64_t> h_counts, h_rec_base;
 
+  // the host checks of a caller's segment, before any of its bytes is read
+  void check_segment(const tezgpu_segment &sg) const {
+    TG_CHECK(sg.data || sg.len == 0, TEZGPU_E_INVALID, "null segment");
+    TG_CHECK(sg.len >= ((sg.flags & TEZGPU_SEG_HAS_HEADER) ? 10u : 6u), TEZGPU_E_FORMAT, "IFile segment shorter than an empty segment");
+    TG_CHECK((int)sg.partition < pipe.conf.num_partitions, TEZGPU_E_INVALID, "segment partition out of range");
+  }
+
   // ---- intake: builds the segment table (segs, d_segs) and launches the header and checksum checks, whose verdicts
   //      check_verdicts() reads.  Segments already on this device are used in place (no copy; kernels handle any byte
   //      alignment); host segments are staged contiguously with 16-byte aligned starts.
   void intake(const tezgpu_segment *in, uint32_t nseg) {
     cudaStream_t st = pipe.stream;
     TG_CUDA(cudaSetDevice(pipe.conf.device));
-    parsed_fixed = false;
     arrays_ready = false;
     segs.resize(nseg);
     bool all_device = nseg > 0;
@@ -314,10 +316,9 @@ class Merger {
       std::stable_sort(seg_orig.begin(), seg_orig.end(), [&](uint32_t a, uint32_t b) { return in[a].partition < in[b].partition; });
     for (uint32_t s = 0; s < nseg; s++) {
       const tezgpu_segment &sg = in[seg_orig[s]];
-      TG_CHECK(sg.data || sg.len == 0, TEZGPU_E_INVALID, "null segment");
+      check_segment(sg);
       const bool hdr = sg.flags & TEZGPU_SEG_HAS_HEADER;
       any_header |= hdr;
-      TG_CHECK(sg.len >= (hdr ? 10u : 6u), TEZGPU_E_FORMAT, "IFile segment shorter than an empty segment");
       segs[s].off = all_device ? (uint64_t)((uintptr_t)sg.data - lo_addr) : off;
       segs[s].len = sg.len;
       segs[s].body0 = hdr ? 4 : 0;
@@ -325,7 +326,6 @@ class Merger {
       segs[s].has_header = (hdr ? 1u : 0u) | ((hdr && (sg.flags & TEZGPU_SEG_VERIFIED)) ? 2u : 0u) |
                            ((hdr && (sg.flags & SEG_DECODED)) ? 4u : 0u);
       segs[s].partition = sg.partition;
-      TG_CHECK((int)sg.partition < pipe.conf.num_partitions, TEZGPU_E_INVALID, "segment partition out of range");
       off = align_up(off + sg.len, 16);
     }
     if (all_device) {
@@ -386,69 +386,28 @@ class Merger {
       check_verdicts();
       return;
     }
+    // ---- merge = stable sort of the union of the runs by the RawComparator
+    bool sorted = false;
     if (count_fixed_records(nseg, FRAMING_MAX_LEN)) {
       // ---- run-table mode: offsets are arithmetic, the stage kernel checks the framing bytes it passes over anyway.
       //      No per-record arrays, no host round trip before the sort's own.
-      cudaStream_t st = pipe.stream;
-      std::vector<uint64_t> roff(nseg);
-      std::vector<uint32_t> rbase(nseg + 1), rpart(nseg);
-      for (uint32_t s = 0; s < nseg; s++) { roff[s] = segs[s].off + segs[s].body0; rbase[s] = (uint32_t)h_rec_base[s]; rpart[s] = segs[s].partition; }
-      rbase[nseg] = (uint32_t)n;
-      const int P = pipe.conf.num_partitions;
-      std::vector<uint32_t> pseg((size_t)P + 1, 0);
-      for (uint32_t s = 0; s < nseg; s++) pseg[segs[s].partition + 1]++;
-      for (int p = 0; p < P; p++) pseg[p + 1] += pseg[p];
-      d_run_pseg.ensure(((size_t)P + 1) * 4);
-      TG_CUDA(cudaMemcpyAsync(d_run_pseg.p, pseg.data(), ((size_t)P + 1) * 4, cudaMemcpyHostToDevice, st));
-      d_run_off.ensure((size_t)nseg * 8); d_run_base.ensure((size_t)(nseg + 1) * 4); d_run_part.ensure((size_t)nseg * 4);
-      TG_CUDA(cudaMemcpyAsync(d_run_off.p, roff.data(), (size_t)nseg * 8, cudaMemcpyHostToDevice, st));
-      TG_CUDA(cudaMemcpyAsync(d_run_base.p, rbase.data(), (size_t)(nseg + 1) * 4, cudaMemcpyHostToDevice, st));
-      TG_CUDA(cudaMemcpyAsync(d_run_part.p, rpart.data(), (size_t)nseg * 4, cudaMemcpyHostToDevice, st));
-      TG_CUDA(cudaStreamSynchronize(st));  // stack-lifetime staging vectors (and: the caller's host segments may go away)
-      const FixedFraming f = fixed_framing(fixed_klen, fixed_vlen);
-      Records r;
-      memset(&r, 0, sizeof(r));
-      r.kv = data;
-      r.kv_bytes = data_slack ? align_up(seg_bytes, 16) + data_slack : seg_bytes;
-      r.n = (uint32_t)n;
-      r.fixed = 1;
-      r.klen = fixed_klen;
-      r.vlen = fixed_vlen;
-      r.use_runs = 1;
-      r.runs.seg_off = d_run_off.as<uint64_t>();
-      r.runs.rec_base = d_run_base.as<uint32_t>();
-      r.runs.seg_part = d_run_part.as<uint32_t>();
-      r.runs.part_seg0 = d_run_pseg.as<uint32_t>();
-      r.runs.nseg = nseg;
-      r.runs.rec_size = f.rec_size;
-      r.runs.hdr_len = f.len;
-      r.runs.hdr_bytes[0] = f.packed(0);
-      r.runs.hdr_bytes[1] = f.packed(1);
-      bool mismatch = false;
       pipe.merge_inputs_plain = true;
       try {
-        pipe.sort_phase(r);
+        pipe.sort_phase(run_table_records(nseg));
+        sorted = true;
       } catch (const FramingMismatch &) {
-        mismatch = true;  // not the fixed framing after all (e.g. run-length encoded input): take the general walk
+        // not the fixed framing after all (e.g. run-length encoded input): take the general walk
       }
-      check_verdicts();
-      if (!mismatch) {
-        parsed_fixed = true;
-        parse_mode = 0;
-        parse_rounds = 0;
-        launches += pipe.state.launches;
-        cursor = 0;
-        have_kvoff = false;
-        return;
-      }
-    } else {
-      check_verdicts();  // also: the caller's host buffers may go away after open()
     }
-    find_records_general(nseg);
-
-    // ---- merge = stable sort of the union of the runs by the RawComparator
-    pipe.merge_inputs_plain = false;
-    pipe.sort_phase(array_records());
+    check_verdicts();  // also: the caller's host buffers may go away after open()
+    if (sorted) {
+      parse_mode = 0;
+      parse_rounds = 0;
+    } else {
+      find_records_general(nseg);
+      pipe.merge_inputs_plain = false;
+      pipe.sort_phase(array_records());
+    }
     launches += pipe.state.launches;
     cursor = 0;
     have_kvoff = false;
@@ -511,12 +470,19 @@ class Merger {
       const uint64_t body = segs[s].body_end - segs[s].body0;
       if (body < 2 || (body - 2) % f.rec_size) return false;
       h_counts[s] = (body - 2) / f.rec_size;
+      h_counts[nseg + s] = h_counts[s] * (fixed_klen + fixed_vlen);
     }
-    for (uint32_t s = 0; s < nseg; s++) { h_rec_base[s] = n; n += h_counts[s]; }
-    h_rec_base[nseg] = n;
-    kv_bytes = n * (uint64_t)(fixed_klen + fixed_vlen);
-    TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one merge");
+    set_record_bases(nseg);
     return true;
+  }
+
+  // h_counts = the records of every segment, then their key + value bytes -> h_rec_base, n and kv_bytes (the window
+  // parser sums the key + value bytes on the device and sets kv_bytes afterwards)
+  void set_record_bases(uint32_t nseg) {
+    n = kv_bytes = 0;
+    for (uint32_t s = 0; s < nseg; s++) { h_rec_base[s] = n; n += h_counts[s]; kv_bytes += h_counts[nseg + s]; }
+    h_rec_base[nseg] = n;
+    TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one merge");
   }
 
   // general path: walk the segments (IFile.Reader semantics), materialise the per-record metadata
@@ -526,7 +492,7 @@ class Merger {
     d_rec_base.ensure((size_t)(nseg + 2) * 8);
     n = 0;
     kv_bytes = 0;
-    if (nseg) open_general_reparse(nseg, h_counts, h_rec_base);
+    if (nseg) open_general_reparse(nseg);
     else record_arrays(0);
     TG_CUDA(cudaGetLastError());
     arrays_ready = true;
@@ -557,29 +523,73 @@ class Merger {
     return r;
   }
 
+  // Records over the run table of the fixed framing (uploaded here): no per-record arrays
+  Records run_table_records(uint32_t nseg) {
+    cudaStream_t st = pipe.stream;
+    std::vector<uint64_t> roff(nseg);
+    std::vector<uint32_t> rbase(nseg + 1), rpart(nseg);
+    for (uint32_t s = 0; s < nseg; s++) { roff[s] = segs[s].off + segs[s].body0; rbase[s] = (uint32_t)h_rec_base[s]; rpart[s] = segs[s].partition; }
+    rbase[nseg] = (uint32_t)n;
+    const int P = pipe.conf.num_partitions;
+    std::vector<uint32_t> pseg((size_t)P + 1, 0);
+    for (uint32_t s = 0; s < nseg; s++) pseg[segs[s].partition + 1]++;
+    for (int p = 0; p < P; p++) pseg[p + 1] += pseg[p];
+    d_run_pseg.ensure(((size_t)P + 1) * 4);
+    TG_CUDA(cudaMemcpyAsync(d_run_pseg.p, pseg.data(), ((size_t)P + 1) * 4, cudaMemcpyHostToDevice, st));
+    d_run_off.ensure((size_t)nseg * 8); d_run_base.ensure((size_t)(nseg + 1) * 4); d_run_part.ensure((size_t)nseg * 4);
+    TG_CUDA(cudaMemcpyAsync(d_run_off.p, roff.data(), (size_t)nseg * 8, cudaMemcpyHostToDevice, st));
+    TG_CUDA(cudaMemcpyAsync(d_run_base.p, rbase.data(), (size_t)(nseg + 1) * 4, cudaMemcpyHostToDevice, st));
+    TG_CUDA(cudaMemcpyAsync(d_run_part.p, rpart.data(), (size_t)nseg * 4, cudaMemcpyHostToDevice, st));
+    TG_CUDA(cudaStreamSynchronize(st));  // stack-lifetime staging vectors (and: the caller's host segments may go away)
+    const FixedFraming f = fixed_framing(fixed_klen, fixed_vlen);
+    Records r;
+    memset(&r, 0, sizeof(r));
+    r.kv = data;
+    r.kv_bytes = data_slack ? align_up(seg_bytes, 16) + data_slack : seg_bytes;
+    r.n = (uint32_t)n;
+    r.fixed = 1;
+    r.klen = fixed_klen;
+    r.vlen = fixed_vlen;
+    r.use_runs = 1;
+    r.runs.seg_off = d_run_off.as<uint64_t>();
+    r.runs.rec_base = d_run_base.as<uint32_t>();
+    r.runs.seg_part = d_run_part.as<uint32_t>();
+    r.runs.part_seg0 = d_run_pseg.as<uint32_t>();
+    r.runs.nseg = nseg;
+    r.runs.rec_size = f.rec_size;
+    r.runs.hdr_len = f.len;
+    r.runs.hdr_bytes[0] = f.packed(0);
+    r.runs.hdr_bytes[1] = f.packed(1);
+    return r;
+  }
+
+  // blocks of the grid-stride kernels over the records
+  uint32_t record_grid() const { return (uint32_t)std::min<uint64_t>(div_up(n, 256), (uint64_t)pipe.num_sms * 16); }
+
+  // the per-record arrays of the fixed framing, in the run table's record numbering (h_rec_base).  Returns the launches.
+  int fill_fixed_arrays() {
+    const uint32_t nseg = (uint32_t)segs.size();
+    d_rec_base.ensure((size_t)(nseg + 2) * 8);
+    TG_CUDA(cudaMemcpyAsync(d_rec_base.p, h_rec_base.data(), (size_t)(nseg + 1) * 8, cudaMemcpyHostToDevice, pipe.stream));
+    const ParseArrays pa = record_arrays(n);
+    if (!n) return 0;
+    k_fill_fixed_arrays<<<record_grid(), 256, 0, pipe.stream>>>(d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), fixed_klen,
+                                                                fixed_vlen, fixed_framing(fixed_klen, fixed_vlen).len, pa);
+    TG_CUDA(cudaGetLastError());
+    return 1;
+  }
+
   // run-table mode keeps no per-record arrays; the record iterator and the general (run-length encoding) emit need
   // them: fill them now (same record numbering, so the sorted order stays valid) and switch the sorter's view over
   void ensure_arrays() {
     if (arrays_ready) return;
-    cudaStream_t st = pipe.stream;
-    const uint32_t nseg = (uint32_t)segs.size();
-    d_rec_base.ensure((size_t)(nseg + 2) * 8);
-    TG_CUDA(cudaMemcpyAsync(d_rec_base.p, h_rec_base.data(), (size_t)(nseg + 1) * 8, cudaMemcpyHostToDevice, st));
-    const ParseArrays pa = record_arrays(n);
-    if (n) {
-      k_fill_fixed_arrays<<<(uint32_t)std::min<uint64_t>(div_up(n, 256), (uint64_t)pipe.num_sms * 16), 256, 0, st>>>(
-          d_segs.as<SegDesc>(), nseg, d_rec_base.as<uint64_t>(), fixed_klen, fixed_vlen, fixed_framing(fixed_klen, fixed_vlen).len, pa);
-      launches++;
-      TG_CUDA(cudaGetLastError());
-    }
+    launches += fill_fixed_arrays();
     Records r = array_records();
     r.fixed = 1;
     r.klen = fixed_klen;
     r.vlen = fixed_vlen;
-    r.cmp = pipe.state.rec.cmp;
-    r.hash_partition = pipe.state.rec.hash_partition;
-    r.num_partitions = pipe.state.rec.num_partitions;
-    r.pbits = pipe.state.rec.pbits;
+    const Records &sorted = pipe.state.rec;   // the comparator and partitioning the sort ran with
+    std::tie(r.cmp, r.hash_partition, r.num_partitions, r.pbits) = std::tie(sorted.cmp, sorted.hash_partition, sorted.num_partitions, sorted.pbits);
     pipe.state.rec = r;
     // the record view changed (explicit offsets instead of the run table): the emit must lay its tiles out again --
     // tile sizes depend on the kernel that serves the view (set_fixed_layout)
@@ -645,15 +655,9 @@ class Merger {
     d_counts.ensure((size_t)(nseg + 1) * 16);
     k_parse_seg_counts<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(d_pwseg.as<PwSeg>(), nseg, d_wbase.as<uint64_t>(), d_counts.as<uint64_t>());
     launches++;
-    uint64_t total = 0;
-    TG_CUDA(cudaMemcpyAsync(&total, d_wbase.as<uint64_t>() + nwin, 8, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaMemcpyAsync(h_counts.data(), d_counts.p, (size_t)nseg * 8, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaStreamSynchronize(st));
-    n = total;
-    TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one merge");
-    uint64_t acc = 0;
-    for (uint32_t s = 0; s < nseg; s++) { h_rec_base[s] = acc; acc += h_counts[s]; }
-    h_rec_base[nseg] = acc;
+    set_record_bases(nseg);
     const ParseArrays pa = record_arrays(n);
     d_carry.ensure((size_t)nwin * 16);
     k_parse_carry<<<grid, PW_THREADS, 0, st>>>(d_pwseg.as<PwSeg>(), nseg, nwin, d_entry[cur].as<uint64_t>(), d_wlast.as<uint64_t>(), d_carry.as<uint64_t>());
@@ -674,7 +678,7 @@ class Merger {
     return true;
   }
 
-  void open_general_reparse(uint32_t nseg, std::vector<uint64_t> &counts, std::vector<uint64_t> &rec_base) {
+  void open_general_reparse(uint32_t nseg) {
     cudaStream_t st = pipe.stream;
     static const bool serial_only = getenv("TEZGPU_PARSE_SERIAL") && atoi(getenv("TEZGPU_PARSE_SERIAL")) != 0;
     parse_mode = 1;
@@ -685,16 +689,12 @@ class Merger {
     k_parse_segments<false><<<(uint32_t)div_up(nseg, PARSE_WARPS), PARSE_WARPS * 32, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, d_counts.as<uint64_t>(),
                                                                      d_counts.as<uint64_t>() + nseg, nullptr, pa, d_bad);
     int bad = 0;
-    TG_CUDA(cudaMemcpyAsync(counts.data(), d_counts.p, (size_t)nseg * 16, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaMemcpyAsync(h_counts.data(), d_counts.p, (size_t)nseg * 16, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaStreamSynchronize(st));
     TG_CHECK(bad == 0, TEZGPU_E_FORMAT, "malformed IFile segment " + std::to_string(bad ? seg_orig[bad - 1] : 0));
-    n = 0;
-    kv_bytes = 0;
-    for (uint32_t s = 0; s < nseg; s++) { rec_base[s] = n; n += counts[s]; kv_bytes += counts[nseg + s]; }
-    rec_base[nseg] = n;
-    TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one merge");
-    TG_CUDA(cudaMemcpyAsync(d_rec_base.p, rec_base.data(), (size_t)(nseg + 1) * 8, cudaMemcpyHostToDevice, st));
+    set_record_bases(nseg);
+    TG_CUDA(cudaMemcpyAsync(d_rec_base.p, h_rec_base.data(), (size_t)(nseg + 1) * 8, cudaMemcpyHostToDevice, st));
     pa = record_arrays(n);
     if (n) k_parse_segments<true><<<(uint32_t)div_up(nseg, PARSE_WARPS), PARSE_WARPS * 32, 0, st>>>(data, d_segs.as<SegDesc>(), nseg, nullptr, nullptr,
                                                                             d_rec_base.as<uint64_t>(), pa, d_bad);
@@ -724,42 +724,40 @@ class Merger {
   DeviceBuffer z_nblk, z_base, z_blks, z_slow;   // LZ4 / zstd: blocks (frames) per segment, their first index, the units, serial-path flags
   void open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg);
 
-  // the writer behind write_*: TezMerger.writeFile semantics, or -- with a combiner -- the combined records, which carry
-  // no segment tags and unique keys (merge mode and the plain writer then write the same bytes)
-  void emit(int writer_rle, uint8_t *d_out_buf, uint64_t cap, uint64_t *out_len, int64_t *index, tezgpu_stats *st) {
-    pipe.emit_out(writer_rle ? 1 : 0, true, raw_output_bound(), d_out_buf, cap, out_len, index, st);
-  }
-
-  // TezMerger.writeFile: one IFile segment, equal adjacent keys written through IFile.REPEAT_KEY
-  void write_device(uint8_t *d_out_buf, uint64_t cap, int writer_rle, int64_t *raw_len, int64_t *part_len, tezgpu_stats *stats) {
-    TG_CHECK(pipe.conf.num_partitions == 1, TEZGPU_E_STATE,
-             "merger was opened with num_partitions > 1: use tezgpu_merge_write_partitions*");
-    int64_t index[3] = {0, 0, 0};
-    uint64_t len = 0;
-    tezgpu_stats st;
-    if (concat) {
-      concat_write(d_out_buf, cap, writer_rle, &len, index, &st);
-    } else {
-      emit(writer_rle, d_out_buf, cap, &len, index, &st);
-      st.output_bytes = (int64_t)kv_bytes;
-      st.kernel_launches += launches - pipe.state.launches;
-    }
-    if (raw_len) *raw_len = index[1];
-    if (part_len) *part_len = index[2];
-    if (stats) *stats = st;
-  }
-
-  void write_partitions_device(uint8_t *d_out_buf, uint64_t cap, int writer_rle, uint64_t *out_len, int64_t *index,
-                               tezgpu_stats *stats) {
+  // the writer behind every write_*: TezMerger.writeFile semantics per partition, or -- with a combiner -- the combined
+  // records, which carry no segment tags and unique keys (merge mode and the plain writer then write the same bytes)
+  void write_device(uint8_t *d_out_buf, uint64_t cap, int writer_rle, uint64_t *out_len, int64_t *index, tezgpu_stats *stats) {
     tezgpu_stats st;
     if (concat) {
       concat_write(d_out_buf, cap, writer_rle, out_len, index, &st);
     } else {
-      emit(writer_rle, d_out_buf, cap, out_len, index, &st);
+      pipe.emit_out(writer_rle ? 1 : 0, true, raw_output_bound(), d_out_buf, cap, out_len, index, &st);
       st.output_bytes = (int64_t)kv_bytes;
       st.kernel_launches += launches - pipe.state.launches;
     }
     if (stats) *stats = st;
+  }
+
+  // where a write into host memory lands: the caller's buffer, which must hold len bytes, or h_out
+  uint8_t *host_out(uint8_t *out, uint64_t cap, uint64_t len) {
+    if (!out) {
+      h_out.ensure(len + 16);
+      return h_out.as<uint8_t>();
+    }
+    TG_CHECK(len <= cap, TEZGPU_E_NOMEM, "output buffer too small for the merged segment");
+    return out;
+  }
+
+  // write_device into d_out, then one copy into host memory (host_out); returns where the *len bytes are
+  const uint8_t *write_host(int writer_rle, uint8_t *out, uint64_t cap, uint64_t *len, int64_t *index, tezgpu_stats *stats) {
+    d_out.ensure(output_bound());
+    write_device(d_out.as<uint8_t>(), d_out.cap, writer_rle, len, index, stats);
+    uint8_t *host = host_out(out, cap, *len);
+    if (*len) {
+      TG_CUDA(cudaMemcpyAsync(host, d_out.p, *len, cudaMemcpyDeviceToHost, pipe.stream));
+      TG_CUDA(cudaStreamSynchronize(pipe.stream));
+    }
+    return host;
   }
 
   void ensure_kvoff() {

@@ -221,10 +221,7 @@ __global__ void k_fetch_crc_check(const FetchSeg *__restrict__ segs, uint32_t ns
   if (s >= nseg) return;
   const FetchSeg sd = segs[s];
   const uint64_t body = sd.len - 4 - (sd.has_header ? 4 : 0);
-  const uint32_t crc = seg_crc[s] ^ crc_shift_bytes(t, 0xFFFFFFFFu, body) ^ 0xFFFFFFFFu;
-  const uint8_t *tr = sd.dst + sd.len - 4;
-  const uint32_t stored = ((uint32_t)tr[0] << 24) | ((uint32_t)tr[1] << 16) | ((uint32_t)tr[2] << 8) | tr[3];
-  if (crc != stored) atomicExch(bad, (int)s + 1);
+  if (crc_from_raw(t, seg_crc[s], body) != load_be32(sd.dst + sd.len - 4)) atomicExch(bad, (int)s + 1);
 }
 
 // number of chunks a range of `len` bytes starting at `src` occupies (at least one, so head/tail bytes always move)

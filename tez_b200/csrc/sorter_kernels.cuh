@@ -1215,12 +1215,10 @@ __global__ void k_finalize_segments(EmitParams e) {
     crc = 0xFFFF0000u;  // crc32(FF FF)
     o += 6;
   } else {
-    // standard CRC = raw remainder xor (0xFFFFFFFF * x^(8*len)) xor 0xFFFFFFFF
-    uint64_t body = s1 - s0 - 8;
-    crc = e.seg_crc[p] ^ crc_shift_bytes(e.crc, 0xFFFFFFFFu, body) ^ 0xFFFFFFFFu;
+    crc = crc_from_raw(e.crc, e.seg_crc[p], s1 - s0 - 8);
     o += s1 - s0 - 4;
   }
-  o[0] = (uint8_t)(crc >> 24); o[1] = (uint8_t)(crc >> 16); o[2] = (uint8_t)(crc >> 8); o[3] = (uint8_t)crc;
+  store_be32(o, crc);
 }
 
 }  // namespace tezgpu
