@@ -12,6 +12,9 @@
  *   - no exceptions cross the boundary; handles are opaque; one producer thread per handle; handles independent.
  *   - the caller owns every buffer it passes, for the duration of the call only; the library owns device memory.
  *   - there is NO CPU fallback: without a CUDA device every compute entry point fails with TEZGPU_E_CUDA.
+ *   - every call runs on its handle's conf.device (or its device argument) and returns with the calling thread's
+ *     CUDA context as it found it; a thread that had none stays on the call's device (no context is created elsewhere).
+ *   - a device ordinal outside [0, tezgpu_device_count()) fails with TEZGPU_E_INVALID ("bad device ordinal").
  */
 #ifndef TEZGPU_H
 #define TEZGPU_H

@@ -81,3 +81,16 @@ def test_no_cpu_fallback_without_a_device(tmp_path):
     with pytest.raises(IOError, match="no CUDA device"):
         out.start()
     assert _lib.load().tezgpu_device_count() == 0
+
+
+@pytest.mark.skipif(__import__("torch").cuda.is_available(), reason="checks the no-GPU failure mode")
+def test_device_argument_calls_without_a_device():
+    """the calls that take a device argument report a missing device as the handle calls do"""
+    from tez_b200 import native
+    import numpy as np
+    calls = [lambda: T.PeerBuffer(16), lambda: T.fetch_ranges([(16, 32, 16)]), lambda: T.fetch_segments_verified([(16, 32, 16)]),
+             lambda: native.shuffle_serve(16, np.zeros((1, 3), dtype=np.int64), "m", 0, 1)]
+    for call in calls:
+        with pytest.raises(_lib.TezGpuError, match="no CUDA device available") as e:
+            call()
+        assert e.value.code == T.E_CUDA

@@ -231,7 +231,6 @@ static inline const char *codec_err_name(int32_t codec, int32_t rc) {
 inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg) {
   if (!pipe.codec) { open(in, nseg); return; }
   cudaStream_t st = pipe.stream;
-  TG_CUDA(cudaSetDevice(pipe.conf.device));
   // which segments are compressed: the header flag byte
   std::vector<uint8_t> hdr((size_t)nseg * 4, 0);
   for (uint32_t s = 0; s < nseg; s++) {

@@ -185,7 +185,6 @@ inline void Merger::concat_write(uint8_t *d_out_buf, uint64_t cap, int writer_rl
                                  tezgpu_stats *stats) {
   TG_CHECK(writer_rle == 0, TEZGPU_E_INVALID,
            "rle " + std::to_string(writer_rle) + ": a concatenating merger writes without run-length encoding (rle must be 0)");
-  TG_CUDA(cudaSetDevice(pipe.conf.device));
   cudaStream_t st = pipe.stream;
   const int P = pipe.conf.num_partitions;
   const uint32_t nseg = (uint32_t)segs.size();
@@ -267,7 +266,6 @@ inline void Merger::concat_write(uint8_t *d_out_buf, uint64_t cap, int writer_rl
 // next_batch / counts: find the records (run table or window parser), then the identity order with no SAME_KEY
 inline void Merger::concat_parse() {
   if (concat_parsed) return;
-  TG_CUDA(cudaSetDevice(pipe.conf.device));
   cudaStream_t st = pipe.stream;
   const uint32_t nseg = (uint32_t)segs.size();
   bool fixed_ok = count_fixed_records(nseg, 8);

@@ -1,5 +1,8 @@
-// device_util.h -- host-side RAII helpers (device / pinned buffers) for libtezgpu.
+// device_util.h -- host-side RAII helpers (device selection, device / pinned buffers) for libtezgpu.
 #pragma once
+#include <cudaTypedefs.h>
+
+#include "../../include/tezgpu.h"
 #include "common.cuh"
 
 namespace tezgpu {
@@ -11,6 +14,51 @@ struct DeviceTally {
   void add(size_t b) { live += b; if (live > peak) peak = live; }
 };
 inline thread_local DeviceTally *g_device_tally = nullptr;
+
+struct TallyScope {
+  DeviceTally *prev;
+  explicit TallyScope(DeviceTally *t) : prev(g_device_tally) { g_device_tally = t; }
+  ~TallyScope() { g_device_tally = prev; }
+};
+
+// The device a C ABI call runs on: every entry point that touches CUDA opens one scope, on its handle's conf.device or
+// its device argument, and everything under it (streams, events, buffers, kernels) uses the current device.  The
+// calling thread's CUDA context is current again when the call returns or throws.  A thread that had none is left on
+// the call's device: selecting device 0, which it reports, would create a context on a device it never used.
+class DeviceScope {
+  CUcontext prev = nullptr;
+  // cuCtxGetCurrent / cuCtxSetCurrent, looked up through the runtime so that the library does not link libcuda
+  struct CtxApi {
+    PFN_cuCtxGetCurrent get = nullptr;
+    PFN_cuCtxSetCurrent set = nullptr;
+    CtxApi() {
+      TG_CUDA(cudaGetDriverEntryPoint("cuCtxGetCurrent", (void **)&get, cudaEnableDefault));
+      TG_CUDA(cudaGetDriverEntryPoint("cuCtxSetCurrent", (void **)&set, cudaEnableDefault));
+      TG_CHECK(get && set, TEZGPU_E_CUDA, "the CUDA driver has no cuCtxGetCurrent / cuCtxSetCurrent");
+    }
+  };
+  static const CtxApi &ctx() {
+    static const CtxApi api;
+    return api;
+  }
+
+ public:
+  explicit DeviceScope(int d) {
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
+      cudaGetLastError();
+      throw Error(TEZGPU_E_CUDA, "no CUDA device available (libtezgpu has no CPU fallback)");
+    }
+    TG_CHECK(d >= 0 && d < n, TEZGPU_E_INVALID, "bad device ordinal");
+    if (ctx().get(&prev) != CUDA_SUCCESS) prev = nullptr;
+    TG_CUDA(cudaSetDevice(d));
+  }
+  ~DeviceScope() {
+    if (prev) ctx().set(prev);
+  }
+  DeviceScope(const DeviceScope &) = delete;
+  DeviceScope &operator=(const DeviceScope &) = delete;
+};
 
 struct DeviceBuffer {
   void *p = nullptr;

@@ -222,12 +222,6 @@ __global__ void k_stitch_finish(const uint32_t *__restrict__ part_raw, const uin
 }
 
 // ------------------------------------------------------------------------------------------------ host loop
-struct TallyScope {
-  DeviceTally *prev;
-  explicit TallyScope(DeviceTally *t) : prev(g_device_tally) { g_device_tally = t; }
-  ~TallyScope() { g_device_tally = prev; }
-};
-
 class BoundedMerge {
  public:
   Merger &m;
@@ -266,7 +260,6 @@ class BoundedMerge {
 
   void open(const tezgpu_segment *segs, uint32_t nseg) {
     TallyScope ts(&tally);
-    TG_CUDA(cudaSetDevice(m.pipe.conf.device));
     uint64_t total = 0;
     in.assign(segs, segs + nseg);
     body0.resize(nseg); body_end.resize(nseg); stored.assign(nseg, 0); check_crc.assign(nseg, 0);

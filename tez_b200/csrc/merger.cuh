@@ -293,7 +293,6 @@ class Merger {
   //      alignment); host segments are staged contiguously with 16-byte aligned starts.
   void intake(const tezgpu_segment *in, uint32_t nseg) {
     cudaStream_t st = pipe.stream;
-    TG_CUDA(cudaSetDevice(pipe.conf.device));
     arrays_ready = false;
     segs.resize(nseg);
     bool all_device = nseg > 0;
@@ -779,7 +778,6 @@ class Merger {
 
   // next()/getKey()/getValue()/isSameKey() in batches
   void next_batch(uint8_t *out_kv, uint64_t cap, tezgpu_kv_index *idx, uint32_t idx_cap, uint32_t *count) {
-    TG_CUDA(cudaSetDevice(pipe.conf.device));
     cudaStream_t st = pipe.stream;
     *count = 0;
     TG_CHECK(!pipe.combiner, TEZGPU_E_STATE, "a merger with a combiner has no record iterator: use tezgpu_merge_write_*");

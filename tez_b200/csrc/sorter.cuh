@@ -5,6 +5,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <memory>
+#include <mutex>
 #include <vector>
 
 #include "../../include/tezgpu.h"
@@ -41,19 +43,24 @@ static inline int partition_bits(int P) {
   return b;
 }
 
-// per-device constant tables (CRC), created once
+// per-device constant tables (CRC), created once per device on the current one (the caller's DeviceScope on `device`)
 struct DeviceConstants {
   CrcTables *d_crc = nullptr;
-  static DeviceConstants &get(int device) {
+  static const DeviceConstants &get(int device) {
     static DeviceConstants inst[64];
+    static std::once_flag built[64];
     DeviceConstants &d = inst[device & 63];
-    if (!d.d_crc) {
-      CrcTables *h = new CrcTables();
+    std::call_once(built[device & 63], [&d] {
+      std::unique_ptr<CrcTables> h(new CrcTables());
       crc_build_tables(*h, EMIT_CRC_STRIDE_WORDS);
-      TG_CUDA(cudaMalloc((void **)&d.d_crc, sizeof(CrcTables)));
-      TG_CUDA(cudaMemcpy(d.d_crc, h, sizeof(CrcTables), cudaMemcpyHostToDevice));
-      delete h;
-    }
+      CrcTables *p = nullptr;
+      TG_CUDA(cudaMalloc((void **)&p, sizeof(CrcTables)));
+      cudaError_t e = cudaMemcpy(p, h.get(), sizeof(CrcTables), cudaMemcpyHostToDevice);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(0);   // a copy from pageable memory can return before it lands
+      if (e != cudaSuccess) cudaFree(p);   // the next call tries again
+      TG_CUDA(e);
+      d.d_crc = p;
+    });
     return d;
   }
 };
@@ -174,20 +181,16 @@ class SortPipeline {
   DeviceBuffer seg_start, tile_start, part_start, d_index, seg_crc, tile_desc, tile_crc, tie_state;
   PinnedBuffer h_small;
 
-  explicit SortPipeline(const tezgpu_conf &c) : conf(c) {
+  // run by the caller before it opens the constructor's DeviceScope: a bad configuration is reported before a bad device
+  static void check_conf(const tezgpu_conf &c) {
     TG_CHECK(c.num_partitions >= 1, TEZGPU_E_INVALID, "num_partitions must be >= 1");
     TG_CHECK(c.comparator >= TEZGPU_CMP_BYTES && c.comparator <= TEZGPU_CMP_LONG, TEZGPU_E_UNSUPPORTED,
              "comparator outside the device-supported set (BYTES, TEXT, BYTESWRITABLE, INT, LONG)");
     TG_CHECK(c.partitioner == TEZGPU_PART_GIVEN || c.partitioner == TEZGPU_PART_HASH || c.partitioner == TEZGPU_PART_TOTAL_ORDER,
              TEZGPU_E_UNSUPPORTED, "partitioner outside the device-supported set (GIVEN, HASH, TOTAL_ORDER)");
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0) {
-      cudaGetLastError();
-      throw Error(TEZGPU_E_CUDA, "no CUDA device available (libtezgpu has no CPU fallback)");
-    }
-    TG_CHECK(c.device >= 0 && c.device < ndev, TEZGPU_E_INVALID, "bad device ordinal");
-    TG_CUDA(cudaSetDevice(c.device));
+  }
+
+  explicit SortPipeline(const tezgpu_conf &c) : conf(c) {
     TG_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
     TG_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, c.device));
     // The path is dominated by sparse reads (16-byte keys out of 80-byte records, 80-byte record gathers): ask L2 to
@@ -234,7 +237,6 @@ class SortPipeline {
   bool have_splits = false;
   // uploads a table build_split_table made; the stream is idle between flushes, so the old table is no longer read
   void set_split_points(const HostSplitTable &t) {
-    TG_CUDA(cudaSetDevice(conf.device));
     const size_t n = t.prefix.size();
     sp_prefix.ensure(std::max<size_t>(n, 1) * 8);
     sp_len.ensure(std::max<size_t>(n, 1) * 4);
@@ -333,7 +335,6 @@ class SortPipeline {
 
   // partition + sort: stage, radix sort of (sort word, index), tie refinement.  Leaves K / order / same / counts.
   void sort_phase(Records rec) {
-    TG_CUDA(cudaSetDevice(conf.device));
     const uint32_t n = rec.n;
     const int P = conf.num_partitions;
     TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one sort");
@@ -571,7 +572,6 @@ class SortPipeline {
   // (empty keys may be run-length encoded too, SORT/TezMerger.java:215-245).
   void emit_phase(int rle, bool merge_mode, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index,
                   tezgpu_stats *stats) {
-    TG_CUDA(cudaSetDevice(conf.device));
     TG_CHECK(((uintptr_t)d_out & 15u) == 0, TEZGPU_E_INVALID, "output buffer must be 16-byte aligned");
     const Records rec = state.rec;
     const uint32_t n = rec.n;

@@ -173,13 +173,19 @@ int32_t tezgpu_sorter_create(const tezgpu_conf *conf, tezgpu_sorter **out) {
   TG_API_BEGIN
   TG_CHECK(conf && out, TEZGPU_E_INVALID, "null argument");
   TG_CHECK(conf->abi_version == TEZGPU_ABI_VERSION, TEZGPU_E_INVALID, "tezgpu_conf.abi_version mismatch");
+  SortPipeline::check_conf(*conf);
+  DeviceScope ds(conf->device);
   *out = new tezgpu_sorter(*conf);
   TG_API_END
 }
 
 int32_t tezgpu_sorter_destroy(tezgpu_sorter *h) {
   TG_API_BEGIN
-  delete h;
+  std::unique_ptr<tezgpu_sorter> own(h);   // deleted also when its device cannot be selected
+  if (h) {
+    DeviceScope ds(h->pipe.conf.device);
+    own.reset();
+  }
   TG_API_END
 }
 
@@ -217,8 +223,8 @@ int32_t tezgpu_sorter_collect_batch(tezgpu_sorter *h, const uint8_t *kv, uint64_
              "sort memory budget exceeded (" + std::to_string(h->payload_bytes + add) + " > " + std::to_string(budget) +
                  " bytes): spill (flush + reset) before collecting more");
   }
+  DeviceScope ds(h->pipe.conf.device);
   cudaStream_t st = h->pipe.stream;
-  TG_CUDA(cudaSetDevice(h->pipe.conf.device));
   const uint64_t base = align_up(h->kv_bytes, 16);  // every batch starts 16-byte aligned
   h->d_kv.grow_preserve(base + kv_bytes + 32, h->kv_bytes, st);
   h->d_koff.grow_preserve((h->n + n) * 8, h->n * 8, st);
@@ -267,8 +273,8 @@ int32_t tezgpu_sorter_collect_fixed(tezgpu_sorter *h, const uint8_t *kv, const i
              "sort memory budget exceeded (" + std::to_string((h->n + n) * stride) + " > " + std::to_string(budget) +
                  " bytes): spill (flush + reset) before collecting more");
   }
+  DeviceScope ds(h->pipe.conf.device);
   cudaStream_t st = h->pipe.stream;
-  TG_CUDA(cudaSetDevice(h->pipe.conf.device));
   h->d_kv.grow_preserve((h->n + n) * stride + 32, h->n * stride, st);
   if (partition) h->d_part.grow_preserve((h->n + n) * 4, h->n * 4, st);
   TG_CUDA(cudaMemcpyAsync(h->d_kv.as<uint8_t>() + h->n * stride, kv, n * stride, cudaMemcpyHostToDevice, st));
@@ -324,6 +330,7 @@ int32_t tezgpu_sorter_flush_to_memory(tezgpu_sorter *h, uint8_t *out, uint64_t o
                                       uint8_t *index_out, int64_t *index, tezgpu_stats *stats) {
   TG_API_BEGIN
   TG_CHECK(h && (out || out_cap == 0), TEZGPU_E_INVALID, "null argument");
+  DeviceScope ds(h->pipe.conf.device);
   std::vector<int64_t> idx;
   sorter_run(h, out, out_cap, out_len, index, stats, idx);
   if (index_out) {
@@ -338,6 +345,7 @@ int32_t tezgpu_sorter_flush(tezgpu_sorter *h, const char *out_path, const char *
                             tezgpu_stats *stats) {
   TG_API_BEGIN
   TG_CHECK(h && out_path && index_path, TEZGPU_E_INVALID, "null argument");
+  DeviceScope ds(h->pipe.conf.device);
   uint64_t bound = tezgpu_sorter_output_bound(h);
   h->h_out.ensure(bound);
   std::vector<int64_t> idx;
@@ -368,6 +376,7 @@ int32_t tezgpu_sorter_sort_device_fixed(tezgpu_sorter *h, const void *d_kv, cons
   r.vlen = h->vlen;
   r.fixed = 1;
   TG_CHECK(((uintptr_t)d_kv & 15u) == 0, TEZGPU_E_INVALID, "device-resident input must be 16-byte aligned");
+  DeviceScope ds(h->pipe.conf.device);
   tezgpu_stats st;
   h->pipe.run(r, (uint8_t *)d_out, out_cap, out_len, index, &st);
   st.output_bytes = (int64_t)(n * ((uint64_t)h->klen + h->vlen));
@@ -408,6 +417,7 @@ int32_t tezgpu_sorter_set_split_points(tezgpu_sorter *h, const uint8_t *keys, co
   TG_CHECK(h->n == 0 && !h->flushed, TEZGPU_E_STATE, "set the split points before the first collect (or after a reset)");
   HostSplitTable t;
   build_split_table(c.comparator, order, c.num_partitions, keys, key_off, key_len, n, t);
+  DeviceScope ds(c.device);
   h->pipe.set_split_points(t);
   TG_API_END
 }
@@ -528,7 +538,7 @@ int32_t tezgpu_peer_alloc(int32_t device, uint64_t bytes, void **dptr, uint8_t *
   TG_API_BEGIN
   TG_CHECK(dptr && handle_out && bytes, TEZGPU_E_INVALID, "null argument");
   static_assert(sizeof(cudaIpcMemHandle_t) == TEZGPU_PEER_HANDLE_BYTES, "export handle size");
-  TG_CUDA(cudaSetDevice(device));
+  DeviceScope ds(device);
   void *p = nullptr;
   TG_CUDA(cudaMalloc(&p, bytes));
   cudaIpcMemHandle_t h;
@@ -544,7 +554,7 @@ int32_t tezgpu_peer_alloc(int32_t device, uint64_t bytes, void **dptr, uint8_t *
 
 int32_t tezgpu_peer_free(int32_t device, void *dptr) {
   TG_API_BEGIN
-  TG_CUDA(cudaSetDevice(device));
+  DeviceScope ds(device);
   if (dptr) TG_CUDA(cudaFree(dptr));
   TG_API_END
 }
@@ -552,7 +562,7 @@ int32_t tezgpu_peer_free(int32_t device, void *dptr) {
 int32_t tezgpu_peer_open(int32_t device, const uint8_t *handle, void **dptr) {
   TG_API_BEGIN
   TG_CHECK(handle && dptr, TEZGPU_E_INVALID, "null argument");
-  TG_CUDA(cudaSetDevice(device));
+  DeviceScope ds(device);
   cudaIpcMemHandle_t h;
   memcpy(&h, handle, sizeof(h));
   void *p = nullptr;
@@ -563,7 +573,7 @@ int32_t tezgpu_peer_open(int32_t device, const uint8_t *handle, void **dptr) {
 
 int32_t tezgpu_peer_close(int32_t device, void *dptr) {
   TG_API_BEGIN
-  TG_CUDA(cudaSetDevice(device));
+  DeviceScope ds(device);
   if (dptr) TG_CUDA(cudaIpcCloseMemHandle(dptr));
   TG_API_END
 }
@@ -583,7 +593,7 @@ int32_t tezgpu_fetch_ranges(int32_t device, const tezgpu_copy_range *ranges, uin
   TG_CHECK(ranges || n == 0, TEZGPU_E_INVALID, "null argument");
   if (ms_kernel) *ms_kernel = 0;
   if (n == 0) return TEZGPU_OK;
-  TG_CUDA(cudaSetDevice(device));
+  DeviceScope ds(device);
   cudaStream_t st = (cudaStream_t)stream;
   std::vector<FetchRange> fr(n);
   uint64_t chunks = 0;
@@ -649,7 +659,7 @@ int32_t tezgpu_fetch_segments_verified(int32_t device, const tezgpu_fetch_segmen
   TG_CHECK(segs || n == 0, TEZGPU_E_INVALID, "null argument");
   if (ms_kernel) *ms_kernel = 0;
   if (n == 0) return TEZGPU_OK;
-  TG_CUDA(cudaSetDevice(device));
+  DeviceScope ds(device);
   cudaStream_t st = (cudaStream_t)stream;
   std::vector<FetchSeg> fs(n);
   std::vector<uint32_t> piece_start(n + 1);
