@@ -63,6 +63,13 @@ int32_t tezrt_output_event(tezrt_output *o, int32_t i, int32_t *type, const uint
                            int32_t *source_index_start, int32_t *count);
 int64_t tezrt_output_counter(tezrt_output *o, const char *name);
 int32_t tezrt_output_num_spills(tezrt_output *o);
+/* The final merge over several spills, after close(): steps = 0 when none ran (one spill, or final merge off), 1 for a
+ * one-step merge, else the key-range steps of the bounded merge; peak_device_bytes and h2d_bytes as
+ * tezgpu_merge_bounded_info, 0 unless the merge ran under tez.runtime.gpu.merge.device.budget.mb.  That key (MiB; 0 or
+ * unset: no budget; below 16: TEZGPU_E_INVALID at initialize) bounds the final merge of an ordered output without a
+ * codec (tezgpu_merge_open_bounded); with a codec the final merge takes one step, as a bounded merge writes no
+ * compressed output.  The unordered outputs concatenate and ignore it. */
+int32_t tezrt_output_merge_info(tezrt_output *o, int32_t *steps, uint64_t *peak_device_bytes, uint64_t *h2d_bytes);
 /* final file.out / file.out.index paths (ExternalSorter.getFinalOutputFile / getFinalIndexFile) */
 const char *tezrt_output_file(tezrt_output *o);
 const char *tezrt_output_index_file(tezrt_output *o);
@@ -98,6 +105,12 @@ int32_t tezrt_input_create_unordered(const char *conf, const char *work_dir, con
                                      int32_t num_physical_inputs, int32_t device, tezrt_input **out);
 /* KeyValueReader.next() + getCurrentKey() / getCurrentValue(): 1 and the next record, 0 at the end */
 int32_t tezrt_input_next_kv(tezrt_input *in, const uint8_t **key, uint32_t *klen, const uint8_t **val, uint32_t *vlen);
+/* The merge behind the reader, after waitForInputReady: as tezrt_output_merge_info.  Under
+ * tez.runtime.gpu.merge.device.budget.mb an OrderedGroupedKVInput decodes its compressed segments with
+ * tezgpu_decode_segments, then merges every segment with tezgpu_merge_open_bounded under the same budget; the peak is
+ * the larger of the two.  The stream and the counters are those of the merge without the key.  UnorderedKVInput
+ * concatenates and ignores the key. */
+int32_t tezrt_input_merge_info(tezrt_input *in, int32_t *steps, uint64_t *peak_device_bytes, uint64_t *h2d_bytes);
 int64_t tezrt_input_counter(tezrt_input *in, const char *name);
 int32_t tezrt_input_destroy(tezrt_input *in);
 

@@ -346,6 +346,20 @@ int32_t tezgpu_merge_open_bounded(const tezgpu_conf *conf, const tezgpu_segment 
  * held at once, and the bytes uploaded from the host segments by all passes.  TEZGPU_E_STATE on a handle that was
  * not opened bounded. */
 int32_t tezgpu_merge_bounded_info(tezgpu_merger *m, int32_t *steps, uint64_t *peak_device_bytes, uint64_t *h2d_bytes);
+/* Decodes compressed HOST segments on the device under a device budget, so that tezgpu_merge_open_bounded (which takes
+ * uncompressed segments only) can merge them.  For every segment whose header flag byte is 1, out[i] receives its
+ * uncompressed IFile segment of raw_len[i] + 4 bytes: TIF\0, the body, the CRC-32 of the body -- what an uncompressed
+ * IFile.Writer writes for the same records.  Other segments are not read past their header and their out[i] may be NULL.
+ * Checksums and streams are checked as tezgpu_merge_open_codec checks them (same codes and messages, naming the
+ * caller's segment index); the decoders are that call's.  The segments are decoded whole, in groups whose staged
+ * compressed bytes, images and decoder workspace stay within budget_bytes (DESIGN.md section 3); *peak_device_bytes
+ * (may be NULL) receives the most device memory the call held at once.  A segment that does not fit the budget on its
+ * own fails with TEZGPU_E_NOMEM naming it and its sizes.  TEZGPU_E_INVALID: a device segment, a budget below
+ * TEZGPU_MERGE_BUDGET_MIN, raw_len NULL (with nseg > 0), out[i] NULL for a compressed segment.  TEZGPU_E_UNSUPPORTED:
+ * a codec other than TEZGPU_CODEC_DEFAULT, _LZ4 and _ZSTD.  Runs on conf->device; conf's other fields are checked as
+ * for a merge. */
+int32_t tezgpu_decode_segments(const tezgpu_conf *conf, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg,
+                               int32_t codec, uint64_t budget_bytes, uint8_t *const *out, uint64_t *peak_device_bytes);
 void *tezgpu_merge_stream(tezgpu_merger *m);
 int32_t tezgpu_merge_close(tezgpu_merger *m);
 

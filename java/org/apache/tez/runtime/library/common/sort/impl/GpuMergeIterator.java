@@ -24,6 +24,7 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
   private static final int BATCH_BYTES = 8 << 20, BATCH_RECORDS = 1 << 16;
 
   private long handle; // tezgpu_merger*
+  private long[] images; // decoded images of a budgeted merge (native memory, freed by close)
   // both grow to fit a record larger than BATCH_BYTES
   private ByteBuffer batch = ByteBuffer.allocateDirect(BATCH_BYTES).order(ByteOrder.nativeOrder());
   private final IntBuffer idx = ByteBuffer.allocateDirect(5 * 4 * BATCH_RECORDS).order(ByteOrder.nativeOrder()).asIntBuffer();
@@ -54,6 +55,38 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
       boolean checkForSameKeys) throws IOException {
     handle = nativeOpen(addresses, lengths, flags, null, 1, rawLengths, codec, comparator,
         Integer.parseInt(System.getenv().getOrDefault("TEZGPU_DEVICE", "0"))); // tezgpu_merge_open_codec
+    if (!checkForSameKeys) nativeSetCheckForSameKeys(handle, false);
+  }
+
+  /**
+   * MergeManager's final merge under tez.runtime.gpu.merge.device.budget.mb (INTEGRATION.md 2d): the merge holds at
+   * most budgetBytes of device memory.  Compressed segments are first decoded on the device, in groups that fit the
+   * budget, into native images of rawLength + 4 bytes that replace them (nativeDecodeSegments: tezgpu_decode_segments);
+   * then every segment is merged in key-range steps (nativeOpenBounded: tezgpu_merge_open_bounded).  The segments must
+   * be in host memory and stay valid until close(), which frees the images.
+   */
+  public GpuMergeIterator(long[] addresses, long[] lengths, int[] flags, long[] rawLengths, int codec, int comparator,
+      boolean checkForSameKeys, long budgetBytes) throws IOException {
+    final int device = Integer.parseInt(System.getenv().getOrDefault("TEZGPU_DEVICE", "0"));
+    addresses = addresses.clone();
+    lengths = lengths.clone();
+    flags = flags.clone();
+    images = new long[addresses.length];
+    if (codec != GpuSorter.CODEC_NONE) {
+      nativeDecodeSegments(addresses, lengths, flags, rawLengths, codec, budgetBytes, device, images);
+      for (int s = 0; s < images.length; s++) {
+        if (images[s] == 0) continue;
+        addresses[s] = images[s];
+        lengths[s] = rawLengths[s] + 4;
+        flags[s] |= SEG_VERIFIED;   // the decode wrote the image's checksum from its bytes
+      }
+    }
+    try {
+      handle = nativeOpenBounded(addresses, lengths, flags, comparator, budgetBytes, device);
+    } catch (IOException e) {
+      nativeFreeImages(images);
+      throw e;
+    }
     if (!checkForSameKeys) nativeSetCheckForSameKeys(handle, false);
   }
 
@@ -122,7 +155,9 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
   @Override
   public void close() throws IOException {
     if (handle != 0) nativeClose(handle);
+    if (images != null) nativeFreeImages(images);
     handle = 0;
+    images = null;
   }
 
   /** PipelinedSorter.flush's final merge: all spills, all partitions, one device pass (PipelinedSorter.java:774-836). */
@@ -139,6 +174,12 @@ public final class GpuMergeIterator implements TezRawKeyValueIterator {
       long[] rawLengths, int codec, int comparator, int device) throws IOException;
   /** native address of a direct buffer (GetDirectBufferAddress), for the segment tables of the open calls */
   static native long nativeAddress(ByteBuffer direct);
+  private static native long nativeOpenBounded(long[] addresses, long[] lengths, int[] flags, int comparator,
+      long budgetBytes, int device) throws IOException;
+  /** images[i] receives the native address of segment i's decoded image (malloc), 0 when it is not compressed */
+  private static native void nativeDecodeSegments(long[] addresses, long[] lengths, int[] flags, long[] rawLengths,
+      int codec, long budgetBytes, int device, long[] images) throws IOException;
+  private static native void nativeFreeImages(long[] images);
   private static native long nativeConcatOpen(long[] addresses, long[] lengths, int[] flags, int[] partitions,
       int numPartitions, long[] rawLengths, int codec, int device) throws IOException;
   private static native void nativeWritePartitions(long h, String out, String index, boolean rle, long[] idx)

@@ -160,6 +160,89 @@ JNIEXPORT jlong JNICALL MERGER(nativeOpen)(JNIEnv *env, jclass cls, jlongArray a
   return open_merger(env, addresses, lengths, flags, partitions, num_partitions, raw_lengths, codec, comparator, device, 0);
 }
 
+/* the segment table of nativeOpenBounded / nativeDecodeSegments (host segments, one partition) */
+static tezgpu_segment *segment_table(JNIEnv *env, jlongArray addresses, jlongArray lengths, jintArray flags, jsize *n) {
+  *n = (*env)->GetArrayLength(env, addresses);
+  jlong *a = (*env)->GetLongArrayElements(env, addresses, NULL), *l = (*env)->GetLongArrayElements(env, lengths, NULL);
+  jint *f = (*env)->GetIntArrayElements(env, flags, NULL);
+  tezgpu_segment *segs = (tezgpu_segment *)calloc((size_t)*n + 1, sizeof(tezgpu_segment));
+  for (jsize i = 0; i < *n; i++) {
+    segs[i].data = (const void *)(intptr_t)a[i];
+    segs[i].len = (uint64_t)l[i];
+    segs[i].flags = (uint32_t)f[i];
+  }
+  (*env)->ReleaseLongArrayElements(env, addresses, a, JNI_ABORT);
+  (*env)->ReleaseLongArrayElements(env, lengths, l, JNI_ABORT);
+  (*env)->ReleaseIntArrayElements(env, flags, f, JNI_ABORT);
+  return segs;
+}
+
+static tezgpu_conf merge_conf(jint comparator, jint device) {
+  tezgpu_conf c;
+  memset(&c, 0, sizeof(c));
+  c.abi_version = TEZGPU_ABI_VERSION;
+  c.device = device;
+  c.num_partitions = 1;
+  c.comparator = comparator;
+  c.partitioner = TEZGPU_PART_GIVEN;
+  c.send_empty_partition_details = 1;
+  return c;
+}
+
+/* MergeManager's final merge under a device budget: tezgpu_merge_open_bounded over uncompressed host segments */
+JNIEXPORT jlong JNICALL MERGER(nativeOpenBounded)(JNIEnv *env, jclass cls, jlongArray addresses, jlongArray lengths,
+                                                  jintArray flags, jint comparator, jlong budget, jint device) {
+  (void)cls;
+  jsize n;
+  tezgpu_segment *segs = segment_table(env, addresses, lengths, flags, &n);
+  tezgpu_conf c = merge_conf(comparator, device);
+  tezgpu_merger *m = NULL;
+  int32_t rc = tezgpu_merge_open_bounded(&c, segs, NULL, (uint32_t)n, TEZGPU_CODEC_NONE, (uint64_t)budget, &m);
+  free(segs);
+  if (failed(env, rc)) return 0;
+  return (jlong)(intptr_t)m;
+}
+
+/* the compressed host segments (TIF\x01) decoded under the budget into malloc'd images of rawLength + 4 bytes, whose
+ * addresses go to images[i] (0 for the other segments) */
+JNIEXPORT void JNICALL MERGER(nativeDecodeSegments)(JNIEnv *env, jclass cls, jlongArray addresses, jlongArray lengths,
+                                                    jintArray flags, jlongArray raw_lengths, jint codec, jlong budget,
+                                                    jint device, jlongArray images) {
+  (void)cls;
+  jsize n;
+  tezgpu_segment *segs = segment_table(env, addresses, lengths, flags, &n);
+  jlong *r = (*env)->GetLongArrayElements(env, raw_lengths, NULL);
+  uint8_t **out = (uint8_t **)calloc((size_t)n + 1, sizeof(uint8_t *));
+  jlong *img = (jlong *)calloc((size_t)n + 1, sizeof(jlong));
+  int32_t rc = TEZGPU_OK;
+  for (jsize i = 0; i < n && rc == TEZGPU_OK; i++) {
+    const uint8_t *h = (const uint8_t *)segs[i].data;
+    if (!(segs[i].flags & TEZGPU_SEG_HAS_HEADER) || segs[i].len < 10 || memcmp(h, "TIF\x01", 4) != 0) continue;
+    out[i] = r[i] > 0 ? (uint8_t *)malloc((size_t)r[i] + 4) : NULL;
+    if (!out[i]) rc = TEZGPU_E_NOMEM;
+  }
+  tezgpu_conf c = merge_conf(TEZGPU_CMP_BYTES, device);
+  if (rc == TEZGPU_OK) rc = tezgpu_decode_segments(&c, segs, (const int64_t *)r, (uint32_t)n, codec, (uint64_t)budget, out, NULL);
+  for (jsize i = 0; i < n; i++) {
+    if (rc != TEZGPU_OK) free(out[i]);
+    else img[i] = (jlong)(intptr_t)out[i];
+  }
+  (*env)->SetLongArrayRegion(env, images, 0, n, img);
+  (*env)->ReleaseLongArrayElements(env, raw_lengths, r, JNI_ABORT);
+  free(img);
+  free(out);
+  free(segs);
+  failed(env, rc);
+}
+
+JNIEXPORT void JNICALL MERGER(nativeFreeImages)(JNIEnv *env, jclass cls, jlongArray images) {
+  (void)cls;
+  jsize n = (*env)->GetArrayLength(env, images);
+  jlong *img = (*env)->GetLongArrayElements(env, images, NULL);
+  for (jsize i = 0; i < n; i++) free((void *)(intptr_t)img[i]);
+  (*env)->ReleaseLongArrayElements(env, images, img, JNI_ABORT);
+}
+
 /* UnorderedPartitionedKVWriter.mergeAll / UnorderedKVReader: records in (segment, position) order, no comparator */
 JNIEXPORT jlong JNICALL MERGER(nativeConcatOpen)(JNIEnv *env, jclass cls, jlongArray addresses, jlongArray lengths,
                                                  jintArray flags, jintArray partitions, jint num_partitions,

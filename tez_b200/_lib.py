@@ -91,6 +91,7 @@ SYMBOLS = [
     ("tezgpu_concat_open", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, _P(_V)]),
     ("tezgpu_merge_open_bounded", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, C.c_uint64, _P(_V)]),
     ("tezgpu_merge_bounded_info", C.c_int32, [_V, _P(C.c_int32), _P(C.c_uint64), _P(C.c_uint64)]),
+    ("tezgpu_decode_segments", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, C.c_uint64, _V, _P(C.c_uint64)]),
     ("tezgpu_debug_crc_concat_emulate", C.c_int32, [_V, _V, C.c_uint32, _P(C.c_uint32)]),
     ("tezgpu_merge_set_check_for_same_keys", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_merge_set_combiner", C.c_int32, [_V, C.c_int32]),
@@ -125,6 +126,7 @@ RT_SYMBOLS = [
     ("tezrt_output_event", C.c_int32, [_V, C.c_int32, _P(C.c_int32), _P(_V), _P(C.c_uint64), _P(C.c_int32), _P(C.c_int32)]),
     ("tezrt_output_counter", C.c_int64, [_V, C.c_char_p]),
     ("tezrt_output_num_spills", C.c_int32, [_V]),
+    ("tezrt_output_merge_info", C.c_int32, [_V, _P(C.c_int32), _P(C.c_uint64), _P(C.c_uint64)]),
     ("tezrt_output_file", C.c_char_p, [_V]),
     ("tezrt_output_index_file", C.c_char_p, [_V]),
     ("tezrt_output_destroy", C.c_int32, [_V]),
@@ -138,6 +140,7 @@ RT_SYMBOLS = [
     ("tezrt_input_wait_ready", C.c_int32, [_V]),
     ("tezrt_input_next", C.c_int32, [_V, _P(_V), _P(C.c_uint32)]),
     ("tezrt_input_next_value", C.c_int32, [_V, _P(_V), _P(C.c_uint32)]),
+    ("tezrt_input_merge_info", C.c_int32, [_V, _P(C.c_int32), _P(C.c_uint64), _P(C.c_uint64)]),
     ("tezrt_input_counter", C.c_int64, [_V, C.c_char_p]),
     ("tezrt_input_destroy", C.c_int32, [_V]),
 ]

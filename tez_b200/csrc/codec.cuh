@@ -222,27 +222,57 @@ static inline const char *codec_err_name(int32_t codec, int32_t rc) {
   }
 }
 
-// Compressed segments (TIF\x01 with a codec set) are staged, their CRC checked (unless the transport verified it),
-// decompressed into images TIF\x00 + body + 4 bytes that the merge reads as verified ordinary segments.  zlib: one warp
-// per segment.  LZ4: one thread per segment walks the block headers (one host round trip for the block count), one warp
-// per block decodes, and a segment the block pass could not take is decoded again serially by one warp.  zstd: the same
-// shape with frames: a segment whose frames all carry Frame_Content_Size is decoded one warp per frame, any other one
-// warp per segment.  Every other segment goes to open() unchanged, so errors keep naming the caller's segment index.
-inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg) {
-  if (!pipe.codec) { open(in, nseg); return; }
-  cudaStream_t st = pipe.stream;
-  // which segments are compressed: the header flag byte
+inline void check_raw_len(uint32_t s, int64_t raw) {
+  TG_CHECK(raw >= 6 && raw < (1ll << 40), TEZGPU_E_INVALID,
+           "segment " + std::to_string(s) + ": raw length " + std::to_string(raw) + " is not a valid IFile rawLength");
+}
+
+// The caller's indices of the compressed segments: header TIF and flag byte 1.  Headers of device segments are read
+// through `st`.
+inline std::vector<uint32_t> compressed_segments(const tezgpu_segment *in, uint32_t nseg, cudaStream_t st) {
   std::vector<uint8_t> hdr((size_t)nseg * 4, 0);
+  bool on_device = false;
   for (uint32_t s = 0; s < nseg; s++) {
     if (!(in[s].flags & TEZGPU_SEG_HAS_HEADER) || in[s].len < 10 || !in[s].data) continue;
-    if (in[s].flags & TEZGPU_SEG_DEVICE) TG_CUDA(cudaMemcpyAsync(&hdr[4 * (size_t)s], in[s].data, 4, cudaMemcpyDeviceToHost, st));
-    else memcpy(&hdr[4 * (size_t)s], in[s].data, 4);
+    if (in[s].flags & TEZGPU_SEG_DEVICE) {
+      TG_CUDA(cudaMemcpyAsync(&hdr[4 * (size_t)s], in[s].data, 4, cudaMemcpyDeviceToHost, st));
+      on_device = true;
+    } else {
+      memcpy(&hdr[4 * (size_t)s], in[s].data, 4);
+    }
   }
-  TG_CUDA(cudaStreamSynchronize(st));
+  if (on_device) TG_CUDA(cudaStreamSynchronize(st));
   std::vector<uint32_t> zs;
   for (uint32_t s = 0; s < nseg; s++)
     if (hdr[4 * s] == 'T' && hdr[4 * s + 1] == 'I' && hdr[4 * s + 2] == 'F' && hdr[4 * s + 3] == 1) zs.push_back(s);
+  return zs;
+}
+
+// Compressed segments go through decode_compressed, and their images TIF\x00 + body + 4 bytes are merged as verified
+// ordinary segments.  Every other segment goes to open() unchanged, so errors keep naming the caller's segment index.
+inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg) {
+  if (!pipe.codec) { open(in, nseg); return; }
+  const std::vector<uint32_t> zs = compressed_segments(in, nseg, pipe.stream);
   if (zs.empty()) { open(in, nseg); return; }
+  decode_compressed(in, raw_len, zs);
+  std::vector<tezgpu_segment> segs2(in, in + nseg);
+  for (size_t i = 0; i < zs.size(); i++) {
+    tezgpu_segment &sg = segs2[zs[i]];
+    sg.data = z_img.as<uint8_t>() + z_img_off[i];
+    sg.len = (uint64_t)raw_len[zs[i]] + 4;
+    sg.flags = TEZGPU_SEG_HAS_HEADER | TEZGPU_SEG_DEVICE | TEZGPU_SEG_VERIFIED | SEG_DECODED;
+  }
+  open(segs2.data(), nseg);
+}
+
+// The segments zs of `in` (caller's indices, all compressed) are staged, their CRC checked (unless the transport
+// verified it), and decompressed into images at z_img + z_img_off[i]: TIF\x00, the body, 4 zero bytes.  zlib: one warp
+// per segment.  LZ4: one thread per segment walks the block headers (one host round trip for the block count), one warp
+// per block decodes, and a segment the block pass could not take is decoded again serially by one warp.  zstd: the same
+// shape with frames: a segment whose frames all carry Frame_Content_Size is decoded one warp per frame, any other one
+// warp per segment.  Returns once every image is complete; errors name the caller's segment index.
+inline void Merger::decode_compressed(const tezgpu_segment *in, const int64_t *raw_len, const std::vector<uint32_t> &zs) {
+  cudaStream_t st = pipe.stream;
   TG_CHECK(raw_len, TEZGPU_E_INVALID, "segment " + std::to_string(zs[0]) + " is compressed: its raw length is required");
   const uint32_t nz = (uint32_t)zs.size();
   uint64_t in_bytes = 0, img_bytes = 0;
@@ -253,8 +283,7 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
   };
   for (uint32_t i = 0; i < nz; i++) {
     const uint32_t s = zs[i];
-    TG_CHECK(raw_len[s] >= 6 && raw_len[s] < (1ll << 40), TEZGPU_E_INVALID,
-             "segment " + std::to_string(s) + ": raw length " + std::to_string(raw_len[s]) + " is not a valid IFile rawLength");
+    check_raw_len(s, raw_len[s]);
     in_off[i] = in_bytes;
     if (!in_place(in[s])) in_bytes = align_up(in_bytes + in[s].len, 16);
     img_off[i] = img_bytes;
@@ -343,14 +372,78 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
   for (uint32_t i = 0; i < nz; i++)
     TG_CHECK(status[i] == Z_OK, TEZGPU_E_FORMAT,
              std::string("compressed segment ") + std::to_string(zs[i]) + ": " + codec_err_name(pipe.codec, status[i]));
-  std::vector<tezgpu_segment> segs2(in, in + nseg);
-  for (uint32_t i = 0; i < nz; i++) {
-    tezgpu_segment &sg = segs2[zs[i]];
-    sg.data = zi[i].dst;
-    sg.len = (uint64_t)raw_len[zs[i]] + 4;
-    sg.flags = TEZGPU_SEG_HAS_HEADER | TEZGPU_SEG_DEVICE | TEZGPU_SEG_VERIFIED | SEG_DECODED;
+  z_img_off = img_off;
+}
+
+// the CRC-32 trailer of every image after its body, from the body's raw remainder in seg_crc
+__global__ void k_image_trailers(uint8_t *__restrict__ img, const SegDesc *__restrict__ sd, uint32_t n,
+                                 const uint32_t *__restrict__ seg_crc, const CrcTables *__restrict__ t) {
+  const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n) return;
+  const SegDesc d = sd[s];
+  store_be32(img + d.off + d.body_end, crc_from_raw(t, seg_crc[s], d.body_end - d.body0));
+}
+
+// ---- tezgpu_decode_segments: the compressed host segments decoded into uncompressed IFile segments in host memory,
+//      in groups that hold at most `budget` device bytes.  A group holds its staged compressed bytes, its images and
+//      the decoder's workspace, bounded by decode_group_bytes; the buffers are released between groups, so the device
+//      holds the Merger's own (`base`, measured by the caller) plus one group at a time.
+constexpr uint64_t DECODE_FIXED_BYTES = 16 << 10;     // the 256-byte rounding of the group's buffers, their slack
+constexpr uint64_t DECODE_BYTES_PER_SEGMENT = 128;    // descriptors, statuses, unit counts, piece starts, CRCs
+constexpr uint64_t DECODE_MIN_UNIT_BYTES = 8;         // the smallest LZ4 block or zstd frame: a decode unit per 8 bytes
+
+inline uint64_t decode_group_bytes(int32_t codec, uint64_t len, uint64_t raw) {
+  const uint64_t units = codec == TEZGPU_CODEC_DEFAULT ? 0 : len / DECODE_MIN_UNIT_BYTES + 1;
+  const uint64_t pieces = div_up(len, CRC_PIECE) + div_up(raw + 4, CRC_PIECE);
+  return align_up(len, 16) + align_up(raw + 4, 16) + units * sizeof(ZUnit) + pieces * sizeof(TileCrc) + DECODE_BYTES_PER_SEGMENT;
+}
+
+inline void Merger::decode_to_host(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg, uint64_t base,
+                                   uint64_t budget, uint8_t *const *out) {
+  cudaStream_t st = pipe.stream;
+  const std::vector<uint32_t> zs = compressed_segments(in, nseg, st);
+  auto decode_group = [&](const std::vector<uint32_t> &g) {
+    decode_compressed(in, raw_len, g);
+    // the trailers: the bodies' remainders (k_crc_pieces / k_crc_combine), then k_image_trailers
+    const uint32_t n = (uint32_t)g.size();
+    std::vector<SegDesc> sd(n);
+    for (uint32_t i = 0; i < n; i++) {
+      const uint64_t raw = (uint64_t)raw_len[g[i]];
+      sd[i] = SegDesc{z_img_off[i], raw + 4, 4, raw, 1u, 0};
+    }
+    TG_CUDA(cudaMemcpyAsync(z_descs.p, sd.data(), (size_t)n * sizeof(SegDesc), cudaMemcpyHostToDevice, st));
+    std::vector<uint32_t> piece_start;
+    launches += segment_remainders(z_img.as<uint8_t>(), sd, z_descs.as<SegDesc>(), [](const SegDesc &) { return true; },
+                                   piece_start, false);
+    k_image_trailers<<<(uint32_t)div_up(n, 128), 128, 0, st>>>(z_img.as<uint8_t>(), z_descs.as<SegDesc>(), n, d_seg_crc.as<uint32_t>(),
+                                                               DeviceConstants::get(pipe.conf.device).d_crc);
+    launches++;
+    TG_CUDA(cudaGetLastError());
+    for (uint32_t i = 0; i < n; i++)
+      TG_CUDA(cudaMemcpyAsync(out[g[i]], z_img.as<uint8_t>() + z_img_off[i], sd[i].len, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaStreamSynchronize(st));   // also: the host tables above live on this stack
+    for (DeviceBuffer *b : {&z_in, &z_img, &z_insegs, &z_status, &z_descs, &z_flag, &z_nblk, &z_base, &z_blks, &z_slow,
+                            &d_piece_start, &d_piece_crc, &d_seg_crc})
+      b->release();
+  };
+  std::vector<uint32_t> group;
+  uint64_t held = 0;
+  for (const uint32_t s : zs) {
+    const int64_t raw = raw_len[s];
+    check_raw_len(s, raw);
+    const uint64_t b = decode_group_bytes(pipe.codec, in[s].len, (uint64_t)raw);
+    TG_CHECK(base + DECODE_FIXED_BYTES + b <= budget, TEZGPU_E_NOMEM,
+             "segment " + std::to_string(s) + " (" + std::to_string(in[s].len) + " compressed bytes, " + std::to_string(raw) +
+                 " raw bytes) does not fit the device budget of " + std::to_string(budget) + " bytes");
+    if (base + DECODE_FIXED_BYTES + held + b > budget) {
+      decode_group(group);
+      group.clear();
+      held = 0;
+    }
+    group.push_back(s);
+    held += b;
   }
-  open(segs2.data(), nseg);
+  if (!group.empty()) decode_group(group);
 }
 
 // host run of the device writer over one body: 78 01, the chunks, Adler-32 (tezgpu_debug_deflate_emulate)

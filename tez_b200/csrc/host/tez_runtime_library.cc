@@ -76,6 +76,7 @@ static const char *K_COMBINER_CLASS = "tez.runtime.combiner.class";
 static const char *K_COMBINE_MIN_SPILLS = "tez.runtime.combine.min.spills";  // TezRuntimeConfiguration:128-130 default 3
 static const char *K_UNORDERED_BUFFER_MB = "tez.runtime.unordered.output.buffer.size-mb";  // :204-206 default 100
 static const char *K_PIPELINED_SHUFFLE = "tez.runtime.pipelined-shuffle.enabled";           // default false
+static const char *K_MERGE_BUDGET_MB = "tez.runtime.gpu.merge.device.budget.mb";           // this project's; default 0
 
 static bool ends_with(const std::string &s, const char *suf) {
   size_t n = strlen(suf);
@@ -325,6 +326,25 @@ static int codec_for(const Configuration &conf) {
   return TEZGPU_CODEC_DEFAULT;
 }
 
+// tez.runtime.gpu.merge.device.budget.mb: the device memory, in MiB, that the reduce-side merge and the output's final
+// merge over several spills may hold (tezgpu_merge_open_bounded; compressed inputs are decoded first with
+// tezgpu_decode_segments).  0 or unset: no budget, the one-step merge as before.  Checked at initialize(), before any
+// device call.  Concatenations (the unordered edges) hold no merge workspace and ignore it.
+static uint64_t merge_budget(const Configuration &c) {
+  const long mb = c.getInt(K_MERGE_BUDGET_MB, 0);
+  RT_CHECK(mb == 0 || mb >= (long)(TEZGPU_MERGE_BUDGET_MIN >> 20), TEZGPU_E_INVALID,
+           std::string(K_MERGE_BUDGET_MB) + "=" + std::to_string(mb) + ": a device budget is at least " +
+               std::to_string(TEZGPU_MERGE_BUDGET_MIN >> 20) + " MiB (0: none)");
+  return (uint64_t)mb << 20;
+}
+
+// what a merge took: steps (0: no merge ran, 1: one step), the most device memory it held at once and the bytes it
+// uploaded from the host (both 0 unless it ran under a budget; the larger of the decode's and the merge's peak)
+struct MergeInfo {
+  int32_t steps = 0;
+  uint64_t peak = 0, h2d = 0;
+};
+
 // ================================================================================================ output side
 // GpuSorter: the ExternalSorter seam (SORT/ExternalSorter.java:74-92,281-288) backed by tezgpu_sorter.  Records are
 // batched on the host and handed to the device; when the collected bytes reach the granted sort memory the device
@@ -353,6 +373,8 @@ struct GpuSorter {
   int combiner = TEZGPU_COMBINE_NONE;    // runs on every spill, and on the final merge from min_spills spills on (:601-609,815-820)
   int min_spills = 3;
   int codec = TEZGPU_CODEC_NONE;         // every spill is compressed; the final merge reads and writes through it
+  uint64_t budget = 0;                   // merge_budget: the final merge of an uncompressed ordered output holds at most this
+  MergeInfo info;                        // of the final merge
   std::map<std::string, int64_t> &counters;
 
   GpuSorter(const tezgpu_conf &c, int64_t mem, bool fm, const std::string &wd, const std::string &u, std::map<std::string, int64_t> &ctr)
@@ -507,15 +529,21 @@ struct GpuSorter {
       gpu_check(tezgpu_concat_open(&mc, cs.data(), craws.data(), (uint32_t)cs.size(), codec, &m));
       rc = tezgpu_merge_write_partitions(m, final_out.c_str(), final_index.c_str(), /*rle=*/0, final_idx.data(), &st);
     } else {
-      gpu_check(tezgpu_merge_open_codec(&mc, segs.data(), raws.data(), (uint32_t)segs.size(), codec, &m));
+      // under a budget the merge runs in key-range steps over the spills in host memory; a bounded merge writes no
+      // compressed output, so a compressed final merge takes one step whatever the budget
+      const bool bounded = budget && !codec;
+      if (bounded) gpu_check(tezgpu_merge_open_bounded(&mc, segs.data(), raws.data(), (uint32_t)segs.size(), codec, budget, &m));
+      else gpu_check(tezgpu_merge_open_codec(&mc, segs.data(), raws.data(), (uint32_t)segs.size(), codec, &m));
       // TezMerger.merge(..., checkForSameKeys = merger.needsRLE()) into Writer(..., rle = merger.needsRLE()), `merger`
       // being the SpanMerger of the last spill (SORT/PipelinedSorter.java:797-814)
       rc = tezgpu_merge_set_check_for_same_keys(m, last_spill_rle);
       if (rc == 0 && combine) rc = tezgpu_merge_set_combiner(m, combiner);
       if (rc == 0)
         rc = tezgpu_merge_write_partitions(m, final_out.c_str(), final_index.c_str(), /*rle=*/last_spill_rle, final_idx.data(), &st);
+      if (rc == 0 && bounded) rc = tezgpu_merge_bounded_info(m, &info.steps, &info.peak, &info.h2d);
     }
     tezgpu_merge_close(m);
+    if (!info.steps) info.steps = 1;
     gpu_check(rc);
     const uint64_t len = (uint64_t)st.file_out_bytes;
     counters["SPILLED_RECORDS"] += st.spilled_records;
@@ -541,6 +569,7 @@ struct Output {
   bool initialized = false, started = false, closed = false;
   bool send_empty = true, final_merge = true;
   bool unordered = false;   // UnorderedPartitionedKVOutput / UnorderedKVOutput: the writer in TEZGPU_SORTER_UNORDERED mode
+  uint64_t budget = 0;      // merge_budget
   bool total_order;         // TotalOrderPartitioner: the device partitions by the split points of the partition file
   std::map<std::string, int64_t> counters;
   GpuSorter *sorter = nullptr;
@@ -551,6 +580,7 @@ struct Output {
   ~Output() { delete sorter; }
 
   void initialize() {
+    budget = merge_budget(conf);
     if (unordered) {
       // UnorderedPartitionedKVWriter.getInitialMemoryRequirement (RL/common/writers/UnorderedPartitionedKVWriter.java:705-716)
       const long mb = conf.getInt(K_UNORDERED_BUFFER_MB, 100);
@@ -616,6 +646,7 @@ struct Output {
     // UnorderedPartitionedKVWriter runs no combiner (and tezgpu_sorter_set_combiner refuses an unordered handle)
     if (const int c = unordered ? 0 : combiner_for(conf)) sorter->set_combiner(c, (int)conf.getInt(K_COMBINE_MIN_SPILLS, 3));
     if (codec) sorter->set_codec(codec);
+    sorter->budget = budget;
     if (total_order)
       gpu_check(tezgpu_sorter_set_split_points(sorter->h, splits.keys.data(), splits.off.data(), splits.len.data(),
                                                (uint32_t)splits.len.size(), split_order));
@@ -729,6 +760,9 @@ struct Input {
   tezgpu_merger *merger = nullptr;
   int cmp = 0;
   int codec = TEZGPU_CODEC_NONE;
+  uint64_t budget = 0;   // merge_budget
+  MergeInfo info;        // one-step merges; a bounded one is asked when merge_info() is called, as it steps while read
+  uint64_t decode_peak = 0;
   // iterator state (RL/common/ValuesIterator.java:91-201)
   std::vector<uint8_t> batch, next_batch_buf;
   std::vector<tezgpu_kv_index> idx;
@@ -753,6 +787,7 @@ struct Input {
     requested = (int64_t)(pct * (double)task_memory);
     cmp = unordered ? TEZGPU_CMP_BYTES : comparator_for(conf);
     codec = codec_for(conf);
+    budget = merge_budget(conf);
     initialized = true;
   }
   void start() {
@@ -832,17 +867,54 @@ struct Input {
       std::vector<int64_t> oraw(segs.size());
       for (size_t i = 0; i < ord.size(); i++) { os[i] = segs[ord[i]]; oraw[i] = seg_raw[ord[i]]; }
       gpu_check(tezgpu_concat_open(&gc, os.data(), oraw.data(), (uint32_t)os.size(), codec, &merger));
+    } else if (budget) {
+      open_bounded(gc, segs);
+      counters["MERGED_MAP_OUTPUTS"] += (int64_t)segs.size();
     } else {
       // MergeManager.finalMerge -> TezMerger.merge; compressed segments are inflated with their index rawLength
       gpu_check(tezgpu_merge_open_codec(&gc, segs.data(), seg_raw.data(), (uint32_t)segs.size(), codec, &merger));
       counters["MERGED_MAP_OUTPUTS"] += (int64_t)segs.size();
     }
-    seg_bytes.clear();
+    info.steps = 1;
+    // a merge in several steps reads the fetched segments until it is closed
+    if (!budget || unordered) seg_bytes.clear();
     seg_raw.clear();
     seg_order.clear();
     batch.resize(8u << 20);
     idx.resize(1u << 16);
     ready = true;
+  }
+  // MergeManager.finalMerge under the budget: the compressed segments are decoded on the device first (their images
+  // replace their fetched bytes), then every segment is merged as an uncompressed host segment in key-range steps
+  void open_bounded(const tezgpu_conf &gc, std::vector<tezgpu_segment> &segs) {
+    std::vector<std::vector<uint8_t>> img(segs.size());
+    std::vector<uint8_t *> out(segs.size(), nullptr);
+    bool any = false;
+    for (size_t i = 0; codec && i < segs.size(); i++)
+      if (seg_bytes[i].size() >= 10 && memcmp(seg_bytes[i].data(), "TIF\x01", 4) == 0) {
+        img[i].resize((size_t)seg_raw[i] + 4);
+        out[i] = img[i].data();
+        any = true;
+      }
+    if (any) {
+      gpu_check(tezgpu_decode_segments(&gc, segs.data(), seg_raw.data(), (uint32_t)segs.size(), codec, budget, out.data(), &decode_peak));
+      for (size_t i = 0; i < segs.size(); i++) {
+        if (!out[i]) continue;
+        seg_bytes[i].swap(img[i]);
+        std::vector<uint8_t>().swap(img[i]);
+        segs[i].data = seg_bytes[i].data();
+        segs[i].len = seg_bytes[i].size();
+        segs[i].flags |= TEZGPU_SEG_VERIFIED;   // the decode wrote the image's checksum from its bytes
+      }
+    }
+    gpu_check(tezgpu_merge_open_bounded(&gc, segs.data(), nullptr, (uint32_t)segs.size(), TEZGPU_CODEC_NONE, budget, &merger));
+  }
+  MergeInfo merge_info() const {
+    if (!merger || !budget || unordered) return info;
+    MergeInfo mi;
+    gpu_check(tezgpu_merge_bounded_info(merger, &mi.steps, &mi.peak, &mi.h2d));
+    mi.peak = std::max(mi.peak, decode_peak);
+    return mi;
   }
   bool fetch() {  // next record of the merged stream into (idx[bi])
     if (eos) return false;
@@ -958,6 +1030,17 @@ int32_t tezrt_output_event(tezrt_output *o, int32_t i, int32_t *type, const uint
 }
 int64_t tezrt_output_counter(tezrt_output *o, const char *name) { auto it = o->o.counters.find(name); return it == o->o.counters.end() ? 0 : it->second; }
 int32_t tezrt_output_num_spills(tezrt_output *o) { return o->o.sorter ? o->o.sorter->num_spills : 0; }
+static void merge_info(const MergeInfo &mi, int32_t *steps, uint64_t *peak, uint64_t *h2d) {
+  if (steps) *steps = mi.steps;
+  if (peak) *peak = mi.peak;
+  if (h2d) *h2d = mi.h2d;
+}
+int32_t tezrt_output_merge_info(tezrt_output *o, int32_t *steps, uint64_t *peak_device_bytes, uint64_t *h2d_bytes) {
+  RT_BEGIN
+  RT_CHECK(o, TEZGPU_E_INVALID, "null handle");
+  merge_info(o->o.sorter ? o->o.sorter->info : MergeInfo(), steps, peak_device_bytes, h2d_bytes);
+  RT_END
+}
 const char *tezrt_output_file(tezrt_output *o) { return o->o.sorter ? o->o.sorter->final_out.c_str() : ""; }
 const char *tezrt_output_index_file(tezrt_output *o) { return o->o.sorter ? o->o.sorter->final_index.c_str() : ""; }
 int32_t tezrt_output_destroy(tezrt_output *o) { delete o; return 0; }
@@ -995,6 +1078,12 @@ int32_t tezrt_input_next(tezrt_input *in, const uint8_t **key, uint32_t *klen) {
 }
 int32_t tezrt_input_next_value(tezrt_input *in, const uint8_t **val, uint32_t *vlen) {
   try { return in->i.next_value(val, vlen) ? 1 : 0; } catch (const Err &e) { g_err = e.what(); return e.code; }
+}
+int32_t tezrt_input_merge_info(tezrt_input *in, int32_t *steps, uint64_t *peak_device_bytes, uint64_t *h2d_bytes) {
+  RT_BEGIN
+  RT_CHECK(in, TEZGPU_E_INVALID, "null handle");
+  merge_info(in->i.merge_info(), steps, peak_device_bytes, h2d_bytes);
+  RT_END
 }
 int64_t tezrt_input_counter(tezrt_input *in, const char *name) { auto it = in->i.counters.find(name); return it == in->i.counters.end() ? 0 : it->second; }
 int32_t tezrt_input_destroy(tezrt_input *in) { delete in; return 0; }

@@ -721,7 +721,11 @@ class Merger {
   // ---- codec (codec.cuh): compressed segments are checked, decompressed into z_img and merged as ordinary segments
   DeviceBuffer z_in, z_img, z_insegs, z_status, z_descs, z_flag;
   DeviceBuffer z_nblk, z_base, z_blks, z_slow;   // LZ4 / zstd: blocks (frames) per segment, their first index, the units, serial-path flags
+  std::vector<uint64_t> z_img_off;                // image of the i-th decoded segment: z_img + z_img_off[i]
   void open_codec(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg);
+  void decode_compressed(const tezgpu_segment *in, const int64_t *raw_len, const std::vector<uint32_t> &zs);
+  void decode_to_host(const tezgpu_segment *in, const int64_t *raw_len, uint32_t nseg, uint64_t base, uint64_t budget,
+                      uint8_t *const *out);
 
   // the writer behind every write_*: TezMerger.writeFile semantics per partition, or -- with a combiner -- the combined
   // records, which carry no segment tags and unique keys (merge mode and the plain writer then write the same bytes)

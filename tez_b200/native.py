@@ -56,6 +56,30 @@ def debug_total_order(keys, split_points, comparator, order=None):
     return part[:len(keys)]
 
 
+def decode_segments(segs, raw_lens, codec, budget, device=0):
+    """The compressed (TIF\\x01) host segments among segs decoded on the device under a budget of device bytes
+    (tezgpu_decode_segments).  Returns (images, peak device bytes): images[i] is segment i's uncompressed IFile segment
+    (TIF\\x00, body, CRC-32 of the body; raw_lens[i] + 4 bytes) or None for a segment that is not compressed."""
+    L = _lib.load()
+    keep = [np.ascontiguousarray(np.frombuffer(s, dtype=np.uint8) if isinstance(s, (bytes, bytearray)) else s, dtype=np.uint8)
+            for s in segs]
+    arr = (Segment * max(1, len(keep)))()
+    imgs = [None] * len(keep)
+    out = (C.c_void_p * max(1, len(keep)))()
+    for i, a in enumerate(keep):
+        arr[i].data = a.ctypes.data if a.size else None
+        arr[i].len = a.size
+        arr[i].flags = SEG_HAS_HEADER
+        if raw_lens is not None and a.size >= 10 and bytes(a[:4]) == b"TIF\x01":
+            imgs[i] = np.empty(int(raw_lens[i]) + 4, dtype=np.uint8)
+            out[i] = imgs[i].ctypes.data
+    raw = None if raw_lens is None else np.ascontiguousarray(raw_lens, dtype=np.int64)
+    conf = make_conf(1, partitioner=PART_GIVEN, device=device)
+    peak = C.c_uint64()
+    check(L.tezgpu_decode_segments(C.byref(conf), arr, _ptr(raw), len(keep), codec, int(budget), out, C.byref(peak)))
+    return [None if m is None else m.tobytes() for m in imgs], peak.value
+
+
 class GpuSorter:
     def __init__(self, num_partitions, combiner=COMBINE_NONE, codec=CODEC_NONE, split_points=None, split_order=None, **kw):
         """combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG runs MRCombiner with IntSumReducer / LongSumReducer on every

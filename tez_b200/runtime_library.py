@@ -16,6 +16,12 @@ from dataclasses import dataclass, field
 from . import _lib
 from ._lib import check_rt
 
+
+def _merge_info(fn, h):
+    steps, peak, h2d = C.c_int32(), C.c_uint64(), C.c_uint64()
+    check_rt(fn(h, C.byref(steps), C.byref(peak), C.byref(h2d)))
+    return steps.value, peak.value, h2d.value
+
 TEXT = "org.apache.hadoop.io.Text"
 INT_WRITABLE = "org.apache.hadoop.io.IntWritable"
 LONG_WRITABLE = "org.apache.hadoop.io.LongWritable"
@@ -153,6 +159,11 @@ class OrderedPartitionedKVOutput:
     def num_spills(self):
         return self._L.tezrt_output_num_spills(self._h)
 
+    def merge_info(self):
+        """(steps, peak device bytes, bytes uploaded) of the final merge over the spills: steps 0 when none ran, 1 for a
+        one-step merge; the bytes are 0 unless tez.runtime.gpu.merge.device.budget.mb bounded it."""
+        return _merge_info(self._L.tezrt_output_merge_info, self._h)
+
     @property
     def final_output_file(self):
         return self._L.tezrt_output_file(self._h).decode()
@@ -271,6 +282,11 @@ class OrderedGroupedKVInput:
 
     def counter(self, name):
         return self._L.tezrt_input_counter(self._h, name.encode())
+
+    def merge_info(self):
+        """(steps, peak device bytes, bytes uploaded) of the merge behind the reader, after waitForInputReady; under
+        tez.runtime.gpu.merge.device.budget.mb the peak covers the decode of compressed inputs too."""
+        return _merge_info(self._L.tezrt_input_merge_info, self._h)
 
     def close(self):
         return []
