@@ -188,6 +188,26 @@ int32_t tezgpu_sorter_reset(tezgpu_sorter *h);
 int32_t tezgpu_sorter_sort_device_fixed(tezgpu_sorter *h, const void *d_kv, const void *d_partition, uint64_t n,
                                         void *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index,
                                         tezgpu_stats *stats);
+/* Device-resident variable-length records: replaces PipelinedSorter.write/collect (SORT/PipelinedSorter.java:387-466)
+ * and flush()+spill() (:558-647,664-859) in one call, for records a GPU producer already holds in HBM -- nothing crosses
+ * PCIe.  Record i's key is d_kv[d_key_off[i] .. d_val_off[i]) and its value d_kv[d_val_off[i] .. + d_val_len[i]), the
+ * triple of collect_batch, but with 64-bit offsets (inputs past 4 GiB) and records in any order, with gaps between them.
+ * Every array lives on conf.device; d_kv must be 16-byte aligned; d_partition may be 0 (HASH, TOTAL_ORDER).  Nothing is
+ * read outside d_kv[0 .. kv_bytes).  A variable-length handle (not fixed), ordered or TEZGPU_SORTER_UNORDERED, with any
+ * comparator, partitioner, combiner and codec; nothing may be collected on it (TEZGPU_E_STATE until reset), and the
+ * call leaves nothing collected.  Before any key byte is read one kernel checks every record -- key_off <= val_off,
+ * val_off - key_off < 2^32, val_off + val_len <= kv_bytes, 0 <= partition < num_partitions -- and fails with
+ * TEZGPU_E_INVALID naming the lowest bad record ("record 1234: ..."); d_out is then untouched.  Output as
+ * tezgpu_sorter_sort_device_fixed: d_out (16-byte aligned without a codec) receives file.out, index and stats are filled
+ * after an internal stream sync; stats.output_bytes = key + value bytes.  out_cap >= tezgpu_sorter_device_output_bound
+ * always suffices; a smaller out_cap that the file does not fit fails with TEZGPU_E_NOMEM and writes nothing. */
+int32_t tezgpu_sorter_sort_device(tezgpu_sorter *h, const void *d_kv, uint64_t kv_bytes, const uint64_t *d_key_off,
+                                  const uint64_t *d_val_off, const uint32_t *d_val_len, const int32_t *d_partition, uint64_t n,
+                                  void *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index, tezgpu_stats *stats);
+/* the out_cap tezgpu_sorter_sort_device always fits for n records in a buffer of kv_bytes (the bound of
+ * tezgpu_sorter_output_bound for those records, with the handle's codec's worst case), known before the sort so that a
+ * caller can size the exchange buffer it sorts into.  0 for a NULL handle. */
+uint64_t tezgpu_sorter_device_output_bound(const tezgpu_sorter *h, uint64_t n, uint64_t kv_bytes);
 /* cudaStream_t of the handle, as an opaque pointer (so callers can record events on it) */
 void *tezgpu_sorter_stream(tezgpu_sorter *h);
 
@@ -447,6 +467,10 @@ uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks);
  * k_emit_fast<5, true>, 2 k_emit_fast4u, 3 k_emit_fast<5, false> (22016-byte images), 4 k_emit<true> (tiles written
  * in pieces, any record size). */
 int32_t tezgpu_debug_fixed_emit_plan(uint32_t klen, uint32_t vlen, int32_t layout, int32_t *kernel, uint32_t *recs_per_tile);
+
+/* diagnostics: tezgpu_sorter_device_output_bound of a handle with num_partitions partitions and codec (TEZGPU_CODEC_*),
+ * computed without a device; 0 for num_partitions < 1 or an unknown codec */
+uint64_t tezgpu_debug_device_output_bound(int32_t num_partitions, int32_t codec, uint64_t n, uint64_t kv_bytes);
 
 /* diagnostics: the checksum algebra of tezgpu_concat_open on the host: bodies[i] (lens[i] bytes, ending in FF FF) are
  * the input bodies; each one's CRC-32 becomes the remainder of its record bytes, those are folded with crc(A||B), and

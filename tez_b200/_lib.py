@@ -61,6 +61,9 @@ SYMBOLS = [
     ("tezgpu_sorter_destroy", C.c_int32, [_V]),
     ("tezgpu_sorter_reset", C.c_int32, [_V]),
     ("tezgpu_sorter_sort_device_fixed", C.c_int32, [_V, _V, _V, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64), _V, _P(Stats)]),
+    ("tezgpu_sorter_sort_device", C.c_int32, [_V, _V, C.c_uint64, _V, _V, _V, _V, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64), _V,
+                                              _P(Stats)]),
+    ("tezgpu_sorter_device_output_bound", C.c_uint64, [_V, C.c_uint64, C.c_uint64]),
     ("tezgpu_sorter_stream", _V, [_V]),
     ("tezgpu_sorter_set_combiner", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_sorter_set_codec", C.c_int32, [_V, C.c_int32]),
@@ -75,6 +78,7 @@ SYMBOLS = [
     ("tezgpu_debug_chunk_fold_emulate", C.c_uint32, [_V, C.c_uint32, C.c_int32]),
     ("tezgpu_debug_run_fold_emulate", C.c_uint32, [_V, C.c_uint32]),
     ("tezgpu_debug_fixed_emit_plan", C.c_int32, [C.c_uint32, C.c_uint32, C.c_int32, _P(C.c_int32), _P(C.c_uint32)]),
+    ("tezgpu_debug_device_output_bound", C.c_uint64, [C.c_int32, C.c_int32, C.c_uint64, C.c_uint64]),
     ("tezgpu_debug_deflate_emulate", C.c_int32, [_V, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_debug_inflate_emulate", C.c_int32, [_V, C.c_uint64, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_debug_lz4_compress_emulate", C.c_int32, [_V, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),

@@ -16,6 +16,7 @@
 #include "merge_steps.cuh"
 #include "sorter.cuh"
 #include "peer_fetch.cuh"
+#include "record_table.cuh"
 
 using namespace tezgpu;
 
@@ -295,6 +296,13 @@ static uint64_t sorter_raw_bound(const tezgpu_sorter *h) {
   return SortPipeline::output_bound(h->n, h->kv_bytes, h->pipe.conf.num_partitions);
 }
 
+// out_cap that always suffices for tezgpu_sorter_sort_device of n records in kv_bytes bytes: the uncompressed file's
+// bound, and with a codec that file's worst case compressed
+static uint64_t device_output_bound(int P, int codec, uint64_t n, uint64_t kv_bytes) {
+  const uint64_t raw = SortPipeline::output_bound(n, kv_bytes, P);
+  return codec ? SortPipeline::codec_bound(codec, raw, P) : raw;
+}
+
 uint64_t tezgpu_sorter_output_bound(const tezgpu_sorter *h) {
   if (!h) return 0;
   const uint64_t raw = sorter_raw_bound(h);
@@ -381,6 +389,70 @@ int32_t tezgpu_sorter_sort_device_fixed(tezgpu_sorter *h, const void *d_kv, cons
   h->pipe.run(r, (uint8_t *)d_out, out_cap, out_len, index, &st);
   st.output_bytes = (int64_t)(n * ((uint64_t)h->klen + h->vlen));
   if (stats) *stats = st;
+  TG_API_END
+}
+
+uint64_t tezgpu_sorter_device_output_bound(const tezgpu_sorter *h, uint64_t n, uint64_t kv_bytes) {
+  return h ? device_output_bound(h->pipe.conf.num_partitions, h->pipe.codec, n, kv_bytes) : 0;
+}
+
+uint64_t tezgpu_debug_device_output_bound(int32_t num_partitions, int32_t codec, uint64_t n, uint64_t kv_bytes) {
+  if (num_partitions < 1 || codec < TEZGPU_CODEC_NONE || codec > TEZGPU_CODEC_ZSTD) return 0;
+  return device_output_bound(num_partitions, codec, n, kv_bytes);
+}
+
+int32_t tezgpu_sorter_sort_device(tezgpu_sorter *h, const void *d_kv, uint64_t kv_bytes, const uint64_t *d_key_off,
+                                  const uint64_t *d_val_off, const uint32_t *d_val_len, const int32_t *d_partition, uint64_t n,
+                                  void *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index, tezgpu_stats *stats) {
+  TG_API_BEGIN
+  TG_CHECK(h && d_out, TEZGPU_E_INVALID, "null argument");
+  TG_CHECK(n == 0 || (d_kv && d_key_off && d_val_off && d_val_len), TEZGPU_E_INVALID, "null argument");
+  TG_CHECK(!h->fixed, TEZGPU_E_STATE, "handle is in fixed-width mode: use tezgpu_sorter_sort_device_fixed");
+  TG_CHECK(h->n == 0, TEZGPU_E_STATE, "records were collected on this handle: reset it first");
+  TG_CHECK(n <= RADIX_MAX_N, TEZGPU_E_INVALID, "more than 2^30-1 records in one sort");
+  check_partition_source(h, d_partition != nullptr);
+  TG_CHECK(((uintptr_t)d_kv & 15u) == 0, TEZGPU_E_INVALID, "device-resident input must be 16-byte aligned");
+  TG_CHECK(h->pipe.codec || ((uintptr_t)d_out & 15u) == 0, TEZGPU_E_INVALID, "output buffer must be 16-byte aligned");
+  DeviceScope ds(h->pipe.conf.device);
+  SortPipeline &pipe = h->pipe;
+  cudaStream_t st = pipe.stream;
+  uint64_t payload = 0;
+  if (n) {
+    // the record table goes into the handle's collect arrays (free: nothing is collected); the verdict borrows the
+    // sort's scratch, which sort_phase clears before it sorts
+    h->d_koff.ensure(n * 8);
+    h->d_klen.ensure(n * 4);
+    h->d_vlen.ensure(n * 4);
+    SortVerdict *v = &pipe.d_scratch()->verdict;
+    TG_CUDA(cudaMemsetAsync(&v->dups, 0xFF, sizeof(v->dups), st));
+    TG_CUDA(cudaMemsetAsync(&v->totals[0], 0, sizeof(v->totals[0]), st));
+    const uint32_t grid = (uint32_t)std::min<uint64_t>(div_up(n, RECTAB_THREADS), (uint64_t)pipe.num_sms * 8);
+    k_record_table<<<grid, RECTAB_THREADS, 0, st>>>(d_key_off, d_val_off, d_val_len, d_partition, (uint32_t)n, kv_bytes,
+                                                    pipe.conf.num_partitions, h->d_koff.as<uint64_t>(), h->d_klen.as<uint32_t>(),
+                                                    h->d_vlen.as<uint32_t>(), &v->dups, (unsigned long long *)&v->totals[0]);
+    TG_CUDA(cudaGetLastError());
+    store_to_host(st, &pipe.h_scratch()->verdict, v, sizeof(SortVerdict));
+    TG_CUDA(cudaGetLastError());
+    TG_CUDA(cudaStreamSynchronize(st));
+    const SortVerdict &hv = pipe.h_scratch()->verdict;
+    TG_CHECK(hv.dups == ~0ull, TEZGPU_E_INVALID,
+             "record " + std::to_string(hv.dups >> RECTAB_REASON_BITS) + ": " +
+                 record_table_reason((uint32_t)(hv.dups & ((1u << RECTAB_REASON_BITS) - 1))));
+    payload = hv.totals[0];
+  }
+  Records r;
+  memset(&r, 0, sizeof(r));
+  r.kv = (const uint8_t *)d_kv;
+  r.kv_bytes = kv_bytes;  // exact: the emit's loads are clamped to it, every other kernel reads inside the records
+  r.key_off = h->d_koff.as<uint64_t>();
+  r.key_len = h->d_klen.as<uint32_t>();
+  r.val_len = h->d_vlen.as<uint32_t>();
+  r.partition = d_partition;
+  r.n = (uint32_t)n;
+  tezgpu_stats s;
+  pipe.run(r, (uint8_t *)d_out, out_cap, out_len, index, &s);
+  s.output_bytes = (int64_t)payload;
+  if (stats) *stats = s;
   TG_API_END
 }
 

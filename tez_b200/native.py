@@ -188,6 +188,22 @@ class GpuSorter:
                                                      _ptr(index), C.byref(st)))
         return out_len.value, index, st.as_dict()
 
+    def sort_device(self, d_kv, kv_bytes, d_key_off, d_val_off, d_val_len, n, d_out, out_cap, d_partition=None):
+        """Device-resident variable-length records (raw device pointers as ints): record i's key is
+        kv[key_off[i] .. val_off[i]) and its value kv[val_off[i] .. + val_len[i]) with uint64 offsets, uint32 value
+        lengths and optional int32 partition ids, all on the handle's device.  Sorts in one call into d_out.  Returns
+        (out_len, index, stats)."""
+        out_len = C.c_uint64()
+        index = np.zeros((self.P, 3), dtype=np.int64)
+        st = Stats()
+        check(self.L.tezgpu_sorter_sort_device(self.h, d_kv, kv_bytes, d_key_off, d_val_off, d_val_len, d_partition, n, d_out,
+                                               out_cap, C.byref(out_len), _ptr(index), C.byref(st)))
+        return out_len.value, index, st.as_dict()
+
+    def device_output_bound(self, n, kv_bytes):
+        """out_cap that sort_device always fits for n records in a buffer of kv_bytes."""
+        return self.L.tezgpu_sorter_device_output_bound(self.h, n, kv_bytes)
+
     def stream(self):
         return self.L.tezgpu_sorter_stream(self.h)
 

@@ -73,6 +73,63 @@ def zipf_ids(first_index, n, seed=5, s=1.1, num_ids=1 << 32, device="cpu"):
     return torch.clamp(rank.to(torch.int64) - 1, 0, num_ids - 1)
 
 
+WORD_MAX = 12
+_WORD_REC = 1 + WORD_MAX + 4   # vint(length) + letters + IntWritable
+
+
+def word_table(vocab, seed=7, s=1.1):
+    """The vocabulary of gen_words, built on the host: (images uint8 [vocab, 17], lengths int64 [vocab], cdf int64
+    [vocab]).  Word w has 3 + h_w % 10 lower-case letters, letter j = (splitmix64((seed << 56) ^ (16 * w + 1 + j)) >> 1) % 26
+    with h_w the same hash at j = -1; its record image is the Text key (vint(length) + letters) followed by IntWritable(1).
+    cdf[w] = floor(2^53 * sum_{v <= w} (v+1)^-s / sum_v (v+1)^-s): rank w is drawn with weight (w+1)^-s (Zipf)."""
+    import numpy as np
+    sbits = (seed << 56)
+    if sbits >= 1 << 63:
+        sbits -= 1 << 64
+    w = torch.arange(vocab, dtype=torch.int64)
+    j = torch.arange(WORD_MAX + 1, dtype=torch.int64)
+    h = _lsr(splitmix64((w.unsqueeze(1) * 16 + j) ^ sbits), 1)
+    lens = 3 + h[:, 0] % 10
+    letters = (97 + h[:, 1:] % 26).to(torch.uint8)
+    img = torch.zeros(vocab, _WORD_REC, dtype=torch.uint8)
+    img[:, 0] = lens.to(torch.uint8)                  # vint of 3..12 is the byte itself
+    pos = torch.arange(WORD_MAX, dtype=torch.int64)
+    img[:, 1:1 + WORD_MAX] = torch.where(pos < lens.unsqueeze(1), letters, torch.zeros_like(letters))
+    one = torch.tensor([0, 0, 0, 1], dtype=torch.uint8)
+    for k in range(4):                                 # IntWritable(1) right behind the letters
+        img[torch.arange(vocab), 1 + lens + k] = one[k]
+    wt = (np.arange(1, vocab + 1, dtype=np.float64)) ** -s
+    cdf = np.floor(np.cumsum(wt) / wt.sum() * float(1 << 53)).astype(np.int64)
+    cdf[-1] = 1 << 53
+    return img, lens + 5, torch.from_numpy(cdf)
+
+
+def gen_words(first_index, n, seed=7, vocab=50000, device="cpu", s=1.1, table=None):
+    """OrderedWordCount map output: record i is a Text key of the word of rank r_i (word_table) and IntWritable(1), where
+    r_i = the first rank whose cdf exceeds splitmix64(((seed + 1) << 56) ^ i) >> 11 -- a Zipf(s) draw in integer
+    arithmetic only, so the records are the same bytes on every device.  Records are packed back to back.  Returns
+    (kv uint8, key_off int64, val_off int64, val_len int32) on `device`: the arrays GpuSorter.sort_device takes (the
+    offsets are the uint64 values, the lengths the uint32 values), kv_bytes = kv.numel()."""
+    img, rec_len, cdf = table if table is not None else word_table(vocab, seed, s)
+    img, rec_len, cdf = img.to(device), rec_len.to(device), cdf.to(device)
+    sbits = ((seed + 1) << 56) & ((1 << 64) - 1)
+    if sbits >= 1 << 63:
+        sbits -= 1 << 64
+    i = torch.arange(first_index, first_index + n, device=device, dtype=torch.int64)
+    u = _lsr(splitmix64(i ^ sbits), 11)
+    rank = torch.clamp(torch.searchsorted(cdf, u, right=True), max=img.shape[0] - 1)
+    size = rec_len[rank]
+    key_off = torch.cumsum(size, 0) - size
+    total = int(size.sum().item()) if n else 0
+    kv = torch.empty(total, dtype=torch.uint8, device=device)
+    for j in range(_WORD_REC):                         # byte j of every record that long
+        m = size > j
+        kv[(key_off + j)[m]] = img[rank[m], j]
+    val_off = key_off + size - 4
+    val_len = torch.full((n,), 4, dtype=torch.int32, device=device)
+    return kv, key_off, val_off, val_len
+
+
 def gen_c5(first_index, n, seed=5, val_len=4096, device="cpu", chunk=1 << 16):
     """BASELINE config 5 records (SURVEY 8d): key = 16 bytes rendered from a Zipf(1.1) id over 2^32 ids (two big-endian
     splitmix64 words of the id, so equal ids <=> equal keys and keys are spread over the partitions), value = val_len
