@@ -324,6 +324,23 @@ int32_t tezgpu_merge_counts(tezgpu_merger *m, uint64_t *records, uint64_t *kv_by
  * to at least key_len + val_len bytes and calls again. */
 int32_t tezgpu_merge_next_batch(tezgpu_merger *m, uint8_t *out_kv, uint64_t cap, tezgpu_kv_index *idx,
                                 uint32_t idx_cap, uint32_t *n);
+/* TezRawKeyValueIterator for a consumer on the device: the next records of the merged stream (the records, order and
+ * same_key that tezgpu_merge_next_batch would return from the same position) written into device memory on conf.device.
+ * Record i of the batch: key = d_kv[d_key_off[i] .. d_val_off[i]), value = d_kv[d_val_off[i] .. + d_val_len[i]), packed
+ * back to back from d_kv[0]; d_same_key[i] = isSameKey() (d_same_key may be NULL).  64-bit offsets: a batch may pass 4 GiB.
+ * The table is the input triple of tezgpu_sorter_sort_device, so a batch can be sorted again without leaving the device.
+ *   A batch is the longest run from the cursor with at most idx_cap records whose bytes fit in kv_cap; *kv_bytes receives
+ *   its bytes, and *n = 0 at the end of the stream.  When the next record alone needs more than kv_cap bytes the call
+ *   fails with TEZGPU_E_NOMEM, *n = 0, *kv_bytes = the bytes that record needs, the cursor where it was and nothing
+ *   written.  Nothing is written past d_kv[*kv_bytes) or past entry *n of the table.
+ *   The cursor is the one of tezgpu_merge_next_batch: the two may be interleaved on one stream.  Every handle
+ *   next_batch serves is served (merges, concatenations, codec and bounded handles; a bounded handle's batches never
+ *   span two of its steps).  Runs on the handle's stream (tezgpu_merge_stream) and returns once the batch is written.
+ *   Checked before anything is launched or written: TEZGPU_E_INVALID for a NULL argument (other than d_same_key) or a
+ *   d_kv that is not 16-byte aligned; TEZGPU_E_STATE for a merger with a combiner, as next_batch. */
+int32_t tezgpu_merge_next_batch_device(tezgpu_merger *m, void *d_kv, uint64_t kv_cap, uint64_t *d_key_off,
+                                       uint64_t *d_val_off, uint32_t *d_val_len, uint8_t *d_same_key,
+                                       uint32_t idx_cap, uint32_t *n, uint64_t *kv_bytes);
 /* replaces TezMerger.writeFile(iter, new IFile.Writer(..., rle)) (SORT/TezMerger.java:215-245): one IFile segment.
  * path may be NULL when out != NULL.  raw_len / part_len as IFile.Writer.getRawLength / getCompressedLength. */
 int32_t tezgpu_merge_write_ifile(tezgpu_merger *m, const char *path, uint8_t *out, uint64_t out_cap, int32_t rle,

@@ -102,6 +102,8 @@ SYMBOLS = [
     ("tezgpu_merge_parse_info", C.c_int32, [_V, _V, _V]),
     ("tezgpu_merge_counts", C.c_int32, [_V, _P(C.c_uint64), _P(C.c_uint64)]),
     ("tezgpu_merge_next_batch", C.c_int32, [_V, _V, C.c_uint64, _P(KvIndex), C.c_uint32, _P(C.c_uint32)]),
+    ("tezgpu_merge_next_batch_device", C.c_int32, [_V, _V, C.c_uint64, _V, _V, _V, _V, C.c_uint32, _P(C.c_uint32),
+                                                   _P(C.c_uint64)]),
     ("tezgpu_merge_write_ifile", C.c_int32, [_V, C.c_char_p, _V, C.c_uint64, C.c_int32, _P(C.c_int64), _P(C.c_int64), _P(Stats)]),
     ("tezgpu_merge_output_bound", C.c_uint64, [_V]),
     ("tezgpu_merge_write_ifile_device", C.c_int32, [_V, _V, C.c_uint64, C.c_int32, _P(C.c_int64), _P(C.c_int64), _P(Stats)]),

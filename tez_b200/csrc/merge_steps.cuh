@@ -535,9 +535,10 @@ class BoundedMerge {
   }
 
   // ---- record iterator across steps
-  void next_batch(uint8_t *out_kv, uint64_t cap, tezgpu_kv_index *idx, uint32_t idx_cap, uint32_t *count) {
+  void next_batch(const BatchDest &d, uint64_t cap, uint32_t idx_cap, uint32_t *count) {
     TallyScope ts(&tally);
     *count = 0;
+    if (d.kv_bytes) *d.kv_bytes = 0;
     TG_CHECK(!m.pipe.combiner, TEZGPU_E_STATE, "a merger with a combiner has no record iterator: use tezgpu_merge_write_*");
     if (idx_cap == 0 || iter == 2) return;
     if (iter == 0) {
@@ -546,7 +547,7 @@ class BoundedMerge {
     }
     while (true) {
       if (in_step && m.cursor < m.n) {
-        m.next_batch(out_kv, cap, idx, idx_cap, count);
+        m.next_batch(d, cap, idx_cap, count);
         if (*count) return;
       }
       in_step = next_step();

@@ -220,25 +220,75 @@ __global__ void k_find_batch(const uint64_t *__restrict__ kv_off, uint32_t n, ui
   *out_count = lo;
 }
 
+// The record table of a batch, in the layout its consumer reads.  put() writes record w: its bytes start at o in the
+// batch, key then value.
+// tezgpu_merge_next_batch: 32-bit array of structs, copied to the caller's tezgpu_kv_index
 struct KvIndexDev { uint32_t key_off, key_len, val_off, val_len, same_key; };
+struct BatchIndexAos {
+  KvIndexDev *idx;
+  __device__ __forceinline__ void put(uint32_t w, uint64_t o, uint32_t kl, uint32_t vl, bool sk) const {
+    KvIndexDev &e = idx[w];
+    e.key_off = (uint32_t)o; e.key_len = kl; e.val_off = (uint32_t)(o + kl); e.val_len = vl; e.same_key = sk ? 1u : 0u;
+  }
+};
+// tezgpu_merge_next_batch_device: struct of arrays with 64-bit offsets, the input triple of tezgpu_sorter_sort_device
+struct BatchIndexSoa {
+  uint64_t *key_off, *val_off;
+  uint32_t *val_len;
+  uint8_t *same_key;   // may be null
+  __device__ __forceinline__ void put(uint32_t w, uint64_t o, uint32_t kl, uint32_t vl, bool sk) const {
+    key_off[w] = o;
+    val_off[w] = o + kl;
+    val_len[w] = vl;
+    if (same_key) same_key[w] = sk ? 1 : 0;
+  }
+};
 
-// one warp per record: copies key then value bytes into the batch buffer and fills the index entry
-__global__ void __launch_bounds__(256)
+constexpr int GATHER_THREADS = 256;
+
+// the 16 bytes at p, any alignment, from the aligned 16-byte words that hold them (both hold bytes of [p, p + 16), so
+// nothing is read from a word without a wanted byte)
+__device__ __forceinline__ uint4 load16_any(const uint8_t *p) {
+  const uintptr_t a = (uintptr_t)p & ~(uintptr_t)15;
+  const uint32_t m = (uint32_t)((uintptr_t)p & 15u);
+  const uint4 lo = *reinterpret_cast<const uint4 *>(a);
+  if (m == 0) return lo;
+  const uint4 hi = *reinterpret_cast<const uint4 *>(a + 16);
+  const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+  const uint32_t k = m >> 2, sh = 8 * (m & 3u);
+  uint32_t s[5];
+#pragma unroll
+  for (int j = 0; j < 5; j++) s[j] = k == 0 ? w[j] : k == 1 ? w[j + 1] : k == 2 ? w[j + 2] : w[j + 3];
+  return make_uint4(__funnelshift_r(s[0], s[1], sh), __funnelshift_r(s[1], s[2], sh), __funnelshift_r(s[2], s[3], sh),
+                    __funnelshift_r(s[3], s[4], sh));
+}
+
+// len bytes src -> dst by the g lanes of a group (lane = rank in the group): the 16-byte words of dst that lie wholly
+// inside the span as 16-byte stores, the bytes before and after them one by one.  Neighbouring records share the
+// edge words, so no lane stores a byte outside its span.
+__device__ __forceinline__ void gather_span(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, uint32_t len,
+                                            uint32_t lane, uint32_t g) {
+  const uint32_t head = min(len, (uint32_t)(-(uintptr_t)dst & 15u));
+  const uint32_t words = (len - head) >> 4, tail = head + (words << 4);
+  for (uint32_t b = lane; b < head; b += g) dst[b] = src[b];
+  for (uint32_t b = tail + lane; b < len; b += g) dst[b] = src[b];
+  uint4 *d16 = reinterpret_cast<uint4 *>(dst + head);
+  const uint8_t *s = src + head;
+  for (uint32_t q = lane; q < words; q += g) d16[q] = load16_any(s + 16ull * q);
+}
+
+// One batch of the record iterator: the record table, one thread per record, and the key then value bytes of every
+// record packed back to back from out[0], 2^lanes_log2 lanes per record (the host sizes the group to the batch's mean
+// record length, so short records do not leave most of a warp idle).  out must be 16-byte aligned.
+template <typename Index>
+__global__ void __launch_bounds__(GATHER_THREADS)
     k_gather_batch(Records rec, const uint32_t *__restrict__ order, const uint8_t *__restrict__ same,
                    const uint64_t *__restrict__ kv_off, uint32_t cursor, uint32_t count, uint8_t *__restrict__ out,
-                   KvIndexDev *__restrict__ idx, int check_same) {
-  const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (w >= count) return;
-  const uint32_t r = cursor + w, i = order[r];
-  const uint64_t o = kv_off[r] - kv_off[cursor];
-  const uint32_t kl = rec.key_len[i], vl = rec.val_len[i];
-  const uint8_t *k = rec.kv + rec.key_off[i];
-  const uint8_t *v = rec.kv + (rec.val_off ? rec.val_off[i] : rec.key_off[i] + kl);
-  for (uint32_t b = lane; b < kl; b += 32) out[o + b] = k[b];
-  for (uint32_t b = lane; b < vl; b += 32) out[o + kl + b] = v[b];
-  if (lane == 0) {
-    KvIndexDev e;
-    e.key_off = (uint32_t)o; e.key_len = kl; e.val_off = (uint32_t)(o + kl); e.val_len = vl;
+                   Index index, int check_same, uint32_t lanes_log2) {
+  const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, nthreads = (uint64_t)gridDim.x * blockDim.x;
+  const uint64_t base = kv_off[cursor];
+  for (uint64_t w = tid; w < count; w += nthreads) {
+    const uint32_t r = cursor + (uint32_t)w, i = order[r];
     // MergeQueue.isSameKey(): read as SAME_KEY from its segment, or (checkForSameKeys) equal to the previous key of
     // another segment
     bool sk = false;
@@ -246,12 +296,32 @@ __global__ void __launch_bounds__(256)
       const uint32_t tag = rec.tag[i], tagp = rec.tag[order[r - 1]];
       sk = (tag & 1u) || (check_same && ((tag >> 1) != (tagp >> 1)));
     }
-    e.same_key = sk ? 1u : 0u;
-    idx[w] = e;
+    index.put((uint32_t)w, kv_off[r] - base, rec.key_len[i], rec.val_len[i], sk);
+  }
+  const uint32_t g = 1u << lanes_log2, lane = (uint32_t)tid & (g - 1);
+  for (uint64_t w = tid >> lanes_log2; w < count; w += nthreads >> lanes_log2) {
+    const uint32_t r = cursor + (uint32_t)w, i = order[r];
+    const uint64_t o = kv_off[r] - base;
+    const uint32_t kl = rec.key_len[i], vl = rec.val_len[i];
+    const uint8_t *k = rec.kv + rec.key_off[i];
+    const uint8_t *v = rec.kv + (rec.val_off ? rec.val_off[i] : rec.key_off[i] + kl);
+    gather_span(out + o, k, kl, lane, g);
+    gather_span(out + o + kl, v, vl, lane, g);
   }
 }
 
 // ------------------------------------------------------------------------------------------------ host orchestration
+// where a batch of the record iterator goes: host memory with the 32-bit index (idx set), or the caller's device
+// buffers with the 64-bit table (idx null; same_key may be null); kv_bytes (may be null) receives the batch's bytes
+struct BatchDest {
+  uint8_t *kv;
+  tezgpu_kv_index *idx;
+  uint64_t *key_off, *val_off;
+  uint32_t *val_len;
+  uint8_t *same_key;
+  uint64_t *kv_bytes;
+};
+
 class Merger {
  public:
   SortPipeline pipe;
@@ -780,15 +850,17 @@ class Merger {
     have_kvoff = true;
   }
 
-  // next()/getKey()/getValue()/isSameKey() in batches
-  void next_batch(uint8_t *out_kv, uint64_t cap, tezgpu_kv_index *idx, uint32_t idx_cap, uint32_t *count) {
+  // next()/getKey()/getValue()/isSameKey() in batches, into host memory (idx != null: tezgpu_merge_next_batch) or into
+  // the caller's device buffers (dev: tezgpu_merge_next_batch_device, whose *kv_bytes receives the batch's bytes)
+  void next_batch(const BatchDest &d, uint64_t cap, uint32_t idx_cap, uint32_t *count) {
     cudaStream_t st = pipe.stream;
     *count = 0;
+    if (d.kv_bytes) *d.kv_bytes = 0;
     TG_CHECK(!pipe.combiner, TEZGPU_E_STATE, "a merger with a combiner has no record iterator: use tezgpu_merge_write_*");
     if (concat) concat_parse();
     if (cursor >= n || idx_cap == 0) return;
     ensure_kvoff();
-    cap = std::min<uint64_t>(cap, 0xFFFFFFFFull);   // tezgpu_kv_index offsets are 32-bit
+    if (d.idx) cap = std::min<uint64_t>(cap, 0xFFFFFFFFull);   // tezgpu_kv_index offsets are 32-bit
     uint32_t *d_cnt = &pipe.d_scratch()->verdict.batch_count;
     k_find_batch<<<1, 1, 0, st>>>(d_kvoff.as<uint64_t>(), (uint32_t)n, (uint32_t)cursor, idx_cap, cap, d_cnt);
     uint32_t cnt = 0;
@@ -804,7 +876,8 @@ class Merger {
       TG_CUDA(cudaMemcpyAsync(&kl, rec.key_len + i, 4, cudaMemcpyDeviceToHost, st));
       TG_CUDA(cudaMemcpyAsync(&vl, rec.val_len + i, 4, cudaMemcpyDeviceToHost, st));
       TG_CUDA(cudaStreamSynchronize(st));
-      idx[0] = tezgpu_kv_index{0, kl, kl, vl, 0};
+      if (d.idx) d.idx[0] = tezgpu_kv_index{0, kl, kl, vl, 0};
+      if (d.kv_bytes) *d.kv_bytes = (uint64_t)kl + vl;
       throw Error(TEZGPU_E_NOMEM, "batch buffer smaller than one record: the next record needs " +
                                       std::to_string((uint64_t)kl + vl) + " bytes");
     }
@@ -813,19 +886,34 @@ class Merger {
     TG_CUDA(cudaMemcpyAsync(&ends[1], d_kvoff.as<uint64_t>() + cursor + cnt, 8, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaStreamSynchronize(st));
     const uint64_t bytes = ends[1] - ends[0];
-    d_batch.ensure(bytes + 16);
-    d_batch_idx.ensure((size_t)cnt * sizeof(KvIndexDev));
-    k_gather_batch<<<(uint32_t)div_up((uint64_t)cnt * 32, 256), 256, 0, st>>>(pipe.state.rec, pipe.state.order, pipe.same.as<uint8_t>(),
-                                                                         d_kvoff.as<uint64_t>(), (uint32_t)cursor, cnt,
-                                                                         d_batch.as<uint8_t>(), d_batch_idx.as<KvIndexDev>(),
-                                                                         pipe.merge_check_same);
-    TG_CUDA(cudaGetLastError());
-    if (bytes) TG_CUDA(cudaMemcpyAsync(out_kv, d_batch.p, bytes, cudaMemcpyDeviceToHost, st));
-    static_assert(sizeof(KvIndexDev) == sizeof(tezgpu_kv_index), "index layout");
-    TG_CUDA(cudaMemcpyAsync(idx, d_batch_idx.p, (size_t)cnt * sizeof(KvIndexDev), cudaMemcpyDeviceToHost, st));
+    if (d.idx) {
+      d_batch.ensure(bytes + 16);
+      d_batch_idx.ensure((size_t)cnt * sizeof(KvIndexDev));
+      gather(cnt, bytes, d_batch.as<uint8_t>(), BatchIndexAos{d_batch_idx.as<KvIndexDev>()});
+      if (bytes) TG_CUDA(cudaMemcpyAsync(d.kv, d_batch.p, bytes, cudaMemcpyDeviceToHost, st));
+      static_assert(sizeof(KvIndexDev) == sizeof(tezgpu_kv_index), "index layout");
+      TG_CUDA(cudaMemcpyAsync(d.idx, d_batch_idx.p, (size_t)cnt * sizeof(KvIndexDev), cudaMemcpyDeviceToHost, st));
+    } else {
+      gather(cnt, bytes, d.kv, BatchIndexSoa{d.key_off, d.val_off, d.val_len, d.same_key});
+    }
     TG_CUDA(cudaStreamSynchronize(st));
     cursor += cnt;
     *count = cnt;
+    if (d.kv_bytes) *d.kv_bytes = bytes;
+  }
+
+  // k_gather_batch of the cnt records at the cursor (bytes of key + value) into out
+  template <typename Index>
+  void gather(uint32_t cnt, uint64_t bytes, uint8_t *out, Index index) {
+    // lanes per record: the power of two nearest above a 32nd of the mean record length, at most a warp
+    uint32_t lanes_log2 = 0;
+    while (lanes_log2 < 5 && (32ull << lanes_log2) * cnt < bytes) lanes_log2++;
+    const uint64_t threads = std::max<uint64_t>(cnt, (uint64_t)cnt << lanes_log2);
+    const uint32_t grid = (uint32_t)std::min<uint64_t>(div_up(threads, GATHER_THREADS), (uint64_t)pipe.num_sms * 16);
+    k_gather_batch<<<grid, GATHER_THREADS, 0, pipe.stream>>>(pipe.state.rec, pipe.state.order, pipe.same.as<uint8_t>(),
+                                                              d_kvoff.as<uint64_t>(), (uint32_t)cursor, cnt, out, index,
+                                                              pipe.merge_check_same, lanes_log2);
+    TG_CUDA(cudaGetLastError());
   }
 };
 

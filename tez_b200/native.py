@@ -346,6 +346,52 @@ class GpuMerger:
                 e = idx[i]
                 yield (raw[e.key_off:e.key_off + e.key_len], raw[e.val_off:e.val_off + e.val_len], bool(e.same_key))
 
+    def next_batch_device(self, d_kv, kv_cap, d_key_off, d_val_off, d_val_len, d_same_key=None, idx_cap=1 << 16):
+        """The next records of the merged stream written into device memory (raw device pointers as ints, on the
+        handle's device; d_kv 16-byte aligned): record i's key is kv[key_off[i] .. val_off[i]) and its value
+        kv[val_off[i] .. + val_len[i]), with uint64 offsets, uint32 value lengths and uint8 isSameKey flags, packed back
+        to back from kv[0] (tezgpu_merge_next_batch_device).  Returns (n, kv_bytes) once the batch is written; n = 0 at
+        the end of the stream.  A record larger than kv_cap raises TezGpuError(E_NOMEM) whose `needed` is the bytes it
+        needs; the stream stays where it was.  The call runs on the merger's own stream (stream()), which nothing orders
+        after the caller's: work the caller queued on the buffers must be complete, or waited for, before the call."""
+        n, kvb = C.c_uint32(), C.c_uint64()
+        rc = self.L.tezgpu_merge_next_batch_device(self.h, d_kv, kv_cap, d_key_off, d_val_off, d_val_len, d_same_key,
+                                                   idx_cap, C.byref(n), C.byref(kvb))
+        try:
+            check(rc)
+        except _lib.TezGpuError as e:
+            e.needed = kvb.value if rc == E_NOMEM else 0
+            raise
+        return n.value, kvb.value
+
+    def records_device(self, batch_records=1 << 16, batch_bytes=1 << 24):
+        """The device twin of records(): yields one batch at a time as torch CUDA tensor views (kv uint8, key_off int64,
+        val_off int64, val_len int32, same_key uint8) over buffers the next batch reuses; the offsets are the uint64 /
+        uint32 values of next_batch_device.  The kv buffer grows to fit a record larger than batch_bytes.  Work the
+        consumer queues on the views on torch's current stream may still be running when it asks for the next batch:
+        the merger's stream waits for that stream before it writes the buffers again."""
+        import torch
+        dev = torch.device("cuda", self.conf.device)
+        mine = torch.cuda.ExternalStream(self.stream(), device=dev)
+        kv = torch.empty(batch_bytes, dtype=torch.uint8, device=dev)
+        ko = torch.empty(batch_records, dtype=torch.int64, device=dev)
+        vo = torch.empty(batch_records, dtype=torch.int64, device=dev)
+        vl = torch.empty(batch_records, dtype=torch.int32, device=dev)
+        sk = torch.empty(batch_records, dtype=torch.uint8, device=dev)
+        while True:
+            mine.wait_stream(torch.cuda.current_stream(dev))
+            try:
+                n, b = self.next_batch_device(kv.data_ptr(), kv.numel(), ko.data_ptr(), vo.data_ptr(), vl.data_ptr(),
+                                              sk.data_ptr(), batch_records)
+            except _lib.TezGpuError as e:
+                if e.code != E_NOMEM or e.needed <= kv.numel():
+                    raise
+                kv = torch.empty(e.needed, dtype=torch.uint8, device=dev)
+                continue
+            if n == 0:
+                return
+            yield kv[:b], ko[:n], vo[:n], vl[:n], sk[:n]
+
     def output_bound(self):
         return self.L.tezgpu_merge_output_bound(self.h)
 
