@@ -239,6 +239,51 @@ int32_t tezgpu_sorter_set_codec(tezgpu_sorter *h, int32_t codec);
 int32_t tezgpu_sorter_set_split_points(tezgpu_sorter *h, const uint8_t *keys, const uint64_t *key_off, const uint32_t *key_len,
                                        uint32_t n, int32_t order);
 
+/* InputSampler.RandomSampler on the device: a sample of the keys of device-resident records, given as the input triple of
+ * tezgpu_sorter_sort_device (key i is d_kv[d_key_off[i] .. d_val_off[i]), the value d_val_len[i] bytes after it), so
+ * that a producer passes the same arrays to both calls.  Record i has the global number gid = gid_base + i and the hash
+ * h = splitmix64(seed ^ gid).  It is a candidate when h < ceil(freq * 2^64), computed exactly from the double freq in
+ * [0, 1]; freq = 1 makes every record one.  Of more than max_samples candidates the max_samples with the smallest
+ * (h, gid) are kept.  So the sample is a function of (seed, gid) alone: records divided between calls (ranks) with the
+ * right gid_base give, capped again by tezgpu_select_split_points, the sample of the whole set.  This is RandomSampler's
+ * contract (a uniform sample of at most numSamples keys at rate freq), not its java.util.Random stream.
+ * Output, in gid order, to host buffers: *count <= max_samples keys back to back in keys (key_off[j], key_len[j]), and
+ * h[j], gid[j]; key_off, key_len, h and gid hold max_samples entries.  When the keys need more than keys_cap bytes the
+ * call fails with TEZGPU_E_NOMEM, *keys_bytes = the bytes they need, *count = 0 and nothing else written.
+ * Before any key byte is read every record gets tezgpu_sorter_sort_device's checks (key_off <= val_off,
+ * val_off - key_off < 2^32, val_off + val_len <= kv_bytes); a bad record fails the call with TEZGPU_E_INVALID naming the
+ * lowest bad index ("record 1234: ...") and nothing written.  TEZGPU_E_INVALID also for a NULL argument, freq outside
+ * [0, 1], n >= 2^32 or gid_base + n past 2^64.  Runs on a stream of the library's: work queued on the records must be
+ * complete before the call; the call returns when its results are on the host. */
+int32_t tezgpu_sample_keys(int32_t device, const void *d_kv, uint64_t kv_bytes, const uint64_t *d_key_off,
+                           const uint64_t *d_val_off, const uint32_t *d_val_len, uint64_t n, uint64_t gid_base, uint64_t seed,
+                           double freq, uint32_t max_samples, uint8_t *keys, uint64_t keys_cap, uint64_t *key_off,
+                           uint32_t *key_len, uint64_t *h, uint64_t *gid, uint32_t *count, uint64_t *keys_bytes);
+
+/* InputSampler.writePartitionFile on the device: the num_partitions - 1 split points of TotalOrderPartitioner from one or
+ * more samples of tezgpu_sample_keys, given together as n host entries (keys, key_off, key_len, h, gid; for example the
+ * union of every rank's sample).  First the global cap: the max_samples smallest (h, gid) of the union, so the result does
+ * not depend on how the records were divided between sample calls.  The kept keys are sorted on the device under
+ * `comparator` by the sort pipeline (ties in gid order), and the splits are picked by writePartitionFile's rule with
+ * Java's float arithmetic:
+ *   float stepSize = len / (float) P; last = -1;
+ *   for i in 1 .. P-1: k = Math.round(stepSize * i); while (last >= k && cmp(samples[last], samples[k]) == 0) ++k;
+ *                      split i-1 = samples[k]; last = k;
+ * `order` is the search order of tezgpu_sorter_set_split_points, with the same pairing rule (TEZGPU_E_INVALID
+ * otherwise); the splits do not depend on it.  Output in that call's layout: split i in split_keys[split_off[i] .. +
+ * split_len[i]), *split_bytes = the bytes written; chosen (may be NULL) receives each split's index in the sorted sample.
+ * Where Java's rule writes a split equal to or below the one before (a skewed sample), the split is returned as Java
+ * writes it, and tezgpu_sorter_set_split_points then refuses it ("Split points are out of order").  Where Java would
+ * fail the call fails with TEZGPU_E_INVALID: an empty sample with P > 1, or a k past the end of the sample
+ * (ArrayIndexOutOfBoundsException); also for a gid that appears twice.  When the splits need more than split_cap bytes,
+ * TEZGPU_E_NOMEM with *split_bytes = the bytes they need and nothing else written.  P = 1 returns no splits.
+ * TEZGPU_E_UNSUPPORTED for an unknown comparator; TEZGPU_E_INVALID for a NULL argument, max_samples above 2^30 - 1 or
+ * n >= 2^32. */
+int32_t tezgpu_select_split_points(int32_t device, int32_t comparator, int32_t order, int32_t num_partitions, uint32_t max_samples,
+                                   const uint8_t *keys, const uint64_t *key_off, const uint32_t *key_len, const uint64_t *h,
+                                   const uint64_t *gid, uint64_t n, uint8_t *split_keys, uint64_t split_cap, uint64_t *split_off,
+                                   uint32_t *split_len, uint64_t *split_bytes, uint64_t *chosen);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Merger: replaces TezMerger.merge(...) -> TezRawKeyValueIterator (SORT/TezMerger.java:717-912,
  * SORT/TezRawKeyValueIterator.java:33-87) as called from OG/MergeManager.java:804-811,899-903,1035-1041,1197-1199
@@ -526,6 +571,11 @@ int32_t tezgpu_debug_sort_words_emulate(const uint8_t *kv, const uint64_t *key_o
 int32_t tezgpu_debug_total_order_emulate(const uint8_t *kv, const uint64_t *key_off, const uint32_t *key_len, uint32_t n,
                                          const uint8_t *splits, const uint64_t *split_off, const uint32_t *split_len,
                                          uint32_t nsplits, int32_t comparator, int32_t order, int32_t *partition);
+
+/* diagnostics: keeps only the bits of `mask` of every hash tezgpu_sample_keys computes (h = splitmix64(seed ^ gid) & mask)
+ * and returns the mask it replaces; ~0 (the default) keeps them all.  splitmix64 is a bijection, so records of one seed
+ * never tie in h: a narrow mask makes them tie, for tests of the cap's order (h, gid).  Process-wide. */
+uint64_t tezgpu_debug_set_sample_hash_mask(uint64_t mask);
 
 #ifdef __cplusplus
 }

@@ -68,6 +68,11 @@ SYMBOLS = [
     ("tezgpu_sorter_set_combiner", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_sorter_set_codec", C.c_int32, [_V, C.c_int32]),
     ("tezgpu_sorter_set_split_points", C.c_int32, [_V, _V, _V, _V, C.c_uint32, C.c_int32]),
+    ("tezgpu_sample_keys", C.c_int32, [C.c_int32, _V, C.c_uint64, _V, _V, _V, C.c_uint64, C.c_uint64, C.c_uint64, C.c_double,
+                                       C.c_uint32, _V, C.c_uint64, _V, _V, _V, _V, _P(C.c_uint32), _P(C.c_uint64)]),
+    ("tezgpu_select_split_points", C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_uint32, _V, _V, _V, _V, _V,
+                                               C.c_uint64, _V, C.c_uint64, _V, _V, _P(C.c_uint64), _V]),
+    ("tezgpu_debug_set_sample_hash_mask", C.c_uint64, [C.c_uint64]),
     ("tezgpu_shuffle_header_size", C.c_uint64, [C.c_char_p, C.c_int64, C.c_int64, C.c_int32]),
     ("tezgpu_shuffle_header_write", C.c_int32, [C.c_char_p, C.c_int64, C.c_int64, C.c_int32, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_shuffle_header_read", C.c_int32, [_V, C.c_uint64, _V, C.c_uint64, _P(C.c_int64), _P(C.c_int64), _P(C.c_int32), _P(C.c_uint64)]),

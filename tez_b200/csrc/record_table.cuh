@@ -22,6 +22,15 @@ static inline std::string record_table_reason(uint32_t r) {
   }
 }
 
+// Why a record (key at ko, value at vo, vl value bytes) does not lie in a buffer of kv_bytes, 0 when it does: the
+// record checks every device-resident record table goes through (k_record_table, the sampler's k_sample_count)
+__host__ __device__ __forceinline__ uint32_t record_bounds_check(uint64_t ko, uint64_t vo, uint32_t vl, uint64_t kv_bytes) {
+  if (vo < ko) return RECTAB_KEY_AFTER_VALUE;
+  if (vo - ko > 0xFFFFFFFFull) return RECTAB_KEY_TOO_LONG;
+  if (vo > kv_bytes || vl > kv_bytes - vo) return RECTAB_PAST_END;
+  return 0;
+}
+
 // One pass over the caller's arrays (64-bit sibling of k_rebase_offsets).  A record is valid when key_off <= val_off,
 // val_off - key_off < 2^32, val_off + val_len <= kv_bytes and, with partition ids, 0 <= partition < P.  first_bad
 // (initialised to ~0) receives min((i << RECTAB_REASON_BITS) | reason) over the invalid records i, so the host names the
@@ -38,11 +47,8 @@ __global__ void __launch_bounds__(RECTAB_THREADS)
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const uint64_t ko = key_off[i], vo = val_off[i];
     const uint32_t vl = val_len[i];
-    uint32_t why = 0;
-    if (vo < ko) why = RECTAB_KEY_AFTER_VALUE;
-    else if (vo - ko > 0xFFFFFFFFull) why = RECTAB_KEY_TOO_LONG;
-    else if (vo > kv_bytes || vl > kv_bytes - vo) why = RECTAB_PAST_END;
-    else if (partition) {
+    uint32_t why = record_bounds_check(ko, vo, vl, kv_bytes);
+    if (!why && partition) {
       const int32_t p = partition[i];
       if (p < 0 || p >= P) why = RECTAB_PARTITION;
     }

@@ -955,3 +955,4 @@ int32_t tezgpu_debug_fixed_emit_plan(uint32_t klen, uint32_t vlen, int32_t layou
 }  // extern "C"
 
 #include "merger_api.inl"
+#include "sample_api.inl"

@@ -98,12 +98,16 @@ struct HostSplitTable {
     return SplitTable{prefix.data(), len.data(), off.data(), blob.data(), (uint32_t)prefix.size(), order};
   }
 };
-static inline void build_split_table(int sort_cmp, int order, int P, const uint8_t *keys, const uint64_t *key_off,
-                                     const uint32_t *key_len, uint32_t n, HostSplitTable &t) {
-  // the handle's own order, or the natural (content) order of Text / BytesWritable keys sorted by raw bytes
+// the search order of split points: the handle's own order, or the natural (content) order of Text / BytesWritable keys
+// sorted by raw bytes
+static inline void check_split_order(int sort_cmp, int order) {
   TG_CHECK(order == sort_cmp || (sort_cmp == CMP_BYTES && (order == CMP_TEXT || order == CMP_BYTESWRITABLE)), TEZGPU_E_INVALID,
            "search order " + std::to_string(order) + " does not fit comparator " + std::to_string(sort_cmp) +
                " (the comparator itself, or TEXT / BYTESWRITABLE under BYTES)");
+}
+static inline void build_split_table(int sort_cmp, int order, int P, const uint8_t *keys, const uint64_t *key_off,
+                                     const uint32_t *key_len, uint32_t n, HostSplitTable &t) {
+  check_split_order(sort_cmp, order);
   TG_CHECK((int64_t)n == (int64_t)P - 1, TEZGPU_E_INVALID, "Wrong number of partitions in keyset");
   TG_CHECK((keys && key_off && key_len) || n == 0, TEZGPU_E_INVALID, "null argument");
   for (uint32_t i = 1; i < n; i++)

@@ -3,6 +3,7 @@
 GpuSorter  ~ ExternalSorter seam (SORT/ExternalSorter.java:74-92): write/collect -> flush -> close.
 GpuMerger  ~ TezMerger.merge(...) -> TezRawKeyValueIterator (SORT/TezMerger.java:717-912).
 """
+import collections
 import ctypes as C
 import os
 import tempfile
@@ -54,6 +55,75 @@ def debug_total_order(keys, split_points, comparator, order=None):
                                              len(split_points), comparator, comparator if order is None else order,
                                              _ptr(part)))
     return part[:len(keys)]
+
+
+KeySample = collections.namedtuple("KeySample", "keys key_off key_len h gid")
+KeySample.__doc__ = """A sample of tezgpu_sample_keys, in gid order (numpy): keys uint8 (the keys back to back), key_off uint64,
+key_len uint32, h uint64 (splitmix64(seed ^ gid)), gid uint64 (the records' global numbers)."""
+
+
+def sample_keys(d_kv, kv_bytes, d_key_off, d_val_off, d_val_len, n, seed, freq, max_samples, gid_base=0, device=0):
+    """RandomSampler on the device (tezgpu_sample_keys): a sample of the keys of device-resident records given as
+    GpuSorter.sort_device's input (raw device pointers as ints).  Record i is numbered gid_base + i; it is a candidate
+    when splitmix64(seed ^ gid) < freq * 2^64, and of more than max_samples candidates those with the smallest
+    (h, gid) are kept.  Returns a KeySample."""
+    L = _lib.load()
+    m = max(1, int(max_samples))
+    ko, kl = np.empty(m, dtype=np.uint64), np.empty(m, dtype=np.uint32)
+    h, gid = np.empty(m, dtype=np.uint64), np.empty(m, dtype=np.uint64)
+    count, need = C.c_uint32(), C.c_uint64()
+    keys = np.empty(max(4096, min(int(n), m) * 32), dtype=np.uint8)
+    while True:
+        rc = L.tezgpu_sample_keys(device, d_kv, kv_bytes, d_key_off, d_val_off, d_val_len, n, gid_base, seed, float(freq),
+                                  max_samples, _ptr(keys), keys.size, _ptr(ko), _ptr(kl), _ptr(h), _ptr(gid), C.byref(count),
+                                  C.byref(need))
+        if rc == E_NOMEM and need.value > keys.size:
+            keys = np.empty(need.value, dtype=np.uint8)
+            continue
+        check(rc)
+        c = count.value
+        return KeySample(keys[:need.value].copy(), ko[:c].copy(), kl[:c].copy(), h[:c].copy(), gid[:c].copy())
+
+
+def concat_samples(samples):
+    """The union of several KeySamples as one (keys rebased), e.g. every rank's sample."""
+    samples = list(samples)
+    if len(samples) == 1:
+        return samples[0]
+    base = np.cumsum([0] + [s.keys.size for s in samples[:-1]]).astype(np.uint64)
+    return KeySample(np.concatenate([s.keys for s in samples]).astype(np.uint8),
+                     np.concatenate([s.key_off + b for s, b in zip(samples, base)]).astype(np.uint64),
+                     np.concatenate([s.key_len for s in samples]).astype(np.uint32),
+                     np.concatenate([s.h for s in samples]).astype(np.uint64),
+                     np.concatenate([s.gid for s in samples]).astype(np.uint64))
+
+
+def sample_key_list(sample):
+    """The keys of a KeySample as a list of bytes."""
+    raw = sample.keys.tobytes()
+    return [raw[o:o + ln] for o, ln in zip(sample.key_off.tolist(), sample.key_len.tolist())]
+
+
+def select_split_points(samples, num_partitions, max_samples, comparator, order=None, device=0, with_chosen=False):
+    """InputSampler.writePartitionFile on the device (tezgpu_select_split_points): the union of the KeySamples capped to
+    the max_samples smallest (h, gid), sorted under `comparator` on the device, and the num_partitions - 1 split points
+    picked by writePartitionFile's rule.  Returns the serialized split keys, the list GpuSorter(partitioner=PART_TOTAL_ORDER,
+    split_points=...) takes, searched in `order` (None = the comparator); with_chosen also their indices in the sorted
+    sample."""
+    L = _lib.load()
+    s = concat_samples([samples] if isinstance(samples, KeySample) else samples)
+    P = int(num_partitions)
+    so, sl = np.empty(max(1, P - 1), dtype=np.uint64), np.empty(max(1, P - 1), dtype=np.uint32)
+    chosen = np.empty(max(1, P - 1), dtype=np.uint64)
+    need = C.c_uint64()
+    out = np.empty(max(16, int(s.key_len.max(initial=0)) * max(0, P - 1)), dtype=np.uint8)   # every split at the longest key
+    check(L.tezgpu_select_split_points(device, comparator, comparator if order is None else order, P, max_samples,
+                                       _ptr(s.keys if s.keys.size else np.zeros(1, np.uint8)), _ptr(s.key_off), _ptr(s.key_len),
+                                       _ptr(s.h), _ptr(s.gid), s.gid.size, _ptr(out), out.size, _ptr(so), _ptr(sl),
+                                       C.byref(need), _ptr(chosen)))
+    raw = out[:need.value].tobytes()
+    splits = [raw[o:o + ln] for o, ln in zip(so[:P - 1].tolist(), sl[:P - 1].tolist())]
+    return (splits, chosen[:P - 1].copy()) if with_chosen else splits
 
 
 def decode_segments(segs, raw_lens, codec, budget, device=0):

@@ -119,6 +119,61 @@ def ring_order(segs, rank, world):
     return sorted((t for t in segs if t[3] != rank), key=lambda t: (t[3] - rank) % world)
 
 
+def total_order_splits(records, num_partitions, freq, max_samples, seed, group=None, comparator=None, order=None, device=0,
+                       timings=None):
+    """TotalOrderPartitioner split points shared by every rank, sampled on the devices: records = (kv, key_off, val_off,
+    val_len), this rank's device tensors in GpuSorter.sort_device's layout (synth.gen_words returns them).  The records
+    are numbered across ranks (gid_base = the records of the lower ranks, from an all-gather of the counts), each rank
+    samples its own (native.sample_keys), the samples are all-gathered, and every rank selects the same splits from their
+    union (native.select_split_points).  With these splits on every rank's TOTAL_ORDER sorter and owner_ranges' blocks of
+    partitions, rank 0's merged output, then rank 1's, ... is one sorted sequence.  A failure on any rank, or splits
+    whose digest differs from rank 0's, raise on every rank.  timings: an optional dict that receives the seconds of the
+    phases sample, all-gather and select."""
+    import hashlib
+    import time
+
+    from . import native
+    from .constants import CMP_BYTES
+    cmp = CMP_BYTES if comparator is None else comparator
+    kv, ko, vo, vl = records
+    n = int(ko.numel())
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+
+    def agree(ok, payload, what):
+        got = [None] * world
+        dist.all_gather_object(got, (ok, payload), group=group)
+        bad = [g for g, (o, _) in enumerate(got) if not o]
+        if bad:
+            raise RuntimeError("total_order_splits: rank %d could not %s (%s)" % (bad[0], what, got[bad[0]][1]))
+        return [p for _, p in got]
+
+    t0 = time.perf_counter()
+    counts = agree(True, n, "count its records")
+    sample, err = None, None
+    try:
+        sample = native.sample_keys(kv.data_ptr(), kv.numel(), ko.data_ptr(), vo.data_ptr(), vl.data_ptr(), n, seed, freq,
+                                    max_samples, gid_base=sum(counts[:rank]), device=device)
+    except Exception as e:  # noqa: BLE001 -- reported on every rank by agree()
+        err = e
+    t1 = time.perf_counter()
+    samples = agree(err is None, sample if err is None else str(err), "sample its keys")
+    t2 = time.perf_counter()
+    splits, err = None, None
+    try:
+        splits = native.select_split_points(samples, num_partitions, max_samples, cmp, order, device=device)
+    except Exception as e:  # noqa: BLE001
+        err = e
+    digest = hashlib.sha256(b"".join(len(s).to_bytes(8, "little") + s for s in splits)).hexdigest() if err is None else None
+    digests = agree(err is None, digest if err is None else str(err), "select the split points")
+    if any(d != digests[0] for d in digests):
+        raise RuntimeError("total_order_splits: the split points of rank %d differ from rank 0's"
+                           % next(g for g, d in enumerate(digests) if d != digests[0]))
+    t3 = time.perf_counter()
+    if timings is not None:
+        timings.update(sample=t1 - t0, all_gather=t2 - t1, select=t3 - t2)
+    return splits
+
+
 class PeerExchange:
     """NVLink pull shuffle.  Each rank owns `slots` exported file.out buffers used round-robin (step k writes slot
     k % slots): with two slots the index all-gather of step k+1 is the only synchronisation needed -- a peer has
