@@ -128,6 +128,11 @@ typedef struct tezgpu_merger tezgpu_merger;
  * device writes one frame per TEZGPU_ZSTD_BLOCK_BYTES raw bytes (the last one shorter): Single_Segment with
  * Frame_Content_Size, one block, no checksum, at most TEZGPU_ZSTD_FRAME_BOUND bytes.  The device reader takes what
  * libzstd's default streaming decoder takes (windows up to 2^27), except dictionaries.
+ * With SNAPPY (org.apache.hadoop.io.compress.SnappyCodec) the stream has Lz4Codec's block framing with one raw Snappy
+ * block per chunk (a varint preamble giving the chunk's raw length, then literal and copy elements).  The device writes
+ * blocks of TEZGPU_SNAPPY_BLOCK_BYTES raw bytes (the last one shorter), one chunk each, no chunk longer than
+ * TEZGPU_SNAPPY_CHUNK_BOUND; a Java reader needs io.compression.codec.snappy.buffersize of at least that (the default
+ * is 262,144).  The device reader takes chunks of at most 262,144 bytes that decode to at most 262,144 bytes each.
  * Other codecs are not on the device. */
 #define TEZGPU_CODEC_NONE 0
 #define TEZGPU_CODEC_DEFAULT 1
@@ -137,6 +142,9 @@ typedef struct tezgpu_merger tezgpu_merger;
 #define TEZGPU_CODEC_ZSTD 3
 #define TEZGPU_ZSTD_BLOCK_BYTES 65024
 #define TEZGPU_ZSTD_FRAME_BOUND (TEZGPU_ZSTD_BLOCK_BYTES + 10) /* a raw frame: magic, descriptor, 2-byte size, block header */
+#define TEZGPU_CODEC_SNAPPY 4
+#define TEZGPU_SNAPPY_BLOCK_BYTES 65024
+#define TEZGPU_SNAPPY_CHUNK_BOUND (3 + 3 + TEZGPU_SNAPPY_BLOCK_BYTES) /* all literal: 3 preamble, 3 literal-tag bytes */
 
 const char *tezgpu_last_error(void);
 int32_t tezgpu_abi_version(void);
@@ -555,6 +563,11 @@ int32_t tezgpu_debug_lz4_decompress_emulate(const uint8_t *z, uint64_t len, uint
 int32_t tezgpu_debug_zstd_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len);
 int32_t tezgpu_debug_zstd_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
                                              uint64_t *out_len);
+/* the same for TEZGPU_CODEC_SNAPPY: snappy_compress gives the block stream the device writes for one body;
+ * snappy_decompress runs the device reader's walk and chunk decoder on one lane and fails with the reason it gives */
+int32_t tezgpu_debug_snappy_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len);
+int32_t tezgpu_debug_snappy_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
+                                               uint64_t *out_len);
 
 /* diagnostics: the 32-bit sort words the variable-width map side gives n keys (key i = kv[key_off[i] ..
  * key_off[i] + key_len[i])), computed on the host with the device's code: the alphabet table built from the byte values

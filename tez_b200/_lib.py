@@ -90,6 +90,8 @@ SYMBOLS = [
     ("tezgpu_debug_lz4_decompress_emulate", C.c_int32, [_V, C.c_uint64, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_debug_zstd_compress_emulate", C.c_int32, [_V, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_debug_zstd_decompress_emulate", C.c_int32, [_V, C.c_uint64, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
+    ("tezgpu_debug_snappy_compress_emulate", C.c_int32, [_V, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
+    ("tezgpu_debug_snappy_decompress_emulate", C.c_int32, [_V, C.c_uint64, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_debug_sort_words_emulate", C.c_int32, [_V, _V, _V, C.c_uint32, C.c_int32, C.c_int32, _V, C.c_int32, _V,
                                                      _P(C.c_uint32), _P(C.c_int32)]),
     ("tezgpu_debug_total_order_emulate", C.c_int32, [_V, _V, _V, C.c_uint32, _V, _V, _V, C.c_uint32, C.c_int32, C.c_int32, _V]),

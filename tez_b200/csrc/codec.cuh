@@ -1,26 +1,29 @@
-// codec.cuh -- DefaultCodec, Lz4Codec and ZStandardCodec on both sides of the shuffle: the compress phase behind every
-// emit (SortPipeline) and the decompress step in front of every merge open (Merger).  Formats, chunk kernels and
-// decoders: deflate.cuh, inflate.cuh (DefaultCodec), lz4.cuh (Lz4Codec), zstd.cuh (ZStandardCodec).  What the codecs
-// share is here: the segment layout and its kernels, the finish of LZ4 and zstd segments, the reader's staging and
-// checksum check, its block-parallel sequence for LZ4 and zstd, and the writers' host runs.
+// codec.cuh -- DefaultCodec, Lz4Codec, ZStandardCodec and SnappyCodec on both sides of the shuffle: the compress phase
+// behind every emit (SortPipeline) and the decompress step in front of every merge open (Merger).  Formats, chunk
+// kernels and decoders: deflate.cuh, inflate.cuh (DefaultCodec), lz4.cuh (Lz4Codec), zstd.cuh (ZStandardCodec),
+// snappy.cuh (SnappyCodec).  What the codecs share is here: the segment layout and its kernels, the finish of LZ4, zstd
+// and Snappy segments, the reader's staging and checksum check, its block-parallel sequence for LZ4 and zstd, and the
+// writers' host runs.
 #pragma once
 #include <memory>
 #include "inflate.cuh"
 #include "lz4.cuh"
 #include "zstd.cuh"
+#include "snappy.cuh"
 #include "merger.cuh"
 
 namespace tezgpu {
 
 // the codecs the device writes and reads (TEZGPU_CODEC_*)
 inline void check_codec(int32_t codec) {
-  TG_CHECK(codec == TEZGPU_CODEC_NONE || codec == TEZGPU_CODEC_DEFAULT || codec == TEZGPU_CODEC_LZ4 || codec == TEZGPU_CODEC_ZSTD,
-           TEZGPU_E_UNSUPPORTED, "codec " + std::to_string(codec) + " is not on the device (DefaultCodec, Lz4Codec and ZStandardCodec only)");
+  TG_CHECK(codec == TEZGPU_CODEC_NONE || codec == TEZGPU_CODEC_DEFAULT || codec == TEZGPU_CODEC_LZ4 || codec == TEZGPU_CODEC_ZSTD ||
+               codec == TEZGPU_CODEC_SNAPPY,
+           TEZGPU_E_UNSUPPORTED, "codec " + std::to_string(codec) + " is not on the device (DefaultCodec, Lz4Codec, ZStandardCodec and SnappyCodec only)");
 }
 
 // How a codec's compressed segment is laid out around its chunks.  zlib: 32 KiB chunks, framed by
-// TIF\x01 78 01 | chunks | Adler-32 CRC; LZ4: blocks of one chunk each (their 8 header bytes in the slot), framed by
-// TIF\x01 | blocks | CRC; zstd: one frame per chunk, framed by TIF\x01 | frames | CRC.
+// TIF\x01 78 01 | chunks | Adler-32 CRC; LZ4 and Snappy: blocks of one chunk each (their 8 header bytes in the slot),
+// framed by TIF\x01 | blocks | CRC; zstd: one frame per chunk, framed by TIF\x01 | frames | CRC.
 struct CodecLayout {
   uint64_t chunk;   // body bytes per chunk
   uint32_t slot;    // device bytes reserved per compressed chunk
@@ -32,6 +35,7 @@ inline CodecLayout codec_layout(int32_t codec) {
   switch (codec) {
     case TEZGPU_CODEC_LZ4: return {L4_BLOCK, L4_SLOT, 8, 4, 0};
     case TEZGPU_CODEC_ZSTD: return {ZS_BLOCK, ZS_SLOT, 8, 4, 0};
+    case TEZGPU_CODEC_SNAPPY: return {SN_BLOCK, SN_SLOT, 8, 4, 0};
     default: return {ZCHUNK, ZSLOT, 14, 6, 4};
   }
 }
@@ -86,7 +90,7 @@ __global__ void k_zpack(const uint8_t *__restrict__ slots, const uint32_t *__res
   for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
 }
 
-// per block-framed (LZ4, zstd) segment: TIF\x01 and the CRC-32 of the stream (the chunks' raw remainders are in seg_crc)
+// per block-framed (LZ4, zstd, Snappy) segment: TIF\x01 and the CRC-32 of the stream (the chunks' raw remainders are in seg_crc)
 __global__ void k_zfinish_blocks(const ZSeg *__restrict__ segs, uint32_t P, const uint32_t *__restrict__ seg_crc,
                                  const CrcTables *__restrict__ t, uint8_t *__restrict__ out) {
   const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -147,6 +151,11 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
         k_zscompress<<<nchunks, ZS_LANES, sizeof(ZsShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
                                                                  z_csize.as<uint32_t>());
         break;
+      case TEZGPU_CODEC_SNAPPY:
+        set_smem_limit<k_sncompress>(conf.device, sizeof(SnShared));
+        k_sncompress<<<nchunks, SN_LANES, sizeof(SnShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
+                                                                 z_csize.as<uint32_t>());
+        break;
       default:
         set_smem_limit<k_zdeflate>(conf.device, sizeof(ZShared));
         z_cadler.ensure((size_t)nchunks * 4);
@@ -184,6 +193,7 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
     switch (codec) {
       case TEZGPU_CODEC_LZ4:
       case TEZGPU_CODEC_ZSTD:
+      case TEZGPU_CODEC_SNAPPY:
         k_zfinish_blocks<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_crc.as<uint32_t>(), d_crc, d_out);
         break;
       default:
@@ -218,6 +228,7 @@ static inline const char *codec_err_name(int32_t codec, int32_t rc) {
   switch (codec) {
     case TEZGPU_CODEC_LZ4: return l4_err_name(rc);
     case TEZGPU_CODEC_ZSTD: return zs_err_name(rc);
+    case TEZGPU_CODEC_SNAPPY: return sn_err_name(rc);
     default: return z_err_name(rc);
   }
 }
@@ -270,7 +281,8 @@ inline void Merger::open_codec(const tezgpu_segment *in, const int64_t *raw_len,
 // per segment.  LZ4: one thread per segment walks the block headers (one host round trip for the block count), one warp
 // per block decodes, and a segment the block pass could not take is decoded again serially by one warp.  zstd: the same
 // shape with frames: a segment whose frames all carry Frame_Content_Size is decoded one warp per frame, any other one
-// warp per segment.  Returns once every image is complete; errors name the caller's segment index.
+// warp per segment.  Snappy: the walk makes every chunk a unit (each states its raw length), one warp per chunk
+// decodes, and each segment reports its first error in stream order.  Returns once every image is complete; errors name the caller's segment index.
 inline void Merger::decode_compressed(const tezgpu_segment *in, const int64_t *raw_len, const std::vector<uint32_t> &zs) {
   cudaStream_t st = pipe.stream;
   TG_CHECK(raw_len, TEZGPU_E_INVALID, "segment " + std::to_string(zs[0]) + " is compressed: its raw length is required");
@@ -358,6 +370,33 @@ inline void Merger::decode_compressed(const tezgpu_segment *in, const int64_t *r
     case TEZGPU_CODEC_ZSTD:
       decode_units(k_zswalk<0>, k_zswalk<1>, k_zsframes, k_zsserial, ZSD_WARPS, "too many zstd frames in one merge");
       break;
+    case TEZGPU_CODEC_SNAPPY: {
+      // the count walk (and the walk errors), one host round trip for the chunk counts, the fill walk, one warp per
+      // chunk, and the image frames with each segment's first error
+      z_nblk.ensure((size_t)nz * 4);
+      z_slow.ensure((size_t)nz * 8);
+      unsigned long long *err = reinterpret_cast<unsigned long long *>(z_slow.p);
+      k_snwalk<0><<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), nullptr, nullptr, err);
+      launches++;
+      TG_CUDA(cudaGetLastError());
+      std::vector<uint32_t> nunit(nz), base(nz);
+      TG_CUDA(cudaMemcpyAsync(nunit.data(), z_nblk.p, (size_t)nz * 4, cudaMemcpyDeviceToHost, st));
+      TG_CUDA(cudaStreamSynchronize(st));
+      uint64_t nu = 0;
+      for (uint32_t i = 0; i < nz; i++) { base[i] = (uint32_t)nu; nu += nunit[i]; }
+      TG_CHECK(nu < (1ull << 32), TEZGPU_E_INVALID, "too many Snappy chunks in one merge");
+      if (nu) {
+        z_base.ensure((size_t)nz * 4);
+        z_blks.ensure((size_t)nu * sizeof(ZUnit));
+        TG_CUDA(cudaMemcpyAsync(z_base.p, base.data(), (size_t)nz * 4, cudaMemcpyHostToDevice, st));
+        k_snwalk<1><<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_nblk.as<uint32_t>(), z_base.as<uint32_t>(),
+                                                               z_blks.as<ZUnit>(), err);
+        k_snchunks<<<(uint32_t)div_up(nu, SNDEC_WARPS), SNDEC_WARPS * 32, 0, st>>>(z_blks.as<ZUnit>(), (uint32_t)nu, err);
+        launches += 2;
+      }
+      k_snfinish<<<(uint32_t)div_up(nz, 128), 128, 0, st>>>(z_insegs.as<ZInSeg>(), nz, err, z_status.as<int32_t>());
+      break;
+    }
     default:
       k_zinflate<<<(uint32_t)div_up(nz, ZINF_WARPS), ZINF_WARPS * 32, 0, st>>>(z_insegs.as<ZInSeg>(), nz, z_status.as<int32_t>());
   }
@@ -393,7 +432,12 @@ constexpr uint64_t DECODE_BYTES_PER_SEGMENT = 128;    // descriptors, statuses, 
 constexpr uint64_t DECODE_MIN_UNIT_BYTES = 8;         // the smallest LZ4 block or zstd frame: a decode unit per 8 bytes
 
 inline uint64_t decode_group_bytes(int32_t codec, uint64_t len, uint64_t raw) {
-  const uint64_t units = codec == TEZGPU_CODEC_DEFAULT ? 0 : len / DECODE_MIN_UNIT_BYTES + 1;
+  uint64_t units;
+  switch (codec) {
+    case TEZGPU_CODEC_DEFAULT: units = 0; break;
+    case TEZGPU_CODEC_SNAPPY: units = len / SN_MIN_UNIT_BYTES + 1; break;   // and the 8-byte error words, within the 128
+    default: units = len / DECODE_MIN_UNIT_BYTES + 1;
+  }
   const uint64_t pieces = div_up(len, CRC_PIECE) + div_up(raw + 4, CRC_PIECE);
   return align_up(len, 16) + align_up(raw + 4, 16) + units * sizeof(ZUnit) + pieces * sizeof(TileCrc) + DECODE_BYTES_PER_SEGMENT;
 }
@@ -487,11 +531,17 @@ static inline std::vector<uint8_t> l4_compress_host(const uint8_t *body, uint64_
 static inline std::vector<uint8_t> zs_compress_host(const uint8_t *body, uint64_t len) {
   return blocks_compress_host<ZsShared>(body, len, ZS_BLOCK, ZS_SLOT, 0, zs_compress_block_host);
 }
+// Snappy: the blocks, each its 8 header bytes and one chunk (tezgpu_debug_snappy_compress_emulate)
+static inline std::vector<uint8_t> sn_compress_host(const uint8_t *body, uint64_t len) {
+  return blocks_compress_host<SnShared>(body, len, SN_BLOCK, SN_SLOT, 8, sn_compress_block_host);
+}
 
 // worst case of the compressed file given the uncompressed file's bound.  zlib: every chunk stored.  LZ4: every block
 // all literals (one token, (n - 15) / 255 + 1 length bytes) plus its 8 header bytes.  zstd: every frame raw (10 bytes
-// of frame and block header).
+// of frame and block header).  Snappy: every block all literals (3 preamble and 3 literal-tag bytes) plus its 8 header
+// bytes.
 inline uint64_t SortPipeline::codec_bound(int codec, uint64_t raw_bound, int P) {
+  if (codec == TEZGPU_CODEC_SNAPPY) return raw_bound + 14 * (raw_bound / SN_BLOCK + (uint64_t)P + 1) + 64;
   if (codec == TEZGPU_CODEC_ZSTD) return raw_bound + 10 * (raw_bound / ZS_BLOCK + (uint64_t)P + 1) + 64;
   if (codec == TEZGPU_CODEC_LZ4) return raw_bound + raw_bound / 255 + 10 * (raw_bound / L4_BLOCK + (uint64_t)P + 1) + 64;
   return raw_bound + 5 * (raw_bound / ZCHUNK + (uint64_t)P + 1) + 11ull * P + 64;

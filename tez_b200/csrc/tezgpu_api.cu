@@ -397,7 +397,7 @@ uint64_t tezgpu_sorter_device_output_bound(const tezgpu_sorter *h, uint64_t n, u
 }
 
 uint64_t tezgpu_debug_device_output_bound(int32_t num_partitions, int32_t codec, uint64_t n, uint64_t kv_bytes) {
-  if (num_partitions < 1 || codec < TEZGPU_CODEC_NONE || codec > TEZGPU_CODEC_ZSTD) return 0;
+  if (num_partitions < 1 || codec < TEZGPU_CODEC_NONE || codec > TEZGPU_CODEC_SNAPPY) return 0;
   return device_output_bound(num_partitions, codec, n, kv_bytes);
 }
 
@@ -540,6 +540,16 @@ int32_t tezgpu_debug_zstd_decompress_emulate(const uint8_t *z, uint64_t len, uin
     std::unique_ptr<ZsDec> d(new ZsDec());
     return zs_decompress(z, len, out, body_len, got, *d);
   });
+}
+
+int32_t tezgpu_debug_snappy_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len) {
+  return compress_emulate(sn_compress_host, body, len, out, cap, out_len);
+}
+
+int32_t tezgpu_debug_snappy_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
+                                               uint64_t *out_len) {
+  return decompress_emulate(TEZGPU_CODEC_SNAPPY, z, len, body_len, out, cap, out_len,
+                            [&](uint64_t *got) { return sn_decompress(z, len, out, body_len, got); });
 }
 
 int32_t tezgpu_debug_crc_concat_emulate(const uint8_t *const *bodies, const uint64_t *lens, uint32_t n, uint32_t *crc) {

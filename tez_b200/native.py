@@ -155,7 +155,8 @@ class GpuSorter:
         """combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG runs MRCombiner with IntSumReducer / LongSumReducer on every
         flush (tezgpu_sorter_set_combiner).  codec: CODEC_DEFAULT writes zlib-compressed segments, CODEC_LZ4 Lz4Codec
         segments (blocks of LZ4_BLOCK_BYTES raw bytes, one chunk each), CODEC_ZSTD ZStandardCodec segments (one frame per
-        ZSTD_BLOCK_BYTES raw bytes) (tezgpu_sorter_set_codec).  split_points: the serialized split keys of a
+        ZSTD_BLOCK_BYTES raw bytes), CODEC_SNAPPY SnappyCodec segments (blocks of SNAPPY_BLOCK_BYTES raw bytes, one chunk
+        each) (tezgpu_sorter_set_codec).  split_points: the serialized split keys of a
         partitioner=PART_TOTAL_ORDER handle, searched in split_order (a CMP_*; None = the handle's comparator)
         (tezgpu_sorter_set_split_points)."""
         self.L = _lib.load()
@@ -179,7 +180,7 @@ class GpuSorter:
         check(self.L.tezgpu_sorter_set_combiner(self.h, combiner))
 
     def set_codec(self, codec):
-        """CODEC_NONE / CODEC_DEFAULT / CODEC_LZ4 / CODEC_ZSTD; before the first collect (or after reset); survives reset."""
+        """CODEC_NONE / CODEC_DEFAULT / CODEC_LZ4 / CODEC_ZSTD / CODEC_SNAPPY; before the first collect (or after reset); survives reset."""
         check(self.L.tezgpu_sorter_set_codec(self.h, codec))
 
     def set_split_points(self, split_points, order=None):
@@ -286,8 +287,8 @@ class GpuMerger:
         verified: optional per-segment booleans -- the transport already checked that segment's checksum
         (TEZGPU_SEG_VERIFIED: fetch_segments_verified), the merge does not read it again to verify.
         combiner: COMBINE_SUM_INT / COMBINE_SUM_LONG combines the merged stream in write_* (tezgpu_merge_set_combiner).
-        codec: CODEC_DEFAULT (zlib), CODEC_LZ4 (Lz4Codec) or CODEC_ZSTD (ZStandardCodec) reads compressed (TIF\\x01) segments of that codec and writes
-        compressed output (tezgpu_merge_open_codec); raw_lens: per-segment rawLength, required for the compressed
+        codec: CODEC_DEFAULT (zlib), CODEC_LZ4 (Lz4Codec), CODEC_ZSTD (ZStandardCodec) or CODEC_SNAPPY (SnappyCodec) reads
+        compressed (TIF\\x01) segments of that codec and writes compressed output (tezgpu_merge_open_codec); raw_lens: per-segment rawLength, required for the compressed
         segments.
         concat: UnorderedPartitionedKVWriter.mergeAll / UnorderedKVReader (tezgpu_concat_open): records leave in
         (segment, position) order, the writes copy the record bytes (rle must be False).

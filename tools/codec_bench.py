@@ -1,9 +1,10 @@
-"""DefaultCodec, Lz4Codec and ZStandardCodec cost on the device: one JSON line per case, no-codec, zlib, LZ4 and zstd runs
-alternating in one process (the *_lz4 fields are Lz4Codec's, the *_zstd fields ZStandardCodec's).
+"""DefaultCodec, Lz4Codec, ZStandardCodec and SnappyCodec cost on the device: one JSON line per case, no-codec, zlib,
+LZ4, zstd and Snappy runs alternating in one process (the *_lz4 fields are Lz4Codec's, the *_zstd fields
+ZStandardCodec's, the *_snappy fields SnappyCodec's).
 
   1. config-2 map side: 1e8 random 80-byte records, P = 64, sort_device_fixed (the stored / all-literal path)
   2. compressible map side: Text words drawn from a Zipf law with IntWritable 1 values, sort_device_fixed
-  3. reduce side: config-3 segments compressed on the host (zlib level 1; LZ4 and zstd by the device writers' host
+  3. reduce side: config-3 segments compressed on the host (zlib level 1; LZ4, zstd and Snappy by the device writers' host
      emulations, zstd's frames taking the one-warp-per-frame path; zstd also as libzstd level-3 one-frame streams
      without content size, the one-warp-per-segment path, where libzstd can be loaded), reopen + write_ifile_device
   4. e2e through host buffers: collect_batch + flush_to_memory of the case-2 records
@@ -35,11 +36,12 @@ def card():
 
 
 def zcap(raw, P):
-    """room for the zlib (every chunk stored), the LZ4 (every block all literals) and the zstd (every frame raw) worst case"""
+    """room for the zlib (every chunk stored), the LZ4 and Snappy (every block all literals) and the zstd (every frame
+    raw) worst case"""
     return raw + raw // 255 + 10 * (raw // 32768 + P + 1) + 11 * P + 64
 
 
-CODECS = (0, T.CODEC_LZ4, T.CODEC_ZSTD, T.CODEC_DEFAULT)   # zlib last: the compressible case reads its output back
+CODECS = (0, T.CODEC_LZ4, T.CODEC_ZSTD, T.CODEC_SNAPPY, T.CODEC_DEFAULT)   # zlib last: the compressible case reads its output back
 
 
 def lz4_stream(body):
@@ -59,6 +61,16 @@ def zstd_stream(body):
     out = (C.c_uint8 * cap)()
     n = C.c_uint64()
     T._lib.check(L.tezgpu_debug_zstd_compress_emulate(body, len(body), out, cap, C.byref(n)))
+    return bytes(out[:n.value])
+
+
+def snappy_stream(body):
+    """the device writer's Snappy stream of one body, run on the host (tezgpu_debug_snappy_compress_emulate)"""
+    L = T._lib.load()
+    cap = len(body) + 14 * (len(body) // T.SNAPPY_BLOCK_BYTES + 2) + 64
+    out = (C.c_uint8 * cap)()
+    n = C.c_uint64()
+    T._lib.check(L.tezgpu_debug_snappy_compress_emulate(body, len(body), out, cap, C.byref(n)))
     return bytes(out[:n.value])
 
 
@@ -136,6 +148,11 @@ def map_side(name, kv, kl, vl, cmp_kind, P, runs, out):
                 ms_runs_zstd=[round(x, 2) for x in res[T.CODEC_ZSTD]])
     extra = line["ms_zstd"] - line["ms_no_codec"]
     line["compress_gbps_derived_zstd"] = round(raw / extra / 1e6, 2) if extra > 0 else None
+    nlen = lens[T.CODEC_SNAPPY][0]
+    line.update(compressed_bytes_snappy=nlen, ratio_snappy=round(nlen / raw, 4), ms_snappy=round(min(res[T.CODEC_SNAPPY]), 2),
+                ms_runs_snappy=[round(x, 2) for x in res[T.CODEC_SNAPPY]])
+    extra = line["ms_snappy"] - line["ms_no_codec"]
+    line["compress_gbps_derived_snappy"] = round(raw / extra / 1e6, 2) if extra > 0 else None
     if name == "compressible":
         # zlib level 1 on the same bodies (the first 8 partitions)
         host = d_out[:zlen].cpu().numpy().tobytes()
@@ -164,6 +181,7 @@ def reduce_side(nseg, seg_bytes, runs, out):
     with ThreadPoolExecutor(16) as ex:
         lsegs = [b"TIF\x01" + z + zlib.crc32(z).to_bytes(4, "big") for z in ex.map(lambda p: lz4_stream(p[4:-4]), plain)]
         ssegs = [b"TIF\x01" + z + zlib.crc32(z).to_bytes(4, "big") for z in ex.map(lambda p: zstd_stream(p[4:-4]), plain)]
+        nsegs = [b"TIF\x01" + z + zlib.crc32(z).to_bytes(4, "big") for z in ex.map(lambda p: snappy_stream(p[4:-4]), plain)]
         jz = list(ex.map(lambda p: libzstd_level3(p[4:-4]), plain))
     jsegs = None if jz[0] is None else [b"TIF\x01" + z + zlib.crc32(z).to_bytes(4, "big") for z in jz]
     if jsegs is None:
@@ -171,11 +189,12 @@ def reduce_side(nseg, seg_bytes, runs, out):
     mz = T.GpuMerger(zsegs, comparator=T.CMP_TEXT, codec=T.CODEC_DEFAULT, raw_lens=raws)
     ml = T.GpuMerger(lsegs, comparator=T.CMP_TEXT, codec=T.CODEC_LZ4, raw_lens=raws)
     ms_ = T.GpuMerger(ssegs, comparator=T.CMP_TEXT, codec=T.CODEC_ZSTD, raw_lens=raws)
+    mn = T.GpuMerger(nsegs, comparator=T.CMP_TEXT, codec=T.CODEC_SNAPPY, raw_lens=raws)
     mp = T.GpuMerger(plain, comparator=T.CMP_TEXT)
-    cap = max(mz.output_bound(), ml.output_bound(), ms_.output_bound(), mp.output_bound())
+    cap = max(mz.output_bound(), ml.output_bound(), ms_.output_bound(), mn.output_bound(), mp.output_bound())
     d_out = torch.empty(cap, dtype=torch.uint8, device="cuda")
     res = {c: [] for c in CODECS + ("java",)}
-    arms = [(0, mp, plain), (T.CODEC_DEFAULT, mz, zsegs), (T.CODEC_LZ4, ml, lsegs), (T.CODEC_ZSTD, ms_, ssegs)]
+    arms = [(0, mp, plain), (T.CODEC_DEFAULT, mz, zsegs), (T.CODEC_LZ4, ml, lsegs), (T.CODEC_ZSTD, ms_, ssegs), (T.CODEC_SNAPPY, mn, nsegs)]
     if jsegs is not None:
         arms.append(("java", ms_, jsegs))
     for r in range(runs + 1):
@@ -197,6 +216,8 @@ def reduce_side(nseg, seg_bytes, runs, out):
                 ms_runs_lz4=[round(x, 2) for x in res[T.CODEC_LZ4]],
                 compressed_in_bytes_zstd=sum(len(z) for z in ssegs), ms_zstd=round(min(res[T.CODEC_ZSTD]), 2),
                 ms_runs_zstd=[round(x, 2) for x in res[T.CODEC_ZSTD]],
+                compressed_in_bytes_snappy=sum(len(z) for z in nsegs), ms_snappy=round(min(res[T.CODEC_SNAPPY]), 2),
+                ms_runs_snappy=[round(x, 2) for x in res[T.CODEC_SNAPPY]],
                 note="codec: reads compressed segments and writes a compressed merged segment")
     if jsegs is not None:
         line.update(compressed_in_bytes_zstd_libzstd3=sum(len(z) for z in jsegs), ms_zstd_libzstd3=round(min(res["java"]), 2),
@@ -205,6 +226,7 @@ def reduce_side(nseg, seg_bytes, runs, out):
     mz.close()
     ml.close()
     ms_.close()
+    mn.close()
     mp.close()
 
 
@@ -233,7 +255,8 @@ def e2e(kv, kl, vl, cmp_kind, P, runs, out):
                     kv_gbps_codec=round(kv.size / min(res[1]) / 1e6, 2), down_bytes_lz4=moved[T.CODEC_LZ4],
                     ms_lz4=round(min(res[T.CODEC_LZ4]), 1), kv_gbps_lz4=round(kv.size / min(res[T.CODEC_LZ4]) / 1e6, 2),
                     down_bytes_zstd=moved[T.CODEC_ZSTD], ms_zstd=round(min(res[T.CODEC_ZSTD]), 1),
-                    kv_gbps_zstd=round(kv.size / min(res[T.CODEC_ZSTD]) / 1e6, 2)))
+                    kv_gbps_zstd=round(kv.size / min(res[T.CODEC_ZSTD]) / 1e6, 2), down_bytes_snappy=moved[T.CODEC_SNAPPY],
+                    ms_snappy=round(min(res[T.CODEC_SNAPPY]), 1), kv_gbps_snappy=round(kv.size / min(res[T.CODEC_SNAPPY]) / 1e6, 2)))
 
 
 def main():
