@@ -538,6 +538,11 @@ uint32_t tezgpu_debug_run_fold_emulate(const uint8_t *data, uint32_t nchunks);
  * in pieces, any record size). */
 int32_t tezgpu_debug_fixed_emit_plan(uint32_t klen, uint32_t vlen, int32_t layout, int32_t *kernel, uint32_t *recs_per_tile);
 
+/* diagnostics: the launch shape of fixed-width emit kernel `kernel` (numbered as in tezgpu_debug_fixed_emit_plan) over
+ * `tiles` tiles on `device`: *ctas CTAs of *groups_per_cta persistent tile groups each.  Group g of CTA b emits tile
+ * b * groups_per_cta + g, then every (ctas * groups_per_cta)-th tile. */
+int32_t tezgpu_debug_emit_grid(int32_t device, int32_t kernel, uint64_t tiles, uint32_t *ctas, uint32_t *groups_per_cta);
+
 /* diagnostics: tezgpu_sorter_device_output_bound of a handle with num_partitions partitions and codec (TEZGPU_CODEC_*),
  * computed without a device; 0 for num_partitions < 1 or an unknown codec */
 uint64_t tezgpu_debug_device_output_bound(int32_t num_partitions, int32_t codec, uint64_t n, uint64_t kv_bytes);

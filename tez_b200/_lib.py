@@ -83,6 +83,7 @@ SYMBOLS = [
     ("tezgpu_debug_chunk_fold_emulate", C.c_uint32, [_V, C.c_uint32, C.c_int32]),
     ("tezgpu_debug_run_fold_emulate", C.c_uint32, [_V, C.c_uint32]),
     ("tezgpu_debug_fixed_emit_plan", C.c_int32, [C.c_uint32, C.c_uint32, C.c_int32, _P(C.c_int32), _P(C.c_uint32)]),
+    ("tezgpu_debug_emit_grid", C.c_int32, [C.c_int32, C.c_int32, C.c_uint64, _P(C.c_uint32), _P(C.c_uint32)]),
     ("tezgpu_debug_device_output_bound", C.c_uint64, [C.c_int32, C.c_int32, C.c_uint64, C.c_uint64]),
     ("tezgpu_debug_deflate_emulate", C.c_int32, [_V, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),
     ("tezgpu_debug_inflate_emulate", C.c_int32, [_V, C.c_uint64, C.c_uint64, _V, C.c_uint64, _P(C.c_uint64)]),

@@ -165,6 +165,42 @@ static inline FixedEmitPlan plan_fixed_emit(const Records &rec, uint32_t rec_siz
   return {FixedEmitKernel::PipeUnaligned, best};
 }
 
+// persistent CTAs of a one-group emit kernel over `tiles` tiles: as many as fit the device at once
+template <typename Kern>
+static inline uint32_t persistent_ctas(Kern kern, int threads, size_t smem, int num_sms, uint64_t tiles) {
+  int per_sm = 0;
+  TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+  return (uint32_t)std::min<uint64_t>(tiles, (uint64_t)num_sms * (per_sm > 0 ? per_sm : 1));
+}
+
+// Launch shape of a fixed-width emit kernel over `tiles` tiles: `ctas` CTAs of `groups` independent tile groups; group
+// g of CTA b takes tile b * groups + g, then every (ctas * groups)-th.  Sets the kernel's shared-memory limit on
+// `device` first where it needs one, so the shape is the one the launch gets.
+struct EmitGrid {
+  uint32_t ctas, groups;
+};
+static inline EmitGrid fixed_emit_grid(int device, int num_sms, FixedEmitKernel kernel, uint64_t tiles) {
+  switch (kernel) {
+    case FixedEmitKernel::Pipe:
+      // One CTA per SM, FE4_GROUPS independent 256-thread groups sharing the lane-private checksum tables (66 KB)
+      // next to their images, indices and parked partials (54 KB): 125 KB keeps the CTA in the 132 KB
+      // shared-memory carveout, which leaves the random gather enough L1 for its loads in flight (larger
+      // footprints measured slower, DESIGN.md §7).
+      set_smem_limit<k_emit_fast4<FE4_UNROLL>>(device, Emit4Smem::TOTAL);
+      return {(uint32_t)std::min<uint64_t>(div_up(tiles, FE4_GROUPS), (uint64_t)num_sms), (uint32_t)FE4_GROUPS};
+    case FixedEmitKernel::Fast:
+      return {persistent_ctas(k_emit_fast<5, true>, FE_THREADS, 0, num_sms, tiles), 1};
+    case FixedEmitKernel::PipeUnaligned:
+      set_smem_limit<k_emit_fast4u<FE4U_UNROLL>>(device, Emit4uSmem::TOTAL);
+      return {persistent_ctas(k_emit_fast4u<FE4U_UNROLL>, FE_THREADS, Emit4uSmem::TOTAL, num_sms, tiles), 1};
+    case FixedEmitKernel::FastUnaligned:
+      return {persistent_ctas(k_emit_fast<5, false>, FE_THREADS, 0, num_sms, tiles), 1};
+    case FixedEmitKernel::General:
+      break;
+  }
+  return {persistent_ctas(k_emit<true>, EMIT_THREADS, 0, num_sms, tiles), 1};
+}
+
 class SortPipeline {
  public:
   tezgpu_conf conf;
@@ -648,39 +684,25 @@ class SortPipeline {
     }
     timer.mark(stream);
     if (tiles) {
-      // persistent CTAs: as many as fit the device at once
-      auto persistent_grid = [&](auto kern, int threads, size_t smem) {
-        int per_sm = 0;
-        TG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
-        return (uint32_t)std::min<uint64_t>(tiles, (uint64_t)num_sms * (per_sm > 0 ? per_sm : 1));
-      };
       if (!fixed_emit) {
-        k_emit<false><<<persistent_grid(k_emit<false>, EMIT_THREADS, 0), EMIT_THREADS, 0, stream>>>(e);
+        k_emit<false><<<persistent_ctas(k_emit<false>, EMIT_THREADS, 0, num_sms, tiles), EMIT_THREADS, 0, stream>>>(e);
       } else {
+        const uint32_t grid = fixed_emit_grid(conf.device, num_sms, kernel, tiles).ctas;
         switch (kernel) {
-          case FixedEmitKernel::Pipe: {
-            // One CTA per SM, FE4_GROUPS independent 256-thread groups sharing the lane-private checksum tables (66 KB)
-            // next to their images, indices and parked partials (54 KB): 125 KB keeps the CTA in the 132 KB
-            // shared-memory carveout, which leaves the random gather enough L1 for its loads in flight (larger
-            // footprints measured slower, DESIGN.md §7).
-            set_smem_limit<k_emit_fast4<FE4_UNROLL>>(conf.device, Emit4Smem::TOTAL);
-            const uint32_t grid = (uint32_t)std::min<uint64_t>(div_up(tiles, FE4_GROUPS), (uint64_t)num_sms);
+          case FixedEmitKernel::Pipe:
             k_emit_fast4<FE4_UNROLL><<<grid, FE_THREADS * FE4_GROUPS, Emit4Smem::TOTAL, stream>>>(fp);
             break;
-          }
           case FixedEmitKernel::Fast:
-            k_emit_fast<5, true><<<persistent_grid(k_emit_fast<5, true>, FE_THREADS, 0), FE_THREADS, 0, stream>>>(fp);
+            k_emit_fast<5, true><<<grid, FE_THREADS, 0, stream>>>(fp);
             break;
           case FixedEmitKernel::PipeUnaligned:
-            set_smem_limit<k_emit_fast4u<FE4U_UNROLL>>(conf.device, Emit4uSmem::TOTAL);
-            k_emit_fast4u<FE4U_UNROLL><<<persistent_grid(k_emit_fast4u<FE4U_UNROLL>, FE_THREADS, Emit4uSmem::TOTAL), FE_THREADS,
-                                         Emit4uSmem::TOTAL, stream>>>(fp);
+            k_emit_fast4u<FE4U_UNROLL><<<grid, FE_THREADS, Emit4uSmem::TOTAL, stream>>>(fp);
             break;
           case FixedEmitKernel::FastUnaligned:
-            k_emit_fast<5, false><<<persistent_grid(k_emit_fast<5, false>, FE_THREADS, 0), FE_THREADS, 0, stream>>>(fp);
+            k_emit_fast<5, false><<<grid, FE_THREADS, 0, stream>>>(fp);
             break;
           case FixedEmitKernel::General:
-            k_emit<true><<<persistent_grid(k_emit<true>, EMIT_THREADS, 0), EMIT_THREADS, 0, stream>>>(e);
+            k_emit<true><<<grid, EMIT_THREADS, 0, stream>>>(e);
             break;
         }
       }

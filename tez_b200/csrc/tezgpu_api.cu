@@ -962,6 +962,20 @@ int32_t tezgpu_debug_fixed_emit_plan(uint32_t klen, uint32_t vlen, int32_t layou
   TG_API_END
 }
 
+int32_t tezgpu_debug_emit_grid(int32_t device, int32_t kernel, uint64_t tiles, uint32_t *ctas, uint32_t *groups_per_cta) {
+  TG_API_BEGIN
+  TG_CHECK(ctas && groups_per_cta, TEZGPU_E_INVALID, "null argument");
+  TG_CHECK(kernel >= 0 && kernel <= (int32_t)FixedEmitKernel::General, TEZGPU_E_INVALID, "kernel must be 0 to 4 (tezgpu_debug_fixed_emit_plan)");
+  TG_CHECK(tiles < (1ull << 32), TEZGPU_E_INVALID, "more than 2^32-1 tiles");
+  DeviceScope ds(device);
+  int sms = 0;
+  TG_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  const EmitGrid g = fixed_emit_grid(device, sms, (FixedEmitKernel)kernel, tiles);
+  *ctas = g.ctas;
+  *groups_per_cta = g.groups;
+  TG_API_END
+}
+
 }  // extern "C"
 
 #include "merger_api.inl"
