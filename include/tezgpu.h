@@ -417,7 +417,8 @@ int32_t tezgpu_merge_write_partitions(tezgpu_merger *m, const char *out_path, co
  * SORT/TezMerger.java:717-912): the k-way merge of tezgpu_merge_open_codec over HOST segments, holding at most
  * budget_bytes of device memory.  budget_bytes = 0: the device's free memory at open; a budget below
  * TEZGPU_MERGE_BUDGET_MIN fails with TEZGPU_E_INVALID, a device segment (TEZGPU_SEG_DEVICE) too.  codec must be
- * TEZGPU_CODEC_NONE (else TEZGPU_E_UNSUPPORTED); raw_len is not read.
+ * TEZGPU_CODEC_NONE (else TEZGPU_E_UNSUPPORTED; compressed output: tezgpu_merge_open_bounded_write_codec); raw_len is
+ * not read.
  *   When the inputs fit the budget with one record per input byte (the worst case of the workspace bound in DESIGN
  *   section 3, "Bounded-memory merge"), the handle takes one step: exactly tezgpu_merge_open.  Otherwise it merges in
  *   key-range steps over windows of the segments; when the first step's windows hold every segment whole and the
@@ -432,6 +433,17 @@ int32_t tezgpu_merge_write_partitions(tezgpu_merger *m, const char *out_path, co
 #define TEZGPU_MERGE_BUDGET_MIN (16ull << 20)
 int32_t tezgpu_merge_open_bounded(const tezgpu_conf *conf, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg,
                                   int32_t codec, uint64_t budget_bytes, tezgpu_merger **out);
+/* The bounded merge with compressed output: tezgpu_merge_open_bounded over the same uncompressed HOST segments, budget
+ * and checks (same codes and messages), whose writes compress with write_codec (TEZGPU_CODEC_NONE, _DEFAULT, _LZ4,
+ * _ZSTD or _SNAPPY; any other fails with TEZGPU_E_UNSUPPORTED before any device call).  NONE: exactly
+ * tezgpu_merge_open_bounded.  A handle that takes one step is exactly tezgpu_merge_open_codec(conf, segs, NULL, nseg,
+ * write_codec).  With several steps, write_ifile and write_partitions write the file and index that handle writes,
+ * byte for byte (rawLength uncompressed, partLength compressed): every step compresses its pieces on the codec's chunk
+ * grid of each partition, so the budget includes the compression workspace (DESIGN section 3).  stats are as the
+ * codec writes give them (physical bytes compressed, ms_total with the compression), output_bound bounds the
+ * compressed bytes once the counts are known; everything else is as for tezgpu_merge_open_bounded. */
+int32_t tezgpu_merge_open_bounded_write_codec(const tezgpu_conf *conf, const tezgpu_segment *segs, uint32_t nseg,
+                                              int32_t write_codec, uint64_t budget_bytes, tezgpu_merger **out);
 /* steps the last pass over the inputs took (1 for a one-step handle), the most device memory the handle's buffers
  * held at once, and the bytes uploaded from the host segments by all passes.  TEZGPU_E_STATE on a handle that was
  * not opened bounded. */
@@ -446,7 +458,7 @@ int32_t tezgpu_merge_bounded_info(tezgpu_merger *m, int32_t *steps, uint64_t *pe
  * (may be NULL) receives the most device memory the call held at once.  A segment that does not fit the budget on its
  * own fails with TEZGPU_E_NOMEM naming it and its sizes.  TEZGPU_E_INVALID: a device segment, a budget below
  * TEZGPU_MERGE_BUDGET_MIN, raw_len NULL (with nseg > 0), out[i] NULL for a compressed segment.  TEZGPU_E_UNSUPPORTED:
- * a codec other than TEZGPU_CODEC_DEFAULT, _LZ4 and _ZSTD.  Runs on conf->device; conf's other fields are checked as
+ * a codec other than TEZGPU_CODEC_DEFAULT, _LZ4, _ZSTD and _SNAPPY.  Runs on conf->device; conf's other fields are checked as
  * for a merge. */
 int32_t tezgpu_decode_segments(const tezgpu_conf *conf, const tezgpu_segment *segs, const int64_t *raw_len, uint32_t nseg,
                                int32_t codec, uint64_t budget_bytes, uint8_t *const *out, uint64_t *peak_device_bytes);
@@ -573,6 +585,14 @@ int32_t tezgpu_debug_zstd_decompress_emulate(const uint8_t *z, uint64_t len, uin
 int32_t tezgpu_debug_snappy_compress_emulate(const uint8_t *body, uint64_t len, uint8_t *out, uint64_t cap, uint64_t *out_len);
 int32_t tezgpu_debug_snappy_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
                                                uint64_t *out_len);
+/* the compressed write of a bounded merge that takes several steps, on the host: the body (len >= 1 bytes) of one
+ * partition cut into pieces at the ncuts non-decreasing offsets cuts[], each piece compressed as a step compresses it
+ * (the chunk grid from the body's start, the carry of the bytes after the last whole chunk, zlib's open chunks and
+ * Adler-32 fold, the CRC-32 fold, checked against the stream).  out receives the codec stream, which is
+ * tezgpu_debug_{deflate,lz4_compress,zstd_compress,snappy_compress}_emulate of the uncut body.  codec: _DEFAULT, _LZ4,
+ * _ZSTD or _SNAPPY. */
+int32_t tezgpu_debug_stitched_compress_emulate(int32_t codec, const uint8_t *body, uint64_t len, const uint64_t *cuts, uint32_t ncuts,
+                                               uint8_t *out, uint64_t cap, uint64_t *out_len);
 
 /* diagnostics: the 32-bit sort words the variable-width map side gives n keys (key i = kv[key_off[i] ..
  * key_off[i] + key_len[i])), computed on the host with the device's code: the alphabet table built from the byte values

@@ -102,6 +102,9 @@ SYMBOLS = [
     ("tezgpu_merge_reopen_codec", C.c_int32, [_V, _P(Segment), _V, C.c_uint32]),
     ("tezgpu_concat_open", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, _P(_V)]),
     ("tezgpu_merge_open_bounded", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, C.c_uint64, _P(_V)]),
+    ("tezgpu_merge_open_bounded_write_codec", C.c_int32, [_P(Conf), _P(Segment), C.c_uint32, C.c_int32, C.c_uint64, _P(_V)]),
+    ("tezgpu_debug_stitched_compress_emulate", C.c_int32, [C.c_int32, _V, C.c_uint64, _V, C.c_uint32, _V, C.c_uint64,
+                                                            _P(C.c_uint64)]),
     ("tezgpu_merge_bounded_info", C.c_int32, [_V, _P(C.c_int32), _P(C.c_uint64), _P(C.c_uint64)]),
     ("tezgpu_decode_segments", C.c_int32, [_P(Conf), _P(Segment), _V, C.c_uint32, C.c_int32, C.c_uint64, _V, _P(C.c_uint64)]),
     ("tezgpu_debug_crc_concat_emulate", C.c_int32, [_V, _V, C.c_uint32, _P(C.c_uint32)]),

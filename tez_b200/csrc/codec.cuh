@@ -103,6 +103,66 @@ __global__ void k_zfinish_blocks(const ZSeg *__restrict__ segs, uint32_t P, cons
   store_be32(o + s.zlen - 4, crc);
 }
 
+// The chunks of the segments hs[0, nseg) in codec zc (host table: body_off into img, body_len, chunk0, nchunks, rank,
+// open; nchunks chunks in all, at least one): each compressed into its slot of z_slots (sizes z_csize, zlib's Adler-32 values
+// z_cadler), their file offsets z_coff, the segments' zstart / zlen (frame: segment bytes outside its chunks) back in
+// hs and on the device in z_segs, and z_crc[s] = the raw CRC remainder of segment s's chunk bytes followed by `tail`
+// zero bytes.  One host round trip (the layout).  Returns the chunk bytes; *launches counts the kernels.
+inline uint64_t SortPipeline::compress_chunks(int32_t zc, const uint8_t *img, ZSeg *hs, uint32_t nseg, uint32_t nchunks,
+                                              uint32_t frame, uint32_t tail, int *launches) {
+  cudaStream_t st = stream;
+  const CodecLayout L = codec_layout(zc);
+  z_segs.ensure((size_t)nseg * sizeof(ZSeg));
+  TG_CUDA(cudaMemcpyAsync(z_segs.p, hs, (size_t)nseg * sizeof(ZSeg), cudaMemcpyHostToDevice, st));
+  z_slots.ensure((size_t)nchunks * L.slot);
+  z_csize.ensure((size_t)nchunks * 4);
+  z_coff.ensure(((size_t)nchunks + 2) * 8);
+  switch (zc) {
+    case TEZGPU_CODEC_LZ4:
+      set_smem_limit<k_l4compress>(conf.device, sizeof(L4Shared));
+      k_l4compress<<<nchunks, L4_LANES, sizeof(L4Shared), st>>>(img, z_segs.as<ZSeg>(), nseg, z_slots.as<uint8_t>(), z_csize.as<uint32_t>());
+      break;
+    case TEZGPU_CODEC_ZSTD:
+      set_smem_limit<k_zscompress>(conf.device, sizeof(ZsShared));
+      k_zscompress<<<nchunks, ZS_LANES, sizeof(ZsShared), st>>>(img, z_segs.as<ZSeg>(), nseg, z_slots.as<uint8_t>(), z_csize.as<uint32_t>());
+      break;
+    case TEZGPU_CODEC_SNAPPY:
+      set_smem_limit<k_sncompress>(conf.device, sizeof(SnShared));
+      k_sncompress<<<nchunks, SN_LANES, sizeof(SnShared), st>>>(img, z_segs.as<ZSeg>(), nseg, z_slots.as<uint8_t>(), z_csize.as<uint32_t>());
+      break;
+    default:
+      set_smem_limit<k_zdeflate>(conf.device, sizeof(ZShared));
+      z_cadler.ensure((size_t)nchunks * 4);
+      k_zdeflate<<<nchunks, ZLANES, sizeof(ZShared), st>>>(img, z_segs.as<ZSeg>(), nseg, z_slots.as<uint8_t>(), z_csize.as<uint32_t>(),
+                                                          z_cadler.as<uint32_t>());
+  }
+  *launches += 1 + scan_u32_exclusive(st, blk, z_csize.as<uint32_t>(), nchunks, z_coff.as<uint64_t>());
+  k_zseg_layout<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), nseg, z_coff.as<uint64_t>(), frame);
+  // checksums of the chunks (k_crc_pieces, one piece per chunk), placed in their segments and folded per segment
+  const CrcTables *d_crc = DeviceConstants::get(conf.device).d_crc;
+  z_descs.ensure((size_t)nchunks * sizeof(SegDesc));
+  z_pstart.ensure(((size_t)nchunks + 1) * 4);
+  z_tc.ensure((size_t)nchunks * sizeof(TileCrc));
+  z_crc.ensure((size_t)nseg * 4);
+  TG_CUDA(cudaMemsetAsync(z_crc.p, 0, (size_t)nseg * 4, st));
+  k_zchunk_descs<<<(uint32_t)div_up((uint64_t)nchunks + 1, 256), 256, 0, st>>>(z_csize.as<uint32_t>(), nchunks, L.slot,
+                                                                            z_descs.as<SegDesc>(), z_pstart.as<uint32_t>());
+  k_crc_pieces<<<nchunks, CRCV_THREADS, 0, st>>>(z_slots.as<uint8_t>(), z_descs.as<SegDesc>(), z_pstart.as<uint32_t>(), nchunks, d_crc,
+                                                 z_tc.as<TileCrc>());
+  k_zcrc_place<<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, z_segs.as<ZSeg>(), nseg,
+                                                              z_coff.as<uint64_t>(), tail);
+  k_crc_combine<<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, d_crc, z_crc.as<uint32_t>());
+  *launches += 5;
+  TG_CUDA(cudaGetLastError());
+  TG_CUDA(cudaMemcpyAsync(hs, z_segs.p, (size_t)nseg * sizeof(ZSeg), cudaMemcpyDeviceToHost, st));
+  TG_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(hs) + (size_t)nseg * sizeof(ZSeg), z_coff.as<uint64_t>() + nchunks, 8,
+                          cudaMemcpyDeviceToHost, st));
+  TG_CUDA(cudaStreamSynchronize(st));
+  uint64_t cbytes;
+  memcpy(&cbytes, reinterpret_cast<uint8_t *>(hs) + (size_t)nseg * sizeof(ZSeg), 8);
+  return cbytes;
+}
+
 // The uncompressed file is in z_img with its index raw_index (start, rawLength, partLength per partition).  Every
 // partition that has a segment gets a compressed one: TIF\x01, the codec stream of the same body (zlib, or LZ4 blocks),
 // CRC-32 of the stream.  index receives (start, the same rawLength, compressed length).  One host round trip (the
@@ -135,59 +195,10 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
   int launches = 0;
   uint64_t total = 0;
   if (nchunks) {
-    z_segs.ensure((size_t)P * sizeof(ZSeg));
-    TG_CUDA(cudaMemcpyAsync(z_segs.p, hs, (size_t)P * sizeof(ZSeg), cudaMemcpyHostToDevice, st));
-    z_slots.ensure((size_t)nchunks * L.slot);
-    z_csize.ensure((size_t)nchunks * 4);
-    z_coff.ensure(((size_t)nchunks + 2) * 8);
-    switch (codec) {
-      case TEZGPU_CODEC_LZ4:
-        set_smem_limit<k_l4compress>(conf.device, sizeof(L4Shared));
-        k_l4compress<<<nchunks, L4_LANES, sizeof(L4Shared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
-                                                                 z_csize.as<uint32_t>());
-        break;
-      case TEZGPU_CODEC_ZSTD:
-        set_smem_limit<k_zscompress>(conf.device, sizeof(ZsShared));
-        k_zscompress<<<nchunks, ZS_LANES, sizeof(ZsShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
-                                                                 z_csize.as<uint32_t>());
-        break;
-      case TEZGPU_CODEC_SNAPPY:
-        set_smem_limit<k_sncompress>(conf.device, sizeof(SnShared));
-        k_sncompress<<<nchunks, SN_LANES, sizeof(SnShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
-                                                                 z_csize.as<uint32_t>());
-        break;
-      default:
-        set_smem_limit<k_zdeflate>(conf.device, sizeof(ZShared));
-        z_cadler.ensure((size_t)nchunks * 4);
-        k_zdeflate<<<nchunks, ZLANES, sizeof(ZShared), st>>>(z_img.as<uint8_t>(), z_segs.as<ZSeg>(), (uint32_t)P, z_slots.as<uint8_t>(),
-                                                            z_csize.as<uint32_t>(), z_cadler.as<uint32_t>());
-    }
-    launches += 1 + scan_u32_exclusive(st, blk, z_csize.as<uint32_t>(), nchunks, z_coff.as<uint64_t>());
-    k_zseg_layout<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_coff.as<uint64_t>(), L.frame);
-    launches++;
-    TG_CUDA(cudaGetLastError());
-    TG_CUDA(cudaMemcpyAsync(hs, z_segs.p, (size_t)P * sizeof(ZSeg), cudaMemcpyDeviceToHost, st));
-    TG_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(hs) + (size_t)P * sizeof(ZSeg), z_coff.as<uint64_t>() + nchunks, 8,
-                            cudaMemcpyDeviceToHost, st));
-    TG_CUDA(cudaStreamSynchronize(st));
-    uint64_t cbytes;
-    memcpy(&cbytes, reinterpret_cast<uint8_t *>(hs) + (size_t)P * sizeof(ZSeg), 8);
+    const uint64_t cbytes = compress_chunks(codec, z_img.as<uint8_t>(), hs, (uint32_t)P, nchunks, L.frame, L.tail, &launches);
     total = cbytes + L.frame * nsegs;
     TG_CHECK(total <= out_cap, TEZGPU_E_NOMEM, "output buffer too small for the compressed file.out");
-    // checksums of the chunks (k_crc_pieces, one piece per chunk), placed in their segments and folded per segment
     const CrcTables *d_crc = DeviceConstants::get(conf.device).d_crc;
-    z_descs.ensure((size_t)nchunks * sizeof(SegDesc));
-    z_pstart.ensure(((size_t)nchunks + 1) * 4);
-    z_tc.ensure((size_t)nchunks * sizeof(TileCrc));
-    z_crc.ensure((size_t)P * 4);
-    TG_CUDA(cudaMemsetAsync(z_crc.p, 0, (size_t)P * 4, st));
-    k_zchunk_descs<<<(uint32_t)div_up((uint64_t)nchunks + 1, 256), 256, 0, st>>>(z_csize.as<uint32_t>(), nchunks, L.slot,
-                                                                              z_descs.as<SegDesc>(), z_pstart.as<uint32_t>());
-    k_crc_pieces<<<nchunks, CRCV_THREADS, 0, st>>>(z_slots.as<uint8_t>(), z_descs.as<SegDesc>(), z_pstart.as<uint32_t>(), nchunks, d_crc,
-                                                   z_tc.as<TileCrc>());
-    k_zcrc_place<<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, z_segs.as<ZSeg>(), (uint32_t)P,
-                                                                z_coff.as<uint64_t>(), L.tail);
-    k_crc_combine<<<(uint32_t)div_up(nchunks, 256), 256, 0, st>>>(z_tc.as<TileCrc>(), nchunks, d_crc, z_crc.as<uint32_t>());
     k_zpack<<<nchunks, 256, 0, st>>>(z_slots.as<uint8_t>(), z_csize.as<uint32_t>(), z_coff.as<uint64_t>(), z_segs.as<ZSeg>(), (uint32_t)P,
                                      L.slot, L.head, d_out);
     switch (codec) {
@@ -200,7 +211,7 @@ inline void SortPipeline::compress_image(const int64_t *raw_index, uint8_t *d_ou
         k_zfinish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(z_segs.as<ZSeg>(), (uint32_t)P, z_cadler.as<uint32_t>(), z_csize.as<uint32_t>(),
                                                            z_crc.as<uint32_t>(), d_crc, d_out);
     }
-    launches += 6;
+    launches += 2;
     TG_CUDA(cudaGetLastError());
   }
   z_timer.mark(st);

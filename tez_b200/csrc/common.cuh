@@ -155,6 +155,9 @@ struct ZSeg {
   uint64_t rank;       // segments before this partition
   uint64_t zstart;     // out: file offset of the compressed segment
   uint64_t zlen;       // out: its length (0: no segment)
+  uint32_t open;       // the body continues after these chunks (a bounded merge's open partition): zlib ends the
+                       // last chunk with the sync-flush block instead of marking it final
+  uint32_t pad;
 };
 
 // chunk c -> its partition: the last p with chunk0 <= c (partitions without a segment own no chunk)

@@ -474,7 +474,7 @@ __global__ void __launch_bounds__(ZLANES)
   const uint32_t clen = (uint32_t)z_min64(ZCHUNK, sg.body_len - a);
   const uint8_t *src = img + sg.body_off + a;
   for (uint32_t i = tid; i < clen; i += ZLANES) sh.data[i] = src[i];
-  if (tid == 0) { sh.clen = clen; sh.last = (k + 1 == sg.nchunks) ? 1 : 0; }
+  if (tid == 0) { sh.clen = clen; sh.last = (k + 1 == sg.nchunks && !sg.open) ? 1 : 0; }
   __syncthreads();
   z_lane<1>(sh, tid, nullptr);
   __syncthreads();

@@ -17,11 +17,21 @@
 // Writes stitch the pieces every step emits: TIF\0 only at the start of a partition, the FF FF EOF markers and the
 // checksum only at its end; the checksum of a partition is folded from the trailers of its pieces (k_stitch_raw,
 // k_crc_combine, k_stitch_finish), so the output is byte-identical to the one-step merge.
+//
+// Compressed writes (tezgpu_merge_open_bounded_write_codec) compress every step's pieces on the codec's chunk grid,
+// counted from the start of each partition's body, so the stream is the one the one-step merge writes: a piece that
+// closes its partition is compressed whole; of the partition the step leaves open only the whole chunks before the
+// piece's last byte are, and the bytes after them (1 to one chunk) wait in a device carry buffer for the partition's
+// next piece.  zlib chunks of an open piece end with the sync-flush block like every inner chunk (ZSeg::open); 78 01
+// is written at a partition's start and the Adler-32 at its end, folded from the chunks' values; the CRC-32 of the
+// compressed bytes is folded across steps like the uncompressed one (k_zstitch_fold, k_zstitch_finish).
 #pragma once
 #include <algorithm>
+#include <memory>
 #include <string>
 #include <vector>
 
+#include "codec.cuh"
 #include "merger.cuh"
 
 namespace tezgpu {
@@ -221,6 +231,167 @@ __global__ void k_stitch_finish(const uint32_t *__restrict__ part_raw, const uin
   crc[p] = crc_from_raw(t, part_raw[p] ^ t->eof_raw, part_body[p] + 2);
 }
 
+// ------------------------------------------------------------------------------------------------ compressed writes
+// Room in front of a step's uncompressed image (DESIGN.md section 3): bytes [0, 2) hold the EOF markers an empty
+// segment compresses, a partition that closes without records of its own compresses its carry and FF FF from
+// [2, 4 + carry), and the carry of a continuing partition is put right in front of its piece in the image.
+constexpr uint64_t STEP_CARRY_ROOM = 65536;
+static_assert(STEP_CARRY_ROOM >= 4 + 4 + L4_BLOCK && L4_BLOCK == ZS_BLOCK && L4_BLOCK == SN_BLOCK && ZCHUNK < L4_BLOCK,
+              "the room holds the EOF markers, the largest carry with its own, and a step image's first TIF header");
+// workspace of one pass per chunk: its slot, its packed bytes (at most a slot), its size, offset, Adler-32, CRC
+// descriptor, piece start and remainder; per partition: the piece table, the running CRC and Adler-32, the chunk
+// bytes and the trailer; fixed: the carry, the room and the scan's block sums with the buffers' rounding
+constexpr uint64_t STEP_CODEC_BYTES_PER_CHUNK_TABLE = 80;
+constexpr uint64_t STEP_CODEC_BYTES_PER_PARTITION = 128;
+constexpr uint64_t STEP_CODEC_FIXED_BYTES = 1ull << 20;
+
+// One piece of a partition's body on the chunk grid: the piece's own n bytes lie at `off` in its source, the carry (the
+// bytes of the partition after its last compressed chunk) right before them.
+struct StitchPlan {
+  uint64_t off;       // first byte compressed now (the carry's first byte)
+  uint64_t len;       // bytes compressed now: whole chunks, or everything when the piece closes the partition
+  uint64_t carry;     // bytes after them, kept for the partition's next piece (at most one chunk)
+  uint32_t nchunks;
+  uint32_t open;      // the partition continues: the last chunk is not the stream's last
+};
+inline StitchPlan plan_stitch_piece(uint64_t chunk, uint64_t carry, uint64_t off, uint64_t n, bool closes) {
+  StitchPlan s;
+  const uint64_t all = carry + n;
+  s.off = off - carry;
+  s.open = closes ? 0 : 1;
+  if (closes) {
+    s.nchunks = (uint32_t)std::max<uint64_t>(1, div_up(all, chunk));
+    s.len = all;
+  } else {
+    // the chunk the piece ends in waits, also a whole one: only the close tells whether it is the stream's last (zlib
+    // marks it final, and a closing piece of no bytes of its own must not add an empty chunk)
+    s.nchunks = (uint32_t)(all ? (all - 1) / chunk : 0);
+    s.len = (uint64_t)s.nchunks * chunk;
+  }
+  s.carry = all - s.len;
+  return s;
+}
+
+// raw CRC remainder (zero initial value, no final xor) of n bytes, bitwise: the host check of the folds below
+static inline uint32_t crc_raw_host(const uint8_t *p, uint64_t n) {
+  uint32_t c = 0;
+  for (uint64_t i = 0; i < n; i++) {
+    c ^= p[i];
+    for (int k = 0; k < 8; k++) c = (c & 1) ? CRC_POLY ^ (c >> 1) : (c >> 1);
+  }
+  return c;
+}
+
+// one chunk through the host run of a codec's device chunk writer, appended to out (zlib: *adler = its Adler-32)
+class ChunkHost {
+ public:
+  explicit ChunkHost(int32_t codec) : codec_(codec), slot_(codec_layout(codec).slot) {
+    switch (codec) {
+      case TEZGPU_CODEC_LZ4: l4_.reset(new L4Shared()); break;
+      case TEZGPU_CODEC_ZSTD: zs_.reset(new ZsShared()); break;
+      case TEZGPU_CODEC_SNAPPY: sn_.reset(new SnShared()); break;
+      default: z_.reset(new ZShared());
+    }
+  }
+  void run(const uint8_t *p, uint32_t clen, bool last, std::vector<uint8_t> &out, uint32_t *adler) {
+    uint32_t n;
+    switch (codec_) {
+      case TEZGPU_CODEC_LZ4: l4_compress_block_host(*l4_, p, clen, slot_.data()); n = 8 + l4_->bytes; break;
+      case TEZGPU_CODEC_ZSTD: zs_compress_block_host(*zs_, p, clen, slot_.data()); n = zs_->bytes; break;
+      case TEZGPU_CODEC_SNAPPY: sn_compress_block_host(*sn_, p, clen, slot_.data()); n = 8 + sn_->bytes; break;
+      default:
+        z_deflate_chunk_host(*z_, p, clen, last, slot_.data());
+        n = z_->bytes;
+        *adler = z_->adler;
+    }
+    out.insert(out.end(), slot_.begin(), slot_.begin() + n);
+  }
+
+ private:
+  int32_t codec_;
+  std::vector<uint8_t> slot_;
+  std::unique_ptr<ZShared> z_;
+  std::unique_ptr<L4Shared> l4_;
+  std::unique_ptr<ZsShared> zs_;
+  std::unique_ptr<SnShared> sn_;
+};
+
+// Host run of the compressed write across steps over one partition body cut into pieces at cuts[0, ncuts)
+// (tezgpu_debug_stitched_compress_emulate): the carry, plan_stitch_piece, the open flag, the Adler-32 fold and the CRC
+// fold of the device path, piece by piece.  Returns the codec stream (zlib: 78 01, chunks, Adler-32), which equals the
+// stream of the uncut body.
+static inline std::vector<uint8_t> stitched_compress_host(int32_t codec, const uint8_t *body, uint64_t len, const uint64_t *cuts,
+                                                          uint32_t ncuts) {
+  const CodecLayout L = codec_layout(codec);
+  const bool zlib = codec == TEZGPU_CODEC_DEFAULT;
+  ChunkHost ch(codec);
+  std::vector<uint8_t> stream, src, carry, piece;
+  if (zlib) stream = {0x78, 0x01};
+  uint32_t adler = 1, raw = 0;   // the body's Adler-32 and the chunk bytes' CRC remainder, folded piece by piece
+  for (uint32_t i = 0; i <= ncuts; i++) {
+    const uint64_t a = i ? cuts[i - 1] : 0, b = i < ncuts ? cuts[i] : len;
+    TG_CHECK(a <= b && b <= len, TEZGPU_E_INVALID, "cuts must be non-decreasing offsets into the body");
+    const bool closes = i == ncuts;
+    src = carry;
+    src.insert(src.end(), body + a, body + b);
+    const StitchPlan pl = plan_stitch_piece(L.chunk, carry.size(), carry.size(), b - a, closes);
+    piece.clear();
+    for (uint32_t k = 0; k < pl.nchunks; k++) {
+      const uint64_t c0 = (uint64_t)k * L.chunk;
+      const uint32_t clen = (uint32_t)std::min<uint64_t>(L.chunk, pl.len - c0);
+      uint32_t ca = 1;
+      ch.run(src.data() + pl.off + c0, clen, !pl.open && k + 1 == pl.nchunks, piece, &ca);
+      if (zlib) adler = z_adler_combine(adler, ca, clen);
+    }
+    raw = crc_multmodp(raw, crc_host_xpow8(piece.size())) ^ crc_raw_host(piece.data(), piece.size());
+    stream.insert(stream.end(), piece.begin(), piece.end());
+    carry.assign(src.begin() + pl.off + pl.len, src.end());
+  }
+  const uint64_t h = zlib ? 2 : 0;
+  TG_CHECK(raw == crc_raw_host(stream.data() + h, stream.size() - h), TEZGPU_E_INVALID,
+           "the folded CRC differs from the CRC of the stitched stream");
+  if (zlib)
+    for (int b = 3; b >= 0; b--) stream.push_back((uint8_t)(adler >> (8 * b)));
+  return stream;
+}
+
+// Per piece of one pass (the pieces of a pass are distinct partitions): the raw CRC remainder of its chunk bytes
+// (seg_crc) and, for zlib, its chunks' Adler-32 values folded into the partition's running values: acc[2p] = remainder
+// of the partition's chunk bytes so far, acc[2p + 1] = Adler-32 of its body so far.
+__global__ void k_zstitch_fold(const ZSeg *__restrict__ segs, const uint32_t *__restrict__ part, uint32_t n,
+                               const uint32_t *__restrict__ seg_crc, const uint32_t *__restrict__ cadler,
+                               const CrcTables *__restrict__ t, uint32_t *__restrict__ acc) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const ZSeg s = segs[i];
+  const uint32_t p = part[i];
+  acc[2 * p] = crc_shift_bytes(t, acc[2 * p], s.zlen) ^ seg_crc[i];
+  if (!cadler) return;
+  uint32_t a = acc[2 * p + 1];
+  for (uint32_t k = 0; k < s.nchunks; k++)
+    a = z_adler_combine(a, cadler[s.chunk0 + k], z_min64(ZCHUNK, s.body_len - (uint64_t)k * ZCHUNK));
+  acc[2 * p + 1] = a;
+}
+
+// per partition with a segment (zb[p]: its chunk bytes): the CRC-32 trailer of its stream; zlib: of 78 01, the chunks
+// and the big-endian Adler-32
+__global__ void k_zstitch_finish(const uint32_t *__restrict__ acc, const uint64_t *__restrict__ zb, uint32_t P, int zlib,
+                                 const CrcTables *__restrict__ t, uint32_t *__restrict__ crc) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P || !zb[p]) return;
+  if (!zlib) {
+    crc[p] = crc_from_raw(t, acc[2 * p], zb[p]);
+    return;
+  }
+  uint32_t hraw = 0, araw = 0;
+  hraw = t->slice[0][(hraw ^ 0x78) & 0xFF] ^ (hraw >> 8);
+  hraw = t->slice[0][(hraw ^ 0x01) & 0xFF] ^ (hraw >> 8);
+  const uint32_t adler = acc[2 * p + 1];
+  for (int b = 3; b >= 0; b--) araw = t->slice[0][(araw ^ (adler >> (8 * b))) & 0xFF] ^ (araw >> 8);
+  const uint32_t raw = crc_shift_bytes(t, hraw, zb[p] + 4) ^ crc_shift_bytes(t, acc[2 * p], 4) ^ araw;
+  crc[p] = crc_from_raw(t, raw, zb[p] + 6);
+}
+
 // ------------------------------------------------------------------------------------------------ host loop
 class BoundedMerge {
  public:
@@ -247,19 +418,33 @@ class BoundedMerge {
   std::vector<uint32_t> win_seg;           // window -> caller's segment
   std::vector<StepScan> scans;
   std::vector<StepCut> cuts;
+  int32_t zcodec = TEZGPU_CODEC_NONE;      // the codec of the written segments (the steps' Merger writes uncompressed)
+  DeviceBuffer d_carry, d_zout, d_zpart, d_zacc, d_zb, d_zcrc;
+  PinnedBuffer h_zout;
 
   BoundedMerge(Merger &mm, uint64_t b, DeviceTally &t) : m(mm), budget(b), tally(t) {}
 
+  // device bytes of one compression pass per chunk (DESIGN.md section 3)
+  uint64_t codec_chunk_bytes() const { return 2ull * codec_layout(zcodec).slot + STEP_CODEC_BYTES_PER_CHUNK_TABLE; }
   uint64_t fixed_bytes() const {
-    return STEP_FIXED_BYTES + STEP_FIXED_PER_PARTITION * (uint64_t)m.pipe.conf.num_partitions +
-           STEP_FIXED_PER_SEGMENT * (uint64_t)in.size();
+    const uint64_t P = (uint64_t)m.pipe.conf.num_partitions;
+    uint64_t b = STEP_FIXED_BYTES + STEP_FIXED_PER_PARTITION * P + STEP_FIXED_PER_SEGMENT * (uint64_t)in.size();
+    // a compressed write: the chunks no image byte pays for (one per piece, the carry's), the tables, room and carry
+    if (zcodec)
+      b += (P + 3) * codec_chunk_bytes() + STEP_CODEC_BYTES_PER_PARTITION * P + 2 * STEP_CARRY_ROOM + STEP_CODEC_FIXED_BYTES;
+    return b;
   }
   uint64_t need(uint64_t w, uint64_t kv, uint64_t n) const {
-    return STEP_BYTES_PER_WINDOW_BYTE * w + STEP_BYTES_PER_KV_BYTE * kv + STEP_BYTES_PER_RECORD * n + fixed_bytes();
+    uint64_t b = STEP_BYTES_PER_WINDOW_BYTE * w + STEP_BYTES_PER_KV_BYTE * kv + STEP_BYTES_PER_RECORD * n + fixed_bytes();
+    if (zcodec)   // the chunks of the step's uncompressed image
+      b += div_up(SortPipeline::output_bound(n, kv, m.pipe.conf.num_partitions), codec_layout(zcodec).chunk) * codec_chunk_bytes();
+    return b;
   }
 
+  // m.pipe.codec on entry: the codec the writes compress with (NONE: uncompressed)
   void open(const tezgpu_segment *segs, uint32_t nseg) {
     TallyScope ts(&tally);
+    zcodec = m.pipe.codec;
     uint64_t total = 0;
     in.assign(segs, segs + nseg);
     body0.resize(nseg); body_end.resize(nseg); stored.assign(nseg, 0); check_crc.assign(nseg, 0);
@@ -282,7 +467,7 @@ class BoundedMerge {
     // one step when the inputs fit with the worst case of one record per byte
     single = need(total + 64, total, total) <= budget;
     if (single) {
-      m.open(segs, nseg);
+      m.open(segs, nseg);   // with the write codec: what tezgpu_merge_open_codec does with uncompressed segments
       steps = 1;
       h2d = total;
       have_counts = true;
@@ -300,6 +485,7 @@ class BoundedMerge {
     std::stable_sort(pmajor.begin(), pmajor.end(), [&](uint32_t a, uint32_t b) { return in[a].partition < in[b].partition; });
     d_bad.ensure(16);
     d_split.ensure(16);
+    m.pipe.codec = TEZGPU_CODEC_NONE;   // the steps write uncompressed pieces; write_compressed compresses them
     // the first step runs here, as every other open parses its inputs before returning
     begin_pass();
     iter = 1;
@@ -309,6 +495,7 @@ class BoundedMerge {
       // the first step took every record: the Merger holds the whole merge, as after a one-step open (the checksums
       // have been checked, the host segments are no longer read)
       single = true;
+      m.pipe.codec = zcodec;
       end_pass();
       in.clear();
     }
@@ -561,7 +748,22 @@ class BoundedMerge {
 
   // ---- writes: every step's pieces stitched into one segment per partition.  out receives file.out, index the
   //      TezIndexRecord triples.
+  static void add_step_stats(tezgpu_stats &sum, const tezgpu_stats &s) {
+    sum.output_records += s.output_records;
+    sum.output_bytes += s.output_bytes;
+    sum.spilled_records += s.spilled_records;
+    sum.rle_used |= s.rle_used;
+    sum.adjacent_equal_keys += s.adjacent_equal_keys;
+    sum.tie_records += s.tie_records;
+    sum.ms_stage += s.ms_stage; sum.ms_sort += s.ms_sort; sum.ms_ties += s.ms_ties; sum.ms_emit += s.ms_emit; sum.ms_total += s.ms_total;
+    sum.kernel_launches += s.kernel_launches;
+  }
+
   void write(int rle, std::vector<uint8_t> &out, std::vector<int64_t> &index, tezgpu_stats *stats) {
+    if (zcodec) {
+      write_compressed(rle, out, index, stats);
+      return;
+    }
     TallyScope ts(&tally);
     cudaStream_t st = m.pipe.stream;
     const int P = m.pipe.conf.num_partitions;
@@ -620,14 +822,7 @@ class BoundedMerge {
         pieces.push_back(pc);
         part_body[p] += body;
       }
-      sum.output_records += s.output_records;
-      sum.output_bytes += s.output_bytes;
-      sum.spilled_records += s.spilled_records;
-      sum.rle_used |= s.rle_used;
-      sum.adjacent_equal_keys += s.adjacent_equal_keys;
-      sum.tie_records += s.tie_records;
-      sum.ms_stage += s.ms_stage; sum.ms_sort += s.ms_sort; sum.ms_ties += s.ms_ties; sum.ms_emit += s.ms_emit; sum.ms_total += s.ms_total;
-      sum.kernel_launches += s.kernel_launches;
+      add_step_stats(sum, s);
     }
     end_pass();
     if (cur >= 0) close_partition(cur);
@@ -662,6 +857,194 @@ class BoundedMerge {
     for (int p = 0; p < P; p++) sum.output_bytes_with_overhead += index[3 * p + 1];
     sum.output_bytes_physical = sum.file_out_bytes = (int64_t)out.size();
     sum.num_spills = 1;
+    if (stats) *stats = sum;
+  }
+
+  // ---- compressed writes (see the top of this file): the file and index the one-step merge with the codec writes.
+  //      Every step that has records writes its uncompressed image behind STEP_CARRY_ROOM bytes of m.d_out and runs
+  //      one pass over its pieces; one more pass after the last step closes what is left.
+  struct StitchJob {
+    uint32_t part;
+    uint64_t off;       // the piece's own bytes in m.d_out (in the room, or in the step image behind it)
+    uint64_t n;
+    bool starts;        // the partition's first piece: TIF\x01 (zlib: and 78 01) in front of it
+    bool closes;        // its last: the trailer after it
+    bool bytes;         // false: a partition without records and without a segment (send_empty_partition_details 1)
+  };
+
+  void write_compressed(int rle, std::vector<uint8_t> &out, std::vector<int64_t> &index, tezgpu_stats *stats) {
+    TallyScope ts(&tally);
+    SortPipeline &pp = m.pipe;
+    cudaStream_t st = pp.stream;
+    const int P = pp.conf.num_partitions;
+    const bool empty_segments = pp.conf.send_empty_partition_details == 0;   // as k_layout
+    const bool zlib = zcodec == TEZGPU_CODEC_DEFAULT;
+    const CodecLayout L = codec_layout(zcodec);
+    const CrcTables *d_crc = DeviceConstants::get(pp.conf.device).d_crc;
+    static const uint8_t kEof[2] = {0xFF, 0xFF};
+    static const uint8_t kHead[6] = {'T', 'I', 'F', 1, 0x78, 0x01};
+    begin_pass();
+    iter = 0;   // the windows are the write's now: a later next_batch starts from the beginning
+    out.clear();
+    index.assign((size_t)P * 3, 0);
+    std::vector<uint64_t> raw((size_t)P, 0), zb((size_t)P, 0);   // per partition: record bytes, compressed chunk bytes
+    std::vector<int64_t> zat((size_t)P, 0);                      // file offset of its segment
+    std::vector<uint32_t> acc((size_t)P * 2);                    // running CRC remainder and Adler-32 (k_zstitch_fold)
+    for (int p = 0; p < P; p++) { acc[2 * p] = 0; acc[2 * p + 1] = 1; }
+    d_zacc.ensure((size_t)P * 8);
+    TG_CUDA(cudaMemcpyAsync(d_zacc.p, acc.data(), (size_t)P * 8, cudaMemcpyHostToDevice, st));
+    d_carry.ensure(STEP_CARRY_ROOM);
+    tezgpu_stats sum;
+    memset(&sum, 0, sizeof(sum));
+    int cur = -1;            // the last partition with records so far
+    bool open = false;       // its segment continues in a later step
+    uint64_t carry = 0;      // its body bytes after its last compressed chunk, in d_carry
+    std::vector<StitchJob> jobs;
+    std::vector<uint32_t> part;
+    std::vector<uint32_t> seg_of;
+    auto done = [&](uint32_t p) {   // every segment of partition p has been read to its end
+      for (size_t s = 0; s < in.size(); s++)
+        if (in[s].partition == p && !finished[s]) return false;
+      return true;
+    };
+    auto close_open = [&] {   // the open partition has no records in this step: its carry and FF FF close it
+      if (open) jobs.push_back({(uint32_t)cur, 2 + carry, 2, false, true, true});
+      open = false;
+    };
+    auto skip_to = [&](int p) {   // partitions before p without records
+      for (int q = cur + 1; q < p; q++) jobs.push_back({(uint32_t)q, 0, 2, true, true, empty_segments});
+    };
+    // one pass: the pieces of `jobs` planned (plan_stitch_piece) and compressed, their bytes appended to out
+    auto pass = [&] {
+      m.d_out.ensure(STEP_CARRY_ROOM);
+      uint8_t *img = m.d_out.as<uint8_t>();
+      pp.z_timer.reset();
+      pp.z_timer.mark(st);
+      int launches = 0;
+      TG_CUDA(cudaMemcpyAsync(img, kEof, 2, cudaMemcpyHostToDevice, st));
+      pp.z_host.ensure(jobs.size() * sizeof(ZSeg) + 64);
+      ZSeg *hs = pp.z_host.as<ZSeg>();
+      seg_of.assign(jobs.size(), ~0u);
+      part.clear();
+      uint32_t nseg = 0, nchunks = 0;
+      for (size_t i = 0; i < jobs.size(); i++) {
+        const StitchJob &j = jobs[i];
+        if (!j.bytes) continue;
+        const uint64_t c = j.starts ? 0 : carry;   // only the open partition continues
+        if (c) TG_CUDA(cudaMemcpyAsync(img + j.off - c, d_carry.p, c, cudaMemcpyDeviceToDevice, st));
+        if (j.off < STEP_CARRY_ROOM) TG_CUDA(cudaMemcpyAsync(img + j.off, kEof, 2, cudaMemcpyHostToDevice, st));
+        const StitchPlan pl = plan_stitch_piece(L.chunk, c, j.off, j.n, j.closes);
+        if (pl.open) {
+          carry = pl.carry;
+          if (carry) TG_CUDA(cudaMemcpyAsync(d_carry.p, img + pl.off + pl.len, carry, cudaMemcpyDeviceToDevice, st));
+        }
+        if (!pl.nchunks) continue;
+        ZSeg &s = hs[nseg];
+        memset(&s, 0, sizeof(s));
+        s.body_off = pl.off;
+        s.body_len = pl.len;
+        s.chunk0 = nchunks;
+        s.nchunks = pl.nchunks;
+        s.rank = nseg;
+        s.open = pl.open;
+        seg_of[i] = nseg++;
+        part.push_back(j.part);
+        nchunks += pl.nchunks;
+      }
+      if (nchunks) {
+        const uint64_t cbytes = pp.compress_chunks(zcodec, img, hs, nseg, nchunks, 0, 0, &launches);
+        d_zout.ensure(cbytes);
+        d_zpart.ensure((size_t)nseg * 4);
+        TG_CUDA(cudaMemcpyAsync(d_zpart.p, part.data(), (size_t)nseg * 4, cudaMemcpyHostToDevice, st));
+        k_zpack<<<nchunks, 256, 0, st>>>(pp.z_slots.as<uint8_t>(), pp.z_csize.as<uint32_t>(), pp.z_coff.as<uint64_t>(), pp.z_segs.as<ZSeg>(),
+                                         nseg, L.slot, 0, d_zout.as<uint8_t>());
+        k_zstitch_fold<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(pp.z_segs.as<ZSeg>(), d_zpart.as<uint32_t>(), nseg, pp.z_crc.as<uint32_t>(),
+                                                                    zlib ? pp.z_cadler.as<uint32_t>() : nullptr, d_crc, d_zacc.as<uint32_t>());
+        launches += 2;
+        TG_CUDA(cudaGetLastError());
+        h_zout.ensure(cbytes);
+        TG_CUDA(cudaMemcpyAsync(h_zout.p, d_zout.p, cbytes, cudaMemcpyDeviceToHost, st));
+      }
+      pp.z_timer.mark(st);
+      TG_CUDA(cudaStreamSynchronize(st));
+      sum.ms_total += pp.z_timer.ms(0, 1);
+      sum.kernel_launches += launches;
+      for (size_t i = 0; i < jobs.size(); i++) {   // hs holds zstart / zlen of every piece with chunks
+        const StitchJob &j = jobs[i];
+        const uint32_t p = j.part;
+        if (!j.bytes) {
+          index[3 * p] = (int64_t)out.size();
+          continue;
+        }
+        if (j.starts) {
+          zat[p] = (int64_t)out.size();
+          out.insert(out.end(), kHead, kHead + (zlib ? 6 : 4));
+        }
+        if (seg_of[i] != ~0u) {
+          const ZSeg &s = hs[seg_of[i]];
+          const uint8_t *z = h_zout.as<uint8_t>() + s.zstart;
+          out.insert(out.end(), z, z + s.zlen);
+          zb[p] += s.zlen;
+        }
+        if (j.closes) {
+          out.insert(out.end(), zlib ? 8 : 4, 0);   // Adler-32 and CRC-32, from the folds below
+          index[3 * p] = zat[p];
+          index[3 * p + 1] = (int64_t)raw[p] + 6;
+          index[3 * p + 2] = (int64_t)out.size() - zat[p];
+        }
+      }
+      jobs.clear();
+    };
+    std::vector<int64_t> idx((size_t)P * 3);
+    while ((in_step = next_step())) {
+      if (!m.n) continue;
+      m.d_out.ensure(STEP_CARRY_ROOM + m.output_bound());
+      uint64_t len = 0;
+      tezgpu_stats s;
+      m.write_device(m.d_out.as<uint8_t>() + STEP_CARRY_ROOM, m.d_out.cap - STEP_CARRY_ROOM, rle, &len, idx.data(), &s);
+      add_step_stats(sum, s);
+      for (int p = 0; p < P; p++) {
+        const int64_t seglen = idx[3 * p + 2];
+        if (seglen <= 10) continue;   // no records of p in this step
+        const bool starts = p != cur;
+        if (starts) {
+          close_open();
+          skip_to(p);
+          cur = p;
+        }
+        const bool closes = done((uint32_t)p);
+        const uint64_t body = (uint64_t)seglen - 10;
+        jobs.push_back({(uint32_t)p, STEP_CARRY_ROOM + (uint64_t)idx[3 * p] + 4, body + (closes ? 2 : 0), starts, closes, true});
+        raw[p] += body;
+        open = !closes;
+      }
+      pass();
+    }
+    end_pass();
+    close_open();
+    skip_to(P);
+    if (!jobs.empty()) pass();
+    // ---- the trailers: CRC-32 of every segment's stream (and zlib's Adler-32) from the folded values
+    d_zb.ensure((size_t)P * 8);
+    d_zcrc.ensure((size_t)P * 4);
+    TG_CUDA(cudaMemcpyAsync(d_zb.p, zb.data(), (size_t)P * 8, cudaMemcpyHostToDevice, st));
+    k_zstitch_finish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(d_zacc.as<uint32_t>(), d_zb.as<uint64_t>(), (uint32_t)P, zlib ? 1 : 0, d_crc,
+                                                                d_zcrc.as<uint32_t>());
+    TG_CUDA(cudaGetLastError());
+    std::vector<uint32_t> crc((size_t)P);
+    TG_CUDA(cudaMemcpyAsync(acc.data(), d_zacc.p, (size_t)P * 8, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaMemcpyAsync(crc.data(), d_zcrc.p, (size_t)P * 4, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaStreamSynchronize(st));
+    for (int p = 0; p < P; p++) {
+      if (!zb[p]) continue;
+      uint8_t *e = out.data() + index[3 * p] + index[3 * p + 2];
+      if (zlib) store_be32(e - 8, acc[2 * p + 1]);
+      store_be32(e - 4, crc[p]);
+    }
+    for (int p = 0; p < P; p++) sum.output_bytes_with_overhead += index[3 * p + 1];
+    sum.output_bytes_physical = sum.file_out_bytes = (int64_t)out.size();
+    sum.num_spills = 1;
+    sum.kernel_launches += 1;
     if (stats) *stats = sum;
   }
 };

@@ -348,6 +348,7 @@ class SortPipeline {
   // worst case of the compressed file given the uncompressed file's bound (codec.cuh)
   static uint64_t codec_bound(int codec, uint64_t raw_bound, int P);
   void compress_image(const int64_t *raw_index, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index, tezgpu_stats *stats);
+  uint64_t compress_chunks(int32_t zc, const uint8_t *img, ZSeg *hs, uint32_t nseg, uint32_t nchunks, uint32_t frame, uint32_t tail, int *launches);
 
   // the emit of the sorted (merged) records: combined or not, compressed or not.  raw_bound bounds the uncompressed file.
   void emit_out(int rle, bool merge_mode, uint64_t raw_bound, uint8_t *d_out, uint64_t out_cap, uint64_t *out_len, int64_t *index,

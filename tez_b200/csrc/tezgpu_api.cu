@@ -546,6 +546,20 @@ int32_t tezgpu_debug_snappy_compress_emulate(const uint8_t *body, uint64_t len, 
   return compress_emulate(sn_compress_host, body, len, out, cap, out_len);
 }
 
+int32_t tezgpu_debug_stitched_compress_emulate(int32_t codec, const uint8_t *body, uint64_t len, const uint64_t *cuts, uint32_t ncuts,
+                                               uint8_t *out, uint64_t cap, uint64_t *out_len) {
+  TG_API_BEGIN
+  TG_CHECK((body || len == 0) && (cuts || ncuts == 0) && out && out_len, TEZGPU_E_INVALID, "null argument");
+  check_codec(codec);
+  TG_CHECK(codec != TEZGPU_CODEC_NONE, TEZGPU_E_INVALID, "tezgpu_debug_stitched_compress_emulate: no codec");
+  TG_CHECK(len > 0, TEZGPU_E_INVALID, "an IFile body holds at least its EOF markers");
+  const std::vector<uint8_t> z = stitched_compress_host(codec, body, len, cuts, ncuts);
+  *out_len = z.size();
+  TG_CHECK(z.size() <= cap, TEZGPU_E_NOMEM, "output buffer too small");
+  memcpy(out, z.data(), z.size());
+  TG_API_END
+}
+
 int32_t tezgpu_debug_snappy_decompress_emulate(const uint8_t *z, uint64_t len, uint64_t body_len, uint8_t *out, uint64_t cap,
                                                uint64_t *out_len) {
   return decompress_emulate(TEZGPU_CODEC_SNAPPY, z, len, body_len, out, cap, out_len,

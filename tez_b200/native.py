@@ -57,6 +57,21 @@ def debug_total_order(keys, split_points, comparator, order=None):
     return part[:len(keys)]
 
 
+def debug_stitched_compress(codec, body, cuts):
+    """The codec stream a bounded merge's compressed write gives one partition body that its steps cut at the offsets
+    `cuts`, computed on the host with the device path's chunk grid, carry and folds (tezgpu_debug_stitched_compress_emulate).
+    It equals the codec's stream of the uncut body."""
+    L = _lib.load()
+    body = bytes(body)
+    c = np.ascontiguousarray(cuts, dtype=np.uint64)
+    cap = len(body) + len(body) // 255 + 16 * (len(body) // 32768 + 2) + 64
+    out = np.empty(cap, dtype=np.uint8)
+    n = C.c_uint64()
+    check(L.tezgpu_debug_stitched_compress_emulate(codec, body, len(body), _ptr(c) if c.size else None, c.size, _ptr(out), cap,
+                                                   C.byref(n)))
+    return out[:n.value].tobytes()
+
+
 KeySample = collections.namedtuple("KeySample", "keys key_off key_len h gid")
 KeySample.__doc__ = """A sample of tezgpu_sample_keys, in gid order (numpy): keys uint8 (the keys back to back), key_off uint64,
 key_len uint32, h uint64 (splitmix64(seed ^ gid)), gid uint64 (the records' global numbers)."""
@@ -282,7 +297,7 @@ class GpuSorter:
 class GpuMerger:
     def __init__(self, segments, comparator=CMP_BYTES, device=0, has_header=True, device_ptrs=False, fixed=None,
                  partitions=None, num_partitions=1, send_empty=True, verified=None, combiner=COMBINE_NONE,
-                 codec=CODEC_NONE, raw_lens=None, concat=False, device_budget=None):
+                 codec=CODEC_NONE, raw_lens=None, concat=False, device_budget=None, write_codec=None):
         """segments: list of bytes / uint8 arrays (host) or (ptr, len) tuples when device_ptrs.
         verified: optional per-segment booleans -- the transport already checked that segment's checksum
         (TEZGPU_SEG_VERIFIED: fetch_segments_verified), the merge does not read it again to verify.
@@ -293,7 +308,12 @@ class GpuMerger:
         concat: UnorderedPartitionedKVWriter.mergeAll / UnorderedKVReader (tezgpu_concat_open): records leave in
         (segment, position) order, the writes copy the record bytes (rle must be False).
         device_budget: bytes of device memory the merge may hold (tezgpu_merge_open_bounded; 0 = the free memory):
-        host segments larger than that merge in key-range steps, with the same stream and output."""
+        host segments larger than that merge in key-range steps, with the same stream and output.
+        write_codec (with device_budget): the bounded merge of uncompressed host segments writes segments of this codec
+        (tezgpu_merge_open_bounded_write_codec), byte for byte what GpuMerger(codec=write_codec) writes."""
+        self.h = C.c_void_p()
+        if write_codec is not None and device_budget is None:
+            raise ValueError("write_codec is the codec of a bounded merge's writes: it needs device_budget (codec= otherwise)")
         self.L = _lib.load()
         self.conf = make_conf(num_partitions, comparator=comparator, partitioner=PART_GIVEN, device=device, fixed=fixed,
                               send_empty=send_empty)
@@ -302,7 +322,10 @@ class GpuMerger:
         arr = self._segments(segments, partitions, verified)
         self.h = C.c_void_p()
         self.bounded = device_budget is not None
-        if self.bounded:
+        if write_codec is not None:
+            check(self.L.tezgpu_merge_open_bounded_write_codec(C.byref(self.conf), arr, len(segments), write_codec,
+                                                               int(device_budget), C.byref(self.h)))
+        elif self.bounded:
             check(self.L.tezgpu_merge_open_bounded(C.byref(self.conf), arr, _ptr(self._raw(raw_lens)), len(segments), codec,
                                                    int(device_budget), C.byref(self.h)))
         elif concat:

@@ -14,6 +14,8 @@ timed region: every run's output has the CRC-32 trailer of its body, every uncom
 bytes (trailer and length; the one-step codec merge writes an Lz4Codec segment), and a sample of the
 segments merged under a 64 MiB budget is byte-exact against the oracle's TezMerger.  The card name and power limit are
 read in the same run.
+
+  --write-codec none,default,lz4,zstd,snappy: instead, the bounded merge's compressed write (write_codec_arm).
 """
 import argparse
 import ctypes as C
@@ -100,6 +102,63 @@ def run(variant, budget, segs, raws, out, imgs):
     return secs, n, steps, h2d, max(peak, decode_peak)
 
 
+WRITE_CODECS = {"none": None, "default": T.CODEC_DEFAULT, "lz4": T.CODEC_LZ4, "zstd": T.CODEC_ZSTD, "snappy": T.CODEC_SNAPPY}
+
+
+def write_codec_arm(args, plain, in_bytes, nseg, nrec, out):
+    """--write-codec: the compressed write of the bounded merge (tezgpu_merge_open_bounded_write_codec) at every budget,
+    beside the bounded uncompressed write at the same budgets and a one-step tezgpu_merge_open_codec write of the
+    whole input (which fits the device unbounded).  Times: host clock around open + write_ifile (rle = 0), one
+    warm-up run per arm, --reps runs.  GB/s are of the uncompressed output (rawLength); ratio = rawLength / partLength.
+    Parity: every bounded compressed write equals the one-step write of its codec byte for byte."""
+    name = card()
+    budgets = sorted((int(float(g) * (1 << 30)) for g in args.budgets_gib.split(",")), reverse=True)
+    for arm in [c for c in args.write_codec.split(",") if c]:
+        codec = WRITE_CODECS[arm]
+        ref, warm = None, False
+        for budget in ([0] if codec else []) + budgets:
+            def once():
+                t0 = time.perf_counter()
+                if budget:
+                    m = T.GpuMerger(plain, comparator=T.CMP_TEXT, device_budget=budget, write_codec=codec)
+                else:
+                    m = T.GpuMerger(plain, comparator=T.CMP_TEXT, codec=codec)
+                with m:
+                    raw, part = C.c_int64(), C.c_int64()
+                    _lib.check(_lib.load().tezgpu_merge_write_ifile(m.h, None, out.ctypes.data, out.size, 0, C.byref(raw),
+                                                                    C.byref(part), None))
+                    secs = time.perf_counter() - t0
+                    steps, peak, _ = m.bounded_info() if budget else (1, None, None)
+                return secs, raw.value, part.value, steps, peak
+            times = []
+            try:
+                if not warm:
+                    once()                                               # warm-up
+                    warm = True
+                for _ in range(args.reps):
+                    secs, raw, part, steps, peak = once()
+                    times.append(secs)
+            except _lib.TezGpuError as e:   # the one-step write of the whole input needs more than the device holds
+                if budget:
+                    raise
+                print(json.dumps({"bench": "bounded_merge_write_codec", "write_codec": arm, "open": "open_codec one step",
+                                  "input_bytes": in_bytes, "error": str(e), "card": name}), flush=True)
+                continue
+            digest = zlib.crc32(out[:part])
+            if ref is None:
+                ref = digest
+            s = sum(times) / len(times)
+            print(json.dumps({
+                "bench": "bounded_merge_write_codec", "write_codec": arm,
+                "open": "bounded_write_codec" if (budget and codec) else ("bounded" if budget else "open_codec one step"),
+                "budget_bytes": budget or None, "input_bytes": in_bytes, "segments": nseg, "records": int(sum(nrec)),
+                "raw_bytes": raw, "written_bytes": part, "ratio": round(raw / part, 3),
+                "ms_per_run": round(s * 1e3, 1), "ms_runs": [round(t * 1e3, 1) for t in times],
+                "raw_gbps": round(raw / s / 1e9, 3), "steps": steps, "peak_device_bytes": peak, "card": name,
+                "parity": {"same_bytes_as_one_step_write": digest == ref if codec else None}}), flush=True)
+            assert not codec or digest == ref, "bounded compressed write differs from the one-step write"
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gib", type=float, default=8.0, help="input bytes in GiB (config-3 segments)")
@@ -107,6 +166,9 @@ def main():
     ap.add_argument("--budgets-gib", default="1,2,4")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--sample-segments", type=int, default=8)
+    ap.add_argument("--write-codec", default="",
+                    help="comma-separated arms (none,default,lz4,zstd,snappy; none = the bounded uncompressed write): measure "
+                         "the bounded merge's compressed write instead of the plain and lz4 variants")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bounded_merge_bench measures the device path: no GPU, no numbers"
     torch.cuda.set_device(0)
@@ -116,6 +178,9 @@ def main():
     del gen
     in_bytes = sum(a.size for a in plain)
     kv_bytes = in_bytes - 10 * nseg - 2 * sum(nrec)
+    if args.write_codec:
+        write_codec_arm(args, plain, in_bytes, nseg, nrec, np.empty(in_bytes + (1 << 20), dtype=np.uint8))
+        return
     # the same records as Lz4Codec segments, written by the device writer (a one-segment merge with the codec)
     lz4, raws = [], []
     for a in plain:
