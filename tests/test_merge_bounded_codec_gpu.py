@@ -12,6 +12,7 @@ import pytest
 from oracle import tez_oracle as O
 import tez_b200 as T
 import lz4_model as L4
+from partitioned_segments import partitioned
 import snappy_model as SN
 import zstd_model as ZS
 
@@ -109,27 +110,11 @@ def test_check_for_same_keys_off(name):
     _check(_c3(), CODECS[name], comparator=T.CMP_TEXT, rle=True, check_same=False)
 
 
-def _partitioned(P=16, G=3, seed=1):
-    """G producers' segments of P partitions: three large partitions (each spans many steps at the floor), small ones,
-    and empty ones first, inside and last"""
-    rng = random.Random(seed)
-    recs = [0, 40000, 300, 0, 3000, 45000, 0, 0, 200, 2500, 50000, 10, 1, 0, 700, 0]
-    segs, parts = [], []
-    for g in range(G):
-        for p in range(P):
-            if not recs[p]:
-                continue
-            keys = sorted(b"k%09d" % rng.randrange(10 ** 9) for _ in range(recs[p]))
-            segs.append(O.write_ifile([(k, b"v%d" % (i % 97) * (1 + i % 3)) for i, k in enumerate(keys)])[0])
-            parts.append(p)
-    return segs, parts, [p for p in range(P) if recs[p] >= 40000]
-
-
 @pytest.mark.parametrize("send_empty", [False, True])
 @pytest.mark.parametrize("name", list(CODECS))
 def test_partitions_spanning_steps_and_empty_partitions(name, send_empty, tmp_path):
     codec = CODECS[name]
-    segs, parts, large = _partitioned()
+    segs, parts, large = partitioned()
     kw = dict(tmp=str(tmp_path), P=16, parts=parts, send_empty=send_empty, comparator=T.CMP_BYTES)
     got = _check(segs, codec, **kw)
     (out, _, index), steps = got[FLOOR]

@@ -9,6 +9,7 @@ import zlib
 import pytest
 
 from oracle import tez_oracle as O
+from partitioned_segments import partitioned
 import tez_b200 as T
 
 pytestmark = pytest.mark.gpu
@@ -84,6 +85,15 @@ def test_fixed_width_run_table_segments_with_interleaved_partitions(tmp_path):
     for fixed in ((16, 64), None):
         # only the lowest unfinished partition gets windows: the uploads stay near the input size, not P times it
         _check_budgets(segs, tmp=str(tmp_path), P=P, parts=parts, fixed=fixed, comparator=T.CMP_BYTES, max_upload=2)
+
+
+@pytest.mark.parametrize("send_empty", [False, True])
+def test_partitions_spanning_steps_and_empty_partitions(send_empty, tmp_path):
+    """P = 16: three partitions that each span many steps at the floor, empty partitions first, inside and last; with
+    send_empty_partition_details off they get the empty segment, on they get no bytes"""
+    segs, parts, large = partitioned()
+    steps = _check_budgets(segs, tmp=str(tmp_path), P=16, parts=parts, send_empty=send_empty, comparator=T.CMP_BYTES)
+    assert steps[-1] >= 3 * len(large)               # the floor
 
 
 def _rle_segments(rng, nseg, per, keyspace, header=True):

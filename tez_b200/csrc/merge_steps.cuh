@@ -14,17 +14,17 @@
 // the record before it); a V_END_MARKER in front of it belongs to the step before, whose piece then ends in FD FF FF.
 // Bytes after a cut are uploaded again by the next step.
 //
-// Writes stitch the pieces every step emits: TIF\0 only at the start of a partition, the FF FF EOF markers and the
-// checksum only at its end; the checksum of a partition is folded from the trailers of its pieces (k_stitch_raw,
-// k_crc_combine, k_stitch_finish), so the output is byte-identical to the one-step merge.
-//
-// Compressed writes (tezgpu_merge_open_bounded_write_codec) compress every step's pieces on the codec's chunk grid,
-// counted from the start of each partition's body, so the stream is the one the one-step merge writes: a piece that
-// closes its partition is compressed whole; of the partition the step leaves open only the whole chunks before the
-// piece's last byte are, and the bytes after them (1 to one chunk) wait in a device carry buffer for the partition's
-// next piece.  zlib chunks of an open piece end with the sync-flush block like every inner chunk (ZSeg::open); 78 01
-// is written at a partition's start and the Adler-32 at its end, folded from the chunks' values; the CRC-32 of the
-// compressed bytes is folded across steps like the uncompressed one (k_zstitch_fold, k_zstitch_finish).
+// Writes stitch the pieces every step emits into the file the one-step merge writes, with or without a codec
+// (tezgpu_merge_open_bounded_write_codec): the header (TIF\0; TIF\x01 with a codec, and 78 01 with zlib) only at the
+// start of a partition, the FF FF EOF markers and the trailer only at its end.  One pass per step takes its pieces.
+// Without a codec a piece is copied as it is.  A codec compresses it on the codec's chunk grid, counted from the
+// start of each partition's body, so the stream is the one the one-step merge writes: a piece that closes its
+// partition is compressed whole; of the partition the step leaves open only the whole chunks before the piece's last
+// byte are, and the bytes after them (1 to one chunk) wait in a device carry buffer for the partition's next piece.
+// zlib chunks of an open piece end with the sync-flush block like every inner chunk (ZSeg::open), and the Adler-32 at
+// a partition's end is folded from the chunks' values.  The CRC-32 trailer is folded across steps from each piece's
+// raw remainder (k_stitch_fold, k_stitch_trailers): a codec's chunk remainders, or, without one, the trailer the
+// step's Merger wrote after the piece.
 #pragma once
 #include <algorithm>
 #include <memory>
@@ -32,6 +32,7 @@
 #include <vector>
 
 #include "codec.cuh"
+#include "concat.cuh"
 #include "merger.cuh"
 
 namespace tezgpu {
@@ -203,38 +204,10 @@ __global__ void k_step_crc_fold(const uint32_t *__restrict__ raw, const StepCrcS
   if (c.last && crc_from_raw(t, a, c.total) != c.stored) atomicExch(bad, (int)c.seg + 1);
 }
 
-// One piece = the records R one step wrote for one partition, between its TIF\0 header and its FF FF EOF markers.  Its
-// trailer is crc(R || FF FF); with the identity of concat.cuh, raw(R || FF FF) = trailer ^ ~0 ^ (~0 * x^(8 len)), and
-// raw(R || FF FF) ^ eof_raw = raw(R) * x^16, which k_crc_combine moves past the pieces after it in the partition.
-struct StitchPiece {
-  uint64_t body;        // bytes of R
-  uint64_t after;       // bytes of the partition's pieces after this one
-  uint32_t trailer;
-  uint32_t partition;
-};
-__global__ void k_stitch_raw(const StitchPiece *__restrict__ pc, uint32_t n, const CrcTables *__restrict__ t,
-                             TileCrc *__restrict__ out) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const StitchPiece c = pc[i];
-  TileCrc tc;
-  tc.raw = crc_to_raw(t, c.trailer, c.body + 2) ^ t->eof_raw;
-  tc.p = c.partition;
-  tc.after = c.after;
-  out[i] = tc;
-}
-// checksum of every partition from the folded remainder of its records (0 without records) and their length
-__global__ void k_stitch_finish(const uint32_t *__restrict__ part_raw, const uint64_t *__restrict__ part_body, uint32_t P,
-                                const CrcTables *__restrict__ t, uint32_t *__restrict__ crc) {
-  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= P) return;
-  crc[p] = crc_from_raw(t, part_raw[p] ^ t->eof_raw, part_body[p] + 2);
-}
-
-// ------------------------------------------------------------------------------------------------ compressed writes
+// ------------------------------------------------------------------------------------------------ stitched writes
 // Room in front of a step's uncompressed image (DESIGN.md section 3): bytes [0, 2) hold the EOF markers an empty
-// segment compresses, a partition that closes without records of its own compresses its carry and FF FF from
-// [2, 4 + carry), and the carry of a continuing partition is put right in front of its piece in the image.
+// segment writes, a partition that closes without records of its own writes its carry and FF FF from [2, 4 + carry),
+// and the carry of a continuing partition is put right in front of its piece in the image.
 constexpr uint64_t STEP_CARRY_ROOM = 65536;
 static_assert(STEP_CARRY_ROOM >= 4 + 4 + L4_BLOCK && L4_BLOCK == ZS_BLOCK && L4_BLOCK == SN_BLOCK && ZCHUNK < L4_BLOCK,
               "the room holds the EOF markers, the largest carry with its own, and a step image's first TIF header");
@@ -355,17 +328,29 @@ static inline std::vector<uint8_t> stitched_compress_host(int32_t codec, const u
   return stream;
 }
 
-// Per piece of one pass (the pieces of a pass are distinct partitions): the raw CRC remainder of its chunk bytes
-// (seg_crc) and, for zlib, its chunks' Adler-32 values folded into the partition's running values: acc[2p] = remainder
-// of the partition's chunk bytes so far, acc[2p + 1] = Adler-32 of its body so far.
-__global__ void k_zstitch_fold(const ZSeg *__restrict__ segs, const uint32_t *__restrict__ part, uint32_t n,
-                               const uint32_t *__restrict__ seg_crc, const uint32_t *__restrict__ cadler,
-                               const CrcTables *__restrict__ t, uint32_t *__restrict__ acc) {
+// Per piece of one pass (the pieces of a pass are distinct partitions): the raw CRC remainder of its s.zlen bytes and,
+// for zlib, its chunks' Adler-32 values folded into the partition's running values: acc[2p] = remainder of the
+// partition's stream bytes so far, acc[2p + 1] = Adler-32 of its body so far.  A codec's piece is its chunk bytes, with
+// remainder seg_crc[i].  Without a codec (seg_crc null) a piece is the image bytes at s.body_off taken whole: records R
+// of a step (FF FF included when it closes the partition), or FF FF alone from the room (remainder eof_raw).  The
+// remainder of R comes from the trailer crc(R || FF FF) the step's Merger wrote behind R || FF FF, through the identity
+// of concat.cuh for an open piece, so the bytes are not read.
+__global__ void k_stitch_fold(const ZSeg *__restrict__ segs, const uint32_t *__restrict__ part, uint32_t n,
+                              const uint32_t *__restrict__ seg_crc, const uint32_t *__restrict__ cadler,
+                              const uint8_t *__restrict__ img, const CrcTables *__restrict__ t, uint32_t *__restrict__ acc) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const ZSeg s = segs[i];
   const uint32_t p = part[i];
-  acc[2 * p] = crc_shift_bytes(t, acc[2 * p], s.zlen) ^ seg_crc[i];
+  uint32_t raw = t->eof_raw;
+  if (seg_crc) {
+    raw = seg_crc[i];
+  } else if (s.body_off >= STEP_CARRY_ROOM) {
+    const uint64_t b = s.zlen + (s.open ? 2 : 0);   // R || FF FF
+    raw = crc_to_raw(t, load_be32(img + s.body_off + b), b);
+    if (s.open) raw = concat_records_raw(raw, *t);
+  }
+  acc[2 * p] = crc_shift_bytes(t, acc[2 * p], s.zlen) ^ raw;
   if (!cadler) return;
   uint32_t a = acc[2 * p + 1];
   for (uint32_t k = 0; k < s.nchunks; k++)
@@ -373,10 +358,10 @@ __global__ void k_zstitch_fold(const ZSeg *__restrict__ segs, const uint32_t *__
   acc[2 * p + 1] = a;
 }
 
-// per partition with a segment (zb[p]: its chunk bytes): the CRC-32 trailer of its stream; zlib: of 78 01, the chunks
+// per partition with a segment (zb[p]: its stream bytes): the CRC-32 trailer of its stream; zlib: of 78 01, the chunks
 // and the big-endian Adler-32
-__global__ void k_zstitch_finish(const uint32_t *__restrict__ acc, const uint64_t *__restrict__ zb, uint32_t P, int zlib,
-                                 const CrcTables *__restrict__ t, uint32_t *__restrict__ crc) {
+__global__ void k_stitch_trailers(const uint32_t *__restrict__ acc, const uint64_t *__restrict__ zb, uint32_t P, int zlib,
+                                  const CrcTables *__restrict__ t, uint32_t *__restrict__ crc) {
   const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= P || !zb[p]) return;
   if (!zlib) {
@@ -413,14 +398,13 @@ class BoundedMerge {
   bool in_step = false, have_counts = false;
   uint64_t pass_n = 0, pass_kv = 0, total_n = 0, total_kv = 0;
   DeviceBuffer d_win, d_wins, d_scan, d_cut, d_split, d_on_split, d_acc, d_crcseg, d_crcsd, d_bad;
-  DeviceBuffer d_pieces, d_piece_tc, d_part_raw, d_part_body, d_part_crc;
   std::vector<StepWin> wins;
   std::vector<uint32_t> win_seg;           // window -> caller's segment
   std::vector<StepScan> scans;
   std::vector<StepCut> cuts;
   int32_t zcodec = TEZGPU_CODEC_NONE;      // the codec of the written segments (the steps' Merger writes uncompressed)
-  DeviceBuffer d_carry, d_zout, d_zpart, d_zacc, d_zb, d_zcrc;
-  PinnedBuffer h_zout;
+  DeviceBuffer d_carry, d_zout, d_piece_part, d_fold, d_stream_bytes, d_trailer;
+  PinnedBuffer h_pass;
 
   BoundedMerge(Merger &mm, uint64_t b, DeviceTally &t) : m(mm), budget(b), tally(t) {}
 
@@ -485,7 +469,7 @@ class BoundedMerge {
     std::stable_sort(pmajor.begin(), pmajor.end(), [&](uint32_t a, uint32_t b) { return in[a].partition < in[b].partition; });
     d_bad.ensure(16);
     d_split.ensure(16);
-    m.pipe.codec = TEZGPU_CODEC_NONE;   // the steps write uncompressed pieces; write_compressed compresses them
+    m.pipe.codec = TEZGPU_CODEC_NONE;   // the steps write uncompressed pieces; write compresses them
     // the first step runs here, as every other open parses its inputs before returning
     begin_pass();
     iter = 1;
@@ -746,159 +730,47 @@ class BoundedMerge {
     }
   }
 
-  // ---- writes: every step's pieces stitched into one segment per partition.  out receives file.out, index the
-  //      TezIndexRecord triples.
-  static void add_step_stats(tezgpu_stats &sum, const tezgpu_stats &s) {
-    sum.output_records += s.output_records;
-    sum.output_bytes += s.output_bytes;
-    sum.spilled_records += s.spilled_records;
-    sum.rle_used |= s.rle_used;
-    sum.adjacent_equal_keys += s.adjacent_equal_keys;
-    sum.tie_records += s.tie_records;
-    sum.ms_stage += s.ms_stage; sum.ms_sort += s.ms_sort; sum.ms_ties += s.ms_ties; sum.ms_emit += s.ms_emit; sum.ms_total += s.ms_total;
-    sum.kernel_launches += s.kernel_launches;
-  }
-
-  void write(int rle, std::vector<uint8_t> &out, std::vector<int64_t> &index, tezgpu_stats *stats) {
-    if (zcodec) {
-      write_compressed(rle, out, index, stats);
-      return;
-    }
-    TallyScope ts(&tally);
-    cudaStream_t st = m.pipe.stream;
-    const int P = m.pipe.conf.num_partitions;
-    const bool empty_segments = m.pipe.conf.send_empty_partition_details == 0;   // as k_layout
-    static const uint8_t kHeader[4] = {'T', 'I', 'F', 0};
-    begin_pass();
-    iter = 0;   // the windows are the write's now: a later next_batch starts from the beginning
-    out.clear();
-    index.assign((size_t)P * 3, 0);
-    std::vector<StitchPiece> pieces;
-    std::vector<uint64_t> part_body((size_t)P, 0);
-    std::vector<int64_t> part_at((size_t)P, -1);
-    tezgpu_stats sum;
-    memset(&sum, 0, sizeof(sum));
-    int cur = -1;
-    auto close_partition = [&](int p) {
-      const uint8_t eof[6] = {0xFF, 0xFF, 0, 0, 0, 0};
-      out.insert(out.end(), eof, eof + 6);
-      index[3 * p + 0] = part_at[p];
-      index[3 * p + 2] = (int64_t)out.size() - part_at[p];
-      index[3 * p + 1] = index[3 * p + 2] - 4;
-    };
-    auto skip_to = [&](int p) {   // partitions before p without records
-      for (int q = cur + 1; q < p; q++) {
-        part_at[q] = (int64_t)out.size();
-        index[3 * q] = part_at[q];
-        if (!empty_segments) continue;
-        out.insert(out.end(), kHeader, kHeader + 4);
-        close_partition(q);
-      }
-    };
-    std::vector<int64_t> idx((size_t)P * 3);
-    while ((in_step = next_step())) {
-      if (!m.n) continue;
-      uint64_t len = 0;
-      tezgpu_stats s;
-      const uint8_t *img = m.write_host(rle, nullptr, 0, &len, idx.data(), &s);
-      for (int p = 0; p < P; p++) {
-        const int64_t seglen = idx[3 * p + 2];
-        if (seglen <= 10) continue;   // no records of p in this step
-        const uint8_t *seg = img + idx[3 * p];
-        if (p != cur) {
-          if (cur >= 0) close_partition(cur);
-          skip_to(p);
-          cur = p;
-          part_at[p] = (int64_t)out.size();
-          out.insert(out.end(), seg, seg + 4);
-        }
-        const uint64_t body = (uint64_t)seglen - 10;
-        out.insert(out.end(), seg + 4, seg + 4 + body);
-        StitchPiece pc;
-        pc.body = body;
-        pc.after = 0;
-        pc.trailer = load_be32(seg + seglen - 4);
-        pc.partition = (uint32_t)p;
-        pieces.push_back(pc);
-        part_body[p] += body;
-      }
-      add_step_stats(sum, s);
-    }
-    end_pass();
-    if (cur >= 0) close_partition(cur);
-    skip_to(P);
-    // ---- the checksum of every partition from the trailers of its pieces
-    for (size_t i = pieces.size(); i-- > 0;) {
-      if (i + 1 < pieces.size() && pieces[i + 1].partition == pieces[i].partition)
-        pieces[i].after = pieces[i + 1].after + pieces[i + 1].body;
-    }
-    const CrcTables *d_crc = DeviceConstants::get(m.pipe.conf.device).d_crc;
-    const uint32_t npc = (uint32_t)pieces.size();
-    d_pieces.ensure(std::max<size_t>(1, npc) * sizeof(StitchPiece));
-    d_piece_tc.ensure(std::max<size_t>(1, npc) * sizeof(TileCrc));
-    d_part_raw.ensure((size_t)P * 4);
-    d_part_body.ensure((size_t)P * 8);
-    d_part_crc.ensure((size_t)P * 4);
-    TG_CUDA(cudaMemsetAsync(d_part_raw.p, 0, (size_t)P * 4, st));
-    TG_CUDA(cudaMemcpyAsync(d_part_body.p, part_body.data(), (size_t)P * 8, cudaMemcpyHostToDevice, st));
-    if (npc) {
-      TG_CUDA(cudaMemcpyAsync(d_pieces.p, pieces.data(), npc * sizeof(StitchPiece), cudaMemcpyHostToDevice, st));
-      k_stitch_raw<<<(uint32_t)div_up(npc, 128), 128, 0, st>>>(d_pieces.as<StitchPiece>(), npc, d_crc, d_piece_tc.as<TileCrc>());
-      k_crc_combine<<<(uint32_t)div_up(npc, 256), 256, 0, st>>>(d_piece_tc.as<TileCrc>(), npc, d_crc, d_part_raw.as<uint32_t>());
-    }
-    k_stitch_finish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(d_part_raw.as<uint32_t>(), d_part_body.as<uint64_t>(), (uint32_t)P,
-                                                               d_crc, d_part_crc.as<uint32_t>());
-    TG_CUDA(cudaGetLastError());
-    std::vector<uint32_t> crc((size_t)P);
-    TG_CUDA(cudaMemcpyAsync(crc.data(), d_part_crc.p, (size_t)P * 4, cudaMemcpyDeviceToHost, st));
-    TG_CUDA(cudaStreamSynchronize(st));
-    for (int p = 0; p < P; p++)
-      if (index[3 * p + 2]) store_be32(out.data() + index[3 * p] + index[3 * p + 2] - 4, crc[p]);
-    for (int p = 0; p < P; p++) sum.output_bytes_with_overhead += index[3 * p + 1];
-    sum.output_bytes_physical = sum.file_out_bytes = (int64_t)out.size();
-    sum.num_spills = 1;
-    if (stats) *stats = sum;
-  }
-
-  // ---- compressed writes (see the top of this file): the file and index the one-step merge with the codec writes.
-  //      Every step that has records writes its uncompressed image behind STEP_CARRY_ROOM bytes of m.d_out and runs
-  //      one pass over its pieces; one more pass after the last step closes what is left.
+  // ---- writes (see the top of this file): the file and index the one-step merge with the write codec writes; out
+  //      receives file.out, index the TezIndexRecord triples.  Every step that has records writes its uncompressed
+  //      image behind STEP_CARRY_ROOM bytes of m.d_out and runs one pass over its pieces; one more pass after the last
+  //      step closes what is left.
   struct StitchJob {
     uint32_t part;
     uint64_t off;       // the piece's own bytes in m.d_out (in the room, or in the step image behind it)
     uint64_t n;
-    bool starts;        // the partition's first piece: TIF\x01 (zlib: and 78 01) in front of it
+    bool starts;        // the partition's first piece: the header in front of it
     bool closes;        // its last: the trailer after it
     bool bytes;         // false: a partition without records and without a segment (send_empty_partition_details 1)
   };
 
-  void write_compressed(int rle, std::vector<uint8_t> &out, std::vector<int64_t> &index, tezgpu_stats *stats) {
+  void write(int rle, std::vector<uint8_t> &out, std::vector<int64_t> &index, tezgpu_stats *stats) {
     TallyScope ts(&tally);
     SortPipeline &pp = m.pipe;
     cudaStream_t st = pp.stream;
     const int P = pp.conf.num_partitions;
     const bool empty_segments = pp.conf.send_empty_partition_details == 0;   // as k_layout
     const bool zlib = zcodec == TEZGPU_CODEC_DEFAULT;
-    const CodecLayout L = codec_layout(zcodec);
+    const CodecLayout L = codec_layout(zcodec);   // with a codec only
     const CrcTables *d_crc = DeviceConstants::get(pp.conf.device).d_crc;
     static const uint8_t kEof[2] = {0xFF, 0xFF};
-    static const uint8_t kHead[6] = {'T', 'I', 'F', 1, 0x78, 0x01};
+    const uint8_t head[6] = {'T', 'I', 'F', (uint8_t)(zcodec ? 1 : 0), 0x78, 0x01};
+    const size_t head_len = zlib ? 6 : 4, trailer_len = zlib ? 8 : 4;   // zlib: 78 01; Adler-32 and CRC-32
     begin_pass();
     iter = 0;   // the windows are the write's now: a later next_batch starts from the beginning
     out.clear();
     index.assign((size_t)P * 3, 0);
-    std::vector<uint64_t> raw((size_t)P, 0), zb((size_t)P, 0);   // per partition: record bytes, compressed chunk bytes
-    std::vector<int64_t> zat((size_t)P, 0);                      // file offset of its segment
-    std::vector<uint32_t> acc((size_t)P * 2);                    // running CRC remainder and Adler-32 (k_zstitch_fold)
+    std::vector<uint64_t> raw((size_t)P, 0), slen((size_t)P, 0);   // per partition: record bytes, stream bytes
+    std::vector<int64_t> at((size_t)P, 0);                          // file offset of its segment
+    std::vector<uint32_t> acc((size_t)P * 2);                       // running CRC remainder and Adler-32 (k_stitch_fold)
     for (int p = 0; p < P; p++) { acc[2 * p] = 0; acc[2 * p + 1] = 1; }
-    d_zacc.ensure((size_t)P * 8);
-    TG_CUDA(cudaMemcpyAsync(d_zacc.p, acc.data(), (size_t)P * 8, cudaMemcpyHostToDevice, st));
-    d_carry.ensure(STEP_CARRY_ROOM);
+    d_fold.ensure((size_t)P * 8);
+    TG_CUDA(cudaMemcpyAsync(d_fold.p, acc.data(), (size_t)P * 8, cudaMemcpyHostToDevice, st));
+    if (zcodec) d_carry.ensure(STEP_CARRY_ROOM);
     tezgpu_stats sum;
     memset(&sum, 0, sizeof(sum));
     int cur = -1;            // the last partition with records so far
     bool open = false;       // its segment continues in a later step
-    uint64_t carry = 0;      // its body bytes after its last compressed chunk, in d_carry
+    uint64_t carry = 0;      // its body bytes after its last compressed chunk, in d_carry (always 0 without a codec)
     std::vector<StitchJob> jobs;
     std::vector<uint32_t> part;
     std::vector<uint32_t> seg_of;
@@ -914,7 +786,8 @@ class BoundedMerge {
     auto skip_to = [&](int p) {   // partitions before p without records
       for (int q = cur + 1; q < p; q++) jobs.push_back({(uint32_t)q, 0, 2, true, true, empty_segments});
     };
-    // one pass: the pieces of `jobs` planned (plan_stitch_piece) and compressed, their bytes appended to out
+    // one pass: the pieces of `jobs` compressed (plan_stitch_piece) or, without a codec, taken whole; their checksums
+    // folded and their bytes appended to out
     auto pass = [&] {
       m.d_out.ensure(STEP_CARRY_ROOM);
       uint8_t *img = m.d_out.as<uint8_t>();
@@ -927,49 +800,67 @@ class BoundedMerge {
       seg_of.assign(jobs.size(), ~0u);
       part.clear();
       uint32_t nseg = 0, nchunks = 0;
+      uint64_t bytes = 0;   // the pass's bytes for h_pass
       for (size_t i = 0; i < jobs.size(); i++) {
         const StitchJob &j = jobs[i];
         if (!j.bytes) continue;
         const uint64_t c = j.starts ? 0 : carry;   // only the open partition continues
         if (c) TG_CUDA(cudaMemcpyAsync(img + j.off - c, d_carry.p, c, cudaMemcpyDeviceToDevice, st));
         if (j.off < STEP_CARRY_ROOM) TG_CUDA(cudaMemcpyAsync(img + j.off, kEof, 2, cudaMemcpyHostToDevice, st));
-        const StitchPlan pl = plan_stitch_piece(L.chunk, c, j.off, j.n, j.closes);
-        if (pl.open) {
-          carry = pl.carry;
-          if (carry) TG_CUDA(cudaMemcpyAsync(d_carry.p, img + pl.off + pl.len, carry, cudaMemcpyDeviceToDevice, st));
-        }
-        if (!pl.nchunks) continue;
         ZSeg &s = hs[nseg];
         memset(&s, 0, sizeof(s));
-        s.body_off = pl.off;
-        s.body_len = pl.len;
-        s.chunk0 = nchunks;
-        s.nchunks = pl.nchunks;
+        if (zcodec) {
+          const StitchPlan pl = plan_stitch_piece(L.chunk, c, j.off, j.n, j.closes);
+          if (pl.open) {
+            carry = pl.carry;
+            if (carry) TG_CUDA(cudaMemcpyAsync(d_carry.p, img + pl.off + pl.len, carry, cudaMemcpyDeviceToDevice, st));
+          }
+          if (!pl.nchunks) continue;
+          s.body_off = pl.off;
+          s.body_len = pl.len;
+          s.chunk0 = nchunks;
+          s.nchunks = pl.nchunks;
+          s.open = pl.open;
+          nchunks += pl.nchunks;
+        } else {   // the piece whole: its bytes reach the host with the image
+          s.body_off = s.zstart = j.off;
+          s.zlen = j.n;
+          s.open = !j.closes;
+          bytes = std::max(bytes, j.off + j.n);
+        }
         s.rank = nseg;
-        s.open = pl.open;
         seg_of[i] = nseg++;
         part.push_back(j.part);
-        nchunks += pl.nchunks;
       }
-      if (nchunks) {
-        const uint64_t cbytes = pp.compress_chunks(zcodec, img, hs, nseg, nchunks, 0, 0, &launches);
-        d_zout.ensure(cbytes);
-        d_zpart.ensure((size_t)nseg * 4);
-        TG_CUDA(cudaMemcpyAsync(d_zpart.p, part.data(), (size_t)nseg * 4, cudaMemcpyHostToDevice, st));
-        k_zpack<<<nchunks, 256, 0, st>>>(pp.z_slots.as<uint8_t>(), pp.z_csize.as<uint32_t>(), pp.z_coff.as<uint64_t>(), pp.z_segs.as<ZSeg>(),
-                                         nseg, L.slot, 0, d_zout.as<uint8_t>());
-        k_zstitch_fold<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(pp.z_segs.as<ZSeg>(), d_zpart.as<uint32_t>(), nseg, pp.z_crc.as<uint32_t>(),
-                                                                    zlib ? pp.z_cadler.as<uint32_t>() : nullptr, d_crc, d_zacc.as<uint32_t>());
-        launches += 2;
+      if (nseg) {
+        const uint8_t *src = img;
+        if (zcodec) {
+          bytes = pp.compress_chunks(zcodec, img, hs, nseg, nchunks, 0, 0, &launches);
+          d_zout.ensure(bytes);
+          k_zpack<<<nchunks, 256, 0, st>>>(pp.z_slots.as<uint8_t>(), pp.z_csize.as<uint32_t>(), pp.z_coff.as<uint64_t>(), pp.z_segs.as<ZSeg>(),
+                                           nseg, L.slot, 0, d_zout.as<uint8_t>());
+          src = d_zout.as<uint8_t>();
+          launches++;
+        } else {
+          pp.z_segs.ensure((size_t)nseg * sizeof(ZSeg));
+          TG_CUDA(cudaMemcpyAsync(pp.z_segs.p, hs, (size_t)nseg * sizeof(ZSeg), cudaMemcpyHostToDevice, st));
+        }
+        d_piece_part.ensure((size_t)nseg * 4);
+        TG_CUDA(cudaMemcpyAsync(d_piece_part.p, part.data(), (size_t)nseg * 4, cudaMemcpyHostToDevice, st));
+        k_stitch_fold<<<(uint32_t)div_up(nseg, 128), 128, 0, st>>>(pp.z_segs.as<ZSeg>(), d_piece_part.as<uint32_t>(), nseg,
+                                                                   zcodec ? pp.z_crc.as<uint32_t>() : nullptr,
+                                                                   zlib ? pp.z_cadler.as<uint32_t>() : nullptr, img, d_crc,
+                                                                   d_fold.as<uint32_t>());
+        launches++;
         TG_CUDA(cudaGetLastError());
-        h_zout.ensure(cbytes);
-        TG_CUDA(cudaMemcpyAsync(h_zout.p, d_zout.p, cbytes, cudaMemcpyDeviceToHost, st));
+        h_pass.ensure(bytes);
+        TG_CUDA(cudaMemcpyAsync(h_pass.p, src, bytes, cudaMemcpyDeviceToHost, st));
       }
       pp.z_timer.mark(st);
       TG_CUDA(cudaStreamSynchronize(st));
       sum.ms_total += pp.z_timer.ms(0, 1);
       sum.kernel_launches += launches;
-      for (size_t i = 0; i < jobs.size(); i++) {   // hs holds zstart / zlen of every piece with chunks
+      for (size_t i = 0; i < jobs.size(); i++) {   // hs holds zstart / zlen of every piece with bytes in h_pass
         const StitchJob &j = jobs[i];
         const uint32_t p = j.part;
         if (!j.bytes) {
@@ -977,20 +868,20 @@ class BoundedMerge {
           continue;
         }
         if (j.starts) {
-          zat[p] = (int64_t)out.size();
-          out.insert(out.end(), kHead, kHead + (zlib ? 6 : 4));
+          at[p] = (int64_t)out.size();
+          out.insert(out.end(), head, head + head_len);
         }
         if (seg_of[i] != ~0u) {
           const ZSeg &s = hs[seg_of[i]];
-          const uint8_t *z = h_zout.as<uint8_t>() + s.zstart;
+          const uint8_t *z = h_pass.as<uint8_t>() + s.zstart;
           out.insert(out.end(), z, z + s.zlen);
-          zb[p] += s.zlen;
+          slen[p] += s.zlen;
         }
         if (j.closes) {
-          out.insert(out.end(), zlib ? 8 : 4, 0);   // Adler-32 and CRC-32, from the folds below
-          index[3 * p] = zat[p];
+          out.insert(out.end(), trailer_len, 0);   // from the folds below
+          index[3 * p] = at[p];
           index[3 * p + 1] = (int64_t)raw[p] + 6;
-          index[3 * p + 2] = (int64_t)out.size() - zat[p];
+          index[3 * p + 2] = (int64_t)out.size() - at[p];
         }
       }
       jobs.clear();
@@ -1002,7 +893,14 @@ class BoundedMerge {
       uint64_t len = 0;
       tezgpu_stats s;
       m.write_device(m.d_out.as<uint8_t>() + STEP_CARRY_ROOM, m.d_out.cap - STEP_CARRY_ROOM, rle, &len, idx.data(), &s);
-      add_step_stats(sum, s);
+      sum.output_records += s.output_records;
+      sum.output_bytes += s.output_bytes;
+      sum.spilled_records += s.spilled_records;
+      sum.rle_used |= s.rle_used;
+      sum.adjacent_equal_keys += s.adjacent_equal_keys;
+      sum.tie_records += s.tie_records;
+      sum.ms_stage += s.ms_stage; sum.ms_sort += s.ms_sort; sum.ms_ties += s.ms_ties; sum.ms_emit += s.ms_emit; sum.ms_total += s.ms_total;
+      sum.kernel_launches += s.kernel_launches;
       for (int p = 0; p < P; p++) {
         const int64_t seglen = idx[3 * p + 2];
         if (seglen <= 10) continue;   // no records of p in this step
@@ -1025,18 +923,18 @@ class BoundedMerge {
     skip_to(P);
     if (!jobs.empty()) pass();
     // ---- the trailers: CRC-32 of every segment's stream (and zlib's Adler-32) from the folded values
-    d_zb.ensure((size_t)P * 8);
-    d_zcrc.ensure((size_t)P * 4);
-    TG_CUDA(cudaMemcpyAsync(d_zb.p, zb.data(), (size_t)P * 8, cudaMemcpyHostToDevice, st));
-    k_zstitch_finish<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(d_zacc.as<uint32_t>(), d_zb.as<uint64_t>(), (uint32_t)P, zlib ? 1 : 0, d_crc,
-                                                                d_zcrc.as<uint32_t>());
+    d_stream_bytes.ensure((size_t)P * 8);
+    d_trailer.ensure((size_t)P * 4);
+    TG_CUDA(cudaMemcpyAsync(d_stream_bytes.p, slen.data(), (size_t)P * 8, cudaMemcpyHostToDevice, st));
+    k_stitch_trailers<<<(uint32_t)div_up(P, 128), 128, 0, st>>>(d_fold.as<uint32_t>(), d_stream_bytes.as<uint64_t>(), (uint32_t)P,
+                                                                 zlib ? 1 : 0, d_crc, d_trailer.as<uint32_t>());
     TG_CUDA(cudaGetLastError());
     std::vector<uint32_t> crc((size_t)P);
-    TG_CUDA(cudaMemcpyAsync(acc.data(), d_zacc.p, (size_t)P * 8, cudaMemcpyDeviceToHost, st));
-    TG_CUDA(cudaMemcpyAsync(crc.data(), d_zcrc.p, (size_t)P * 4, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaMemcpyAsync(acc.data(), d_fold.p, (size_t)P * 8, cudaMemcpyDeviceToHost, st));
+    TG_CUDA(cudaMemcpyAsync(crc.data(), d_trailer.p, (size_t)P * 4, cudaMemcpyDeviceToHost, st));
     TG_CUDA(cudaStreamSynchronize(st));
     for (int p = 0; p < P; p++) {
-      if (!zb[p]) continue;
+      if (!slen[p]) continue;
       uint8_t *e = out.data() + index[3 * p] + index[3 * p + 2];
       if (zlib) store_be32(e - 8, acc[2 * p + 1]);
       store_be32(e - 4, crc[p]);

@@ -152,7 +152,7 @@ def write_codec_arm(args, plain, in_bytes, nseg, nrec, out):
                 "bench": "bounded_merge_write_codec", "write_codec": arm,
                 "open": "bounded_write_codec" if (budget and codec) else ("bounded" if budget else "open_codec one step"),
                 "budget_bytes": budget or None, "input_bytes": in_bytes, "segments": nseg, "records": int(sum(nrec)),
-                "raw_bytes": raw, "written_bytes": part, "ratio": round(raw / part, 3),
+                "raw_bytes": raw, "written_bytes": part, "crc32": digest, "ratio": round(raw / part, 3),
                 "ms_per_run": round(s * 1e3, 1), "ms_runs": [round(t * 1e3, 1) for t in times],
                 "raw_gbps": round(raw / s / 1e9, 3), "steps": steps, "peak_device_bytes": peak, "card": name,
                 "parity": {"same_bytes_as_one_step_write": digest == ref if codec else None}}), flush=True)
