@@ -17,7 +17,6 @@ from tez_b200.constants import CODEC_DEFAULT, CODEC_LZ4, CODEC_ZSTD, E_FORMAT
 import codec_model as CM
 import lz4_model as L4
 import zstd_model as ZS
-from test_codec_cpu import _zhdr
 
 
 class Case:
@@ -178,7 +177,7 @@ def deflate_member(blocks, cinfo=7):
     """One zlib member of the given blocks and its body.  A block is ("stored", data), ("fixed", tokens) or
     ("dynamic", tokens, lit_lengths, dist_lengths); tokens are literal byte values and M(length, distance)."""
     w = BitW()
-    w.out += _zhdr(cinfo)
+    w.out += CM.zhdr(cinfo)
     body = bytearray()
     for bi, blk in enumerate(blocks):
         w.put(int(bi + 1 == len(blocks)), 1)
@@ -415,7 +414,7 @@ def deflate_large(block, total):
     d = len(block)
     assert d == 4096 and total > d + 258 * 64
     w = BitW()
-    w.out += _zhdr(7)
+    w.out += CM.zhdr(7)
     w.put(1, 1)
     w.put(1, 2)
     lc, dc = canonical(FIXED_LIT), canonical(FIXED_DIST)

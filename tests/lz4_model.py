@@ -242,6 +242,14 @@ def java_stream(writes, compress=lambda d: lz4_compress(d), max_input=MAX_INPUT)
     return bytes(out)
 
 
+def java_chunk(d, hc=False):
+    """liblz4's chunk (LZ4_compress_HC where hc) where liblz4 can be loaded, else an all-literal chunk (the block framing
+    is Java's either way)"""
+    if liblz4() is not None:
+        return lz4_compress(d, mode="hc" if hc else "fast")
+    return lit(d)
+
+
 def segment(z):
     """TIF\\x01 + stream + CRC-32 of the stream"""
     return b"TIF\x01" + bytes(z) + zlib.crc32(bytes(z)).to_bytes(4, "big")
@@ -258,3 +266,42 @@ def fixture():
     assert pos == len(data)
     return res
 
+
+# ------------------------------------------------------------------------------------------------ hand-made streams
+def blk(raw, *chunks):
+    return raw.to_bytes(4, "big") + b"".join(len(c).to_bytes(4, "big") + c for c in chunks)
+
+
+def lit(data):
+    n = len(data)
+    if n < 15:
+        return bytes([n << 4]) + data
+    r, ext = n - 15, b""
+    while r >= 255:
+        ext += b"\xff"; r -= 255
+    return b"\xf0" + ext + bytes([r]) + data
+
+
+def malformed():
+    good = lit(b"hello world, hello")                      # 18 literal bytes
+    cases = {
+        "truncated_block_header": (blk(18, good)[:2], 18),
+        "truncated_chunk_header": (blk(18, good)[:6], 18),
+        "chunk_past_the_end": (blk(18, good)[:-1], 18),
+        # 'a', then a match of 262,144 bytes at offset 1, then 5 literals: 262,150 bytes from a 1,038-byte chunk
+        "chunk_decodes_past_262144": (blk(262150, b"\x1fa\x01\x00" + b"\xff" * 1027 + bytes([240]) + lit(b"xxxxx")), 262150),
+        "block_raw_zero": (blk(0, good) + blk(18, good), 18),
+        "block_sum_too_large": (blk(18, good) + blk(18, good), 30),
+        "block_sum_too_small": (blk(18, good), 20),
+        "trailing_bytes": (blk(18, good) + b"\x00", 18),
+        "trailing_zero_block": (blk(18, good) + b"\x00\x00\x00\x00", 18),
+        "over_decode": (blk(10, good), 10),
+        "offset_zero": (blk(13, bytes([0x40]) + b"abcd\x00\x00" + lit(b"xxxxx")), 13),
+        "offset_too_far": (blk(13, bytes([0x40]) + b"abcd\x05\x00" + lit(b"xxxxx")), 13),
+        "literal_run_past_the_end": (blk(19, bytes([0xF0, 4]) + b"hello world, hello"), 19),
+        "match_at_the_end": (blk(8, bytes([0x40]) + b"abcd\x04\x00"), 8),
+        "short_last_literals": (blk(9, bytes([0x40]) + b"abcd\x04\x00" + lit(b"x")), 9),
+        "empty_chunk": (blk(18, b""), 18),
+        "chunk_over_262144": (blk(18, good)[:4] + (262145).to_bytes(4, "big") + good + bytes(262145 - len(good)), 18),
+    }
+    return cases

@@ -9,6 +9,7 @@ import zlib
 
 from tez_b200 import _lib
 from tez_b200.constants import SNAPPY_BLOCK_BYTES, SNAPPY_CHUNK_BOUND
+import codec_model as CM
 from lz4_model import ifile_writes, java_stream as _java_stream   # noqa: F401  (the framing is Lz4Codec's)
 
 CHUNK_CAP = 262144                            # io.compression.codec.snappy.buffersize default: SnappyDecompressor's buffer
@@ -209,6 +210,13 @@ def java_stream(writes, compress=None):
     return _java_stream(writes, compress=compress or snappy_compress, max_input=MAX_INPUT)
 
 
+def java_chunk(d):
+    """libsnappy's chunk where pyarrow imports, else an all-literal chunk (the block framing is Java's either way)"""
+    if pyarrow() is not None:
+        return snappy_compress(d)
+    return varint(len(d)) + lit(bytes(d))
+
+
 def segment(z):
     """TIF\\x01 + stream + CRC-32 of the stream"""
     return b"TIF\x01" + bytes(z) + zlib.crc32(bytes(z)).to_bytes(4, "big")
@@ -335,4 +343,55 @@ def mutants(streams, count, seed):
         else:
             expect += rng.choice((-1, 1))
         res.append((bytes(zz), max(expect, 0)))
+    return res
+
+
+# ------------------------------------------------------------------------------------------------ malformed and mutated streams
+def blk(raw, *chunks):
+    return raw.to_bytes(4, "big") + b"".join(len(c).to_bytes(4, "big") + c for c in chunks)
+
+
+def malformed():
+    """{name: (stream, expect, reason)}"""
+    body = CM.wordcount_body(n=300, vocab=40, seed=1)
+    z = compress_emulate(body)
+    (raw, (c,)), = blocks(z)
+    abcd = lit(b"abcd")
+    return {
+        "preamble_runs_past_5_bytes": (blk(8, b"\xff\xff\xff\xff\xff\x01" + abcd), 8, "invalid chunk preamble"),
+        "preamble_fifth_byte_over_15": (blk(8, b"\x80\x80\x80\x80\x10" + abcd), 8, "invalid chunk preamble"),
+        "preamble_zero": (blk(8, b"\x00", varint(8) + abcd + copy(4, 4, 1)), 8, "invalid chunk preamble"),
+        "preamble_over_262144": (blk(300000, varint(262145) + abcd), 300000, "invalid chunk preamble"),
+        "preamble_truncated": (blk(200, b"\xc8"), 200, "invalid chunk preamble"),
+        "offset_zero": (blk(8, varint(8) + abcd + copy(0, 4, 1)), 8, "invalid copy offset"),
+        "offset_zero_copy4": (blk(8, varint(8) + abcd + copy(0, 4, 4)), 8, "invalid copy offset"),
+        "offset_past_the_output": (blk(8, varint(8) + abcd + copy(5, 4, 2)), 8, "invalid copy offset"),
+        "literal_past_the_chunk": (blk(10, varint(10) + bytes([9 << 2]) + b"abc"), 10, "literal past the end of the chunk"),
+        "literal_length_bytes_past_the_chunk": (blk(100, varint(100) + bytes([61 << 2, 99])), 100, "literal past the end of the chunk"),
+        "copy_past_the_chunk": (blk(8, varint(8) + abcd + bytes([2 | (3 << 2), 4])), 8, "copy past the end of the chunk"),
+        "copy4_past_the_chunk": (blk(8, varint(8) + abcd + bytes([3 | (3 << 2), 4, 0, 0])), 8, "copy past the end of the chunk"),
+        "short_output": (blk(9, varint(9) + abcd + copy(4, 4, 1)), 9, "chunk decodes short of its preamble length"),
+        "long_output_copy": (blk(7, varint(7) + abcd + copy(4, 4, 1)), 7, "chunk decodes past its preamble length"),
+        "long_output_literal": (blk(3, varint(3) + abcd), 3, "chunk decodes past its preamble length"),
+        "trailing_element": (blk(4, varint(4) + abcd + copy(4, 4, 1)), 4, "chunk decodes past its preamble length"),
+        "trailing_bytes": (z + b"\0\0\0\0", len(body), "bytes after the last block"),
+        "chunks_short_of_the_block": (blk(raw + 1, c), len(body) + 1, "truncated block header"),
+        "chunks_past_the_block": (blk(raw - 1, c), len(body) - 1, "chunks decode past their block's raw length"),
+        "blocks_short_of_rawlength": (z, len(body) + 1, "decompressed length differs from rawLength - 4"),
+        "blocks_past_rawlength": (z, len(body) - 1, "block raw length outside the remaining rawLength - 4"),
+        "block_raw_zero": (blk(0, c), len(body), "block raw length outside the remaining rawLength - 4"),
+        "chunk_over_262144": (blk(8, b"") [:4] + (262145).to_bytes(4, "big") + b"\0" * 262145, 8,
+                              "chunk length over 262144 or past the end of the stream"),
+        "chunk_past_the_stream": (z[:-1], len(body), "chunk length over 262144 or past the end of the stream"),
+        "truncated_header": (z[:6], len(body), "truncated block header"),
+        "second_of_two_chunks_bad": (blk(16, varint(8) + abcd + copy(4, 4, 1), varint(8) + abcd + copy(9, 4, 1)), 16,
+                                     "invalid copy offset"),
+    }
+
+
+def corpus_streams():
+    """(body, stream) pairs the mutant corpus corrupts: device-written, Java-framed libsnappy-like and crafted"""
+    bodies = [CM.wordcount_body(n=300, vocab=40, seed=s) for s in range(3)] + [random.Random(9).randbytes(600)]
+    res = [(b, compress_emulate(b)) for b in bodies]
+    res += [(decode_chunk(c), one_block([c])) for _, c in crafted_chunks() if len(c) < 4096]
     return res

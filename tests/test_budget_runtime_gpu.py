@@ -18,7 +18,7 @@ from tez_b200.runtime_library import (INT_WRITABLE, TEXT, InputContext, LocalOut
 import combine_model as CBM
 import lz4_model as L4M
 import zstd_model as ZSM
-from test_runtime_library_gpu import _run_output
+from plugin_runs import run_output
 
 pytestmark = pytest.mark.gpu
 KEY = "tez.runtime.gpu.merge.device.budget.mb"
@@ -147,7 +147,7 @@ def test_decode_segment_larger_than_the_budget():
 
 # ------------------------------------------------------------------------------------------------ input
 def _producers(tmp_path, codecs, n):
-    return [_run_output(tmp_path / ("t%d" % t), dict(WC, **_codec_conf(c)), _words(n, seed=100 + t), 1,
+    return [run_output(tmp_path / ("t%d" % t), dict(WC, **_codec_conf(c)), _words(n, seed=100 + t), 1,
                         uid="attempt_1_0001_1_00_%06d_0_10001" % t) for t, c in enumerate(codecs)]
 
 
@@ -183,7 +183,7 @@ def test_input_under_budget_reads_what_it_reads_without(tmp_path, codecs):
 
 # ------------------------------------------------------------------------------------------------ output
 def _output(tmp, conf, recs):
-    out, events = _run_output(tmp, conf, recs, 4)
+    out, events = run_output(tmp, conf, recs, 4)
     with open(out.final_output_file, "rb") as f, open(out.final_index_file, "rb") as fi:
         return out, f.read(), fi.read()
 

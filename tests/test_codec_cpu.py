@@ -12,10 +12,6 @@ from tez_b200.runtime_library import TEXT, OrderedPartitionedKVOutput, OutputCon
 from tez_b200._lib import TezGpuError
 import codec_model as M
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-# the fixture's rawLengths and compressed segment lengths (TestIFile.java:395-397)
-FIXTURE_RAWS = [2392, 102314, 42576, 31432, 25090]
-FIXTURE_COMPRESSED = [723, 25396, 10926, 8203, 6665]
 C = M.CHUNK
 
 
@@ -107,77 +103,16 @@ def test_reader_several_members_in_one_body(members):
 
 
 def test_reader_fixture_segments():
-    data = open(os.path.join(GOLDEN, "TestIFile_concatenated_compressed.bin"), "rb").read()
-    pos = 0
-    for c, raw in zip(FIXTURE_COMPRESSED, FIXTURE_RAWS):
-        seg = data[pos:pos + c]
-        pos += c
+    for seg, raw in M.fixture():
         out = M.inflate_emulate(seg[4:-4], raw - 4)
         assert len(out) == raw - 4
         assert out == zlib.decompress(seg[4:-4])
 
 
 # ------------------------------------------------------------------------------------------------ malformed streams
-class Bits:
-    """LSB-first bit string builder (Huffman codes are given MSB first, as RFC 1951 writes them)."""
-
-    def __init__(self):
-        self.bits = []
-
-    def put(self, v, n):
-        self.bits += [(v >> i) & 1 for i in range(n)]
-        return self
-
-    def huff(self, code, n):
-        self.bits += [(code >> (n - 1 - i)) & 1 for i in range(n)]
-        return self
-
-    def bytes(self):
-        b = self.bits + [0] * (-len(self.bits) % 8)
-        return bytes(sum(b[i + k] << k for k in range(8)) for i in range(0, len(b), 8))
-
-
-def _zhdr(cinfo=7, fdict=0):
-    cmf = (cinfo << 4) | 8
-    flg = fdict << 5
-    flg |= (31 - ((cmf << 8) | flg) % 31) % 31
-    return bytes([cmf, flg])
-
-
-def _adler(b):
-    return zlib.adler32(b).to_bytes(4, "big")
-
-
-def _malformed():
-    good = zlib.compress(b"hello hello hello hello", 6)
-    cases = {
-        "bad_check": b"\x78\x02" + good[2:],
-        "bad_method": bytes([0x77, good[1]]) + good[2:],
-        "fdict": _zhdr(fdict=1) + b"\0\0\0\0" + good[2:],
-        "btype3": _zhdr() + Bits().put(1, 1).put(3, 2).bytes() + b"\0" * 8,
-        "stored_nlen": _zhdr() + b"\x01\x05\x00\x00\x00hello" + _adler(b"hello"),
-        # code-length code: all 19 lengths 1 -> over-subscribed
-        "cl_oversubscribed": _zhdr() + Bits().put(1, 1).put(2, 2).put(0, 5).put(0, 5).put(15, 4).put(0x49249249249249, 57).bytes() + b"\0" * 8,
-        # code-length code: one code of length 1 -> incomplete (never allowed for this code)
-        "cl_incomplete": _zhdr() + Bits().put(1, 1).put(2, 2).put(0, 5).put(0, 5).put(0, 4).put(1, 3).put(0, 9).bytes() + b"\0" * 8,
-        # literal/length symbol 286 in a fixed block (8-bit code 11000110)
-        "len_symbol_286": _zhdr() + Bits().put(1, 1).put(1, 2).huff(0b11000110, 8).bytes() + b"\0" * 6,
-        # 'a', then length 3 (symbol 257, 0000001) with distance symbol 30 (11110)
-        "dist_symbol_30": _zhdr() + Bits().put(1, 1).put(1, 2).huff(0x30 + ord("a"), 8).huff(1, 7).huff(30, 5).huff(0, 7).bytes() + b"\0" * 4,
-        # length 3 at distance 1 before any output
-        "dist_too_far": _zhdr() + Bits().put(1, 1).put(1, 2).huff(1, 7).huff(0, 5).huff(0, 7).bytes() + b"\0" * 4,
-        "truncated": good[:-3],
-        "truncated_header": good[:1],
-        "adler": good[:-1] + bytes([good[-1] ^ 1]),
-        "trailing_garbage": good + b"\x00",
-        "trailing_partial_member": good + good[:5],
-    }
-    return cases, len(b"hello hello hello hello")
-
-
-@pytest.mark.parametrize("case", sorted(_malformed()[0]))
+@pytest.mark.parametrize("case", sorted(M.malformed()[0]))
 def test_reader_malformed_streams_fail_with_format_error(case):
-    cases, n = _malformed()
+    cases, n = M.malformed()
     z = cases[case]
     with pytest.raises(Exception):
         M.hadoop_inflate(z)

@@ -18,9 +18,9 @@ import tez_b200 as T
 from tez_b200 import native
 from tez_b200._lib import TezGpuError
 import codec_lanes_model as M
-import test_codec_cpu
-import test_lz4_cpu
-import test_zstd_cpu
+import codec_model as CM
+import lz4_model as L4
+import zstd_model as ZS
 
 pytestmark = pytest.mark.gpu
 CODECS = ["default", "lz4", "zstd"]
@@ -116,11 +116,11 @@ def test_corrupted_streams_the_emulation_refuses_fail_with_its_reason(codec):
 def _malformed(codec):
     """the malformed-stream tables of the CPU suites: [(name, stream, body length)]"""
     if codec == "default":
-        cases, n = test_codec_cpu._malformed()
+        cases, n = CM.malformed()
         return [(k, z, n) for k, z in sorted(cases.items())]
     if codec == "lz4":
-        return [(k, z, n) for k, (z, n) in sorted(test_lz4_cpu._malformed().items())]
-    return [(k, z, n) for k, (z, n, _) in sorted(test_zstd_cpu._malformed().items())]
+        return [(k, z, n) for k, (z, n) in sorted(L4.malformed().items())]
+    return [(k, z, n) for k, (z, n, _) in sorted(ZS.malformed().items())]
 
 
 @pytest.mark.parametrize("codec", CODECS)

@@ -8,14 +8,11 @@ import pytest
 
 import tez_b200 as T
 import codec_model as M
+import codec_table as CT
 import codec_writer_cases as W
 import lz4_model as L4
 import snappy_model as SN
 import zstd_model as ZS
-
-EMULATE = {T.CODEC_DEFAULT: M.deflate_emulate, T.CODEC_LZ4: L4.compress_emulate, T.CODEC_SNAPPY: SN.compress_emulate,
-           T.CODEC_ZSTD: ZS.compress_emulate}
-
 
 # ------------------------------------------------------------------------------------------------ stream parsers
 def lz4_sequences(chunk):
@@ -163,26 +160,6 @@ def zlib_chunks(z):
         pos = q + 4
 
 
-def independent_decode(codec, z, body):
-    if codec == T.CODEC_DEFAULT:
-        d = zlib.decompressobj()
-        out = d.decompress(z)
-        assert d.eof and not d.unused_data
-        return out
-    if codec == T.CODEC_LZ4:
-        if L4.liblz4() is None:
-            return L4.decode_stream(z, len(body))
-        return b"".join(L4.lz4_decompress_safe(c) for c in block_chunks(z, codec))
-    if codec == T.CODEC_SNAPPY:
-        out = SN.decode_stream(z, len(body))
-        if SN.pyarrow():
-            assert SN.decode_stream(z, len(body), chunk=SN.libsnappy_chunk) == out, "libsnappy and the model differ"
-        return out
-    if ZS.libzstd() is None:
-        pytest.skip("libzstd is not loadable here")
-    return ZS.hadoop_read(z, len(body))
-
-
 # ------------------------------------------------------------------------------------------------ the cases
 @pytest.mark.parametrize("name", list(W.GEOMETRY))
 def test_lengths_cover_every_schedule_edge(name):
@@ -208,8 +185,8 @@ def test_record_framing_absorbs_every_vint_width():
 def test_host_writer_decodes_to_every_body(name):
     g = W.GEOMETRY[name]
     for c in W.cases(g):
-        z = EMULATE[g.codec](c.body)
-        assert independent_decode(g.codec, z, c.body) == c.body, c
+        z = CT.CODECS[name].emulate(c.body)
+        assert CT.CODECS[name].independent(z, len(c.body)) == c.body, c
 
 
 @pytest.mark.parametrize("name", list(W.GEOMETRY))
@@ -217,7 +194,7 @@ def test_random_bodies_are_stored_literal_or_raw(name):
     g = W.GEOMETRY[name]
     for n in (g.slice + 1, g.chunk, 3 * g.chunk + 7):
         c = W.make_case(g, "random", n)
-        z = EMULATE[g.codec](c.body)
+        z = CT.CODECS[name].emulate(c.body)
         if g.codec == T.CODEC_DEFAULT:
             # every chunk is stored, except a last chunk of a few bytes, which is smaller as a fixed-Huffman block
             types = [t for t, _ in zlib_chunks(z)]
@@ -240,7 +217,7 @@ def test_slice_periodic_matches_reach_one_slice_back(name):
     """in every chunk, every lane after the first finds its first match exactly one slice back"""
     g = W.GEOMETRY[name]
     c = W.make_case(g, "slice_periodic", 2 * g.chunk + 100)
-    z = EMULATE[g.codec](c.body)
+    z = CT.CODECS[name].emulate(c.body)
     for k, ch in enumerate(block_chunks(z, g.codec)):
         parse = lz4_sequences(ch) if g.codec == T.CODEC_LZ4 else snappy_elements(ch)
         pos, first = 0, {}
@@ -263,7 +240,7 @@ def test_literal_gaps_are_literal_runs_across_lane_edges():
     for name in ("lz4", "snappy"):
         g = W.GEOMETRY[name]
         c = W.make_case(g, "literal_gaps", g.chunk)
-        z = EMULATE[g.codec](c.body)
+        z = CT.CODECS[name].emulate(c.body)
         ch = block_chunks(z, g.codec)[0]
         if name == "lz4":
             lits = [lit for lit, off, _ in lz4_sequences(ch) if off]

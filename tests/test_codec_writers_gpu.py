@@ -14,9 +14,9 @@ import tez_b200 as T
 from tez_b200 import native
 from tez_b200._lib import TezGpuError
 from oracle import tez_oracle as O
+import codec_table as CT
 import codec_writer_cases as W
 import combine_model as CM
-from test_codec_writers_cpu import EMULATE, independent_decode
 
 pytestmark = pytest.mark.gpu
 BUDGET = 16 << 30
@@ -26,10 +26,10 @@ _STREAM = {}
 
 def _stream(codec, body):
     """the host run of the writer on body, decoded once by an independent reader"""
-    key = (codec, body)
+    key = (codec.name, body)
     if key not in _STREAM:
-        z = EMULATE[codec](body)
-        assert independent_decode(codec, z, body) == body
+        z = codec.emulate(body)
+        assert codec.independent(z, len(body)) == body
         _STREAM[key] = z
     return _STREAM[key]
 
@@ -87,7 +87,7 @@ def check_file(codec, out, index, plain, pindex, bodies=None):
         raws.append(raw)
         want.append(body)
     assert pos == len(out)
-    imgs, _ = native.decode_segments(segs, raws, codec, BUDGET)
+    imgs, _ = native.decode_segments(segs, raws, codec.id, BUDGET)
     for i, (img, body) in enumerate(zip(imgs, want)):
         assert img[4:-4] == body, "the device reader's body of segment %d" % i
     return len(segs)
@@ -114,7 +114,7 @@ def test_sorter_crafted_partitions(name, send_empty):
         plain, pindex, _ = _sort(P, recs, parts, T.CODEC_NONE, send_empty)
         out, index, st = _sort(P, recs, parts, g.codec, send_empty)
         assert st["file_out_bytes"] == len(out)
-        nseg = check_file(g.codec, out, index, plain, pindex, None if send_empty else bodies)
+        nseg = check_file(CT.CODECS[name], out, index, plain, pindex, None if send_empty else bodies)
         assert nseg == len(recs) + (0 if send_empty else P - len(recs)), oname
 
 
@@ -142,7 +142,7 @@ def test_merger_crafted_partitions(name, send_empty, tmp_path):
             parts.append(p)
     plain, pindex = _merge(segs, parts, P, T.CODEC_NONE, send_empty, str(tmp_path))
     out, index = _merge(segs, parts, P, g.codec, send_empty, str(tmp_path))
-    check_file(g.codec, out, index, plain, pindex, None if send_empty else bodies)
+    check_file(CT.CODECS[name], out, index, plain, pindex, None if send_empty else bodies)
 
 
 @pytest.mark.parametrize("which", ["all", "first", "last"])
@@ -158,7 +158,7 @@ def test_many_partitions(name, which):
     for send_empty in (False, True):
         plain, pindex, _ = _sort(P, recs, parts, T.CODEC_NONE, send_empty)
         out, index, _ = _sort(P, recs, parts, g.codec, send_empty)
-        check_file(g.codec, out, index, plain, pindex)
+        check_file(CT.CODECS[name], out, index, plain, pindex)
 
 
 def _dev(a, dtype):
@@ -181,7 +181,7 @@ def test_output_bound_and_exact_capacity(name):
     P = 12 + 200 + 3
     plain, pindex, _ = _sort(P, recs, parts, T.CODEC_NONE, False)
     out, index, _ = _sort(P, recs, parts, g.codec, False)
-    check_file(g.codec, out, index, plain, pindex)
+    check_file(CT.CODECS[name], out, index, plain, pindex)
     kv, ko, kl, vl, vo = CM.pack(recs)
     kv = np.concatenate([kv, np.zeros(64, np.uint8)])
     kv_bytes = int(ko[-1]) + int(kl[-1]) + int(vl[-1])

@@ -159,48 +159,9 @@ def test_emulated_reader_decodes_the_fixture():
     assert max(multi) >= 3   # the long value's block
 
 
-def _blk(raw, *chunks):
-    return raw.to_bytes(4, "big") + b"".join(len(c).to_bytes(4, "big") + c for c in chunks)
-
-
-def _lit(data):
-    n = len(data)
-    if n < 15:
-        return bytes([n << 4]) + data
-    r, ext = n - 15, b""
-    while r >= 255:
-        ext += b"\xff"; r -= 255
-    return b"\xf0" + ext + bytes([r]) + data
-
-
-def _malformed():
-    good = _lit(b"hello world, hello")                      # 18 literal bytes
-    cases = {
-        "truncated_block_header": (_blk(18, good)[:2], 18),
-        "truncated_chunk_header": (_blk(18, good)[:6], 18),
-        "chunk_past_the_end": (_blk(18, good)[:-1], 18),
-        # 'a', then a match of 262,144 bytes at offset 1, then 5 literals: 262,150 bytes from a 1,038-byte chunk
-        "chunk_decodes_past_262144": (_blk(262150, b"\x1fa\x01\x00" + b"\xff" * 1027 + bytes([240]) + _lit(b"xxxxx")), 262150),
-        "block_raw_zero": (_blk(0, good) + _blk(18, good), 18),
-        "block_sum_too_large": (_blk(18, good) + _blk(18, good), 30),
-        "block_sum_too_small": (_blk(18, good), 20),
-        "trailing_bytes": (_blk(18, good) + b"\x00", 18),
-        "trailing_zero_block": (_blk(18, good) + b"\x00\x00\x00\x00", 18),
-        "over_decode": (_blk(10, good), 10),
-        "offset_zero": (_blk(13, bytes([0x40]) + b"abcd\x00\x00" + _lit(b"xxxxx")), 13),
-        "offset_too_far": (_blk(13, bytes([0x40]) + b"abcd\x05\x00" + _lit(b"xxxxx")), 13),
-        "literal_run_past_the_end": (_blk(19, bytes([0xF0, 4]) + b"hello world, hello"), 19),
-        "match_at_the_end": (_blk(8, bytes([0x40]) + b"abcd\x04\x00"), 8),
-        "short_last_literals": (_blk(9, bytes([0x40]) + b"abcd\x04\x00" + _lit(b"x")), 9),
-        "empty_chunk": (_blk(18, b""), 18),
-        "chunk_over_262144": (_blk(18, good)[:4] + (262145).to_bytes(4, "big") + good + bytes(262145 - len(good)), 18),
-    }
-    return cases
-
-
-@pytest.mark.parametrize("case", sorted(_malformed()))
+@pytest.mark.parametrize("case", sorted(M.malformed()))
 def test_malformed_streams_fail_with_format_error(case):
-    z, n = _malformed()[case]
+    z, n = M.malformed()[case]
     with pytest.raises(M.Lz4FormatError):
         M.decode_stream(z, n)
     with pytest.raises(TezGpuError) as e:
@@ -211,7 +172,7 @@ def test_malformed_streams_fail_with_format_error(case):
 
 def test_multi_chunk_block_decodes_on_the_exact_path():
     a, b = b"0123456789" * 3, b"abcdefghij" * 2
-    z = _blk(50, _lit(a), _lit(b)) + _blk(3, _lit(b"end"))
+    z = M.blk(50, M.lit(a), M.lit(b)) + M.blk(3, M.lit(b"end"))
     assert M.decode_stream(z, 53) == a + b + b"end" == M.decompress_emulate(z, 53)
 
 

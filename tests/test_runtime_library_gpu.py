@@ -14,20 +14,9 @@ import tez_b200 as T
 from tez_b200.runtime_library import (BYTES_WRITABLE, INT_WRITABLE, LONG_WRITABLE, TEXT, TEZ_BYTES_COMPARATOR, InputContext,
                                       LocalOutput, OrderedGroupedKVInput, OrderedPartitionedKVOutput, OutputContext,
                                       empty_partitions_from_payload, parse_proto)
+from plugin_runs import consume, run_output
 
 pytestmark = pytest.mark.gpu
-
-
-def _run_output(tmp, conf, records, P, uid="attempt_1_0001_1_00_000000_0_10001", mem=1 << 30):
-    ctx = OutputContext(conf, str(tmp), unique_identifier=uid, total_memory_available_to_task=mem)
-    out = OrderedPartitionedKVOutput(ctx, P)
-    assert out.initialize() == []
-    out.start()
-    w = out.getWriter()
-    for k, v in records:
-        w.write(k, v)
-    events = out.close()
-    return out, events
 
 
 @pytest.mark.parametrize("sorter", ["PIPELINED", "LEGACY"])
@@ -41,7 +30,7 @@ def test_output_lifecycle_files_events_counters(tmp_path, sorter, send_empty):
     conf = {"tez.runtime.key.class": TEXT, "tez.runtime.value.class": INT_WRITABLE, "tez.runtime.sorter.class": sorter,
             "tez.runtime.empty.partitions.info-via-events.enabled": send_empty,
             "tez.runtime.report.partition.stats": "precise"}
-    out, events = _run_output(tmp_path, conf, recs, P)
+    out, events = run_output(tmp_path, conf, recs, P)
     # files: output/<uid>/file.out + .index, mode 0640 (TezTaskOutputFiles, TezSpillRecord.SPILL_FILE_PERMS)
     f, fi = out.final_output_file, out.final_index_file
     assert f == str(tmp_path / "output" / out.context.unique_identifier / "file.out") and fi == f + ".index"
@@ -85,7 +74,7 @@ def test_multiple_spills_and_final_merge_match_single_sort(tmp_path):
     recs = [(bytes(r[:16]), bytes(r[16:])) for r in rows]
     conf = {"tez.runtime.key.class": BYTES_WRITABLE, "tez.runtime.key.comparator.class": TEZ_BYTES_COMPARATOR,
             "tez.runtime.io.sort.mb": 1}
-    out, events = _run_output(tmp_path, conf, recs, P)
+    out, events = run_output(tmp_path, conf, recs, P)
     assert out.num_spills >= 4
     exp = O.pipelined_sort_fixed(O.sorter_conf(P), kv, 16, 64)
     assert open(out.final_output_file, "rb").read() == exp["file_out"]
@@ -121,7 +110,7 @@ def test_final_merge_of_every_key_class_matches_single_sort(tmp_path, key_class,
     conf = {"tez.runtime.key.class": key_class, "tez.runtime.io.sort.mb": 1}
     if comparator_class:
         conf["tez.runtime.key.comparator.class"] = comparator_class
-    out, events = _run_output(tmp_path, conf, recs, P)
+    out, events = run_output(tmp_path, conf, recs, P)
     assert out.num_spills >= 4
     kv = b"".join(k + v for k, v in recs)
     ko = np.cumsum([0] + [len(k) + len(v) for k, v in recs[:-1]])
@@ -154,7 +143,7 @@ def test_multi_spill_final_merge_with_duplicate_keys(tmp_path, dup_pct):
     recs = [(k, zlib.crc32(k).to_bytes(4, "big") * 16) for k in keys]
     conf = {"tez.runtime.key.class": BYTES_WRITABLE, "tez.runtime.key.comparator.class": TEZ_BYTES_COMPARATOR,
             "tez.runtime.io.sort.mb": 1}
-    out, events = _run_output(tmp_path, conf, recs, P)
+    out, events = run_output(tmp_path, conf, recs, P)
     assert out.num_spills >= 4
     kv = np.frombuffer(b"".join(k + v for k, v in recs), dtype=np.uint8)
     rle = dup_pct > 10
@@ -177,7 +166,7 @@ def test_pipelined_shuffle_spill_events_reach_the_input(tmp_path):
     conf = {"tez.runtime.key.class": BYTES_WRITABLE, "tez.runtime.key.comparator.class": TEZ_BYTES_COMPARATOR,
             "tez.runtime.io.sort.mb": 1, "tez.runtime.enable.final-merge.in.output": False,
             "tez.runtime.report.partition.stats": "precise"}
-    out, events = _run_output(tmp_path, conf, recs, P)
+    out, events = run_output(tmp_path, conf, recs, P)
     S = out.num_spills
     assert S >= 3
     dms = [e for e in events if e.type == "CompositeDataMovementEvent"]
@@ -242,22 +231,6 @@ def test_custom_partitioner_results_are_passed_through(tmp_path):
     assert got == [list(range(-50, -10)), list(range(-10, 10)), list(range(10, 50))]
 
 
-def _consume(tmp, conf, producers, partition, P):
-    inp = OrderedGroupedKVInput(InputContext(conf, str(tmp)), len(producers))
-    inp.initialize()
-    inp.start()
-    evs = []
-    for i, (out, events) in enumerate(producers):
-        empties = empty_partitions_from_payload(events[-1].payload, P)
-        evs.append(LocalOutput(i, out.final_output_file, out.final_index_file, partition, empty=partition in empties))
-    inp.handleEvents(evs)
-    r = inp.getReader()
-    groups = []
-    while r.next():
-        groups.append((r.getCurrentKey(), list(r.getCurrentValues())))
-    return inp, groups
-
-
 def test_ordered_word_count_two_edges(tmp_path):
     """TestTezJobs.testOrderedWordCount (tez-tests/.../TestTezJobs.java:748-854): words a_1..a_10 with counts 20,18,..,2;
     tokenizer -> (word,1) -> summation -> (count, word) -> sorter: final order by count then the known answer."""
@@ -270,12 +243,12 @@ def test_ordered_word_count_two_edges(tmp_path):
     producers = []
     for t in range(3):                                   # three tokenizer tasks
         mine = words[t::3]
-        producers.append(_run_output(tmp_path / ("t%d" % t), conf1, [(O.text(w), O.int_writable(1)) for w in mine], P,
+        producers.append(run_output(tmp_path / ("t%d" % t), conf1, [(O.text(w), O.int_writable(1)) for w in mine], P,
                                      uid="attempt_1_0001_1_00_%06d_0_10001" % t))
     counts = {}
     records_seen = 0
     for p in range(P):                                   # P summation tasks
-        inp, groups = _consume(tmp_path / ("s%d" % p), conf1, producers, p, P)
+        inp, groups = consume(tmp_path / ("s%d" % p), conf1, producers, p, P)
         for k, vals in groups:
             word = k[1:].decode()
             assert word not in counts
@@ -287,9 +260,9 @@ def test_ordered_word_count_two_edges(tmp_path):
     assert counts == {"a_%d" % i: 22 - 2 * i for i in range(1, 11)}
     # second edge: (IntWritable count, Text word), one reducer (OrderedWordCount.java:156-160)
     conf2 = {"tez.runtime.key.class": INT_WRITABLE, "tez.runtime.value.class": TEXT}
-    prod2 = [_run_output(tmp_path / "sum", conf2, [(O.int_writable(c), O.text(w)) for w, c in counts.items()], 1,
+    prod2 = [run_output(tmp_path / "sum", conf2, [(O.int_writable(c), O.text(w)) for w, c in counts.items()], 1,
                          uid="attempt_1_0001_1_01_000000_0_10001")]
-    _, groups = _consume(tmp_path / "sorter", conf2, prod2, 0, 1)
+    _, groups = consume(tmp_path / "sorter", conf2, prod2, 0, 1)
     final = [(int.from_bytes(k, "big", signed=True), v[0][1:].decode()) for k, v in groups]
     assert final == [(22 - 2 * i, "a_%d" % i) for i in range(10, 0, -1)]
 
@@ -305,11 +278,11 @@ def test_input_groups_values_across_producers_and_skips_empty(tmp_path):
             k = bytes([rng.randint(0, 40)]) * rng.randint(1, 3)
             v = zlib.crc32(k).to_bytes(4, "big") + bytes([t])
             recs.append((k, v))
-        producers.append(_run_output(tmp_path / ("m%d" % t), conf, recs, P, uid="attempt_1_0001_1_00_%06d_0_1" % t))
+        producers.append(run_output(tmp_path / ("m%d" % t), conf, recs, P, uid="attempt_1_0001_1_00_%06d_0_1" % t))
         for k, v in recs:
             if O.partition_of(O.CMP_BYTES, k, P) == 1:
                 expect.setdefault(k, []).append(v)
-    inp, groups = _consume(tmp_path / "r1", conf, producers, 1, P)
+    inp, groups = consume(tmp_path / "r1", conf, producers, 1, P)
     assert [k for k, _ in groups] == sorted(expect)
     for k, vals in groups:
         assert sorted(vals) == sorted(expect[k])

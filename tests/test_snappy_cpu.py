@@ -130,49 +130,7 @@ def test_crafted_chunks_have_the_elements_their_names_claim():
         assert M.decompress_emulate(M.one_block([c]), M.preamble(c)[0]) == M.decode_chunk(c), name
 
 
-def _blk(raw, *chunks):
-    return raw.to_bytes(4, "big") + b"".join(len(c).to_bytes(4, "big") + c for c in chunks)
-
-
-def _malformed():
-    """{name: (stream, expect, reason)}"""
-    body = CM.wordcount_body(n=300, vocab=40, seed=1)
-    z = M.compress_emulate(body)
-    (raw, (c,)), = M.blocks(z)
-    abcd = M.lit(b"abcd")
-    return {
-        "preamble_runs_past_5_bytes": (_blk(8, b"\xff\xff\xff\xff\xff\x01" + abcd), 8, "invalid chunk preamble"),
-        "preamble_fifth_byte_over_15": (_blk(8, b"\x80\x80\x80\x80\x10" + abcd), 8, "invalid chunk preamble"),
-        "preamble_zero": (_blk(8, b"\x00", M.varint(8) + abcd + M.copy(4, 4, 1)), 8, "invalid chunk preamble"),
-        "preamble_over_262144": (_blk(300000, M.varint(262145) + abcd), 300000, "invalid chunk preamble"),
-        "preamble_truncated": (_blk(200, b"\xc8"), 200, "invalid chunk preamble"),
-        "offset_zero": (_blk(8, M.varint(8) + abcd + M.copy(0, 4, 1)), 8, "invalid copy offset"),
-        "offset_zero_copy4": (_blk(8, M.varint(8) + abcd + M.copy(0, 4, 4)), 8, "invalid copy offset"),
-        "offset_past_the_output": (_blk(8, M.varint(8) + abcd + M.copy(5, 4, 2)), 8, "invalid copy offset"),
-        "literal_past_the_chunk": (_blk(10, M.varint(10) + bytes([9 << 2]) + b"abc"), 10, "literal past the end of the chunk"),
-        "literal_length_bytes_past_the_chunk": (_blk(100, M.varint(100) + bytes([61 << 2, 99])), 100, "literal past the end of the chunk"),
-        "copy_past_the_chunk": (_blk(8, M.varint(8) + abcd + bytes([2 | (3 << 2), 4])), 8, "copy past the end of the chunk"),
-        "copy4_past_the_chunk": (_blk(8, M.varint(8) + abcd + bytes([3 | (3 << 2), 4, 0, 0])), 8, "copy past the end of the chunk"),
-        "short_output": (_blk(9, M.varint(9) + abcd + M.copy(4, 4, 1)), 9, "chunk decodes short of its preamble length"),
-        "long_output_copy": (_blk(7, M.varint(7) + abcd + M.copy(4, 4, 1)), 7, "chunk decodes past its preamble length"),
-        "long_output_literal": (_blk(3, M.varint(3) + abcd), 3, "chunk decodes past its preamble length"),
-        "trailing_element": (_blk(4, M.varint(4) + abcd + M.copy(4, 4, 1)), 4, "chunk decodes past its preamble length"),
-        "trailing_bytes": (z + b"\0\0\0\0", len(body), "bytes after the last block"),
-        "chunks_short_of_the_block": (_blk(raw + 1, c), len(body) + 1, "truncated block header"),
-        "chunks_past_the_block": (_blk(raw - 1, c), len(body) - 1, "chunks decode past their block's raw length"),
-        "blocks_short_of_rawlength": (z, len(body) + 1, "decompressed length differs from rawLength - 4"),
-        "blocks_past_rawlength": (z, len(body) - 1, "block raw length outside the remaining rawLength - 4"),
-        "block_raw_zero": (_blk(0, c), len(body), "block raw length outside the remaining rawLength - 4"),
-        "chunk_over_262144": (_blk(8, b"") [:4] + (262145).to_bytes(4, "big") + b"\0" * 262145, 8,
-                              "chunk length over 262144 or past the end of the stream"),
-        "chunk_past_the_stream": (z[:-1], len(body), "chunk length over 262144 or past the end of the stream"),
-        "truncated_header": (z[:6], len(body), "truncated block header"),
-        "second_of_two_chunks_bad": (_blk(16, M.varint(8) + abcd + M.copy(4, 4, 1), M.varint(8) + abcd + M.copy(9, 4, 1)), 16,
-                                     "invalid copy offset"),
-    }
-
-
-MALFORMED = _malformed()
+MALFORMED = M.malformed()
 
 
 @pytest.mark.parametrize("case", sorted(MALFORMED))
@@ -188,20 +146,12 @@ def test_malformed_streams_fail_with_format_error(case):
 def test_first_error_in_stream_order_wins():
     """a walk error after a bad chunk: the chunk's reason, as the serial emulation meets it"""
     abcd = M.lit(b"abcd")
-    z = _blk(8, M.varint(8) + abcd + M.copy(0, 4, 1)) + b"\0\0"
+    z = M.blk(8, M.varint(8) + abcd + M.copy(0, 4, 1)) + b"\0\0"
     with pytest.raises(TezGpuError, match="invalid copy offset"):
         M.decompress_emulate(z, 16)
-    z = _blk(8, M.varint(8) + abcd + M.copy(4, 4, 1)) + b"\0\0"
+    z = M.blk(8, M.varint(8) + abcd + M.copy(4, 4, 1)) + b"\0\0"
     with pytest.raises(TezGpuError, match="truncated block header"):
         M.decompress_emulate(z, 16)
-
-
-def corpus_streams():
-    """(body, stream) pairs the mutant corpus corrupts: device-written, Java-framed libsnappy-like and crafted"""
-    bodies = [CM.wordcount_body(n=300, vocab=40, seed=s) for s in range(3)] + [random.Random(9).randbytes(600)]
-    res = [(b, M.compress_emulate(b)) for b in bodies]
-    res += [(M.decode_chunk(c), M.one_block([c])) for _, c in M.crafted_chunks() if len(c) < 4096]
-    return res
 
 
 def _verdict(fn):
@@ -215,7 +165,7 @@ def test_mutants_emulation_model_and_libsnappy_agree():
     """3000 seeded mutants: the emulation and the model give the same bytes or the same reason; libsnappy (framing
     as ours) decodes the same ones to the same bytes."""
     fails = 0
-    for i, (z, e) in enumerate(M.mutants(corpus_streams(), 3000, seed=4321)):
+    for i, (z, e) in enumerate(M.mutants(M.corpus_streams(), 3000, seed=4321)):
         emu = _verdict(lambda: M.decompress_emulate(z, e))
         mod = _verdict(lambda: M.decode_stream(z, e))
         assert emu == mod, (i, z.hex(), e)

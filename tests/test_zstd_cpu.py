@@ -166,78 +166,19 @@ def test_reader_agrees_with_libzstd_on_tiny_and_rle_bodies(body):
     assert kinds >= {1}
 
 
-# ---- hand-made streams: one for every error reason
-def _bh(last, bt, size):
-    return (int(last) | bt << 1 | size << 3).to_bytes(3, "little")
-
-
-def _frame(content, fcs=None, checksum=None, fhd_extra=0, window=None, did=None):
-    """a frame of the given block bytes; Single_Segment with a 1-byte Frame_Content_Size when fcs is given, else a
-    Window_Descriptor byte (default 0: 1 KiB)"""
-    fhd = fhd_extra | (4 if checksum is not None else 0) | (1 if did is not None else 0)
-    h = b""
-    if fcs is not None:
-        fhd |= 0x20
-    else:
-        h += bytes([window or 0])
-    if did is not None:
-        h += bytes([did])
-    if fcs is not None:
-        h += bytes([fcs])
-    return M.MAGIC + bytes([fhd]) + h + content + (checksum if checksum is not None else b"")
-
-
-def _raw(data, last=True):
-    return _bh(last, 0, len(data)) + data
-
-
-def _seq_block(lit, ll_sym, of_sym, ml_sym, bits):
-    """a compressed block: raw literals, one sequence with RLE tables for LL / OF / ML, and its bitstream"""
-    content = bytes([len(lit) << 3]) + lit + bytes([1, 0x54, ll_sym, of_sym, ml_sym]) + bits
-    return _bh(True, 2, len(content)) + content
-
-
-def _malformed():
-    good = _frame(_raw(b"abcd"), fcs=4)
-    return {
-        # name: (stream, expected body length, reason)
-        "bad_magic": (b"\x00" * 4 + good, 4, "bad frame magic"),
-        "reserved_bit": (_frame(_raw(b"abcd"), fcs=4, fhd_extra=0x08), 4, "reserved bit set"),
-        "reserved_sequence_modes": (_frame(_bh(True, 2, 7) + bytes([0x20]) + b"abcd" + bytes([1, 0x01])), 4, "reserved bit set"),
-        "dictionary_id": (_frame(_raw(b"abcd"), fcs=4, did=5), 4, "dictionary id set"),
-        "window_too_large": (_frame(_raw(b"abcd"), window=18 << 3), 4, "window size over 2^27"),
-        "block_type_3": (_frame(_bh(True, 3, 4) + b"abcd", fcs=4), 4, "reserved block type"),
-        "block_over_maximum": (_frame(_raw(b"abcdefgh"), fcs=4), 4, "block over Block_Maximum_Size"),
-        "treeless_without_table": (_frame(_bh(True, 2, 6) + bytes([0x43, 0x40, 0x00, 0x00, 0x00, 0x00])), 4,
-                                   "malformed literals section"),
-        "bytes_after_zero_sequences": (_frame(_bh(True, 2, 7) + bytes([0x20]) + b"abcd" + b"\x00\x00"), 4,
-                                       "malformed sequences section"),
-        "sequence_bitstream_zero_last_byte": (_frame(_seq_block(b"abcd", 4, 0, 1, b"\x00")), 8, "bitstream not consumed exactly"),
-        "sequence_bitstream_left_over": (_frame(_seq_block(b"abcd", 4, 0, 1, b"\x07")), 8, "bitstream not consumed exactly"),
-        "offset_beyond_output": (_frame(_seq_block(b"abcd", 4, 5, 1, b"\x20")), 8, "invalid match offset"),
-        "offset_zero": (_frame(_seq_block(b"abcd", 0, 1, 1, b"\x03")), 8, "invalid match offset"),
-        "content_size_mismatch": (_frame(_raw(b"abcd"), fcs=5), 5, "decoded size differs from Frame_Content_Size"),
-        "checksum_mismatch": (_frame(_raw(b"abcd"), fcs=4, checksum=b"\x00\x01\x02\x03"), 4, "content checksum mismatch"),
-        "frames_short_of_raw_length": (good, 6, "decompressed length differs from rawLength - 4"),
-        "frames_past_raw_length": (good + good, 6, "decompressed length differs from rawLength - 4"),
-        "trailing_bytes": (good + b"xy", 4, "bytes after the last frame"),
-        "truncated": (good[:-1], 4, "truncated frame"),
-    }
-
-
 def test_hand_made_valid_sequences_decode_like_libzstd():
     """the builders of the malformed cases make valid streams with valid parameters: a repeat offset (offset 1); the
     compressed blocks go into frames with a 1 KiB window, as a Single_Segment frame's Block_Maximum_Size would be its
     content size"""
-    z = _frame(_seq_block(b"abcd", 4, 0, 1, b"\x01"))
+    z = M.make_frame(M.seq_block(b"abcd", 4, 0, 1, b"\x01"))
     assert M.decompress_emulate(z, 8) == b"abcddddd"
     if M.libzstd():
         assert M.hadoop_read(z, 8) == b"abcddddd"
 
 
-@pytest.mark.parametrize("case", sorted(_malformed()))
+@pytest.mark.parametrize("case", sorted(M.malformed()))
 def test_malformed_streams_fail_with_format_error(case):
-    z, n, reason = _malformed()[case]
+    z, n, reason = M.malformed()[case]
     with pytest.raises(TezGpuError) as e:
         M.decompress_emulate(z, n)
     assert e.value.code == T.E_FORMAT

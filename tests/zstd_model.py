@@ -207,3 +207,62 @@ def fixture():
         pos += e["part_length"]
     assert pos == len(data)
     return res
+
+
+# ---- hand-made streams: one for every error reason
+def block_header(last, bt, size):
+    return (int(last) | bt << 1 | size << 3).to_bytes(3, "little")
+
+
+def make_frame(content, fcs=None, checksum=None, fhd_extra=0, window=None, did=None):
+    """a frame of the given block bytes; Single_Segment with a 1-byte Frame_Content_Size when fcs is given, else a
+    Window_Descriptor byte (default 0: 1 KiB)"""
+    fhd = fhd_extra | (4 if checksum is not None else 0) | (1 if did is not None else 0)
+    h = b""
+    if fcs is not None:
+        fhd |= 0x20
+    else:
+        h += bytes([window or 0])
+    if did is not None:
+        h += bytes([did])
+    if fcs is not None:
+        h += bytes([fcs])
+    return MAGIC + bytes([fhd]) + h + content + (checksum if checksum is not None else b"")
+
+
+def raw_block(data, last=True):
+    return block_header(last, 0, len(data)) + data
+
+
+def seq_block(lit, ll_sym, of_sym, ml_sym, bits):
+    """a compressed block: raw literals, one sequence with RLE tables for LL / OF / ML, and its bitstream"""
+    content = bytes([len(lit) << 3]) + lit + bytes([1, 0x54, ll_sym, of_sym, ml_sym]) + bits
+    return block_header(True, 2, len(content)) + content
+
+
+def malformed():
+    good = make_frame(raw_block(b"abcd"), fcs=4)
+    return {
+        # name: (stream, expected body length, reason)
+        "bad_magic": (b"\x00" * 4 + good, 4, "bad frame magic"),
+        "reserved_bit": (make_frame(raw_block(b"abcd"), fcs=4, fhd_extra=0x08), 4, "reserved bit set"),
+        "reserved_sequence_modes": (make_frame(block_header(True, 2, 7) + bytes([0x20]) + b"abcd" + bytes([1, 0x01])), 4, "reserved bit set"),
+        "dictionary_id": (make_frame(raw_block(b"abcd"), fcs=4, did=5), 4, "dictionary id set"),
+        "window_too_large": (make_frame(raw_block(b"abcd"), window=18 << 3), 4, "window size over 2^27"),
+        "block_type_3": (make_frame(block_header(True, 3, 4) + b"abcd", fcs=4), 4, "reserved block type"),
+        "block_over_maximum": (make_frame(raw_block(b"abcdefgh"), fcs=4), 4, "block over Block_Maximum_Size"),
+        "treeless_without_table": (make_frame(block_header(True, 2, 6) + bytes([0x43, 0x40, 0x00, 0x00, 0x00, 0x00])), 4,
+                                   "malformed literals section"),
+        "bytes_after_zero_sequences": (make_frame(block_header(True, 2, 7) + bytes([0x20]) + b"abcd" + b"\x00\x00"), 4,
+                                       "malformed sequences section"),
+        "sequence_bitstream_zero_last_byte": (make_frame(seq_block(b"abcd", 4, 0, 1, b"\x00")), 8, "bitstream not consumed exactly"),
+        "sequence_bitstream_left_over": (make_frame(seq_block(b"abcd", 4, 0, 1, b"\x07")), 8, "bitstream not consumed exactly"),
+        "offset_beyond_output": (make_frame(seq_block(b"abcd", 4, 5, 1, b"\x20")), 8, "invalid match offset"),
+        "offset_zero": (make_frame(seq_block(b"abcd", 0, 1, 1, b"\x03")), 8, "invalid match offset"),
+        "content_size_mismatch": (make_frame(raw_block(b"abcd"), fcs=5), 5, "decoded size differs from Frame_Content_Size"),
+        "checksum_mismatch": (make_frame(raw_block(b"abcd"), fcs=4, checksum=b"\x00\x01\x02\x03"), 4, "content checksum mismatch"),
+        "frames_short_of_raw_length": (good, 6, "decompressed length differs from rawLength - 4"),
+        "frames_past_raw_length": (good + good, 6, "decompressed length differs from rawLength - 4"),
+        "trailing_bytes": (good + b"xy", 4, "bytes after the last frame"),
+        "truncated": (good[:-1], 4, "truncated frame"),
+    }
